@@ -1,22 +1,22 @@
 #!/usr/bin/env python
-"""bench.py — benchmarks of the zstdmt hot path on B200 (one JSON line per run, the driver's contract).
+"""bench.py — benchmarks of the zstdmt hot path on H100 (one JSON line per run).
 
-    python bench.py --gpus N --steps K --warmup W [--mode M]        (N>1: under torchrun, one rank per GPU)
+    python bench.py --gpus N --steps K --warmup W [--mode M] [--dump-outputs DIR]   (N>1: under torchrun, one rank per GPU)
     python bench.py --impl reference [--mode M] ...                  (the reference's own pthread + liblz4/libzstd path on the host cores)
 
 Modes = the BASELINE.json configs (default: lz4-compress, the config the headline metric is quoted on):
     lz4-compress    configs[1]  lz4-mt level 1, 8 GiB Silesia-mix per GPU, 1 MiB chunks                 (weak scaling)
-    lz4-decompress  configs[2]  lz4-mt decompress-only, 32 GiB stream framed by the REFERENCE, 1->8 GPUs  (strong scaling)
+    lz4-decompress  configs[2]  lz4-mt decompress-only, 16 GiB stream framed by the REFERENCE, 1->8 GPUs  (strong scaling)
     zstd-compress   configs[3]  zstd-mt level 3, 8 GiB synthetic text per GPU, 1 MiB chunks              (weak scaling)
     zstd-mix        configs[4]  zstd-mt level 3, Silesia-mix, 4 MiB chunks, 8 GiB per GPU (64 GiB at 8)  (weak scaling)
-The default run also carries short device-timed legs of the other configs in `extra` (so the driver's 1->8 sweep
-records them at every N); `--no-extra` drops them.
+The default run also carries short device-timed legs of the other configs in `extra` (so a 1->8 GPU sweep records
+them at every N); `--no-extra` drops them.
 
 A step = one pass of the per-chunk hot path over the whole batch:
   value    : GB/s of (bytes in + bytes out), device-timed with CUDA events, inputs resident in HBM, max over ranks
   e2e      : the same metric through the reference-shaped callback API with HOST buffers — ONE call on rank 0 that deals
              its batches over all N GPUs (ZSTDMT_GPUS=0..N-1) and reassembles the frames in order; H2D/D2H inside
-  roofline : the dominant kernel of the mode against the measured HBM copy peak
+  roofline : the dominant kernel of the mode against the HBM peak
   cpu_baseline : the unmodified reference (oracle/_ref) on this box's cores, bounded sample (N=1 only)
 Multi-GPU: chunks are dealt round-robin in batches of 8 (the product's granularity), no collective on the data path.
 """
@@ -42,10 +42,10 @@ MODES = {
     "lz4-compress": dict(codec="lz4", op="c", kind="mix", chunk_mib=1, gib=8.0, level=1, scaling="weak",
                          metric="lz4-mt level-1 compress throughput, bytes in + framed bytes out",
                          workload="lz4-mt level 1, 8 GiB synthetic Silesia-mix generator, 1 MiB chunks, per GPU (BASELINE configs[1])"),
-    "lz4-decompress": dict(codec="lz4", op="d", kind="mix", chunk_mib=1, gib=32.0, level=1, scaling="strong",
+    "lz4-decompress": dict(codec="lz4", op="d", kind="mix", chunk_mib=1, gib=16.0, level=1, scaling="strong",
                            metric="lz4-mt decompress throughput, framed bytes in + bytes out",
-                           workload="lz4-mt decompress-only, 32 GiB stream pre-framed by the reference (LZ4MT_compressCCtx level 1, 1 MiB chunks, "
-                                    "linked blocks; a 2 GiB framed Silesia-mix segment tiled 16x), split over the GPUs (BASELINE configs[2])"),
+                           workload="lz4-mt decompress-only, 16 GiB stream pre-framed by the reference (LZ4MT_compressCCtx level 1, 1 MiB chunks, "
+                                    "linked blocks; a 2 GiB framed Silesia-mix segment tiled 8x), split over the GPUs (BASELINE configs[2])"),
     "zstd-compress": dict(codec="zstd", op="c", kind="text", chunk_mib=1, gib=8.0, level=3, scaling="weak",
                           metric="zstd-mt level-3 compress throughput, bytes in + framed bytes out",
                           workload="zstd-mt level 3, 8 GiB synthetic text, 1 MiB chunks, per GPU (BASELINE configs[3])"),
@@ -70,9 +70,15 @@ def parse_args():
     ap.add_argument("--ref-sample-gib", type=float, default=float(os.environ.get("ZMT_BENCH_REF_GIB", "2")))
     ap.add_argument("--e2e-steps", type=int, default=0, help="steps of the end-to-end leg (default min(steps, 8))")
     ap.add_argument("--no-extra", action="store_true")
-    ap.add_argument("--no-e2e", action="store_true", help="device-timed leg only (profiling runs under ncu)")
+    ap.add_argument("--no-e2e", action="store_true", help="device-timed leg only (profiling runs)")
     ap.add_argument("--no-bind", action="store_true", help="do not bind the rank's process to the CPUs next to its GPU")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy (rank 0), "
+                         "with DIR/inputs.json naming where the inputs came from")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs writes the GPU path's outputs; the reference arm has none to write")
+    return args
 
 
 def measured_peaks():
@@ -82,7 +88,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
 class ClockSampler:
@@ -128,18 +134,6 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
-
-
-def traffic_per_launch(kernel_key, algorithmic_bytes):
-    """DRAM bytes per launch of a kernel: dram__bytes_read.sum + dram__bytes_write.sum of ONE ncu --set full capture
-    (profiles/r2_traffic.json, else r1; made at a smaller size), scaled by algorithmic bytes to this launch."""
-    for name in ("r2_traffic.json", "r1_traffic.json"):
-        try:
-            t = json.load(open(os.path.join(ROOT, "profiles", name)))[kernel_key]
-            return float(t["dram_bytes"]) / float(t["algorithmic_bytes"]) * algorithmic_bytes
-        except Exception:
-            continue
-    return None
 
 
 def cpu_model():
@@ -238,7 +232,7 @@ def run_reference(args):
         "impl": "reference", "metric": M["metric"], "value": gbs, "unit": "GB/s",
         "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": tot / args.steps * 1e3,
         "higher_is_better": True, "scaling": M["scaling"], "vs_baseline": None, "dtype": "u8", "data": "synthetic",
-        "config": {"workload": M["workload"] + " — this arm: a %d MiB sample of it per step (a throughput; the B200 arm runs the full size)" % (n >> 20),
+        "config": {"workload": M["workload"] + " — this arm: a %d MiB sample of it per step (a throughput; the GPU arm runs the full size)" % (n >> 20),
                    "mode": args.mode, "chunk_bytes": chunk, "sample_bytes_per_step": n, "threads": threads},
         "cpu_baseline": {"value": gbs, "unit": "GB/s", "cores": threads, "kind": "reference", "sample": sample, "cpu_model": cpu_model()},
         "e2e": {"value": gbs, "unit": "GB/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -247,7 +241,7 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-# =============================================================================== B200 arm
+# =============================================================================== GPU arm
 class Job:
     """torch.distributed plumbing: NCCL for the timing all-reduces, a gloo group for host-side barriers."""
 
@@ -308,6 +302,29 @@ def to_device(torch, host, d=None):
     return d
 
 
+DUMP_SAMPLES = 4 << 20    # positions sampled from a byte stream too large to dump whole (16 MB as float32)
+
+
+def dump_outputs(job, out_dir, inputs, arrays):
+    """--dump-outputs: `arrays` maps a name to (device tensor, whole).  A whole array is written as float64 (offsets,
+    sizes, statuses: exact below 2**53); a byte stream as float32 at DUMP_SAMPLES positions drawn with a fixed seed from
+    its length, so two builds that return the same bytes write the same files.  `inputs` (written as inputs.json) says
+    where the inputs came from: dumps are only comparable when it is the same.  Rank 0 only."""
+    if out_dir is None or job.rank != 0:
+        return
+    torch = job.torch
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "inputs.json"), "w") as f:
+        json.dump(inputs, f, indent=1)
+    for name, (t, whole) in arrays.items():
+        if whole:
+            a = t.cpu().numpy().astype(np.float64)
+        else:
+            pos = np.sort(np.random.default_rng(0).integers(0, max(t.numel(), 1), size=min(t.numel(), DUMP_SAMPLES)))
+            a = t[torch.from_numpy(pos).to(t.device)].cpu().numpy().astype(np.float32)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def timed_steps(job, L, fn, steps, warmup):
     """W untimed + K timed calls of fn() on job.stream, bracketed by barrier + synchronize; per-kernel CUDA-event times
     from zmt_prof_*.  Returns (max-over-ranks ms total, this rank's ms total, kernel ms per launch[], launches[], clocks)."""
@@ -341,7 +358,7 @@ def roofline(kms, algorithmic_bytes, ids):
         return None
     achieved = algorithmic_bytes / (kms[k] * 1e-3) / 1e9
     return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic_per_launch(KERNEL_NAMES[k], algorithmic_bytes), "kernel": KERNEL_NAMES[k], "kernel_ms": kms[k],
+            "kernel": KERNEL_NAMES[k], "kernel_ms": kms[k],
             "peak_source": peak_src, "algorithmic_bytes_per_launch": algorithmic_bytes}
 
 
@@ -391,6 +408,9 @@ def leg_compress(job, args, M, gib, steps, warmup, full):
     comp = (z.Lz4DeviceCompressor if lz4 else z.ZstdDeviceCompressor)(n, chunk)
     dev_ms, my_ms, kms, cnt, clocks = timed_steps(job, L, lambda: comp.run(d_in, job.stream), steps, warmup)
     framed = int(comp.frame_off[-1].item())
+    if full:
+        dump_outputs(job, args.dump_outputs, {"mode": args.mode, "workload": M["workload"], "bytes": n},
+                     {"frame_off": (comp.frame_off, True), "framed_sample": (comp.out[:framed], False)})
     alg_mine = n + framed
     total_alg = job.reduce(alg_mine, "sum")
     ids = [0, 1, 2, 3, 4] if lz4 else [7, 8]
@@ -524,7 +544,7 @@ def cpu_baseline(args, M, src, n, chunk, codec_fn_c, codec_fn_d, with_decode):
 
 
 # ------------------------------------------------------------------------------- decompress leg (configs[2])
-def leg_lz4_decompress(job, args, M, total_gib, steps, warmup, seg_gib=2.0):
+def leg_lz4_decompress(job, args, M, total_gib, steps, warmup, seg_gib=2.0, dump=False):
     """Device-timed decode of a stream framed by the reference: a `seg_gib` framed segment tiled to `total_gib`, tiles
     dealt round-robin over the ranks (strong scaling).  Falls back to a GPU-framed segment when oracle/_ref is absent."""
     import zstdmt_b200 as z
@@ -566,6 +586,9 @@ def leg_lz4_decompress(job, args, M, total_gib, steps, warmup, seg_gib=2.0):
     for i in range(k):
         assert torch.equal(dout[i * seg:(i + 1) * seg], d_src), "decode of the reference-framed stream differs from the source (tile %d)" % i
     dev_ms, my_ms, kms, cnt, clocks = timed_steps(job, L, run, steps, warmup)
+    if dump:
+        dump_outputs(job, args.dump_outputs, {"mode": args.mode, "workload": M["workload"], "bytes": seg * tiles, "framed_by": framer},
+                     {"status": (dec.status, True), "out_size": (dec.out_size, True), "out_sample": (dec.out, False)})
     alg_mine = (framed.size + seg) * len(mine)
     total_alg = job.reduce(alg_mine, "sum")
     ids = [5, 10, 6]
@@ -634,12 +657,12 @@ def run_b200(args):
             if job.rank == 0:
                 extra["decompress_own_stream"]["e2e_gbs"] = v
         cfg_par = "chunks dealt round-robin in batches of %d over %d GPU(s), no collective" % (DEAL_BATCH, job.world)
-        l2 = "inputs (%.1f GiB per GPU) larger than L2" % (leg["n"] / GIB)
+        l2 = "inputs (%.1f GiB per GPU) larger than the 50 MB L2" % (leg["n"] / GIB)
     else:
-        leg = leg_lz4_decompress(job, args, M, size, steps, warmup)
+        leg = leg_lz4_decompress(job, args, M, size, steps, warmup, dump=True)
         e2e = None if args.no_e2e else e2e_lz4_decompress(job, leg, min(e2e_steps, 5))
         cfg_par = "tiles of the framed stream dealt round-robin over %d GPU(s), no collective" % job.world
-        l2 = "inputs (%.1f GiB framed per GPU) larger than L2" % (leg["alg_mine"] / GIB / 2)
+        l2 = "inputs (%.1f GiB framed per GPU) larger than the 50 MB L2" % (leg["alg_mine"] / GIB / 2)
     line = {
         "metric": M["metric"], "value": leg["value"], "unit": "GB/s", "n_gpus": job.world, "steps": steps, "warmup": warmup,
         "ms_per_step": leg["ms_per_step"], "higher_is_better": True, "scaling": M["scaling"], "vs_baseline": None, "dtype": "u8", "data": "synthetic",
@@ -676,7 +699,7 @@ def run_b200(args):
                     os.sched_setaffinity(0, cpus)
         except Exception as e:  # the baseline must never take the GPU result down with it
             line["cpu_baseline"] = {"value": None, "unit": "GB/s", "cores": 0, "kind": "reference", "sample": "failed: %r" % (e,)}
-    # ---- short legs of the other configs (device-timed; recorded at every N by the driver's sweep)
+    # ---- short legs of the other configs (device-timed; recorded at every N of a GPU-count sweep)
     if not args.no_extra and args.mode == "lz4-compress":
         leg.pop("_keep", None)
         del h_out

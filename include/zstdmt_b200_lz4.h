@@ -1,12 +1,12 @@
 /* zstdmt_b200_lz4.h — drop-in C boundary for the LZ4 half of zstdmt's hot path.
  *
- * libzstdmt_b200.so exports every symbol that /root/reference/lib/lz4-mt.h
+ * libzstdmt_b200.so exports every symbol that lib/lz4-mt.h
  * declares (lz4-mt.h:39-61 error handling, :67-89 buffer + callbacks, :106-159
  * contexts), with the same argument meaning and error convention, so a program
  * written against the reference (programs/lz4-mt.c:24-43 -> programs/main.c)
  * links against this library unchanged.  Behind the boundary the pthread pool +
  * liblz4 of lib/lz4-mt_compress.c / lib/lz4-mt_decompress.c is replaced by a
- * host pipeline feeding sm_100a CUDA kernels (DESIGN.md).
+ * host pipeline feeding sm_90a CUDA kernels (DESIGN.md).
  *
  * Each entry point cites the reference definition it replaces.
  */

@@ -1,6 +1,6 @@
 /* zstdmt_b200_zstd.h — drop-in C boundary for the Zstandard half of zstdmt's hot path.
  *
- * Same contract as /root/reference/lib/zstd-mt.h (:41-60 errors, :67-93 buffer +
+ * Same contract as lib/zstd-mt.h (:41-60 errors, :67-93 buffer +
  * callbacks, :115-205 contexts).  The symbols the reference really exports carry
  * the ZSTDCB_ prefix (programs/zstd-mt.c:24-43 binds them); the ZSTDMT_ names of
  * lib/README.md:43-76 / BASELINE.json are exported as aliases of the same code.

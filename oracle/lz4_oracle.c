@@ -3,12 +3,12 @@
  * CPU restatement of the LZ4 side of zstdmt's per-chunk hot path:
  *   - XXH32                      (content + header checksum inside LZ4F; liblz4 v1.9.4 xxhash.c [ext])
  *   - LZ4 block decode           (what LZ4F_decompress does per block; call site
- *                                 /root/reference/lib/lz4-mt_decompress.c:349-351)
+ *                                 lib/lz4-mt_decompress.c:349-351)
  *   - LZ4 frame decode / encode  (LZ4F_compressFrame call site lib/lz4-mt_compress.c:280-283;
  *                                 preferences lib/lz4-mt_compress.c:141-146)
  *   - the 12-byte skippable container (lib/lz4-mt_compress.c:293-298 write,
  *                                 lib/lz4-mt_decompress.c:192-281 read)
- *   - orc_lz4_block_compress_b200: the bit-exact CPU twin of OUR sm_100a
+ *   - orc_lz4_block_compress_b200: the bit-exact CPU twin of OUR sm_90a
  *     compressor (the reference's compressed bytes are not a parity target;
  *     BASELINE.json north_star: "produces a stream the reference CPU path
  *     decompresses to the identical input").
@@ -98,7 +98,7 @@ long orc_lz4_block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size
     return (long)(op - dst);
 }
 
-/* --------------------------------- B200 compressor twin (deterministic spec)
+/* --------------------------------- GPU compressor twin (deterministic spec)
  * Spec shared with zstdmt_b200/csrc/lz4_kernels.cu (DESIGN.md "LZ4 encoder"):
  *   eligible(i)  : i + 12 <= n                (LZ4 MFLIMIT: no match starts in the last 12 bytes)
  *   v(i)         : LE32 at i;  h(i) = (v * 2654435761) >> 20          (12-bit hash)

@@ -3,7 +3,7 @@
  * Hand-declared subset of the liblz4 v1.9.4 frame API (public ABI of
  * /usr/lib/x86_64-linux-gnu/liblz4.so.1.9.4; the image ships the .so but no
  * dev headers).  Exists only so that the UNMODIFIED reference wrapper
- * (/root/reference/lib/lz4-mt_*.c) can be compiled into oracle/_ref/ — see
+ * (lib/lz4-mt_*.c) can be compiled into oracle/_ref/ — see
  * oracle/Makefile.  Struct layouts follow the documented v1.9.4 ABI
  * (sizeof(LZ4F_frameInfo_t)==32, sizeof(LZ4F_preferences_t)==56; checked by
  * tests/test_oracle_ref.py).  Nothing in the product links against this.

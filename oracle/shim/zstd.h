@@ -2,7 +2,7 @@
  *
  * Hand-declared subset of the libzstd stable API (ABI of the image's
  * /usr/lib/x86_64-linux-gnu/libzstd.so.1.5.5; no dev headers installed).
- * Lets the UNMODIFIED reference wrapper (/root/reference/lib/zstd-mt_*.c)
+ * Lets the UNMODIFIED reference wrapper (lib/zstd-mt_*.c)
  * compile into oracle/_ref/ (oracle/Makefile).  The reference pins v1.5.6
  * (programs/Makefile:11); 1.5.5 is format-identical.  Not used by the product.
  */

@@ -2,8 +2,8 @@
  *
  * CPU restatement of the Zstandard frame decoder (RFC 8878 [ext]) — the
  * arithmetic behind ZSTD_decompressStream at
- * /root/reference/lib/zstd-mt_decompress.c:456,625 (libzstd v1.5.6 is a
- * build-time clone, programs/Makefile:11,245, not in /root/reference).
+ * lib/zstd-mt_decompress.c:456,625 (libzstd v1.5.6 is a
+ * build-time clone, programs/Makefile:11,245, not in the reference tree).
  * Full format: raw / RLE / compressed blocks; literals raw / RLE / Huffman
  * (1 or 4 streams, direct or FSE-coded weights, treeless reuse); sequences
  * with predefined / RLE / FSE-described / repeat tables; repeat offsets;

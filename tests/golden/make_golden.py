@@ -1,6 +1,6 @@
 """Generate tests/golden/*.bin with the REAL reference (oracle/_ref: unmodified
-lib/{lz4,zstd}-mt_*.c + liblz4 1.9.4 / libzstd 1.5.5).  Run in the build container only
-(needs /root/reference at oracle build time); the fixtures are committed."""
+lib/{lz4,zstd}-mt_*.c + liblz4 1.9.4 / libzstd 1.5.5).  Needs the reference tree at oracle
+build time (oracle/Makefile REF); the fixtures are committed, so the suite does not."""
 import json
 import os
 import sys
@@ -20,6 +20,15 @@ CASES = [
     ("zstd", 3, z.GEN_TEXT, 200000, 1 << 20, 0),
     ("zstd", 3, z.GEN_MIX, 3 * 65536 + 5, 65536, 2),
     ("zstd", 1, z.GEN_MIX, 131072 * 2 + 9, 1 << 20, 5),
+    # Small streams of what the suite otherwise only checks against a live reference build.  zstd level 19, mix class 2, one
+    # two-block frame: block 0 has FSE-described sequence tables, block 1 treeless literals and Repeat_Mode tables (both
+    # only legal after a first block).  LZ4 level 9, mix class 7: one frame of two linked blocks (FLG 0x4C).  Random bytes:
+    # raw zstd blocks / stored LZ4 blocks.  Zeros: RLE zstd blocks.
+    ("zstd", 19, z.GEN_MIX, 131072 + 512, 1 << 20, 2),
+    ("zstd", 3, z.GEN_RANDOM, 2 * 1024 + 99, 1024, 0),
+    ("zstd", 1, z.GEN_ZEROS, 3 * 16384 + 999, 16384, 0),
+    ("lz4", 9, z.GEN_MIX, 65536 + 8192, 1 << 20, 7),
+    ("lz4", 1, z.GEN_RANDOM, 2 * 1024 + 99, 1024, 0),
 ]
 
 man = {"generator": "tests/golden/make_golden.py", "cases": []}

@@ -1,7 +1,7 @@
 """The reference's own integration test (programs/Makefile:252-260: random data -> ./$m-mt -z -> ./$m-mt -d -> cmp), run with
 the reference's UNMODIFIED CLI (programs/main.c via programs/{lz4,zstd}-mt.c) linked against libzstdmt_b200.so
-(oracle/Makefile target `cli`; binaries live in oracle/_ref/, built where /root/reference exists).  Also crosses the
-two implementations: files written by the B200-backed tool are read by the reference-backed tool and vice versa."""
+(oracle/Makefile target `cli`; binaries live in oracle/_ref/, built where the reference tree exists).  Also crosses the
+two implementations: files written by the GPU-backed tool are read by the reference-backed tool and vice versa."""
 import os
 import subprocess
 
@@ -18,7 +18,7 @@ REFDIR = os.path.join(ROOT, "oracle", "_ref")
 def tool(name):
     p = os.path.join(REFDIR, name)
     if not os.path.exists(p):
-        pytest.skip(name + " not built (needs /root/reference at build time)")
+        pytest.skip(name + " not built (needs the reference tree at build time)")
     return p
 
 
@@ -52,7 +52,7 @@ def test_reference_make_tests_roundtrip(gpu, tmp_path, codec):
 
 @pytest.mark.parametrize("codec,level", [("lz4", "-1"), ("zstd", "-3")])
 def test_cross_with_reference_cli(gpu, tmp_path, codec, level):
-    """B200-written file -> reference tool decodes; reference-written file -> B200 tool decodes (compressible data)."""
+    """GPU-written file -> reference tool decodes; reference-written file -> GPU tool decodes (compressible data)."""
     data = z.gen_stream(z.GEN_MIX, (9 << 20) + 12345, 1 << 20)
     src = tmp_path / "mix.bin"
     src.write_bytes(data.tobytes())

@@ -1,4 +1,4 @@
-"""GPU parity tests for the LZ4 path (run on the B200 box: pytest -m gpu).
+"""GPU parity tests for the LZ4 path (needs an H100: pytest -m gpu).
 
 Bars (BASELINE.json north_star):
   * decode: bit-exact with the original for reference-produced streams;
@@ -143,6 +143,8 @@ def test_decode_golden_fixtures(torch):
         back, status, osz = gpu_decompress(torch, framed, chunk_sizes(case["n"], case["chunk"]))
         assert not status.any(), (case, status)
         assert np.array_equal(back[: case["n"]], src), case
+        rc, back2, st = z.decompress_mem(z.CODEC_LZ4, framed, case["n"] + 16, threads=4)           # and through LZ4MT_decompressDCtx
+        assert rc == 0 and np.array_equal(back2, src) and st["frames"] == case["frames"], case
 
 
 def test_decode_detects_corruption(torch):

@@ -163,8 +163,10 @@ def test_decode_golden_fixtures(torch):
         back, status, dec = gpu_decompress(torch, framed)
         assert not status.any(), (case, status)
         assert np.array_equal(back[: case["n"]], src), case
+        rc, back2, st = z.decompress_mem(z.CODEC_ZSTD, framed, case["n"] + 16, threads=4)          # and through ZSTDCB_decompressDCtx
+        assert rc == 0 and np.array_equal(back2, src) and st["frames"] == case["frames"], case
         seen += 1
-    assert seen >= 3
+    assert seen >= 6
 
 
 def test_decode_detects_corruption(torch):

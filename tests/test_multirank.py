@@ -1,7 +1,7 @@
 """CPU test of the N>1 path (no collective on the data path): world_size-2 gloo processes each own the chunks
 `rank, rank+2, ...` (what bench.py --gpus N and ZSTDMT_GPUS do), frame them independently, and the frames
 re-serialised by global chunk index must equal the single-process stream byte for byte (SURVEY.md fact 0.7:
-output is independent of how chunks are dealt).  The per-rank "codec" here is the oracle's CPU twin of the B200
+output is independent of how chunks are dealt).  The per-rank "codec" here is the oracle's CPU twin of the GPU
 encoder (tests only); what is under test is the dealing + reassembly logic and the generator's (first, stride)."""
 import os
 import sys

@@ -17,8 +17,8 @@ print("n", n, "->", f.size, "ratio %.3f" % (n / max(1, f.size)), "head", f[:24].
 rc, back = o.orc_decode(o.CODEC_ZSTD, f, n)
 print("oracle decode rc", rc, "ok", back.size == n and np.array_equal(back, src))
 if rc != 0 or not np.array_equal(back, src):
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    f.tofile(os.path.join(ROOT, "gpurun_out", "bad_framed.bin")); src.tofile(os.path.join(ROOT, "gpurun_out", "bad_src.bin"))
+    os.makedirs(os.path.join(ROOT, "debug_out"), exist_ok=True)
+    f.tofile(os.path.join(ROOT, "debug_out", "bad_framed.bin")); src.tofile(os.path.join(ROOT, "debug_out", "bad_src.bin"))
 if o.have_ref():
     for T in (1, 3):
         rc, b2, st = o.ref_decompress(o.CODEC_ZSTD, f, n, threads=T)

@@ -1,4 +1,5 @@
-"""Summarise an ncu --set full report into profiles/<name>.md (key metrics + hottest source lines)."""
+"""Summarise an ncu --set full report into prof_out/<name>.md (key metrics + hottest source lines); prof_out/ is git-ignored,
+copy a summary elsewhere to keep it."""
 import csv, os, subprocess, sys
 rep, kernel, name = sys.argv[1], sys.argv[2], sys.argv[3]
 note = sys.argv[4] if len(sys.argv) > 4 else ""
@@ -25,5 +26,6 @@ for h, u, v in zip(hdr, units, vals):
         except ValueError: pass
 lines = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ncu_lines.py"), rep, kernel], capture_output=True, text=True, env=dict(os.environ, TOP="25")).stdout
 out += ["", "Hottest CUDA source lines (warp-stall samples; `-lineinfo`):", "", "```", lines.rstrip(), "```", ""]
-open(os.path.join(ROOT, "profiles", name + ".md"), "w").write("\n".join(out))
-print("wrote profiles/%s.md" % name)
+os.makedirs(os.path.join(ROOT, "prof_out"), exist_ok=True)
+open(os.path.join(ROOT, "prof_out", name + ".md"), "w").write("\n".join(out))
+print("wrote prof_out/%s.md" % name)

@@ -27,8 +27,8 @@ for ci in range(-(-n // chunk)):
     print("chunk", ci, "size", part.size, "->", g.size, "oracle rc", rc, "ok", ok)
     if not ok and bad is None:
         bad = ci
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        part.tofile(os.path.join(ROOT, "gpurun_out", "bad_src.bin")); g.tofile(os.path.join(ROOT, "gpurun_out", "bad_framed.bin"))
+        os.makedirs(os.path.join(ROOT, "debug_out"), exist_ok=True)
+        part.tofile(os.path.join(ROOT, "debug_out", "bad_src.bin")); g.tofile(os.path.join(ROOT, "debug_out", "bad_framed.bin"))
         if o.have_ref():
             rc2, b2, _ = o.ref_decompress(o.CODEC_ZSTD, g, part.size, threads=1); print("  libzstd rc", rc2, "ok", rc2 == 0 and np.array_equal(b2, part))
 print("first bad chunk", bad)

@@ -1,6 +1,6 @@
-"""zstdmt_b200 — B200-native replacement for zstdmt's per-chunk LZ4 / Zstandard hot path.
+"""zstdmt_b200 — GPU-native (H100) replacement for zstdmt's per-chunk LZ4 / Zstandard hot path.
 
-The product is the C-ABI shared library ``libzstdmt_b200.so`` (CUDA kernels for sm_100a +
+The product is the C-ABI shared library ``libzstdmt_b200.so`` (CUDA kernels for sm_90a +
 host pipeline exporting LZ4MT_* / ZSTDCB_* / ZSTDMT_*, see include/).  This module is only
 the thin ctypes binding used by tests and bench.py; it never computes anything itself and it
 raises if the native library is missing (no Python / CPU fallback).

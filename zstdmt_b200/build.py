@@ -1,10 +1,10 @@
 """Build the in-tree native libraries (no torch extension machinery, plain nvcc / gcc).
 
-  zstdmt_b200/libzstdmt_b200.so   CUDA kernels (sm_100a) + host pipeline + C-ABI   [the product]
+  zstdmt_b200/libzstdmt_b200.so   CUDA kernels (sm_90a) + host pipeline + C-ABI   [the product]
   zstdmt_b200/libzmt_datagen.so   synthetic input generator (harness/datagen.c)     [bench / test harness, no dependencies]
   zstdmt_b200/libzmt_memio.so     in-memory fn_read / fn_write drivers of the C-ABI [bench / test harness, links the product]
   oracle/liboracle.so             CPU restatement                                  [test infrastructure]
-  oracle/_ref/libzstdmt_ref.so    unmodified reference wrapper, only when /root/reference exists
+  oracle/_ref/libzstdmt_ref.so    unmodified reference wrapper, only where the reference tree exists (oracle/Makefile REF)
 """
 import os
 import subprocess
@@ -19,7 +19,7 @@ LIB_GEN = os.path.join(HERE, "libzmt_datagen.so")
 LIB_MEMIO = os.path.join(HERE, "libzmt_memio.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-pthread", "-shared",
 ]
 
@@ -82,7 +82,7 @@ def build_oracle():
 
 
 def build_cli():
-    """Reference CLI (unmodified programs/main.c) linked against the product library — only where /root/reference exists."""
+    """Reference CLI (unmodified programs/main.c) linked against the product library — only where the reference tree exists."""
     subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "cli"], capture_output=True, text=True)
 
 

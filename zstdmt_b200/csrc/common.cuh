@@ -1,4 +1,4 @@
-// common.cuh — device helpers shared by the sm_100a kernels (LZ4 + zstd paths).
+// common.cuh — device helpers shared by the sm_90a kernels (LZ4 + zstd paths).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,9 +1,9 @@
 // host_api.cpp — the drop-in boundary: LZ4MT_* / ZSTDCB_* (+ ZSTDMT_* aliases) on top of the CUDA kernels.
 //
 // Replaces the pthread worker pools of
-//   /root/reference/lib/lz4-mt_compress.c:207-353   (pt_compress, pt_write, LZ4MT_compressCCtx)
-//   /root/reference/lib/lz4-mt_decompress.c:165-567 (pt_read, pt_decompress, pt_write, LZ4MT_decompressDCtx)
-//   /root/reference/lib/zstd-mt_compress.c:177-392  and  lib/zstd-mt_decompress.c:209-843
+//   lib/lz4-mt_compress.c:207-353   (pt_compress, pt_write, LZ4MT_compressCCtx)
+//   lib/lz4-mt_decompress.c:165-567 (pt_read, pt_decompress, pt_write, LZ4MT_decompressDCtx)
+//   lib/zstd-mt_compress.c:177-392  and  lib/zstd-mt_decompress.c:209-843
 // with one software pipeline per call:
 //
 //   reader thread  : fn_read -> pinned staging slot (B chunks / frames per slot)
@@ -413,10 +413,8 @@ size_t compress_run(Ctx* c, GenRdWr* rw)
     const size_t chunk = c->inputsize;
     // Slots in flight: the call is bound by the serialised callbacks (one memcpy stream); a GPU turns a batch around in a
     // fraction of the time the reader needs to fill the next one, so more devices do not need more slots per device — one each
-    // is enough.  Measured on the 2-socket Xeon hosts of the B200 pool (one GPU, 4 GiB, GB/s end to end): 4 slots x 8 MiB 18.2
-    // (the default), 4 x 4 MiB 15.8, 4 x 16 MiB 14.4, 8 x 8 MiB 13.7, 8 x 4 MiB 9.9, 16 x 2 MiB 5.2: a ring that outgrows the
-    // last-level cache slows the callbacks' memcpy, and small batches pay the per-batch launch + copy latency.  A call over 8
-    // devices therefore runs 8 x 8 MiB (14.3 GB/s): sharing a 4-slot host ring between 8 device-side slots is the open lead.
+    // is enough.  4 slots x 8 MiB measured best end to end on 2-socket Xeon hosts (not re-measured with an H100): a ring that
+    // outgrows the last-level cache slows the callbacks' memcpy, and small batches pay the per-batch launch + copy latency.
     if (P.slots.empty()) {
         c->devs = env_devices();
         if (c->devs.empty()) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
@@ -777,9 +775,9 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     Pipe& P = c->pipe;
     const bool is_zstd = c->codec == CODEC_ZSTD;
     const uint32_t kBlkCap = 32768;
-    // decode batches must hold enough frames to fill the GPU (one warp per 64 KiB block): 32 MiB of frames measured best
+    // decode batches must hold enough frames to fill the GPU (one warp per 64 KiB block; a linked-block frame is a chain)
     const size_t in_cap0 = (env_size("ZSTDMT_B200_DBATCH_MB", 32) << 20), out_cap0 = in_cap0 * 2, tab_cap = 8192;
-    const uint64_t piece_bytes = (uint64_t)env_size("ZSTDMT_B200_D2H_PIECE_MB", 2) << 20;      // 0: whole slot right after the kernels (measured 0 / 2 / 4 / 8 MiB: 12.8 / 15.1 / 14.3 / 12.8 GB/s)
+    const uint64_t piece_bytes = (uint64_t)env_size("ZSTDMT_B200_D2H_PIECE_MB", 2) << 20;      // 0: whole slot right after the kernels
 
     // ---- stream-type sniffing on the calling thread (LZ4MT_decompressDCtx, lz4-mt_decompress.c:503-520;
     //      ZSTDCB_decompressDCtx, zstd-mt_decompress.c:721-759)
@@ -1133,7 +1131,7 @@ const char* status_string(size_t st)
     case ZMT_ST_CONTENT_CHECKSUM: return "ERROR_contentChecksum_invalid";
     case ZMT_ST_CONTENT_SIZE: return "ERROR_frameSize_wrong";
     case ZMT_ST_TRAILING: return "trailing bytes after frame";
-    case ZMT_ST_UNSUPPORTED: return "stream type not supported by the B200 path";
+    case ZMT_ST_UNSUPPORTED: return "stream type not supported by the GPU path";
     case ZMT_ST_CUDA: return "CUDA runtime / kernel failure";
     case ZMT_ST_BAD_ARG: return "bad argument";
     }

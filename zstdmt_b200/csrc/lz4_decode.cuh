@@ -1,7 +1,7 @@
 // lz4_decode.cuh — LZ4F frame decoder (included by lz4_kernels.cu).
 //
 // Replaces the arithmetic of LZ4F_decompress as the reference calls it per frame
-// (/root/reference/lib/lz4-mt_decompress.c:349-351), for whole batches of frames at once.
+// (lib/lz4-mt_decompress.c:349-351), for whole batches of frames at once.
 //
 // Work unit = one warp per LZ4F block (64 KiB .. 4 MiB of output), two passes over every block:
 //

@@ -1,10 +1,10 @@
-// lz4_kernels.cu — hand-written sm_100a kernels: the LZ77 front end shared by both codecs, the LZ4 back end
+// lz4_kernels.cu — hand-written sm_90a kernels: the LZ77 front end shared by both codecs, the LZ4 back end
 // (block format, XXH32, frame pack; the decoder is in lz4_decode.cuh) and the launchers of the Zstandard encoder (entropy stage in
 // zstd_entropy.cuh; the Zstandard decoder lives in zstd_decode.cu).
 //
 // Replaces the arithmetic the reference reaches through
-//   LZ4F_compressFrame   (/root/reference/lib/lz4-mt_compress.c:280-283)
-//   LZ4F_decompress      (/root/reference/lib/lz4-mt_decompress.c:349-351)
+//   LZ4F_compressFrame   (lib/lz4-mt_compress.c:280-283)
+//   LZ4F_decompress      (lib/lz4-mt_decompress.c:349-351)
 // plus the 12-byte skippable container write (lib/lz4-mt_compress.c:293-298).
 //
 // Kernels
@@ -42,7 +42,7 @@ __device__ __forceinline__ uint64_t zmt_chunk_len(const uint32_t* __restrict__ c
 
 // A CTA barrier preceded by a warp reconvergence: the data-dependent phases leave warps split into
 // independently scheduled groups, and an aligned BAR.SYNC + the uniform-datapath branches ptxas places
-// after it (BRA.U) must only ever be executed by whole warps (else: 'illegal instruction' on sm_100).
+// after it (BRA.U) must only ever be executed by whole warps (else: 'illegal instruction').
 #define CTA_SYNC() do { __syncwarp(); __syncthreads(); } while (0)
 
 // ============================================================================ compressor
@@ -861,9 +861,9 @@ static inline int zmt_sm_count()
 {
     static int n[64];
     int dev = 0; cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 148;
+    if (dev < 0 || dev >= 64) return 132;
     std::lock_guard<std::mutex> g(g_dev_mu);
-    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 148; }
+    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 132; }
     return n[dev];
 }
 
@@ -984,7 +984,7 @@ extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint
 }
 
 // ---------------------------------------------------------------- zstd compress
-#define ZSTD_MAX_GRID (148u * 2u * 4u)       // the workspace holds one ZScratch per CTA of the largest grid (B200: 148 SMs)
+#define ZSTD_MAX_GRID (132u * 2u * 4u)       // the workspace holds one ZScratch per CTA of the largest grid (H100 SXM: 132 SMs)
 static inline uint32_t zstd_grid(uint32_t nblocks) { uint32_t m = (uint32_t)(zmt_sm_count() * 2 * 4); if (m > ZSTD_MAX_GRID) m = ZSTD_MAX_GRID; return nblocks < m ? nblocks : m; }
 
 extern "C" size_t zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size)
@@ -1083,8 +1083,8 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
         const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8);
         const uint32_t need = (nslots + LZD_WARPS - 1) / LZD_WARPS;
         ZmtProfScope ps(ZMT_K_LZ4_DEXEC, stream);
-        // measured (profiles/r2_lz4_exec_staged_ab.md): the shared-memory step window wins at every size (4 GiB: 12.2 vs 17.0 ms,
-        // 32 GiB: 53.3 vs 56.7 ms); ZSTDMT_B200_LZ4_STAGED=0 keeps the plain variant for A/B
+        // the shared-memory step window turns a chain of matches feeding each other into SMEM round trips instead of L2 ones
+        // (DESIGN.md §3.2); ZSTDMT_B200_LZ4_STAGED=0 keeps the plain variant for A/B
         static const char* force = getenv("ZSTDMT_B200_LZ4_STAGED");
         const bool staged = force ? (*force == '1') : true;
         if (staged)

@@ -12,7 +12,7 @@
 // Shared memory: only what crosses the teams is double-buffered (off, M, V, entry positions, path mask: 9.5 KB per
 // buffer).  Piece lengths do not cross: the front end does not store them, the marking walk of the back end
 // recomputes them for the true-path pieces only (it has the slack), which keeps the 32-bit hash table and its
-// single-pass atomicMax.  (A 16-bit table was tried first: CAS loop 15 %, two-pass atomicMax 8 % of all instructions.)
+// single-pass atomicMax.  (A 16-bit table needs a CAS loop or a two-pass atomicMax per insert, both more instructions.)
 #pragma once
 
 #define P_TEAM      256u

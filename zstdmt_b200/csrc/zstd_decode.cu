@@ -1,5 +1,5 @@
-// zstd_decode.cu — Zstandard frame decoding on sm_100a (the ZSTD_decompressStream step of
-// /root/reference/lib/zstd-mt_decompress.c:442-527, one frame per 12-byte container header).
+// zstd_decode.cu — Zstandard frame decoding on sm_90a (the ZSTD_decompressStream step of
+// lib/zstd-mt_decompress.c:442-527, one frame per 12-byte container header).
 //
 // Kernels per batch, all block-parallel (a zstd frame of a 1 MiB chunk has ~64 blocks of ours, 8 of libzstd's):
 //   zstd_seq_predef_kernel   one LANE per block: the sequences of blocks on the predefined FSE tables (everything our encoder
@@ -444,8 +444,8 @@ __device__ uint32_t zd_block(ZWarpTabs& W, const uint8_t* __restrict__ src, uint
                 !zd_seq_table(to, (modes >> 4) & 3, W.of, W.pof, 5, W.norm, qp, qn, 8, 31, hp, &need) ||
                 !zd_seq_table(tm, (modes >> 2) & 3, W.ml, W.pml, 6, W.norm, qp, qn, 9, 52, hp, &need)) { rc = need ? ZD_NEEDS_SEQ : ZMT_ST_BLOCK; break; }
             if (fs) { fs->ll = tl; fs->of = to; fs->ml = tm; fs->have_tabs = true; }
-            BackBits R;                                           // (the one-refill-per-sequence reader of the lane-per-block kernel needs two
-            if (!R.init(qp, qn)) { rc = ZMT_ST_BLOCK; break; }    //  refills here — described tables, offsets to 31 bits — and measured slower: 6.9 -> 8.5 ms)
+            BackBits R;                                           // (the one-refill-per-sequence reader of the lane-per-block kernel would need
+            if (!R.init(qp, qn)) { rc = ZMT_ST_BLOCK; break; }    //  two refills here — described tables, offsets to 31 bits — so it is not used)
             uint32_t sLL = R.read(tl.log), sOF = R.read(to.log), sML = R.read(tm.log);
             uint32_t r0 = fs ? fs->rep[0] : 1, r1 = fs ? fs->rep[1] : 4, r2 = fs ? fs->rep[2] : 8;
             for (uint32_t i = 0; i < nseq; i++) {
@@ -503,7 +503,7 @@ __device__ __forceinline__ void zd_load_predef(ZWarpTabs& W, uint32_t lane)
 
 // ---------------------------------------------------------------- kernel 0: sequences of predefined-table blocks, one LANE per block
 // The three interleaved FSE states of a block are one serial chain; a warp that walks one chain on one lane wastes 31
-// issue slots of every instruction (round 1: 1.56 active lanes per instruction, the kernel issue-bound at 71 %).  Blocks
+// issue slots of every instruction.  Blocks
 // whose three tables are the predefined ones (every block our encoder writes; `Compression_Modes` = 0) need no per-block
 // table memory, so here every lane walks the chain of its own block: 32 chains per warp instruction.  Blocks with
 // described / RLE / repeated tables are left to the warp-per-block kernel below (seq_done stays 0).
@@ -1318,9 +1318,9 @@ static int zd_sm_count()
 {
     static std::mutex mu; static int n[64];
     int dev = 0; cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 148;
+    if (dev < 0 || dev >= 64) return 132;
     std::lock_guard<std::mutex> g(mu);
-    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 148; }
+    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 132; }
     return n[dev];
 }
 

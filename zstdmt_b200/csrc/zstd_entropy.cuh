@@ -2,7 +2,7 @@
 //
 // Replaces, for one ~16 KiB "sub-block" of sequences + literals produced by the shared LZ77 front end
 // (lz4_kernels.cu), what ZSTD_compress does after match finding at the reference call site
-// /root/reference/lib/zstd-mt_compress.c:284-286:
+// lib/zstd-mt_compress.c:284-286:
 //   literals  : raw / RLE / Huffman (4 streams, tree described by direct 4-bit weights)
 //   sequences : LL / OF / ML codes + extra bits on the PREDEFINED FSE tables (mode 0,0,0), the three state
 //               chains run chunk-parallel on the 32 lanes of one warp (speculative entry states, verified),
@@ -385,8 +385,7 @@ __device__ uint32_t z_encode_block(ZEnt& Z, const ZFseShared& F, ZScratch* zs, u
                 const uint32_t direct = maxsym <= 128 ? 1 + (maxsym + 1) / 2 : 0xFFFFu;
                 // The FSE form is built only where it is mandatory (a symbol above 128).  Where the direct form exists it costs
                 // <= 65 bytes per block, the FSE form would save ~30 of them (0.4 % of the output on text) — and this single-thread
-                // step was the longest wait of the whole stage (16.5 % of the kernel's stall samples, profiles/r2_zstd_compress_blocks.md).
-                // -DZ_ALWAYS_FSE_WEIGHTS=1 restores the round-1 behaviour.
+                // step is a serial wait for the whole CTA.  -DZ_ALWAYS_FSE_WEIGHTS=1 builds the FSE form wherever it is smaller.
                 const uint32_t fl = (direct == 0xFFFFu || Z_ALWAYS_FSE_WEIGHTS) ? z_fse_weights(Z, maxsym, maxbits) : 0u;
                 Z.wdesc_len = (fl && fl < direct) ? fl : (direct != 0xFFFFu ? 0u : 0xFFFFu);       // 0: direct form, 0xFFFF: no valid form
             }

@@ -1,7 +1,7 @@
 /* datagen.c — deterministic synthetic inputs for parity tests and bench.py (SURVEY.md §8d).
  *
  * The reference ships no corpus (its only test compresses /dev/urandom,
- * /root/reference/programs/Makefile:252-260) and Silesia is not in the image, so
+ * programs/Makefile:252-260) and Silesia is not part of this repository, so
  * the workloads BASELINE.json names are generated:
  *   ZMT_GEN_ZEROS  0x00 bytes                                   (config 1)
  *   ZMT_GEN_TEXT   Zipf(s=1) words from a 4096-word vocabulary  (config 4)

@@ -8,7 +8,7 @@
  *   - into oracle/_ref/libzstdmt_ref.so with -DGLUE_PREFIX=ref_ (drives the
  *     unmodified reference wrapper + liblz4/libzstd)
  * so the e2e and cpu_baseline numbers go through byte-identical callbacks.
- * The callback contract mirrored here: /root/reference/lib/lz4-mt.h:67-89,
+ * The callback contract mirrored here: lib/lz4-mt.h:67-89,
  * lib/zstd-mt.h:67-93, CLI callbacks programs/main.c:172-200.
  */
 #include <stddef.h>
