@@ -147,7 +147,8 @@ static long fse_read_ncount(const uint8_t* src, size_t n, int16_t* norm, int* ns
 #define HUF_MAXBITS 11
 typedef struct { uint8_t sym[1 << HUF_MAXBITS]; uint8_t nb[1 << HUF_MAXBITS]; int maxbits; int valid; } huf_dtab;
 
-static int huf_build(huf_dtab* h, const uint8_t* weights, int nw /* explicit weights */)
+/* `full` (may be NULL) receives the weights of all nw + 1 symbols, the implied last one included */
+static int huf_build(huf_dtab* h, const uint8_t* weights, int nw /* explicit weights */, uint8_t* full)
 {
     uint32_t total = 0, rank[HUF_MAXBITS + 2], left; int i, maxbits, lastw, nsym = nw + 1;
     uint8_t w[256];
@@ -174,10 +175,12 @@ static int huf_build(huf_dtab* h, const uint8_t* weights, int nw /* explicit wei
         }
     }
     h->maxbits = maxbits; h->valid = 1;
+    if (full) memcpy(full, w, (size_t)nsym);
     return 0;
 }
 
-static int huf_read_tree(huf_dtab* h, const uint8_t* src, size_t n, size_t* used)
+/* *form: 0 direct 4-bit weights, 1 FSE-coded; *nwl: weights listed; full: see huf_build */
+static int huf_read_tree(huf_dtab* h, const uint8_t* src, size_t n, size_t* used, int* form, int* nwl, uint8_t* full)
 {
     uint8_t weights[256]; int nw = 0; unsigned hb;
     if (n < 1) return -1;
@@ -207,7 +210,8 @@ static int huf_read_tree(huf_dtab* h, const uint8_t* src, size_t n, size_t* used
         }
         *used = 1 + (size_t)hb;
     }
-    return huf_build(h, weights, nw);
+    *form = hb < 128; *nwl = nw;
+    return huf_build(h, weights, nw, full);
 }
 
 static int huf_decode_stream(const huf_dtab* h, const uint8_t* src, size_t n, uint8_t* dst, size_t count)
@@ -257,7 +261,9 @@ static int read_seq_table(fse_dtab* t, int* have, int mode, const uint8_t** ip, 
     }
 }
 
-static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase, size_t dstPos, size_t dstCap, size_t* produced)
+/* tr: trace sink, NULL when decoding normally; tb / tw: this block's record and weights (set up by the caller) */
+static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase, size_t dstPos, size_t dstCap, size_t* produced,
+                        orc_zstd_trace_t* tr, int32_t* tb, uint8_t* tw)
 {
     const uint8_t* ip = src; const uint8_t* const iend = src + n;
     uint8_t* lit = NULL; size_t litSize = 0; int rc = ORC_ERR_CORRUPT;
@@ -272,6 +278,7 @@ static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase,
             else if (sf == 1) { if (n < 2) return ORC_ERR_CORRUPT; regen = (b0 >> 4) | ((size_t)ip[1] << 4); hl = 2; }
             else { if (n < 3) return ORC_ERR_CORRUPT; regen = (b0 >> 4) | ((size_t)ip[1] << 4) | ((size_t)ip[2] << 12); hl = 3; }
             ip += hl;
+            if (tr) { tb[ORC_ZT_LIT_TYPE] = (int32_t)type; tb[ORC_ZT_LIT_SF] = (int32_t)sf; tb[ORC_ZT_LIT_HDR] = (int32_t)hl; tb[ORC_ZT_LIT_REGEN] = (int32_t)regen; }
             lit = (uint8_t*)malloc(regen + 1); litSize = regen;
             if (type == 0) { if ((size_t)(iend - ip) < regen) goto done; memcpy(lit, ip, regen); ip += regen; }
             else { if (iend - ip < 1) goto done; memset(lit, *ip, regen); ip++; }
@@ -280,12 +287,22 @@ static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase,
             else if (sf == 2) { if (n < 4) return ORC_ERR_CORRUPT; { uint32_t v = rd32(ip); regen = (v >> 4) & 0x3FFF; comp = (v >> 18) & 0x3FFF; } hl = 4; streams = 4; }
             else { if (n < 5) return ORC_ERR_CORRUPT; { uint64_t v = (uint64_t)rd32(ip) | ((uint64_t)ip[4] << 32); regen = (size_t)((v >> 4) & 0x3FFFF); comp = (size_t)((v >> 22) & 0x3FFFF); } hl = 5; streams = 4; }
             ip += hl;
+            if (tr) {
+                tb[ORC_ZT_LIT_TYPE] = (int32_t)type; tb[ORC_ZT_LIT_SF] = (int32_t)sf; tb[ORC_ZT_LIT_HDR] = (int32_t)hl;
+                tb[ORC_ZT_LIT_REGEN] = (int32_t)regen; tb[ORC_ZT_LIT_COMP] = (int32_t)comp; tb[ORC_ZT_LIT_STREAMS] = streams;
+            }
             if ((size_t)(iend - ip) < comp) return ORC_ERR_CORRUPT;
             lit = (uint8_t*)malloc(regen + 1); litSize = regen;
             {
                 const uint8_t* lp = ip; const uint8_t* const lend = ip + comp;
-                if (type == 2) { size_t used = 0; if (huf_read_tree(&z->huf, lp, comp, &used)) goto done; lp += used; }
+                if (type == 2) {
+                    size_t used = 0; int form = 0, nwl = 0;
+                    if (huf_read_tree(&z->huf, lp, comp, &used, &form, &nwl, tw)) goto done;
+                    lp += used;
+                    if (tr) { tb[ORC_ZT_TREE_FORM] = form; tb[ORC_ZT_TREE_BYTES] = (int32_t)used; tb[ORC_ZT_NWEIGHTS] = nwl; tb[ORC_ZT_MAXBITS] = z->huf.maxbits; }
+                }
                 else if (!z->huf.valid) goto done;
+                else if (tr) tb[ORC_ZT_MAXBITS] = z->huf.maxbits;
                 if (streams == 1) { if (huf_decode_stream(&z->huf, lp, (size_t)(lend - lp), lit, regen)) goto done; }
                 else {
                     size_t s1, s2, s3, s4, per = (regen + 3) / 4;
@@ -298,9 +315,15 @@ static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase,
                     if (huf_decode_stream(&z->huf, lp + s1, s2, lit + per, per)) goto done;
                     if (huf_decode_stream(&z->huf, lp + s1 + s2, s3, lit + 2 * per, per)) goto done;
                     if (huf_decode_stream(&z->huf, lp + s1 + s2 + s3, s4, lit + 3 * per, regen - 3 * per)) goto done;
+                    if (tr) { tb[ORC_ZT_S1] = (int32_t)s1; tb[ORC_ZT_S2] = (int32_t)s2; tb[ORC_ZT_S3] = (int32_t)s3; tb[ORC_ZT_S4] = (int32_t)s4; }
                 }
             }
             ip += comp;
+        }
+        if (tr) {
+            if (litSize > tr->max_lits - tr->nlits) { rc = ORC_ERR_DST_SMALL; goto done; }
+            tb[ORC_ZT_LIT_FIRST] = (int32_t)tr->nlits;
+            memcpy(tr->lits + tr->nlits, lit, litSize); tr->nlits += litSize;
         }
     }
     /* ---- sequences section ---- */
@@ -312,10 +335,15 @@ static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase,
         else if (b0 < 128) nseq = b0;
         else if (b0 < 255) { if (ip >= iend) goto done; nseq = ((size_t)(b0 - 128) << 8) + *ip++; }
         else { if (iend - ip < 2) goto done; nseq = (size_t)ip[0] + ((size_t)ip[1] << 8) + 0x7F00; ip += 2; }
+        if (tr) {
+            tb[ORC_ZT_NSEQ] = (int32_t)nseq; tb[ORC_ZT_NSEQ_BYTES] = b0 < 128 ? 1 : b0 < 255 ? 2 : 3; tb[ORC_ZT_SEQ_FIRST] = (int32_t)tr->nseqs;
+            if (nseq > tr->max_seqs - tr->nseqs) { rc = ORC_ERR_DST_SMALL; goto done; }
+        }
         if (nseq) {
             unsigned modes; bbits b; uint32_t sLL, sOF, sML; size_t i;
             if (ip >= iend) goto done;
             modes = *ip++;
+            if (tr) tb[ORC_ZT_MODES] = (int32_t)modes;
             if (modes & 3) goto done;
             if (read_seq_table(&z->ll, &z->have_ll, (modes >> 6) & 3, &ip, iend, LL_defnorm, 36, 6, 9, 35)) goto done;
             if (read_seq_table(&z->of, &z->have_of, (modes >> 4) & 3, &ip, iend, OF_defnorm, 29, 5, 8, 31)) goto done;
@@ -346,6 +374,7 @@ static int decode_block(zctx* z, const uint8_t* src, size_t n, uint8_t* dstBase,
                     sOF = z->of.base[sOF] + (uint32_t)bb_read(&b, z->of.nb[sOF]);
                 }
                 if (b.off < 0) goto done;
+                if (tr) { uint32_t* t = tr->seq + 4 * tr->nseqs++; t[0] = (uint32_t)ll; t[1] = (uint32_t)ofv; t[2] = (uint32_t)ml; t[3] = (uint32_t)offset; }
                 if (ll > litSize - litPos) goto done;
                 if (ll + ml > (size_t)(oend - op)) { rc = ORC_ERR_DST_SMALL; goto done; }
                 memcpy(op, lit + litPos, ll); op += ll; litPos += ll;
@@ -395,10 +424,10 @@ uint64_t orc_zstd_content_size(const uint8_t* src, size_t srcSize)
     return fcs;
 }
 
-int orc_zstd_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed)
+static int decode_frame(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed, orc_zstd_trace_t* tr)
 {
     size_t hs, pos, total = 0; uint64_t fcs, win; int hasFcs, hasChk, rc, last = 0;
-    zctx* z;
+    zctx* z; int32_t* tb = NULL; uint8_t* tw = NULL;
     rc = parse_frame_header(src, srcSize, &hs, &fcs, &hasFcs, &hasChk, &win);
     if (rc != ORC_OK) return rc;
     z = (zctx*)calloc(1, sizeof(zctx));
@@ -410,22 +439,34 @@ int orc_zstd_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dst
         bh = src[pos] | (src[pos + 1] << 8) | ((uint32_t)src[pos + 2] << 16); pos += 3;
         last = bh & 1; type = (bh >> 1) & 3; bs = bh >> 3;
         if (type == 3 || bs > 128 * 1024) { rc = ORC_ERR_CORRUPT; goto out; }
+        if (tr) {
+            int k;
+            if (tr->nblocks >= tr->max_blocks) { rc = ORC_ERR_DST_SMALL; goto out; }
+            tb = tr->blk + tr->nblocks * ORC_ZT_NF; tw = tr->weights + tr->nblocks * 256;
+            for (k = 0; k < ORC_ZT_NF; k++) tb[k] = -1;
+            memset(tw, 0, 256);
+            tb[ORC_ZT_TYPE] = (int32_t)type; tb[ORC_ZT_LAST] = last; tb[ORC_ZT_BSIZE] = (int32_t)bs;
+        }
         if (type == 0) {
             if (srcSize - pos < bs) { rc = ORC_ERR_TRUNCATED; goto out; }
             if (bs > dstCap - total) { rc = ORC_ERR_DST_SMALL; goto out; }
             memcpy(dst + total, src + pos, bs); total += bs; pos += bs;
+            if (tr) tb[ORC_ZT_REGEN] = (int32_t)bs;
         } else if (type == 1) {
             if (srcSize - pos < 1) { rc = ORC_ERR_TRUNCATED; goto out; }
             if (bs > dstCap - total) { rc = ORC_ERR_DST_SMALL; goto out; }
             memset(dst + total, src[pos], bs); total += bs; pos += 1;
+            if (tr) tb[ORC_ZT_REGEN] = (int32_t)bs;
         } else {
             size_t produced = 0;
             if (srcSize - pos < bs) { rc = ORC_ERR_TRUNCATED; goto out; }
-            rc = decode_block(z, src + pos, bs, dst, total, dstCap, &produced);
+            rc = decode_block(z, src + pos, bs, dst, total, dstCap, &produced, tr, tb, tw);
             if (rc != ORC_OK) goto out;
             if (produced > 128 * 1024) { rc = ORC_ERR_CORRUPT; goto out; }
             total += produced; pos += bs;
+            if (tr) tb[ORC_ZT_REGEN] = (int32_t)produced;
         }
+        if (tr) tr->nblocks++;
     }
     if (hasChk) {
         if (srcSize - pos < 4) { rc = ORC_ERR_TRUNCATED; goto out; }
@@ -439,4 +480,16 @@ int orc_zstd_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dst
 out:
     free(z);
     return rc;
+}
+
+int orc_zstd_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed)
+{
+    return decode_frame(src, srcSize, dst, dstCap, outSize, consumed, NULL);
+}
+
+int orc_zstd_trace(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed, orc_zstd_trace_t* tr)
+{
+    if (!tr) return ORC_ERR_UNSUPPORTED;
+    tr->nblocks = tr->nseqs = tr->nlits = 0;
+    return decode_frame(src, srcSize, dst, dstCap, outSize, consumed, tr);
 }

@@ -89,3 +89,74 @@ def orc_encode_lz4(data, chunk=1 << 20):
 def xxh32(data, seed=0):
     data = _arr(data)
     return orc().orc_xxh32(data.ctypes.data, data.size, seed)
+
+
+# ---- zstd block trace (orc_zstd_trace) ----
+# columns of ZstdTrace.blk, in the order of the ORC_ZT_* enum of oracle/oracle.h
+ZT_FIELDS = ("type", "last", "bsize", "regen", "lit_type", "lit_sf", "lit_hdr", "lit_regen", "lit_comp", "lit_streams",
+             "s1", "s2", "s3", "s4", "tree_form", "tree_bytes", "nweights", "maxbits", "nseq", "nseq_bytes", "modes",
+             "seq_first", "lit_first")
+ZT = {name: i for i, name in enumerate(ZT_FIELDS)}
+
+
+class _ZTrace(ctypes.Structure):
+    _fields_ = [("max_blocks", c_sz), ("max_seqs", c_sz), ("max_lits", c_sz),
+                ("blk", c_vp), ("weights", c_vp), ("seq", c_vp), ("lits", c_vp),
+                ("nblocks", c_sz), ("nseqs", c_sz), ("nlits", c_sz)]
+
+
+class ZstdTrace:
+    """What every block of one zstd frame contained, as numpy arrays.
+    blk[b, ZT[field]] (int32, -1 where the field does not apply); weights[b] (256 Huffman weights, the implied last one
+    included); seq[i] = (literal length, Offset_Value as coded, match length, resolved offset); lits: the decoded literal
+    sections of the compressed blocks back to back (block b's start at blk[b, ZT["lit_first"]]); content: the frame's
+    decoded bytes."""
+
+    def __init__(self, blk, weights, seq, lits, content, consumed):
+        self.blk, self.weights, self.seq, self.lits, self.content, self.consumed = blk, weights, seq, lits, content, consumed
+
+    def col(self, name):
+        return self.blk[:, ZT[name]]
+
+    def block_lits(self, b):
+        a = int(self.blk[b, ZT["lit_first"]])
+        return self.lits[a: a + int(self.blk[b, ZT["lit_regen"]])]
+
+    def block_seqs(self, b):
+        a = int(self.blk[b, ZT["seq_first"]])
+        return self.seq[a: a + max(0, int(self.blk[b, ZT["nseq"]]))]
+
+
+def zstd_trace(frame, out_cap=None):
+    """orc_zstd_trace on one zstd frame (starting at the zstd magic).  Raises on a decode error."""
+    frame = _arr(frame)
+    L = orc()
+    if not hasattr(L, "_zt_ready"):
+        L.orc_zstd_trace.restype = ctypes.c_int
+        L.orc_zstd_trace.argtypes = [c_vp, c_sz, c_vp, c_sz, ctypes.POINTER(c_sz), ctypes.POINTER(c_sz), ctypes.POINTER(_ZTrace)]
+        L.orc_zstd_content_size.restype = ctypes.c_uint64; L.orc_zstd_content_size.argtypes = [c_vp, c_sz]
+        L._zt_ready = True
+    if out_cap is None:
+        fcs = L.orc_zstd_content_size(frame.ctypes.data, frame.size)
+        out_cap = int(fcs) if fcs != (1 << 64) - 1 else 128 << 20
+    mb, ms, ml = frame.size // 3 + 2, out_cap // 3 + 2, out_cap + 1
+    blk = np.empty((mb, len(ZT_FIELDS)), np.int32); w = np.empty((mb, 256), np.uint8)
+    seq = np.empty((ms, 4), np.uint32); lits = np.empty(ml, np.uint8); out = np.empty(out_cap + 1, np.uint8)
+    t = _ZTrace(mb, ms, ml, blk.ctypes.data, w.ctypes.data, seq.ctypes.data, lits.ctypes.data, 0, 0, 0)
+    got, used = c_sz(0), c_sz(0)
+    rc = L.orc_zstd_trace(frame.ctypes.data, frame.size, out.ctypes.data, out.size, ctypes.byref(got), ctypes.byref(used), ctypes.byref(t))
+    if rc != 0:
+        raise ValueError("orc_zstd_trace failed: %d" % rc)
+    return ZstdTrace(blk[: t.nblocks].copy(), w[: t.nblocks].copy(), seq[: t.nseqs].copy(), lits[: t.nlits].copy(),
+                     out[: got.value].copy(), used.value)
+
+
+def mt_frames(framed):
+    """The zstd / LZ4 frames of a framed stream (each after its 12-byte skippable header)."""
+    framed = _arr(framed)
+    cap = framed.size // 12 + 1
+    offs = np.empty(cap, np.uint64); cs = np.empty(cap, np.uint32)
+    n = orc().orc_mt_scan(framed.ctypes.data, framed.size, offs.ctypes.data, cs.ctypes.data, cap)
+    if n < 0:
+        raise ValueError("orc_mt_scan failed: %d" % n)
+    return [framed[int(offs[i]) + 12: int(offs[i]) + 12 + int(cs[i])] for i in range(n)]
