@@ -68,7 +68,10 @@ struct __align__(16) PipeSmem {
     uint32_t Cont[C_TILE / 32];
     uint8_t  len[C_TILE];                 // piece length per selected piece start (written by the marking walk)
     uint16_t piece[P_MAXPIECE];
-    uint16_t hidx[C_TILE / 4];            // heads: one per sequence, sequences hold a match of >= 4 bytes
+    union {                               // segprev is read by head detection, before the heads are written
+        uint16_t hidx[C_TILE / 4];        // heads: one per sequence, sequences hold a match of >= 4 bytes
+        uint16_t segprev[C_CHAINS];       // per segment: 1 + start of the last non-Cont piece before it (0: none)
+    };
     uint32_t longl[2 * (C_TILE / (C_LONGLIT + 1) + 2)];   // jobs: literal runs > C_LONGLIT (start | length << 16, output offset) -- at most
                                                            // 4096/37 + 1 pending per tile -- and 255-runs of match lengths >= 1290 (count, offset | 1<<31)
     __align__(16) uint32_t scanws[16];
@@ -101,6 +104,31 @@ __device__ __forceinline__ uint32_t team_exscan1(uint32_t v, uint32_t* ws, uint3
 #pragma unroll
     for (uint32_t k = 0; k < 8; k++) { tot += x[k]; if (k < twid) base += x[k]; }
     *total = tot;
+    return base + inc - v;
+}
+
+// the piece-list scan: team_exscan1 of v plus, with the same barrier, the exclusive max of m (m is 0 or grows with
+// the thread index, so that is the last nonzero m below this thread).  `ws`: sums in words 0-7, maxima in words 8-15.
+template <uint32_t BARID>
+__device__ __forceinline__ uint32_t team_exscan_pieces(uint32_t v, uint32_t m, uint32_t* ws, uint32_t* total, uint32_t* mprev,
+                                                      uint32_t twid, uint32_t lane)
+{
+    uint32_t inc = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(ZMT_FULL_MASK, inc, d); if (lane >= (uint32_t)d) inc += y; }
+    const uint32_t below = __ballot_sync(ZMT_FULL_MASK, m != 0) & ((1u << lane) - 1);
+    uint32_t mex = __shfl_sync(ZMT_FULL_MASK, m, below ? 31 - __clz(below) : 0);
+    if (!below) mex = 0;
+    if (lane == 31) { ws[twid] = inc; ws[8 + twid] = m ? m : mex; }
+    bar_sync<BARID, P_TEAM>();
+    const uint4 a = *reinterpret_cast<const uint4*>(ws), b = *reinterpret_cast<const uint4*>(ws + 4);
+    const uint4 c = *reinterpret_cast<const uint4*>(ws + 8), d = *reinterpret_cast<const uint4*>(ws + 12);
+    const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, y[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w};
+    uint32_t base = 0, tot = 0, mx = mex;
+#pragma unroll
+    for (uint32_t k = 0; k < 8; k++) { tot += x[k]; if (k < twid) { base += x[k]; mx = max(mx, y[k]); } }
+    *total = tot;
+    *mprev = mx;
     return base + inc - v;
 }
 
@@ -152,42 +180,56 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                 uint32_t anyM = 0;
 #pragma unroll 1
                 for (uint32_t r = 0; r < C_TILE / C_ROUND; r++) {
-                    constexpr uint32_t KPR = C_ROUND / P_TEAM;
-                    uint32_t hreg[KPR];
+                    // four consecutive positions per thread: three aligned words hold the windows of all four, the four
+                    // offsets go out as one 8-byte store, and eight lanes' 4-bit slices make one M word
+                    static_assert(C_ROUND == 4 * P_TEAM, "a round is four positions per thread");
+                    const uint32_t rel = r * C_ROUND + 4 * ttid, i = t0 + rel;
+                    const uint32_t* w = reinterpret_cast<const uint32_t*>(S.in) + (i >> 2);
+                    const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
+                    uint32_t hreg[4], tab[4], o[4], m4 = 0;
+                    // the four table reads, then the four window reads, are issued together: no position waits on another
 #pragma unroll
-                    for (uint32_t k = 0; k < KPR; k++) {
-                        const uint32_t rel = r * C_ROUND + k * P_TEAM + ttid, i = t0 + rel;
-                        const bool ok = (i + 12 <= n);
-                        const uint32_t* w = reinterpret_cast<const uint32_t*>(S.in) + (i >> 2);
-                        const uint32_t sh = (i & 3) * 8;
-                        const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
-                        const uint32_t v = __funnelshift_r(w1, w2, sh), pv = __funnelshift_r(w0, w1, sh);
-                        const uint32_t h = (v * 2654435761u) >> (32 - C_HASHLOG);
-                        hreg[k] = ok ? h : 0xFFFFFFFFu;
-                        uint32_t o = 0;
-                        if (ok) {
-                            if (i >= 1 && __funnelshift_r(pv, v, 24) == v) o = 1;
-                            else if (i >= 2 && __funnelshift_r(pv, v, 16) == v) o = 2;
-                            else if (i >= 3 && __funnelshift_r(pv, v, 8) == v) o = 3;
-                            else if (i >= 4 && pv == v) o = 4;
-                            else {
-                                const uint32_t t = S.tab[h];
-                                if (t && lds32u(S.in, t - 1) == v) o = i - (t - 1);
-                            }
-                        }
-                        T.off[rel] = (uint16_t)o;
-                        const uint32_t mw = __ballot_sync(ZMT_FULL_MASK, o != 0);
-                        if (lane == 0) T.M[rel >> 5] = mw;
-                        anyM |= mw;
+                    for (uint32_t k = 0; k < 4; k++) {
+                        hreg[k] = (__funnelshift_r(w1, w2, 8 * k) * 2654435761u) >> (32 - C_HASHLOG);
+                        tab[k] = S.tab[hreg[k]];
                     }
+#pragma unroll
+                    for (uint32_t k = 0; k < 4; k++) {
+                        const uint32_t ik = i + k;
+                        const bool ok = (ik + 12 <= n);
+                        const uint32_t v = __funnelshift_r(w1, w2, 8 * k), pv = __funnelshift_r(w0, w1, 8 * k);
+                        const uint32_t t = tab[k];
+                        const bool hit = t && lds32u(S.in, t ? t - 1 : 0) == v;
+                        o[k] = 0;
+                        if (ok) {
+                            if (ik >= 1 && __funnelshift_r(pv, v, 24) == v) o[k] = 1;
+                            else if (ik >= 2 && __funnelshift_r(pv, v, 16) == v) o[k] = 2;
+                            else if (ik >= 3 && __funnelshift_r(pv, v, 8) == v) o[k] = 3;
+                            else if (ik >= 4 && pv == v) o[k] = 4;
+                            else if (hit) o[k] = ik - (t - 1);
+                        }
+                        if (!ok) hreg[k] = 0xFFFFFFFFu;
+                        m4 |= (uint32_t)(o[k] != 0) << k;
+                    }
+                    *reinterpret_cast<uint2*>(&T.off[rel]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+                    uint32_t mw = m4 << (4 * (lane & 7));
+                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 1);
+                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 2);
+                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 4);
+                    if ((lane & 7) == 0) T.M[rel >> 5] = mw;
+                    anyM |= mw;
                     TEAM_A_SYNC();
                     if (r == 0 && ttid == 0) S.a_any[b ^ 1] = 0;       // every reader of the previous tile's flag is past it
 #pragma unroll
-                    for (uint32_t k = 0; k < KPR; k++)
-                        if (hreg[k] != 0xFFFFFFFFu) atomicMax(&S.tab[hreg[k]], t0 + r * C_ROUND + k * P_TEAM + ttid + 1);
+                    for (uint32_t k = 0; k < 4; k++) {
+                        bool last = hreg[k] != 0xFFFFFFFFu;     // a later position of the quad with the same hash wins anyway
+#pragma unroll
+                        for (uint32_t k2 = k + 1; k2 < 4; k2++) last &= hreg[k2] != hreg[k];
+                        if (last) atomicMax(&S.tab[hreg[k]], i + k + 1);
+                    }
                     TEAM_A_SYNC();
                 }
-                if (lane == 0 && anyM) atomicOr(&S.a_any[b], 1u);
+                if ((lane & 7) == 0 && anyM) atomicOr(&S.a_any[b], 1u);   // anyM covers the lane's group of eight
                 TEAM_A_SYNC();
                 const bool tile_has_match = S.a_any[b] != 0;
                 const bool do_parse = !((!tile_has_match && !e_din) || e >= t1);
@@ -251,28 +293,39 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                     TEAM_B_SYNC();
                     uint32_t np;
                     {
-                        uint32_t w = ttid < C_TILE / 32 ? S.Sel[ttid] : 0;
-                        uint32_t base = team_exscan1<PB_B>(__popc(w), S.scanws, 0, &np, twid, lane);
-                        while (w) { const uint32_t bit = __ffs(w) - 1; w &= w - 1; S.piece[base++] = (uint16_t)(ttid * 32 + bit); }
+                        // one segment (16 positions) per thread.  segprev[j]: 1 + start of the last non-Cont piece before
+                        // segment j (0: none), the piece whose offset a Cont piece at the start of segment j continues
+                        const uint32_t sh = 16 * (ttid & 1);
+                        uint32_t w = (S.Sel[ttid >> 1] >> sh) & 0xFFFFu;
+                        const uint32_t nc = w & ~(S.Cont[ttid >> 1] >> sh);
+                        const uint32_t last = nc ? ttid * C_SEG + (31 - __clz(nc)) + 1 : 0u;
+                        uint32_t prev;
+                        uint32_t base = team_exscan_pieces<PB_B>(__popc(w), last, S.scanws, &np, &prev, twid, lane);
+                        S.segprev[ttid] = (uint16_t)prev;
+                        while (w) { const uint32_t bit = __ffs(w) - 1; w &= w - 1; S.piece[base++] = (uint16_t)(ttid * C_SEG + bit); }
                     }
                     TEAM_B_SYNC();
                     if (np == 0) break;
+                    // pieces and sequences are dealt in runs of ceil(count / 256) per thread, so every warp shares the work
                     uint32_t nh_local = 0, headmask = 0;
-                    constexpr uint32_t PPT = P_MAXPIECE / P_TEAM;
+                    const uint32_t ppt = (np + P_TEAM - 1) / P_TEAM;
 #pragma unroll
-                    for (uint32_t k = 0; k < PPT; k++) {
-                        const uint32_t r = ttid * PPT + k;
-                        if (r < np) {
+                    for (uint32_t k = 0; k < P_MAXPIECE / P_TEAM; k++) {
+                        const uint32_t r = ttid * ppt + k;
+                        if (k < ppt && r < np) {
                             const uint32_t pr = S.piece[r];
                             bool head = !((S.Cont[pr >> 5] >> (pr & 31)) & 1);
                             if (head) {
                                 uint32_t pend, poff;
                                 if (r == 0) { pend = pd_valid ? pd_end : 0xFFFFFFFFu; poff = pd_off; }
                                 else {
-                                    uint32_t q = r - 1, pb = S.piece[q];
+                                    const uint32_t pb = S.piece[r - 1];
                                     pend = t0 + pb + S.len[pb];
-                                    while (((S.Cont[pb >> 5] >> (pb & 31)) & 1) && q > 0) { q--; pb = S.piece[q]; }
-                                    poff = ((S.Cont[pb >> 5] >> (pb & 31)) & 1) ? pd_off : T.off[pb];
+                                    if (!((S.Cont[pb >> 5] >> (pb & 31)) & 1)) poff = T.off[pb];
+                                    else {                      // Cont pieces start at a segment boundary (c_walk cuts there)
+                                        const uint32_t sp = S.segprev[pb / C_SEG];
+                                        poff = sp ? T.off[sp - 1] : pd_off;
+                                    }
                                 }
                                 if (pend == t0 + pr && poff == T.off[pr]) head = false;
                             }
@@ -283,7 +336,7 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                     {
                         uint32_t hb = team_exscan1<PB_B>(nh_local, S.scanws, 1, &nh, twid, lane);
 #pragma unroll
-                        for (uint32_t k = 0; k < PPT; k++) if (headmask & (1u << k)) S.hidx[hb++] = (uint16_t)(ttid * PPT + k);
+                        for (uint32_t k = 0; k < P_MAXPIECE / P_TEAM; k++) if (headmask & (1u << k)) S.hidx[hb++] = (uint16_t)(ttid * ppt + k);
                     }
                     TEAM_B_SYNC();
                     const uint32_t lastp = S.piece[np - 1];
@@ -292,11 +345,12 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                     if (pd_valid && S.hidx[0] > 0) { const uint32_t pb = S.piece[S.hidx[0] - 1]; pd_end = t0 + pb + S.len[pb]; }
                     const uint32_t nemit = pd_valid + nh - 1;
                     constexpr uint32_t SPT = 1024 / P_TEAM;
+                    const uint32_t spt = (nemit + P_TEAM - 1) / P_TEAM;
                     uint32_t sz = 0, e_lit0[SPT], e_lit[SPT], e_off[SPT], e_len[SPT], cnt = 0;
 #pragma unroll
                     for (uint32_t k = 0; k < SPT; k++) {
-                        const uint32_t sidx = ttid * SPT + k;
-                        if (sidx < nemit) {
+                        const uint32_t sidx = ttid * spt + k;
+                        if (k < spt && sidx < nemit) {
                             uint32_t ls, st, of, en;
                             if (pd_valid && sidx == 0) { ls = pd_lit; st = pd_start; of = pd_off; en = pd_end; }
                             else {
