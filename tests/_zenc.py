@@ -1,5 +1,5 @@
-"""Plain-Python restatement of the choices the GPU zstd encoder (lz4_kernels.cu lz77_blocks_kernel<1>, zstd_entropy.cuh)
-makes on top of the shared LZ77 parse, for tests that hold its output to them:
+"""Plain-Python restatement of the choices the GPU zstd encoder (lz4_kernels.cu zstd_blocks_kernel, zstd_entropy.cuh)
+makes on top of the LZ77 parse it shares with the LZ4 compressor (lz4_pipe.cuh), for tests that hold its output to them:
   - the parse: the LZ4 sequences of the bit-exact CPU twin orc_lz4_block_compress_b200 on the same 64 KiB window;
   - the sub-block cut: every 4 tiles (16 KiB) a block is closed at the start of the match still pending there;
   - the Huffman code: two-queue tree, length-limited to 11 bits (huf_lengths).

@@ -1,4 +1,4 @@
-"""The GPU zstd encoder (lz77_blocks_kernel<1> + z_encode_block) held block by block to what it means to produce
+"""The GPU zstd encoder (zstd_blocks_kernel + z_encode_block) held block by block to what it means to produce
 (pytest -m gpu).  Every frame is traced by the oracle (orc_zstd_trace) and checked against:
   (a) the parse: each compressed sub-block's sequences are the CPU twin's LZ4 sequences whose matches start inside it,
       and the sub-blocks are cut where _zenc.sub_blocks says;

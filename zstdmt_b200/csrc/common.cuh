@@ -147,23 +147,3 @@ __device__ __forceinline__ uint32_t block_exscan(uint32_t v, uint32_t* ws, uint3
     *total = ws[32];
     return inc - v + ws[wid];
 }
-
-// One-barrier variant: every thread sums the warp totals itself.  `ws` holds two 16-word halves used alternately
-// (`parity` flips per call), so a call never overwrites totals that a slow reader of the previous call still needs,
-// provided the caller does not issue two calls with the same parity without a CTA barrier in between (the barrier
-// inside the intermediate call is enough).  blockDim.x <= 512.
-__device__ __forceinline__ uint32_t block_exscan1(uint32_t v, uint32_t* ws, uint32_t parity, uint32_t* total)
-{
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-    uint32_t inc = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(ZMT_FULL_MASK, inc, d); if (lane >= (uint32_t)d) inc += y; }
-    uint32_t* w = ws + 16 * (parity & 1);
-    if (lane == 31) w[wid] = inc;
-    __syncwarp();
-    __syncthreads();
-    uint32_t base = 0, tot = 0;
-    for (uint32_t k = 0; k < nw; k++) { const uint32_t x = w[k]; if (k < wid) base += x; tot += x; }
-    *total = tot;
-    return base + inc - v;
-}

@@ -8,9 +8,11 @@
 // plus the 12-byte skippable container write (lib/lz4-mt_compress.c:293-298).
 //
 // Kernels
-//   lz77_blocks_kernel<codec,NT> one CTA per 64 KiB block (LZ4F block / zstd match window); block staged in SMEM by the TMA
-//                               unit (cp.async.bulk); round-synchronous hash candidates,
-//                               speculative-chain parallel greedy parse, scan-based emission.
+//   lz4_blocks_pipe_kernel      (lz4_pipe.cuh) one CTA per 64 KiB LZ4F block, block staged in SMEM by the TMA unit
+//                               (cp.async.bulk); round-synchronous hash candidates, speculative-chain parallel greedy
+//                               parse, scan-based emission, as two teams pipelined over 4 KiB tiles.
+//   zstd_blocks_kernel          one CTA per 64 KiB zstd match window: the same parse functions run by a single team,
+//                               sequences and literals to a scratch, entropy stage (zstd_entropy.cuh) every 4 tiles.
 //   xxh32_kernel                4 lanes per chunk (the 4 XXH32 accumulators), 8 chunks per warp.
 //   lz4_frame_sizes_kernel / lz4_frame_pack_kernel
 //                               frame size per chunk -> exclusive scan -> compaction of the block
@@ -48,50 +50,57 @@ __device__ __forceinline__ uint64_t zmt_chunk_len(const uint32_t* __restrict__ c
 // ============================================================================ compressor
 #define LZ4_BLK      65536u
 #define C_CHAINS     256u          // speculative chains per tile (one per 16-byte segment)
-#define C_NT         C_CHAINS      // smem arrays below are per chain
 #define C_TILE       4096u         // positions parsed per tile
-#define C_SEG        16u           // C_TILE / C_NT : positions owned by one speculative chain
+#define C_SEG        16u           // C_TILE / C_CHAINS : positions owned by one speculative chain
 #define C_ROUND      1024u         // hash-table update granularity
 #define C_HASHLOG    12
-#define C_MAXPIECE   1536u         // >= max pieces per tile (4096/4 match pieces + 256 continuation pieces), multiple of 512
+#define C_MAXPIECE   1280u         // 4096/4 match pieces + 256 continuation pieces, multiple of 256
 #define C_LONGLIT    32u           // literal runs longer than this are copied cooperatively
 #define C_END        0xFFFFu       // link: chain leaves the tile
 
-struct __align__(16) CompressSmem {
-    static constexpr bool relen = false;   // chain walks cache piece lengths in len[] for the marking walk
-    uint8_t  pad0[16];                    // bytes "before" the block (read by the 8-byte window of phase 1, never matched)
+// ---- shared-memory parts of the two LZ77 kernels (PipeSmem: LZ4, ZstdSmem: Zstandard)
+struct __align__(16) LzStage {
+    uint8_t  pad0[16];                    // bytes "before" the block (read by the 8-byte window of the candidate rounds, never matched)
     uint8_t  in[LZ4_BLK + 32];            // block bytes + zero pad
-    uint32_t tab[1 << C_HASHLOG];         // hash -> 1 + position
-    // ---- tile arrays (dead between tiles: the zstd entropy stage aliases them, see ZEnt)
-    uint16_t off[C_TILE];                 // per tile position: candidate offset (0 = none)
-    uint8_t  len[C_TILE];                 // per piece start: piece length (<= 19)
-    uint32_t M[C_TILE / 32];              // has-candidate bits
-    uint32_t V[C_TILE / 32];              // visited-by-own-chain bits
-    uint32_t Sel[C_TILE / 32];            // pieces on the true greedy chain
-    uint32_t Cont[C_TILE / 32];           // ... that continue the previous piece's match across a segment boundary
-    uint32_t xfree[C_NT];                 // own-walk exit position (absolute)
-    uint16_t xdin[C_NT];                  // own-walk exit: offset of the match we are still inside (0 = free)
-    uint32_t mpos[C_NT];                  // merge position / tile exit (absolute)
-    uint32_t min_[C_NT];                  // entry (free) position of a reachable chain
-    uint16_t link[C_NT];                  // chain this chain merges into (C_END: leaves the tile)
-    uint16_t jump[C_NT];
-    uint16_t entry[8];                    // per warp: first chain of the true path inside it (0xFFFF: none)
-    uint16_t piece[C_MAXPIECE];           // tile-relative start of the r-th selected piece
-    uint16_t hidx[C_MAXPIECE];            // piece index of the h-th head
-    uint32_t longl[3 * (C_TILE / C_LONGLIT + 2)];
-    // ---- end of tile arrays
-    ZFseShared fse;                       // zstd: predefined FSE encoding tables (unused by the LZ4 instantiation)
-    uint32_t scanws[40];                  // block_exscan / block_exscan1 scratch (two 16-word halves + total)
-    uint32_t nlong;
-    uint32_t e_next;                      // chain state entering the next tile: position ...
-    uint32_t d_next;                      // ... and offset of the match still open there (0 = free)
-    uint64_t mbar;
 };
 
-static_assert(offsetof(CompressSmem, fse) - offsetof(CompressSmem, off) >= sizeof(ZEnt), "entropy scratch must fit in the tile arrays");
+// what the front end hands the back end for one tile (double-buffered in the LZ4 pipeline)
+struct __align__(16) PipeTile {
+    uint16_t off[C_TILE];                 // candidate offset per tile position (0 = none)
+    uint32_t M[C_TILE / 32];              // has-candidate bits
+    uint32_t V[C_TILE / 32];              // visited-by-own-chain bits
+    uint8_t  min_[C_CHAINS];              // entry position of a chain on the true path, relative to its own segment (< 16)
+    uint32_t pathmask[C_CHAINS / 32];     // chains on the true path
+    uint32_t k0, e_din, do_parse, pad;    // entry chain, offset of the match open at the entry, tile has work
+};
+
+// front end, per tile: chain walks and the true path
+struct LzFront {
+    uint32_t xfree[C_CHAINS];             // own-walk exit position (absolute); then the lanes on a chain's way inside its warp
+    uint32_t mpos[C_CHAINS];              // merge position / tile exit (absolute)
+    uint16_t xdin[C_CHAINS];              // own-walk exit: offset of the match we are still inside (0 = free)
+    uint16_t link[C_CHAINS];              // chain this chain merges into (C_END: leaves the tile)
+    uint8_t  jump[C_CHAINS];              // terminal chain reached without leaving the warp
+    uint16_t entry[8];                    // per warp: first chain of the true path inside it (0xFFFF: none)
+    uint32_t e_next, d_next;              // parse state entering the next tile: position, offset of the match still open there
+};
+
+// back end, per tile: marking, piece merge, emission
+struct LzBack {
+    uint32_t Sel[C_TILE / 32];            // pieces on the true greedy chain
+    uint32_t Cont[C_TILE / 32];           // ... that continue the previous piece's match across a segment boundary
+    uint8_t  len[C_TILE];                 // piece length per selected piece start (written by the marking walk)
+    uint16_t piece[C_MAXPIECE];           // tile-relative start of the r-th selected piece
+    union {                               // segprev is read by head detection, before the heads are written
+        uint16_t hidx[C_TILE / 4];        // heads: one per sequence, sequences hold a match of >= 4 bytes
+        uint16_t segprev[C_CHAINS];       // per segment: 1 + start of the last non-Cont piece before it (0: none)
+    };
+    uint32_t longl[2 * (C_TILE / (C_LONGLIT + 1) + 2)];   // jobs: literal runs > C_LONGLIT (start | length << 16, output offset) -- at most
+                                                           // 4096/37 + 1 pending per tile -- and 255-runs of match lengths >= 1290 (count, offset | 1<<31)
+};
 
 // number of bytes (<= cap) for which s[p + i] == s[p + i - d].  Word compares only: the last, partial word gets a
-// sentinel bit at byte `cap` (reads run at most 3 bytes past p + cap: S.in carries 32 pad bytes).
+// sentinel bit at byte `cap` (reads run at most 3 bytes past p + cap: LzStage::in carries 32 pad bytes).
 __device__ __forceinline__ uint32_t c_extend(const uint8_t* s, uint32_t p, uint32_t d, uint32_t cap)
 {
     uint32_t L = 0;
@@ -107,11 +116,12 @@ __device__ __forceinline__ uint32_t c_extend(const uint8_t* s, uint32_t p, uint3
 // Walk one speculative chain through the tile.  The greedy parse is evaluated piecewise: a match is cut at
 // the first segment boundary that leaves it >= 4 bytes, and continues ("inside", din = its offset) into the
 // next segment, so no lane ever compares more than 19 bytes per step.  Pieces are merged again at emission.
-//   MODE 0: own segment only (sets V, caches len, exit state -> xfree/xdin)
-//   MODE 1: continuation until it merges into another chain or leaves the tile (-> link/mpos)
-//   MODE 2: re-walk of a chain that is on the true path: marks Sel/Cont (same steps as MODE 0 + 1)
-template <int MODE, class SM>
-__device__ __forceinline__ void c_walk(SM& S, uint32_t k, uint32_t p, uint32_t din, uint32_t t0, uint32_t limit)
+//   MODE 0: own segment only (sets V, exit state -> X.xfree/X.xdin)                      X: LzFront
+//   MODE 1: continuation until it merges into another chain or leaves the tile (-> X.link/X.mpos)
+//   MODE 2: re-walk of a chain that is on the true path: marks X.Sel/X.Cont and the piece lengths X.len
+//           (same steps as MODE 0 + 1)                                                    X: LzBack
+template <int MODE, class OUT>
+__device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, uint32_t k, uint32_t p, uint32_t din, uint32_t t0, uint32_t limit)
 {
     const uint32_t t1 = t0 + C_TILE;
     uint32_t lk = 0xFFFFFFFFu, mp = 0;
@@ -122,48 +132,43 @@ __device__ __forceinline__ void c_walk(SM& S, uint32_t k, uint32_t p, uint32_t d
         if (MODE == 0 && j != k) { mp = p; done = true; continue; }
         if (din) {
             // inside a match with offset din that covered everything up to the boundary p
-            if (MODE != 0 && j != k && ((S.M[rel >> 5] >> (rel & 31)) & 1) && S.off[rel] == din) {
+            if (MODE != 0 && j != k && ((T.M[rel >> 5] >> (rel & 31)) & 1) && T.off[rel] == din) {
                 lk = j; mp = p; done = true; continue;          // chain j's own first step is this very match
             }
             uint32_t cap = p < limit ? limit - p : 0; if (cap > C_SEG) cap = C_SEG;
-            const uint32_t E = c_extend(S.in, p, din, cap);
-            if (MODE == 2 && E) { atomicOr(&S.Sel[rel >> 5], 1u << (rel & 31)); atomicOr(&S.Cont[rel >> 5], 1u << (rel & 31)); S.len[rel] = (uint8_t)E; }
+            const uint32_t E = c_extend(in, p, din, cap);
+            if constexpr (MODE == 2) {
+                if (E) { atomicOr(&X.Sel[rel >> 5], 1u << (rel & 31)); atomicOr(&X.Cont[rel >> 5], 1u << (rel & 31)); X.len[rel] = (uint8_t)E; }
+            }
             p += E;
             if (E != C_SEG) din = 0;
             continue;
         }
         if (MODE != 0 && j != k && (rel & (C_SEG - 1)) == 0) { lk = j; mp = p; done = true; continue; }
-        uint32_t bits = (S.M[rel >> 5] >> (rel & 16)) & 0xFFFFu;     // this segment's 16 candidate bits
+        uint32_t bits = (T.M[rel >> 5] >> (rel & 16)) & 0xFFFFu;     // this segment's 16 candidate bits
         bits &= 0xFFFFu << (rel & 15);
         if (!bits) {                                                   // segment exhausted: free at its end
             const uint32_t nx = t0 + (j + 1) * C_SEG;
             if (MODE == 0) { mp = nx; done = true; }
-            else if (j + 1 == C_NT) { lk = C_END; mp = t1; done = true; }
+            else if (j + 1 == C_CHAINS) { lk = C_END; mp = t1; done = true; }
             else if (j != k) { lk = j + 1; mp = nx; done = true; }
             else p = nx;
             continue;
         }
         const uint32_t qr = (rel & ~15u) + (__ffs(bits) - 1), q = t0 + qr;
-        if (MODE != 0 && j != k && ((S.V[qr >> 5] >> (qr & 31)) & 1)) { lk = j; mp = q; done = true; continue; }
-        const uint32_t d = S.off[qr];
+        if (MODE != 0 && j != k && ((T.V[qr >> 5] >> (qr & 31)) & 1)) { lk = j; mp = q; done = true; continue; }
+        const uint32_t d = T.off[qr];
         uint32_t B = (q & ~(C_SEG - 1)) + C_SEG;                     // cut at the first boundary leaving >= 4 bytes
         if (B - q < 4) B += C_SEG;
-        uint32_t L;
-        if (MODE == 2 && !SM::relen) { atomicOr(&S.Sel[qr >> 5], 1u << (qr & 31)); L = S.len[qr]; }
-        else {
-            const uint32_t end = B < limit ? B : limit;
-            L = 4 + c_extend(S.in, q + 4, d, end - (q + 4));        // first 4 bytes are known equal; q + 4 <= limit always
-            if (MODE == 2) { atomicOr(&S.Sel[qr >> 5], 1u << (qr & 31)); S.len[qr] = (uint8_t)L; }   // relen: len[] belongs to the marking team
-            else {
-                if (!SM::relen) S.len[qr] = (uint8_t)L;
-                if (MODE == 0) atomicOr(&S.V[qr >> 5], 1u << (qr & 31));
-            }
-        }
+        const uint32_t end = B < limit ? B : limit;
+        const uint32_t L = 4 + c_extend(in, q + 4, d, end - (q + 4));  // first 4 bytes are known equal; q + 4 <= limit always
+        if constexpr (MODE == 2) { atomicOr(&X.Sel[qr >> 5], 1u << (qr & 31)); X.len[qr] = (uint8_t)L; }
+        if constexpr (MODE == 0) atomicOr(&T.V[qr >> 5], 1u << (qr & 31));
         p = q + L;
         if (p == B) din = d;                                          // reached the boundary: still inside the match
     }
-    if (MODE == 0) { S.xfree[k] = mp; S.xdin[k] = (uint16_t)din; }
-    if (MODE == 1) { S.link[k] = (uint16_t)lk; S.mpos[k] = mp; if (lk == C_END) S.xdin[k] = (uint16_t)din; }
+    if constexpr (MODE == 0) { X.xfree[k] = mp; X.xdin[k] = (uint16_t)din; }
+    if constexpr (MODE == 1) { X.link[k] = (uint16_t)lk; X.mpos[k] = mp; if (lk == C_END) X.xdin[k] = (uint16_t)din; }
 }
 
 __device__ __forceinline__ uint32_t c_seq_size(uint32_t lit, uint32_t L)
@@ -174,68 +179,79 @@ __device__ __forceinline__ uint32_t c_seq_size(uint32_t lit, uint32_t L)
     return s;
 }
 
-// writes one LZ4 sequence at op (token, lengths, offset); literals longer than C_LONGLIT are queued for a
-// warp-cooperative copy.  Returns the encoded size.
-template <class SM>
-__device__ __forceinline__ uint32_t c_emit_seq(SM& S, uint8_t* dst, uint32_t o, uint32_t lit_start, uint32_t lit, uint32_t off, uint32_t mlen)
+// writes one LZ4 sequence at dst + o (token, lengths, offset) and returns its size.  No serial 255-runs: the 255 bytes of a
+// literal length exist only when lit >= 270 > C_LONGLIT, and the warp that copies that literal run writes them
+// (c_long_job); literal runs longer than C_LONGLIT and long match-length runs are queued as jobs in K.longl.
+__device__ __forceinline__ uint32_t c_emit_seq(const uint8_t* in, LzBack& K, uint32_t& nlong, uint8_t* dst, uint32_t o,
+                                               uint32_t lit_start, uint32_t lit, uint32_t off, uint32_t mlen)
 {
+    static_assert(C_LONGLIT < 15 + 255, "literal-length 255 runs must imply the cooperative path");
     uint8_t* op = dst + o;
     const uint32_t ml = mlen - 4;
     *op++ = (uint8_t)(((lit >= 15 ? 15u : lit) << 4) | (ml >= 15 ? 15u : ml));
-    if (SM::relen) {
-        // pipelined kernel: no serial 255-runs.  The 255 bytes of a literal length exist only when lit >= 270 > C_LONGLIT
-        // and are written by the warp that copies that literal run; long match-length runs become a fill job.
-        static_assert(C_LONGLIT < 15 + 255, "literal-length 255 runs must imply the cooperative path");
-        if (lit >= 15) { const uint32_t x = lit - 15, nf = x / 255; op += nf; *op++ = (uint8_t)(x - nf * 255); }
-        if (lit <= C_LONGLIT) { for (uint32_t i = 0; i < lit; i++) op[i] = S.in[lit_start + i]; }
-        else { const uint32_t s = atomicAdd(&S.nlong, 1u); S.longl[2 * s] = lit_start | (lit << 16); S.longl[2 * s + 1] = (uint32_t)(op - dst); }
-        op += lit;
-        *op++ = (uint8_t)off; *op++ = (uint8_t)(off >> 8);
-        if (ml >= 15) {
-            const uint32_t x = ml - 15, nf = x / 255;
-            if (nf > 4) { const uint32_t s = atomicAdd(&S.nlong, 1u); S.longl[2 * s] = nf; S.longl[2 * s + 1] = (uint32_t)(op - dst) | 0x80000000u; op += nf; }
-            else for (uint32_t i = 0; i < nf; i++) *op++ = 255;
-            *op++ = (uint8_t)(x - nf * 255);
-        }
-        return (uint32_t)(op - (dst + o));
-    }
-    if (lit >= 15) { uint32_t x = lit - 15; while (x >= 255) { *op++ = 255; x -= 255; } *op++ = (uint8_t)x; }
-    if (lit <= C_LONGLIT) { for (uint32_t i = 0; i < lit; i++) op[i] = S.in[lit_start + i]; }
-    else { const uint32_t s = atomicAdd(&S.nlong, 1u); S.longl[3 * s] = lit_start; S.longl[3 * s + 1] = (uint32_t)(op - dst); S.longl[3 * s + 2] = lit; }
+    if (lit >= 15) { const uint32_t x = lit - 15, nf = x / 255; op += nf; *op++ = (uint8_t)(x - nf * 255); }
+    if (lit <= C_LONGLIT) { for (uint32_t i = 0; i < lit; i++) op[i] = in[lit_start + i]; }
+    else { const uint32_t s = atomicAdd(&nlong, 1u); K.longl[2 * s] = lit_start | (lit << 16); K.longl[2 * s + 1] = (uint32_t)(op - dst); }
     op += lit;
     *op++ = (uint8_t)off; *op++ = (uint8_t)(off >> 8);
-    if (ml >= 15) { uint32_t x = ml - 15; while (x >= 255) { *op++ = 255; x -= 255; } *op++ = (uint8_t)x; }
+    if (ml >= 15) {
+        const uint32_t x = ml - 15, nf = x / 255;
+        if (nf > 4) { const uint32_t s = atomicAdd(&nlong, 1u); K.longl[2 * s] = nf; K.longl[2 * s + 1] = (uint32_t)(op - dst) | 0x80000000u; op += nf; }
+        else for (uint32_t i = 0; i < nf; i++) *op++ = 255;
+        *op++ = (uint8_t)(x - nf * 255);
+    }
     return (uint32_t)(op - (dst + o));
 }
 
-// pipelined kernel: one job of the long list, done by `nthr` threads (thread index t): a literal run with the 255 bytes
-// of its length field, or a run of 255 bytes of a match length
-template <class SM>
-__device__ __forceinline__ void c_long_job(SM& S, uint8_t* dst, uint32_t s, uint32_t t, uint32_t nthr)
+// one job of the long list, done by `nthr` threads (thread index t): a literal run with the 255 bytes of its length
+// field, or a run of 255 bytes of a match length
+__device__ __forceinline__ void c_long_job(const uint8_t* in, const LzBack& K, uint8_t* dst, uint32_t s, uint32_t t, uint32_t nthr)
 {
-    const uint32_t a = S.longl[2 * s], dp = S.longl[2 * s + 1];
+    const uint32_t a = K.longl[2 * s], dp = K.longl[2 * s + 1];
     if (dp & 0x80000000u) { uint8_t* q = dst + (dp & 0x7FFFFFFFu); for (uint32_t i = t; i < a; i += nthr) q[i] = 255; return; }
     const uint32_t sp = a & 0xFFFFu, ln = a >> 16;
-    for (uint32_t i = t; i < ln; i += nthr) dst[dp + i] = S.in[sp + i];
+    for (uint32_t i = t; i < ln; i += nthr) dst[dp + i] = in[sp + i];
     const uint32_t nf = (ln - 15) / 255;                       // ln > C_LONGLIT >= 15
     uint8_t* q = dst + dp - 1 - nf;
     for (uint32_t i = t; i < nf; i += nthr) q[i] = 255;
 }
 
-// CODEC 0: LZ4 block format out.  CODEC 1: Zstandard blocks out (same candidates + parse, entropy stage per ~16 KiB).
-template <int CODEC, int NTHREADS>
-__global__ void __launch_bounds__(NTHREADS, 2)
-lz77_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
+#include "lz4_pipe.cuh"
+
+// ============================================================================ Zstandard encoder: LZ77 + entropy stage
+// The LZ4 compressor's front and back end (lz4_pipe.cuh) run by one team of 256 threads, tile after tile, and the
+// sequences go to the scratch instead of an LZ4 stream.  Every 4 tiles the entropy stage turns what was gathered into
+// a Zstandard block; it is written for the whole CTA, and its shared memory reuses the tile arrays, which are dead
+// between tiles.
+struct __align__(16) ZstdSmem {
+    LzStage  stage;
+    uint32_t tab[1 << C_HASHLOG];         // hash -> 1 + position
+    union {
+        struct { PipeTile tile; LzFront fe; LzBack be; } lz;
+        ZEnt ent;
+    };
+    ZFseShared fse;                       // predefined FSE encoding tables
+    __align__(16) uint32_t scanws[40];    // team_exscan* (16 words) and the entropy stage's block_exscan (33 words)
+    uint32_t any[2];                      // tile has a candidate, per tile parity (lz_candidates)
+    uint32_t nlong;
+    uint64_t mbar;
+};
+static_assert(sizeof(ZstdSmem) + 1024 <= (228 * 1024) / 2, "two CTAs per SM");
+
+__global__ void __launch_bounds__(P_TEAM, 2)
+zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
                    uint32_t bpc, uint8_t* __restrict__ tmp, uint32_t* __restrict__ blk_csize, uint32_t nblocks, uint32_t flags,
                    ZScratch* __restrict__ zscratch)
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    CompressSmem& S = *reinterpret_cast<CompressSmem*>(smem_raw);
-    constexpr uint32_t NT = NTHREADS;                         // threads per CTA (chains stay C_CHAINS = 256)
-    static_assert(NT == 256 || NT == 512, "NT");
-    static_assert(CODEC == 0 || NT == 256, "the zstd entropy stage is written for 256 threads");
+    ZstdSmem& S = *reinterpret_cast<ZstdSmem*>(smem_raw);
+    constexpr uint32_t NT = P_TEAM;
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (CODEC == 1) z_load_fse_shared(S.fse, tid, NT);
+    PipeTile& T = S.lz.tile;
+    LzBack& K = S.lz.be;
+    ZScratch* const zs = zscratch + blockIdx.x;
+    auto cta_sync = [] () { CTA_SYNC(); };
+    z_load_fse_shared(S.fse, tid, NT);
 
     for (uint32_t blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
         const uint32_t chunk = blk / bpc, bic = blk % bpc;
@@ -245,306 +261,89 @@ lz77_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
         uint32_t n = 0;
         if (boff < cbytes) n = (uint32_t)((cbytes - boff) < LZ4_BLK ? (cbytes - boff) : LZ4_BLK);
         if (n == 0) { if (tid == 0) blk_csize[blk] = 0; continue; }
-        const uint8_t* src = in + cbase + boff;
         uint8_t* dst = tmp + (uint64_t)blk * ZMT_LZ4_TMP_STRIDE;
 
-        // ---- stage the block into shared memory (TMA bulk copy when 16-byte aligned)
         CTA_SYNC();                                       // previous block fully consumed
-        const uint32_t nb16 = ((((uintptr_t)src & 15) == 0) && !(flags & 1)) ? (n & ~15u) : 0;
-        if (tid == 0) { if (nb16) mbar_init(&S.mbar, 1); S.nlong = 0; }
-        CTA_SYNC();
-        if (tid == 0 && nb16) { mbar_expect_tx(&S.mbar, nb16); bulk_g2s(S.in, src, nb16, &S.mbar); }
-        for (uint32_t i = nb16 + tid; i < n; i += NT) S.in[i] = src[i];
-        for (uint32_t i = n + tid; i < ((n + 3) & ~3u) + 32 && i < LZ4_BLK + 32; i += NT) S.in[i] = 0;
-        if (tid < 16) S.pad0[tid] = 0;
-        for (uint32_t i = tid; i < (1u << C_HASHLOG); i += NT) S.tab[i] = 0;
-        // one thread observes the TMA completion; the CTA barrier publishes the staged bytes to everyone
-        if (tid == 0 && nb16) { mbar_wait(&S.mbar, 0); asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&S.mbar))); }
-        CTA_SYNC();
+        if (tid == 0) { S.nlong = 0; S.any[0] = 0; S.any[1] = 0; }
+        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, flags, tid);
 
         const uint32_t limit = n >= 5 ? n - 5 : 0;        // matches end at or before n-5
-        uint32_t e = 0, e_din = 0, out_pos = 0;           // CTA-uniform parse state (position, offset of the open match)
-        // pending sequence: its match may still grow in the next tile, so it is emitted one tile late
-        uint32_t pd_valid = 0, pd_lit = 0, pd_start = 0, pd_off = 0, pd_end = 0;
-        // zstd: sequences / literals gathered for the current sub-block, content already emitted into blocks
-        ZScratch* const zs = CODEC == 1 ? zscratch + blockIdx.x : nullptr;
-        ZEnt& ZE = *reinterpret_cast<ZEnt*>(&S.off[0]);
-        uint32_t z_nseq = 0, z_nlit = 0, z_pos = 0, z_tiles = 0;
+        uint32_t e = 0, e_din = 0, out_pos = 0;
+        LzPending pd = {0, 0, 0, 0, 0};
+        // sequences / literals gathered for the current sub-block, content already emitted into blocks
+        uint32_t z_nseq = 0, z_nlit = 0, z_pos = 0;
         const bool z_last_of_chunk = (boff + n == cbytes);
-        auto cta_sync = [] () { CTA_SYNC(); };
 
-        for (uint32_t t0 = 0; t0 < n; t0 += C_TILE) {
-            // ---------------- phase 1: candidates (4 rounds of 1024 positions)
-            if (tid < C_TILE / 32) { S.V[tid] = 0; S.Sel[tid] = 0; S.Cont[tid] = 0; }
-            uint32_t anyM = 0;
-#pragma unroll 1
-            for (uint32_t r = 0; r < C_TILE / C_ROUND; r++) {
-                constexpr uint32_t KPR = C_ROUND / NT;       // positions per thread per round
-                uint32_t hreg[KPR];
-#pragma unroll
-                for (uint32_t k = 0; k < KPR; k++) {
-                    const uint32_t rel = r * C_ROUND + k * NT + tid, i = t0 + rel;
-                    const bool ok = (i + 12 <= n);
-                    // 8-byte window: bytes i-4 .. i+3  (S.in is preceded by 16 pad bytes, so word -1 exists)
-                    const uint32_t* w = reinterpret_cast<const uint32_t*>(S.in) + (i >> 2);
-                    const uint32_t sh = (i & 3) * 8;
-                    const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
-                    const uint32_t v = __funnelshift_r(w1, w2, sh), pv = __funnelshift_r(w0, w1, sh);
-                    const uint32_t h = (v * 2654435761u) >> (32 - C_HASHLOG);
-                    hreg[k] = ok ? h : 0xFFFFFFFFu;
-                    uint32_t o = 0;
-                    if (ok) {
-                        // short-period candidates d = 1..4: v(i-d) is a byte-shift of the window
-                        if (i >= 1 && __funnelshift_r(pv, v, 24) == v) o = 1;
-                        else if (i >= 2 && __funnelshift_r(pv, v, 16) == v) o = 2;
-                        else if (i >= 3 && __funnelshift_r(pv, v, 8) == v) o = 3;
-                        else if (i >= 4 && pv == v) o = 4;
-                        else {
-                            const uint32_t t = S.tab[h];
-                            if (t && lds32u(S.in, t - 1) == v) o = i - (t - 1);
-                        }
-                    }
-                    S.off[rel] = (uint16_t)o;
-                    const uint32_t mw = __ballot_sync(ZMT_FULL_MASK, o != 0);
-                    if (lane == 0) S.M[rel >> 5] = mw;
-                    anyM |= mw;
-                }
-                CTA_SYNC();
-#pragma unroll
-                for (uint32_t k = 0; k < KPR; k++)
-                    if (hreg[k] != 0xFFFFFFFFu) atomicMax(&S.tab[hreg[k]], t0 + r * C_ROUND + k * NT + tid + 1);
-                CTA_SYNC();
-            }
+        for (uint32_t ti = 0, t0 = 0; t0 < n; ti++, t0 += C_TILE) {
             const uint32_t t1 = t0 + C_TILE;
-            __syncwarp();
-            const int tile_has_match = __syncthreads_or(anyM != 0);
-            const bool do_parse = !((!tile_has_match && !e_din) || e >= t1);
-            if (!do_parse) { if (e < t1) e = t1; }         // nothing to parse in this tile
-            else do {
-            // ---------------- phase 2: speculative chains (own segment, then continuation)
-            const uint32_t k0 = (e - t0) / C_SEG;
-            const uint32_t seg0 = t0 + tid * C_SEG;
-            const bool is_chain = tid < C_CHAINS;          // threads beyond the chains only help in the data-parallel phases
-            const bool alive = is_chain && tid >= k0;
-            if (alive) c_walk<0>(S, tid, tid == k0 ? e : seg0, tid == k0 ? e_din : 0u, t0, limit);
-            else if (is_chain) S.link[tid] = (uint16_t)tid;   // dead: self link, never reached
-            CTA_SYNC();
-            if (alive) c_walk<1>(S, tid, S.xfree[tid], S.xdin[tid], t0, limit);
-            CTA_SYNC();
-            // ---------------- phase 3: which chains lie on the true path (entry k0, follow the links)
-            // Links only go forward.  Each warp resolves its own 32 chains with shuffles (pointer doubling on lane
-            // indices: terminal chain + bitmask of the lanes on the way), one thread then hops from warp to warp
-            // (<= 8 hops), and each warp reads its path mask back: 2 CTA barriers instead of 18.
-            bool on_path;
-            {
-                const uint32_t lk = is_chain ? S.link[tid] : tid;
-                const bool inwarp = is_chain && (lk != C_END) && (lk != tid) && ((lk >> 5) == wid);
-                uint32_t jmp = inwarp ? (lk & 31) : lane;                 // next lane inside this warp (self = terminal)
-                uint32_t pm = (1u << lane) | (1u << jmp);
+            const bool has_match = lz_candidates<0>(S.stage.in, S.tab, T, S.any, ti & 1, t0, n, tid, lane);
+            if (lz_chains<0>(S.stage.in, T, S.lz.fe, has_match, e, e_din, t0, limit, tid, lane)) {
+                uint32_t tile_end;
+                const uint32_t nh = lz_heads<0>(S.stage.in, T, K, S.scanws, pd, tile_end, t0, limit, tid, lane);
+                if (nh) {
+                    const LzRun R = lz_seq_run(T, K, pd, nh, t0, tid);
+                    uint32_t sz = 0;                          // (sequences << 18) | literal bytes
 #pragma unroll
-                for (int r = 0; r < 5; r++) { pm |= __shfl_sync(ZMT_FULL_MASK, pm, jmp); jmp = __shfl_sync(ZMT_FULL_MASK, jmp, jmp); }
-                if (is_chain) {
-                    S.jump[tid] = (uint16_t)(32 * wid + jmp);              // terminal chain reached from tid without leaving the warp
-                    S.xfree[tid] = pm;                                     // lanes on that way (xfree is dead after the continuation walk)
-                }
-                if (tid < 8) S.entry[tid] = 0xFFFFu;
-                CTA_SYNC();
-                if (tid == 0) {
-                    uint32_t cur = k0;
-                    S.min_[k0] = e;
-                    for (;;) {
-                        S.entry[cur >> 5] = (uint16_t)cur;
-                        const uint32_t t = S.jump[cur], tl = S.link[t];
-                        if (tl == C_END) { S.e_next = S.mpos[t]; S.d_next = S.xdin[t]; break; }
-                        S.min_[tl] = S.mpos[t];                            // entry position of the next warp's first chain on the path
-                        cur = tl;
+                    for (uint32_t k = 0; k < LZ_SPT; k++) if (k < R.cnt) sz += (1u << 18) | R.lit[k];
+                    uint32_t total;
+                    const uint32_t o = team_exscan1<0>(sz, S.scanws, 0, &total, wid, lane);
+                    uint32_t si = z_nseq + (o >> 18), li = z_nlit + (o & 0x3FFFF);
+#pragma unroll
+                    for (uint32_t k = 0; k < LZ_SPT; k++) {
+                        if (k >= R.cnt) break;
+                        ZSeq q; q.litlen = R.lit[k]; q.off = (uint16_t)R.off[k]; q.mlen = (uint16_t)R.len[k];
+                        zs->seq[si++] = q;
+                        if (R.lit[k] <= C_LONGLIT) { for (uint32_t i = 0; i < R.lit[k]; i++) zs->lit[li + i] = S.stage.in[R.lit0[k] + i]; }
+                        else { const uint32_t s = atomicAdd(&S.nlong, 1u); K.longl[2 * s] = R.lit0[k] | (R.lit[k] << 16); K.longl[2 * s + 1] = li; }
+                        li += R.lit[k];
                     }
+                    team_sync<0>();
+                    // long literal runs, one warp each (a plain copy: unlike the LZ4 jobs, no length field goes with them)
+                    const uint32_t nl = S.nlong;
+                    for (uint32_t s = wid; s < nl; s += NT / 32) {
+                        const uint32_t a = K.longl[2 * s], dp = K.longl[2 * s + 1], sp = a & 0xFFFFu, ln = a >> 16;
+                        for (uint32_t i = lane; i < ln; i += 32) zs->lit[dp + i] = S.stage.in[sp + i];
+                    }
+                    z_nseq += total >> 18; z_nlit += total & 0x3FFFF;
+                    lz_next_pending(T, K, pd, nh, tile_end, t0);
+                    team_sync<0>();
+                    if (tid == 0) S.nlong = 0;
                 }
-                CTA_SYNC();
-                const uint32_t a = is_chain ? S.entry[wid] : 0xFFFFu;
-                on_path = (a != 0xFFFFu) && ((S.xfree[a] >> lane) & 1u);
-                if (on_path && inwarp) S.min_[lk] = S.mpos[tid];           // in-warp successor: entry position = my merge position
-                __syncwarp();
             }
-            // ---------------- phase 4: mark the pieces of the true chain
-            if (on_path) c_walk<2>(S, tid, S.min_[tid], tid == k0 ? e_din : 0u, t0, limit);
-            CTA_SYNC();
-            e = S.e_next; e_din = S.d_next;
 
-            // ---------------- phase 5: merge pieces into sequences, emit all but the last (it may still grow)
-            uint32_t np;
-            {
-                uint32_t w = tid < C_TILE / 32 ? S.Sel[tid] : 0;
-                uint32_t base = block_exscan1(__popc(w), S.scanws, 0, &np);
-                while (w) { const uint32_t b = __ffs(w) - 1; w &= w - 1; S.piece[base++] = (uint16_t)(tid * 32 + b); }
-            }
-            CTA_SYNC();
-            if (np == 0) break;
-            // piece r is a HEAD unless it continues the previous piece's match: flagged continuation, or contiguous with the
-            // same offset (the effective offset of a flagged piece is that of the nearest unflagged piece before it)
-            uint32_t nh_local = 0, headmask = 0;
-            constexpr uint32_t PPT = C_MAXPIECE / NT;     // pieces per thread
-#pragma unroll
-            for (uint32_t k = 0; k < PPT; k++) {
-                const uint32_t r = tid * PPT + k;
-                if (r < np) {
-                    const uint32_t pr = S.piece[r];
-                    bool head = !((S.Cont[pr >> 5] >> (pr & 31)) & 1);
-                    if (head) {
-                        uint32_t pend, poff;                         // end and effective offset of what precedes piece r
-                        if (r == 0) { pend = pd_valid ? pd_end : 0xFFFFFFFFu; poff = pd_off; }
-                        else {
-                            uint32_t b = r - 1, pb = S.piece[b];
-                            pend = t0 + pb + S.len[pb];
-                            while (((S.Cont[pb >> 5] >> (pb & 31)) & 1) && b > 0) { b--; pb = S.piece[b]; }
-                            poff = ((S.Cont[pb >> 5] >> (pb & 31)) & 1) ? pd_off : S.off[pb];
-                        }
-                        if (pend == t0 + pr && poff == S.off[pr]) head = false;
-                    }
-                    if (head) { headmask |= 1u << k; nh_local++; }
-                }
-            }
-            uint32_t nh;
-            {
-                uint32_t hb = block_exscan1(nh_local, S.scanws, 1, &nh);
-#pragma unroll
-                for (uint32_t k = 0; k < PPT; k++) if (headmask & (1u << k)) S.hidx[hb++] = (uint16_t)(tid * PPT + k);
-            }
-            CTA_SYNC();
-            const uint32_t lastp = S.piece[np - 1];
-            const uint32_t tile_end = t0 + lastp + S.len[lastp];     // end of the last piece of this tile
-            if (nh == 0) { pd_end = tile_end; break; }               // every piece extends the pending sequence
-            if (pd_valid && S.hidx[0] > 0) { const uint32_t pb = S.piece[S.hidx[0] - 1]; pd_end = t0 + pb + S.len[pb]; }
-            // sequences to emit now: [pending] + heads 0 .. nh-2 ; head nh-1 becomes the new pending sequence
-            const uint32_t nemit = pd_valid + nh - 1;
-            constexpr uint32_t SPT = 1024 / NT;           // sequences per thread (at most 1024 per tile)
-            uint32_t sz = 0, e_lit0[SPT], e_lit[SPT], e_off[SPT], e_len[SPT], cnt = 0;
-#pragma unroll
-            for (uint32_t k = 0; k < SPT; k++) {
-                const uint32_t sidx = tid * SPT + k;
-                if (sidx < nemit) {
-                    uint32_t ls, st, of, en;
-                    if (pd_valid && sidx == 0) { ls = pd_lit; st = pd_start; of = pd_off; en = pd_end; }
-                    else {
-                        const uint32_t h = sidx - pd_valid;          // head index, h <= nh-2
-                        const uint32_t pi = S.hidx[h], pr = S.piece[pi];
-                        const uint32_t pl = S.piece[S.hidx[h + 1] - 1];
-                        st = t0 + pr; of = S.off[pr]; en = t0 + pl + S.len[pl];
-                        if (h == 0) ls = pd_valid ? pd_end : pd_lit;     // pd_lit doubles as "end of everything emitted so far"
-                        else { const uint32_t pp = S.piece[pi - 1]; ls = t0 + pp + S.len[pp]; }
-                    }
-                    e_lit0[k] = ls; e_lit[k] = st - ls; e_off[k] = of; e_len[k] = en - st;
-                    sz += CODEC == 0 ? c_seq_size(e_lit[k], e_len[k]) : ((1u << 18) | e_lit[k]); cnt++;   // zstd: (count, literal bytes) packed
-                }
-            }
-            uint32_t total;
-            uint32_t o = block_exscan1(sz, S.scanws, 0, &total);
-            if (CODEC == 0) {
-                o += out_pos;
-#pragma unroll
-                for (uint32_t k = 0; k < SPT; k++) {
-                    if (k >= cnt) break;
-                    o += c_emit_seq(S, dst, o, e_lit0[k], e_lit[k], e_off[k], e_len[k]);
-                }
-            } else {
-                uint32_t si = z_nseq + (o >> 18), li = z_nlit + (o & 0x3FFFF);
-#pragma unroll
-                for (uint32_t k = 0; k < SPT; k++) {
-                    if (k >= cnt) break;
-                    ZSeq q; q.litlen = e_lit[k]; q.off = (uint16_t)e_off[k]; q.mlen = (uint16_t)e_len[k];
-                    zs->seq[si++] = q;
-                    if (e_lit[k] <= C_LONGLIT) { for (uint32_t i = 0; i < e_lit[k]; i++) zs->lit[li + i] = S.in[e_lit0[k] + i]; }
-                    else { const uint32_t s = atomicAdd(&S.nlong, 1u); S.longl[3 * s] = e_lit0[k]; S.longl[3 * s + 1] = li; S.longl[3 * s + 2] = e_lit[k]; }
-                    li += e_lit[k];
-                }
-            }
-            CTA_SYNC();
-            {   // cooperative copies of long literal runs: one warp per run
-                const uint32_t nl = S.nlong;
-                uint8_t* const ldst = CODEC == 0 ? dst : zs->lit;
-                for (uint32_t s = wid; s < nl; s += NT / 32) {
-                    const uint32_t sp = S.longl[3 * s], dp = S.longl[3 * s + 1], ln = S.longl[3 * s + 2];
-                    for (uint32_t i = lane; i < ln; i += 32) ldst[dp + i] = S.in[sp + i];
-                }
-                if (CODEC == 0) out_pos += total; else { z_nseq += total >> 18; z_nlit += total & 0x3FFFF; }
-                // new pending = last head of this tile
-                const uint32_t pi = S.hidx[nh - 1], pr = S.piece[pi];
-                uint32_t ls;
-                if (nh >= 2 || pd_valid) { if (pi > 0) { const uint32_t pp = S.piece[pi - 1]; ls = t0 + pp + S.len[pp]; } else ls = pd_end; }
-                else ls = pd_lit;                          // first sequence of the block: literals start where emission stands (0)
-                pd_valid = 1; pd_lit = ls; pd_start = t0 + pr; pd_off = S.off[pr]; pd_end = tile_end;
+            // ---------------- close a block every 4 tiles (not at the end of the window: the final flush does that)
+            if ((ti & 3) == 3 && t1 < n) {
                 CTA_SYNC();
-                if (tid == 0) S.nlong = 0;
-            }
-            } while (0);
-
-            if (CODEC == 1) {
-                // ---------------- zstd: close a block every 4 tiles (not at the end of the window: the final flush does that)
-                z_tiles++;
-                if ((z_tiles & 3) == 0 && t1 < n) {
-                    CTA_SYNC();
-                    // trailing literals up to C: everything before the pending match (or all parsed bytes when nothing is pending)
-                    const uint32_t cover = pd_valid ? pd_lit : z_pos;
-                    const uint32_t C = pd_valid ? pd_start : t1;
-                    for (uint32_t i = tid; i < C - cover; i += NT) zs->lit[z_nlit + i] = S.in[cover + i];
-                    const uint32_t nl = z_nlit + (C - cover);
-                    CTA_SYNC();
-                    if (C > z_pos) out_pos += z_encode_block(ZE, S.fse, zs, z_nseq, nl, S.in + z_pos, C - z_pos, false, dst + out_pos, S.scanws, cta_sync);
-                    z_pos = C; pd_lit = C;                  // literals before C are emitted: the next sequence's literal run starts here
-                    z_nseq = 0; z_nlit = 0;
-                }
+                // trailing literals up to C: everything before the pending match (or all parsed bytes when nothing is pending)
+                const uint32_t cover = pd.valid ? pd.lit : z_pos;
+                const uint32_t C = pd.valid ? pd.start : t1;
+                for (uint32_t i = tid; i < C - cover; i += NT) zs->lit[z_nlit + i] = S.stage.in[cover + i];
+                const uint32_t nl = z_nlit + (C - cover);
+                CTA_SYNC();
+                if (C > z_pos) out_pos += z_encode_block(S.ent, S.fse, zs, z_nseq, nl, S.stage.in + z_pos, C - z_pos, false, dst + out_pos, S.scanws, cta_sync);
+                z_pos = C; pd.lit = C;                  // literals before C are emitted: the next sequence's literal run starts here
+                z_nseq = 0; z_nlit = 0;
             }
         }
 
         // ---------------- flush the pending sequence + last literals
-        if (CODEC == 1) {
-            CTA_SYNC();
-            uint32_t anchor = z_pos;
-            if (pd_valid) {
-                anchor = pd_end;
-                const uint32_t ll = pd_start - pd_lit;
-                if (tid == 0) { ZSeq q; q.litlen = ll; q.off = (uint16_t)pd_off; q.mlen = (uint16_t)(pd_end - pd_start); zs->seq[z_nseq] = q; }
-                for (uint32_t i = tid; i < ll; i += NT) zs->lit[z_nlit + i] = S.in[pd_lit + i];
-                z_nseq++; z_nlit += ll;
-            }
-            for (uint32_t i = tid; i < n - anchor; i += NT) zs->lit[z_nlit + i] = S.in[anchor + i];
-            z_nlit += n - anchor;
-            CTA_SYNC();
-            // the frame's last block carries the Last_Block bit; an empty raw block does when nothing is left
-            out_pos += z_encode_block(ZE, S.fse, zs, z_nseq, z_nlit, S.in + z_pos, n - z_pos, z_last_of_chunk, dst + out_pos, S.scanws, cta_sync);
-            if (tid == 0) blk_csize[blk] = out_pos;
-        } else {
-            uint32_t anchor = 0;
-            if (pd_valid) {
-                anchor = pd_end;
-                if (tid == 0) (void)c_emit_seq(S, dst, out_pos, pd_lit, pd_start - pd_lit, pd_off, pd_end - pd_start);
-                out_pos += c_seq_size(pd_start - pd_lit, pd_end - pd_start);
-                CTA_SYNC();
-                if (S.nlong) {                              // its literal run was long: copy it with the whole CTA
-                    const uint32_t sp = S.longl[0], dp = S.longl[1], ln = S.longl[2];
-                    for (uint32_t i = tid; i < ln; i += NT) dst[dp + i] = S.in[sp + i];
-                }
-            }
-            const uint32_t lit = n - anchor;
-            const uint32_t fin = out_pos + 1 + lit + (lit >= 15 ? 1 + (lit - 15) / 255 : 0);
-            if (fin >= n) { if (tid == 0) blk_csize[blk] = n | 0x80000000u; }   // stored block (LZ4F rule)
-            else {
-                uint8_t* op = dst + out_pos;
-                uint32_t hl = 1;
-                if (lit >= 15) hl += 1 + (lit - 15) / 255;
-                if (tid == 0) {
-                    uint8_t* q = op;
-                    *q++ = (uint8_t)((lit >= 15 ? 15u : lit) << 4);
-                    if (lit >= 15) { uint32_t x = lit - 15; while (x >= 255) { *q++ = 255; x -= 255; } *q++ = (uint8_t)x; }
-                    blk_csize[blk] = fin;
-                }
-                for (uint32_t i = tid; i < lit; i += NT) op[hl + i] = S.in[anchor + i];
-            }
+        CTA_SYNC();
+        uint32_t anchor = z_pos;
+        if (pd.valid) {
+            anchor = pd.end;
+            const uint32_t ll = pd.start - pd.lit;
+            if (tid == 0) { ZSeq q; q.litlen = ll; q.off = (uint16_t)pd.off; q.mlen = (uint16_t)(pd.end - pd.start); zs->seq[z_nseq] = q; }
+            for (uint32_t i = tid; i < ll; i += NT) zs->lit[z_nlit + i] = S.stage.in[pd.lit + i];
+            z_nseq++; z_nlit += ll;
         }
+        for (uint32_t i = tid; i < n - anchor; i += NT) zs->lit[z_nlit + i] = S.stage.in[anchor + i];
+        z_nlit += n - anchor;
+        CTA_SYNC();
+        // the frame's last block carries the Last_Block bit; an empty raw block does when nothing is left
+        out_pos += z_encode_block(S.ent, S.fse, zs, z_nseq, z_nlit, S.stage.in + z_pos, n - z_pos, z_last_of_chunk, dst + out_pos, S.scanws, cta_sync);
+        if (tid == 0) blk_csize[blk] = out_pos;
     }
 }
-
-#include "lz4_pipe.cuh"
 
 // ============================================================================ XXH32 (content checksum)
 // One warp per buffer.  XXH32 is four serial accumulator chains (one per 32-bit word of every 16-byte
@@ -929,31 +728,20 @@ extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint
     uint32_t* chk = (uint32_t*)w; w += (((uint64_t)nchunks * 4 + 255) & ~255ull);
     uint64_t* frame_size = (uint64_t*)w;
 
-    constexpr int LZ4_NT = 512;                    // 2 CTAs x 16 warps per SM: throughput scales ~linearly with resident warps (DESIGN.md §3)
-    cudaFuncSetAttribute(lz77_blocks_kernel<0, LZ4_NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CompressSmem));
+    // 2 CTAs x 16 warps per SM: throughput scales ~linearly with resident warps (DESIGN.md §3)
+    cudaFuncSetAttribute(lz4_blocks_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PipeSmem));
     const uint32_t maxc = (uint32_t)(zmt_sm_count() * 2 * 8);
     uint32_t gridc = nblocks < maxc ? nblocks : maxc;
-    size_t smem_bytes = sizeof(CompressSmem);
-    if (getenv("ZSTDMT_B200_OCC1")) {          // experiment knob: pad shared memory so that only one CTA fits per SM
-        smem_bytes = 200 * 1024;
-        cudaFuncSetAttribute(lz77_blocks_kernel<0, LZ4_NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    static bool occ_shown = false;
+    if (!occ_shown && getenv("ZSTDMT_B200_SHOW_OCC")) {
+        int nb = 0; occ_shown = true;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, lz4_blocks_pipe_kernel, 2 * P_TEAM, sizeof(PipeSmem));
+        fprintf(stderr, "[zstdmt_b200] lz4_blocks_pipe_kernel: %d CTAs/SM, %zu B smem\n", nb, sizeof(PipeSmem));
     }
-    static const bool no_pipe = getenv("ZSTDMT_B200_NOPIPE") != nullptr;   // A/B knob: single-team schedule (same output bytes)
     const ZmtSide side = zmt_side_stream();
     if (side.ok) cudaEventRecord(side.fork, stream);
     { ZmtProfScope ps(ZMT_K_LZ4_COMPRESS, stream);
-    if (no_pipe || smem_bytes != sizeof(CompressSmem))
-        lz77_blocks_kernel<0, LZ4_NT><<<gridc, LZ4_NT, smem_bytes, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u, nullptr);
-    else {
-        cudaFuncSetAttribute(lz4_blocks_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PipeSmem));
-        static bool occ_shown = false;
-        if (!occ_shown && getenv("ZSTDMT_B200_SHOW_OCC")) {
-            int nb = 0; occ_shown = true;
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, lz4_blocks_pipe_kernel, 2 * P_TEAM, sizeof(PipeSmem));
-            fprintf(stderr, "[zstdmt_b200] lz4_blocks_pipe_kernel: %d CTAs/SM, %zu B smem\n", nb, sizeof(PipeSmem));
-        }
-        lz4_blocks_pipe_kernel<<<gridc, 2 * P_TEAM, sizeof(PipeSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u);
-    } }
+    lz4_blocks_pipe_kernel<<<gridc, 2 * P_TEAM, sizeof(PipeSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u); }
     zmt_dbg_check(stream, "lz4 block compressor");
     // The content checksum only reads the input.  It cannot share an SM with the compressor (two compressor CTAs hold every
     // register of an SM), but enqueued on a side stream BEHIND the compressor's launch it fills the SMs the compressor's last,
@@ -1022,11 +810,11 @@ extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uin
     uint64_t* frame_size = (uint64_t*)w; w += ((((uint64_t)nchunks + 1) * 8 + 255) & ~255ull);
     ZScratch* zsc = (ZScratch*)w;
     static_assert(sizeof(ZScratch) % 8 == 0, "scratch stride");
-    cudaFuncSetAttribute(lz77_blocks_kernel<1, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CompressSmem));
+    cudaFuncSetAttribute(zstd_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZstdSmem));
     const uint32_t gridc = zstd_grid(nblocks);
     { ZmtProfScope ps(ZMT_K_ZSTD_COMPRESS, stream);
-    lz77_blocks_kernel<1, 256><<<gridc, 256, sizeof(CompressSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u, zsc); }
-    zmt_dbg_check(stream, "lz77_blocks_kernel<zstd>");
+    zstd_blocks_kernel<<<gridc, P_TEAM, sizeof(ZstdSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u, zsc); }
+    zmt_dbg_check(stream, "zstd_blocks_kernel");
     zstd_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size);
     scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks);
     const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);

@@ -1,16 +1,19 @@
-// lz4_pipe.cuh — the LZ4 block compressor as a two-team software pipeline (included by lz4_kernels.cu).
+// lz4_pipe.cuh — the LZ77 parse as team functions, and the LZ4 block compressor that runs it as a two-team software
+// pipeline (included by lz4_kernels.cu, whose Zstandard encoder runs the same functions with a single team).
 //
-// Same algorithm and same output bytes as lz77_blocks_kernel<0,*> (oracle twin: orc_lz4_block_compress_b200);
-// what changes is the schedule.  The per-tile work splits into a front end that carries (e, e_din) from tile to
-// tile — candidates, speculative chain walks, path resolution — and a back end that carries the pending
-// sequence and the output cursor — marking, piece merge, emission.  Neither needs the other's carry, so a CTA of
+// Oracle twin of the parse: orc_lz4_block_compress_b200.  The per-tile work splits into a front end that carries
+// (e, e_din) from tile to tile — candidates, speculative chain walks, path resolution — and a back end that carries the
+// pending sequence and the output cursor — marking, piece merge, emission.  Neither needs the other's carry, so a CTA of
 // 512 threads runs them as two teams of 256, the front end one tile ahead of the back end, over a
 // double-buffered set of tile arrays.  Hand-off is by named barriers (bar.arrive / bar.sync, count 512):
 // FULL[b] producer -> consumer, EMPTY[b] consumer -> producer.  With 2 CTAs per SM this gives four independent
 // instruction streams per SM instead of two (the kernel is issue/latency bound: DESIGN.md §3).
 //
-// Shared memory: only what crosses the teams is double-buffered (off, M, V, entry positions, path mask: 9.5 KB per
-// buffer).  Piece lengths do not cross: the front end does not store them, the marking walk of the back end
+// Every phase below is run by one team of P_TEAM threads and takes that team's barrier id: PB_A / PB_B here, 0 in the
+// Zstandard encoder, whose CTA is one team.
+//
+// Shared memory: only what crosses the teams is double-buffered (PipeTile: off, M, V, entry positions, path mask: 9.5 KB
+// per buffer).  Piece lengths do not cross: the front end does not store them, the marking walk of the back end
 // recomputes them for the true-path pieces only (it has the slack), which keeps the 32-bit hash table and its
 // single-pass atomicMax.  (A 16-bit table needs a CAS loop or a two-pass atomicMax per insert, both more instructions.)
 #pragma once
@@ -20,7 +23,7 @@
 #define PB_B        2u
 #define PB_FULL0    3u
 #define PB_EMPTY0   5u
-#define P_MAXPIECE  1280u         // 4096/4 match pieces + 256 continuation pieces, multiple of 256
+#define LZ_SPT      (1024u / P_TEAM)   // sequences per thread at most (<= 1024 per tile)
 
 // Barrier ids are immediates: ptxas reserves only the ids it sees (a register id makes it reserve all 16,
 // and barriers are an occupancy resource).
@@ -37,56 +40,8 @@ __device__ __forceinline__ void bar_arrive()
     __threadfence_block();
     asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(NTHREADS) : "memory");
 }
-#define TEAM_A_SYNC()   bar_sync<PB_A, P_TEAM>()
-#define TEAM_B_SYNC()   bar_sync<PB_B, P_TEAM>()
-
-struct __align__(16) PipeTile {
-    uint16_t off[C_TILE];                 // candidate offset per tile position (0 = none)
-    uint32_t M[C_TILE / 32];              // has-candidate bits
-    uint32_t V[C_TILE / 32];              // visited-by-own-chain bits
-    uint8_t  min_[C_CHAINS];              // entry position of a chain on the true path, relative to its own segment (< 16)
-    uint32_t pathmask[C_CHAINS / 32];     // chains on the true path
-    uint32_t k0, e_din, do_parse, pad;    // entry chain, offset of the match open at the entry, tile has work
-};
-
-struct __align__(16) PipeSmem {
-    uint8_t  pad0[16];
-    uint8_t  in[LZ4_BLK + 32];
-    uint32_t tab[1 << C_HASHLOG];         // hash -> 1 + position
-    PipeTile tile[2];
-    // ---- front end (team A)
-    uint32_t xfree[C_CHAINS];
-    uint32_t mpos[C_CHAINS];
-    uint16_t xdin[C_CHAINS];
-    uint16_t link[C_CHAINS];
-    uint8_t  jump[C_CHAINS];
-    uint16_t entry[8];
-    uint32_t e_next, d_next;
-    uint32_t a_any[2];
-    // ---- back end (team B)
-    uint32_t Sel[C_TILE / 32];
-    uint32_t Cont[C_TILE / 32];
-    uint8_t  len[C_TILE];                 // piece length per selected piece start (written by the marking walk)
-    uint16_t piece[P_MAXPIECE];
-    union {                               // segprev is read by head detection, before the heads are written
-        uint16_t hidx[C_TILE / 4];        // heads: one per sequence, sequences hold a match of >= 4 bytes
-        uint16_t segprev[C_CHAINS];       // per segment: 1 + start of the last non-Cont piece before it (0: none)
-    };
-    uint32_t longl[2 * (C_TILE / (C_LONGLIT + 1) + 2)];   // jobs: literal runs > C_LONGLIT (start | length << 16, output offset) -- at most
-                                                           // 4096/37 + 1 pending per tile -- and 255-runs of match lengths >= 1290 (count, offset | 1<<31)
-    __align__(16) uint32_t scanws[16];
-    uint32_t nlong;
-    uint32_t fin_anchor, fin_out;
-    uint64_t mbar;
-};
-static_assert(sizeof(PipeSmem) + 1024 <= (228 * 1024) / 2, "two CTAs per SM");
-
-// what c_walk / c_emit_seq touch, with the tile arrays of the current buffer
-struct PipeView {
-    static constexpr bool relen = true;   // the front end does not keep piece lengths: the marking walk recomputes them
-    const uint8_t* in; uint16_t* off; uint8_t* len; uint32_t* M; uint32_t* V; uint32_t* Sel; uint32_t* Cont;
-    uint32_t* xfree; uint16_t* xdin; uint16_t* link; uint32_t* mpos; uint32_t* longl; uint32_t& nlong;
-};
+template <uint32_t BARID>
+__device__ __forceinline__ void team_sync() { bar_sync<BARID, P_TEAM>(); }
 
 // exclusive scan over one team (8 warps); one team barrier; `ws` = two 8-word halves used alternately
 template <uint32_t BARID>
@@ -97,7 +52,7 @@ __device__ __forceinline__ uint32_t team_exscan1(uint32_t v, uint32_t* ws, uint3
     for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(ZMT_FULL_MASK, inc, d); if (lane >= (uint32_t)d) inc += y; }
     uint32_t* w = ws + 8 * (parity & 1);
     if (lane == 31) w[twid] = inc;
-    bar_sync<BARID, P_TEAM>();
+    team_sync<BARID>();
     const uint4 a = *reinterpret_cast<const uint4*>(w), b = *reinterpret_cast<const uint4*>(w + 4);
     const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
     uint32_t base = 0, tot = 0;
@@ -120,7 +75,7 @@ __device__ __forceinline__ uint32_t team_exscan_pieces(uint32_t v, uint32_t m, u
     uint32_t mex = __shfl_sync(ZMT_FULL_MASK, m, below ? 31 - __clz(below) : 0);
     if (!below) mex = 0;
     if (lane == 31) { ws[twid] = inc; ws[8 + twid] = m ? m : mex; }
-    bar_sync<BARID, P_TEAM>();
+    team_sync<BARID>();
     const uint4 a = *reinterpret_cast<const uint4*>(ws), b = *reinterpret_cast<const uint4*>(ws + 4);
     const uint4 c = *reinterpret_cast<const uint4*>(ws + 8), d = *reinterpret_cast<const uint4*>(ws + 12);
     const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, y[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w};
@@ -131,6 +86,275 @@ __device__ __forceinline__ uint32_t team_exscan_pieces(uint32_t v, uint32_t m, u
     *mprev = mx;
     return base + inc - v;
 }
+
+// ---------------------------------------------------------------- block staging (whole CTA, NT threads)
+// Stages the n bytes at src into St.in (TMA bulk copy when 16-byte aligned), zeroes the pads and the hash table.  The
+// caller has a CTA barrier between the previous block's last reader and this call.
+template <uint32_t NT>
+__device__ __forceinline__ void lz_stage(LzStage& St, uint32_t* tab, uint64_t* mbar, const uint8_t* src, uint32_t n, uint32_t flags, uint32_t tid)
+{
+    const uint32_t nb16 = ((((uintptr_t)src & 15) == 0) && !(flags & 1)) ? (n & ~15u) : 0;
+    if (tid == 0 && nb16) mbar_init(mbar, 1);
+    CTA_SYNC();
+    if (tid == 0 && nb16) { mbar_expect_tx(mbar, nb16); bulk_g2s(St.in, src, nb16, mbar); }
+    for (uint32_t i = nb16 + tid; i < n; i += NT) St.in[i] = src[i];
+    for (uint32_t i = n + tid; i < ((n + 3) & ~3u) + 32 && i < LZ4_BLK + 32; i += NT) St.in[i] = 0;
+    if (tid < 16) St.pad0[tid] = 0;
+    for (uint32_t i = tid; i < (1u << C_HASHLOG); i += NT) tab[i] = 0;
+    // one thread observes the TMA completion; the CTA barrier publishes the staged bytes to everyone
+    if (tid == 0 && nb16) { mbar_wait(mbar, 0); asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(mbar))); }
+    CTA_SYNC();
+}
+
+// ---------------------------------------------------------------- front end
+// Candidate rounds of the tile at t0 (4 rounds of 1024 positions): fills T.off and T.M, clears T.V.  Returns, uniform
+// over the team, whether the tile has a candidate.  any[2] holds that flag per tile parity b; any[b ^ 1] is cleared in
+// round 0, once every reader of the previous tile's flag is past the round's first barrier.
+template <uint32_t BARID>
+__device__ __forceinline__ bool lz_candidates(const uint8_t* in, uint32_t* tab, PipeTile& T, uint32_t* any, uint32_t b,
+                                              uint32_t t0, uint32_t n, uint32_t ttid, uint32_t lane)
+{
+    if (ttid < C_TILE / 32) T.V[ttid] = 0;
+    uint32_t anyM = 0;
+#pragma unroll 1
+    for (uint32_t r = 0; r < C_TILE / C_ROUND; r++) {
+        // four consecutive positions per thread: three aligned words hold the windows of all four, the four
+        // offsets go out as one 8-byte store, and eight lanes' 4-bit slices make one M word
+        static_assert(C_ROUND == 4 * P_TEAM, "a round is four positions per thread");
+        const uint32_t rel = r * C_ROUND + 4 * ttid, i = t0 + rel;
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(in) + (i >> 2);
+        const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
+        uint32_t hreg[4], tv[4], o[4], m4 = 0;
+        // the four table reads, then the four window reads, are issued together: no position waits on another
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
+            hreg[k] = (__funnelshift_r(w1, w2, 8 * k) * 2654435761u) >> (32 - C_HASHLOG);
+            tv[k] = tab[hreg[k]];
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
+            const uint32_t ik = i + k;
+            const bool ok = (ik + 12 <= n);
+            const uint32_t v = __funnelshift_r(w1, w2, 8 * k), pv = __funnelshift_r(w0, w1, 8 * k);
+            const uint32_t t = tv[k];
+            const bool hit = t && lds32u(in, t ? t - 1 : 0) == v;
+            o[k] = 0;
+            if (ok) {
+                // short-period candidates d = 1..4: v(i-d) is a byte-shift of the window
+                if (ik >= 1 && __funnelshift_r(pv, v, 24) == v) o[k] = 1;
+                else if (ik >= 2 && __funnelshift_r(pv, v, 16) == v) o[k] = 2;
+                else if (ik >= 3 && __funnelshift_r(pv, v, 8) == v) o[k] = 3;
+                else if (ik >= 4 && pv == v) o[k] = 4;
+                else if (hit) o[k] = ik - (t - 1);
+            }
+            if (!ok) hreg[k] = 0xFFFFFFFFu;
+            m4 |= (uint32_t)(o[k] != 0) << k;
+        }
+        *reinterpret_cast<uint2*>(&T.off[rel]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+        uint32_t mw = m4 << (4 * (lane & 7));
+        mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 1);
+        mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 2);
+        mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 4);
+        if ((lane & 7) == 0) T.M[rel >> 5] = mw;
+        anyM |= mw;
+        team_sync<BARID>();
+        if (r == 0 && ttid == 0) any[b ^ 1] = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
+            bool last = hreg[k] != 0xFFFFFFFFu;     // a later position of the quad with the same hash wins anyway
+#pragma unroll
+            for (uint32_t k2 = k + 1; k2 < 4; k2++) last &= hreg[k2] != hreg[k];
+            if (last) atomicMax(&tab[hreg[k]], i + k + 1);
+        }
+        team_sync<BARID>();
+    }
+    if ((lane & 7) == 0 && anyM) atomicOr(&any[b], 1u);   // anyM covers the lane's group of eight
+    team_sync<BARID>();
+    return any[b] != 0;
+}
+
+// Speculative chains (own segment, then continuation) and the true path through the tile, entered at e inside a match
+// of offset e_din (0: free).  Hands the path to the back end (T.k0, T.e_din, T.min_, T.pathmask, T.do_parse) and moves
+// (e, e_din) to where it leaves the tile.  A tile without candidates or open match, or one the parse has already passed,
+// is skipped.  Returns T.do_parse.
+template <uint32_t BARID>
+__device__ __forceinline__ bool lz_chains(const uint8_t* in, PipeTile& T, LzFront& F, bool has_match, uint32_t& e, uint32_t& e_din,
+                                          uint32_t t0, uint32_t limit, uint32_t ttid, uint32_t lane)
+{
+    const uint32_t t1 = t0 + C_TILE, twid = ttid >> 5;
+    if ((!has_match && !e_din) || e >= t1) {
+        if (e < t1) e = t1;
+        if (ttid == 0) T.do_parse = 0;
+        return false;
+    }
+    const uint32_t k0 = (e - t0) / C_SEG;
+    const uint32_t seg0 = t0 + ttid * C_SEG;
+    const bool alive = ttid >= k0;
+    if (alive) c_walk<0>(in, T, F, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
+    else F.link[ttid] = (uint16_t)ttid;                 // dead: self link, never reached
+    team_sync<BARID>();
+    if (alive) c_walk<1>(in, T, F, ttid, F.xfree[ttid], F.xdin[ttid], t0, limit);
+    team_sync<BARID>();
+    // Which chains lie on the true path (entry k0, follow the links).  Links only go forward.  Each warp resolves its
+    // own 32 chains with shuffles (pointer doubling on lane indices: terminal chain + bitmask of the lanes on the way),
+    // one thread then hops from warp to warp (<= 8 hops), and each warp reads its path mask back: 2 barriers, not 18.
+    const uint32_t lk = F.link[ttid];
+    const bool inwarp = (lk != C_END) && (lk != ttid) && ((lk >> 5) == twid);
+    uint32_t jmp = inwarp ? (lk & 31) : lane;                 // next lane inside this warp (self = terminal)
+    uint32_t pm = (1u << lane) | (1u << jmp);
+#pragma unroll
+    for (int r = 0; r < 5; r++) { pm |= __shfl_sync(ZMT_FULL_MASK, pm, jmp); jmp = __shfl_sync(ZMT_FULL_MASK, jmp, jmp); }
+    F.jump[ttid] = (uint8_t)(32 * twid + jmp);
+    F.xfree[ttid] = pm;                                       // xfree is dead after the continuation walk
+    if (ttid < 8) F.entry[ttid] = 0xFFFFu;
+    team_sync<BARID>();
+    if (ttid == 0) {
+        uint32_t cur = k0;
+        T.min_[k0] = (uint8_t)((e - t0) & (C_SEG - 1));
+        for (;;) {
+            F.entry[cur >> 5] = (uint16_t)cur;
+            const uint32_t t = F.jump[cur], tl = F.link[t];
+            if (tl == C_END) { F.e_next = F.mpos[t]; F.d_next = F.xdin[t]; break; }
+            T.min_[tl] = (uint8_t)((F.mpos[t] - t0) & (C_SEG - 1));   // entry position of the next warp's first chain on the path
+            cur = tl;
+        }
+        T.k0 = k0; T.e_din = e_din; T.do_parse = 1;
+    }
+    team_sync<BARID>();
+    const uint32_t a = F.entry[twid];
+    const uint32_t pmask = (a != 0xFFFFu) ? F.xfree[a] : 0u;
+    if (lane == 0) T.pathmask[twid] = pmask;
+    // in-warp successor: its entry position is my merge position
+    if (((pmask >> lane) & 1u) && inwarp) T.min_[lk] = (uint8_t)((F.mpos[ttid] - t0) & (C_SEG - 1));
+    e = F.e_next; e_din = F.d_next;
+    return true;
+}
+
+// ---------------------------------------------------------------- back end
+// pending sequence: the last one found so far; its match may still grow in the next tile, so it is emitted one tile late
+struct LzPending { uint32_t valid, lit, start, off, end; };
+
+// Marks the pieces of the true path (c_walk recomputes their lengths), lists them, and finds the HEADS: piece r starts
+// a sequence unless it continues the previous piece's match -- flagged continuation, or contiguous with the same
+// offset (the effective offset of a flagged piece is that of the nearest unflagged piece before it).  Returns the
+// number of heads nh (0 when nothing is marked); the pending match grows over the pieces before the first head.
+template <uint32_t BARID>
+__device__ __forceinline__ uint32_t lz_heads(const uint8_t* in, PipeTile& T, LzBack& K, uint32_t* scanws, LzPending& pd, uint32_t& tile_end,
+                                             uint32_t t0, uint32_t limit, uint32_t ttid, uint32_t lane)
+{
+    const uint32_t twid = ttid >> 5, k0 = T.k0;
+    if (ttid < C_TILE / 32) { K.Sel[ttid] = 0; K.Cont[ttid] = 0; }
+    team_sync<BARID>();
+    if ((T.pathmask[twid] >> lane) & 1u) c_walk<2>(in, T, K, ttid, t0 + ttid * C_SEG + T.min_[ttid], ttid == k0 ? T.e_din : 0u, t0, limit);
+    team_sync<BARID>();
+    uint32_t np;
+    {
+        // one segment (16 positions) per thread.  segprev[j]: 1 + start of the last non-Cont piece before
+        // segment j (0: none), the piece whose offset a Cont piece at the start of segment j continues
+        const uint32_t sh = 16 * (ttid & 1);
+        uint32_t w = (K.Sel[ttid >> 1] >> sh) & 0xFFFFu;
+        const uint32_t nc = w & ~(K.Cont[ttid >> 1] >> sh);
+        const uint32_t last = nc ? ttid * C_SEG + (31 - __clz(nc)) + 1 : 0u;
+        uint32_t prev;
+        uint32_t base = team_exscan_pieces<BARID>(__popc(w), last, scanws, &np, &prev, twid, lane);
+        K.segprev[ttid] = (uint16_t)prev;
+        while (w) { const uint32_t bit = __ffs(w) - 1; w &= w - 1; K.piece[base++] = (uint16_t)(ttid * C_SEG + bit); }
+    }
+    team_sync<BARID>();
+    if (np == 0) return 0;
+    // pieces are dealt in runs of ceil(np / 256) per thread, so every warp shares the work
+    uint32_t nh_local = 0, headmask = 0;
+    const uint32_t ppt = (np + P_TEAM - 1) / P_TEAM;
+#pragma unroll
+    for (uint32_t k = 0; k < C_MAXPIECE / P_TEAM; k++) {
+        const uint32_t r = ttid * ppt + k;
+        if (k < ppt && r < np) {
+            const uint32_t pr = K.piece[r];
+            bool head = !((K.Cont[pr >> 5] >> (pr & 31)) & 1);
+            if (head) {
+                uint32_t pend, poff;                         // end and effective offset of what precedes piece r
+                if (r == 0) { pend = pd.valid ? pd.end : 0xFFFFFFFFu; poff = pd.off; }
+                else {
+                    const uint32_t pb = K.piece[r - 1];
+                    pend = t0 + pb + K.len[pb];
+                    if (!((K.Cont[pb >> 5] >> (pb & 31)) & 1)) poff = T.off[pb];
+                    else {                      // Cont pieces start at a segment boundary (c_walk cuts there)
+                        const uint32_t sp = K.segprev[pb / C_SEG];
+                        poff = sp ? T.off[sp - 1] : pd.off;
+                    }
+                }
+                if (pend == t0 + pr && poff == T.off[pr]) head = false;
+            }
+            if (head) { headmask |= 1u << k; nh_local++; }
+        }
+    }
+    uint32_t nh;
+    {
+        uint32_t hb = team_exscan1<BARID>(nh_local, scanws, 1, &nh, twid, lane);
+#pragma unroll
+        for (uint32_t k = 0; k < C_MAXPIECE / P_TEAM; k++) if (headmask & (1u << k)) K.hidx[hb++] = (uint16_t)(ttid * ppt + k);
+    }
+    team_sync<BARID>();
+    const uint32_t lastp = K.piece[np - 1];
+    tile_end = t0 + lastp + K.len[lastp];                     // end of the last piece of this tile
+    if (nh == 0) pd.end = tile_end;                           // every piece extends the pending sequence
+    else if (pd.valid && K.hidx[0] > 0) { const uint32_t pb = K.piece[K.hidx[0] - 1]; pd.end = t0 + pb + K.len[pb]; }
+    return nh;
+}
+
+// this thread's run of the sequences the tile closes: [pending] + heads 0 .. nh-2, dealt in runs of ceil(count / 256)
+// per thread (head nh-1 becomes the new pending sequence: lz_next_pending).  Per sequence: literals start, literal
+// length, offset, match length.
+struct LzRun { uint32_t cnt, lit0[LZ_SPT], lit[LZ_SPT], off[LZ_SPT], len[LZ_SPT]; };
+__device__ __forceinline__ LzRun lz_seq_run(const PipeTile& T, const LzBack& K, const LzPending& pd, uint32_t nh, uint32_t t0, uint32_t ttid)
+{
+    LzRun R; R.cnt = 0;
+    const uint32_t nemit = pd.valid + nh - 1;
+    const uint32_t spt = (nemit + P_TEAM - 1) / P_TEAM;
+#pragma unroll
+    for (uint32_t k = 0; k < LZ_SPT; k++) {
+        const uint32_t sidx = ttid * spt + k;
+        if (k < spt && sidx < nemit) {
+            uint32_t ls, st, of, en;
+            if (pd.valid && sidx == 0) { ls = pd.lit; st = pd.start; of = pd.off; en = pd.end; }
+            else {
+                const uint32_t h = sidx - pd.valid;          // head index, h <= nh-2
+                const uint32_t pi = K.hidx[h], pr = K.piece[pi];
+                const uint32_t pl = K.piece[K.hidx[h + 1] - 1];
+                st = t0 + pr; of = T.off[pr]; en = t0 + pl + K.len[pl];
+                if (h == 0) ls = pd.valid ? pd.end : pd.lit;     // pd.lit doubles as "end of everything emitted so far"
+                else { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + K.len[pp]; }
+            }
+            R.lit0[k] = ls; R.lit[k] = st - ls; R.off[k] = of; R.len[k] = en - st; R.cnt++;
+        }
+    }
+    return R;
+}
+
+// after emission: the last head of the tile becomes the pending sequence
+__device__ __forceinline__ void lz_next_pending(const PipeTile& T, const LzBack& K, LzPending& pd, uint32_t nh, uint32_t tile_end, uint32_t t0)
+{
+    const uint32_t pi = K.hidx[nh - 1], pr = K.piece[pi];
+    uint32_t ls;
+    if (nh >= 2 || pd.valid) { if (pi > 0) { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + K.len[pp]; } else ls = pd.end; }
+    else ls = pd.lit;                          // first sequence of the block: literals start where emission stands (0)
+    pd.valid = 1; pd.lit = ls; pd.start = t0 + pr; pd.off = T.off[pr]; pd.end = tile_end;
+}
+
+// ---------------------------------------------------------------- the LZ4 pipeline
+struct __align__(16) PipeSmem {
+    LzStage  stage;
+    uint32_t tab[1 << C_HASHLOG];         // hash -> 1 + position
+    PipeTile tile[2];
+    LzFront  fe;                          // team A
+    uint32_t a_any[2];
+    LzBack   be;                          // team B
+    __align__(16) uint32_t scanws[16];
+    uint32_t nlong;
+    uint32_t fin_anchor, fin_out;
+    uint64_t mbar;
+};
+static_assert(sizeof(PipeSmem) + 1024 <= (228 * 1024) / 2, "two CTAs per SM");
 
 __global__ void __launch_bounds__(2 * P_TEAM, 2)
 lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
@@ -150,21 +374,11 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
         uint32_t n = 0;
         if (boff < cbytes) n = (uint32_t)((cbytes - boff) < LZ4_BLK ? (cbytes - boff) : LZ4_BLK);
         if (n == 0) { if (tid == 0) blk_csize[blk] = 0; continue; }
-        const uint8_t* src = in + cbase + boff;
         uint8_t* dst = tmp + (uint64_t)blk * ZMT_LZ4_TMP_STRIDE;
 
-        // ---- stage the block into shared memory (TMA bulk copy when 16-byte aligned); all 512 threads
         CTA_SYNC();                                       // previous block fully consumed
-        const uint32_t nb16 = ((((uintptr_t)src & 15) == 0) && !(flags & 1)) ? (n & ~15u) : 0;
-        if (tid == 0) { if (nb16) mbar_init(&S.mbar, 1); S.nlong = 0; S.a_any[0] = 0; S.a_any[1] = 0; }
-        CTA_SYNC();
-        if (tid == 0 && nb16) { mbar_expect_tx(&S.mbar, nb16); bulk_g2s(S.in, src, nb16, &S.mbar); }
-        for (uint32_t i = nb16 + tid; i < n; i += NT) S.in[i] = src[i];
-        for (uint32_t i = n + tid; i < ((n + 3) & ~3u) + 32 && i < LZ4_BLK + 32; i += NT) S.in[i] = 0;
-        if (tid < 16) S.pad0[tid] = 0;
-        for (uint32_t i = tid; i < (1u << C_HASHLOG); i += NT) S.tab[i] = 0;
-        if (tid == 0 && nb16) { mbar_wait(&S.mbar, 0); asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&S.mbar))); }
-        CTA_SYNC();
+        if (tid == 0) { S.nlong = 0; S.a_any[0] = 0; S.a_any[1] = 0; }
+        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, flags, tid);
 
         const uint32_t limit = n >= 5 ? n - 5 : 0;        // matches end at or before n-5
         const uint32_t ntiles = (n + C_TILE - 1) / C_TILE;
@@ -173,232 +387,57 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
             // =========================================================== front end: candidates, chains, true path
             uint32_t e = 0, e_din = 0;                    // team-uniform parse state (position, offset of the open match)
             for (uint32_t ti = 0; ti < ntiles; ti++) {
-                const uint32_t t0 = ti * C_TILE, t1 = t0 + C_TILE, b = ti & 1;
+                const uint32_t t0 = ti * C_TILE, b = ti & 1;
                 PipeTile& T = S.tile[b];
                 if (ti >= 2) { if (b) bar_sync<PB_EMPTY0 + 1, 2 * P_TEAM>(); else bar_sync<PB_EMPTY0, 2 * P_TEAM>(); }               // back end released this buffer (tile ti-2)
-                if (ttid < C_TILE / 32) T.V[ttid] = 0;
-                uint32_t anyM = 0;
-#pragma unroll 1
-                for (uint32_t r = 0; r < C_TILE / C_ROUND; r++) {
-                    // four consecutive positions per thread: three aligned words hold the windows of all four, the four
-                    // offsets go out as one 8-byte store, and eight lanes' 4-bit slices make one M word
-                    static_assert(C_ROUND == 4 * P_TEAM, "a round is four positions per thread");
-                    const uint32_t rel = r * C_ROUND + 4 * ttid, i = t0 + rel;
-                    const uint32_t* w = reinterpret_cast<const uint32_t*>(S.in) + (i >> 2);
-                    const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
-                    uint32_t hreg[4], tab[4], o[4], m4 = 0;
-                    // the four table reads, then the four window reads, are issued together: no position waits on another
-#pragma unroll
-                    for (uint32_t k = 0; k < 4; k++) {
-                        hreg[k] = (__funnelshift_r(w1, w2, 8 * k) * 2654435761u) >> (32 - C_HASHLOG);
-                        tab[k] = S.tab[hreg[k]];
-                    }
-#pragma unroll
-                    for (uint32_t k = 0; k < 4; k++) {
-                        const uint32_t ik = i + k;
-                        const bool ok = (ik + 12 <= n);
-                        const uint32_t v = __funnelshift_r(w1, w2, 8 * k), pv = __funnelshift_r(w0, w1, 8 * k);
-                        const uint32_t t = tab[k];
-                        const bool hit = t && lds32u(S.in, t ? t - 1 : 0) == v;
-                        o[k] = 0;
-                        if (ok) {
-                            if (ik >= 1 && __funnelshift_r(pv, v, 24) == v) o[k] = 1;
-                            else if (ik >= 2 && __funnelshift_r(pv, v, 16) == v) o[k] = 2;
-                            else if (ik >= 3 && __funnelshift_r(pv, v, 8) == v) o[k] = 3;
-                            else if (ik >= 4 && pv == v) o[k] = 4;
-                            else if (hit) o[k] = ik - (t - 1);
-                        }
-                        if (!ok) hreg[k] = 0xFFFFFFFFu;
-                        m4 |= (uint32_t)(o[k] != 0) << k;
-                    }
-                    *reinterpret_cast<uint2*>(&T.off[rel]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
-                    uint32_t mw = m4 << (4 * (lane & 7));
-                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 1);
-                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 2);
-                    mw |= __shfl_xor_sync(ZMT_FULL_MASK, mw, 4);
-                    if ((lane & 7) == 0) T.M[rel >> 5] = mw;
-                    anyM |= mw;
-                    TEAM_A_SYNC();
-                    if (r == 0 && ttid == 0) S.a_any[b ^ 1] = 0;       // every reader of the previous tile's flag is past it
-#pragma unroll
-                    for (uint32_t k = 0; k < 4; k++) {
-                        bool last = hreg[k] != 0xFFFFFFFFu;     // a later position of the quad with the same hash wins anyway
-#pragma unroll
-                        for (uint32_t k2 = k + 1; k2 < 4; k2++) last &= hreg[k2] != hreg[k];
-                        if (last) atomicMax(&S.tab[hreg[k]], i + k + 1);
-                    }
-                    TEAM_A_SYNC();
-                }
-                if ((lane & 7) == 0 && anyM) atomicOr(&S.a_any[b], 1u);   // anyM covers the lane's group of eight
-                TEAM_A_SYNC();
-                const bool tile_has_match = S.a_any[b] != 0;
-                const bool do_parse = !((!tile_has_match && !e_din) || e >= t1);
-                if (!do_parse) { if (e < t1) e = t1; if (ttid == 0) T.do_parse = 0; }
-                else {
-                    PipeView W{S.in, T.off, nullptr, T.M, T.V, S.Sel, S.Cont, S.xfree, S.xdin, S.link, S.mpos, S.longl, S.nlong};
-                    const uint32_t k0 = (e - t0) / C_SEG;
-                    const uint32_t seg0 = t0 + ttid * C_SEG;
-                    const bool alive = ttid >= k0;
-                    if (alive) c_walk<0>(W, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
-                    else S.link[ttid] = (uint16_t)ttid;                 // dead: self link, never reached
-                    TEAM_A_SYNC();
-                    if (alive) c_walk<1>(W, ttid, S.xfree[ttid], S.xdin[ttid], t0, limit);
-                    TEAM_A_SYNC();
-                    // which chains lie on the true path (see lz77_blocks_kernel phase 3)
-                    const uint32_t lk = S.link[ttid];
-                    const bool inwarp = (lk != C_END) && (lk != ttid) && ((lk >> 5) == twid);
-                    uint32_t jmp = inwarp ? (lk & 31) : lane;
-                    uint32_t pm = (1u << lane) | (1u << jmp);
-#pragma unroll
-                    for (int r = 0; r < 5; r++) { pm |= __shfl_sync(ZMT_FULL_MASK, pm, jmp); jmp = __shfl_sync(ZMT_FULL_MASK, jmp, jmp); }
-                    S.jump[ttid] = (uint8_t)(32 * twid + jmp);
-                    S.xfree[ttid] = pm;
-                    if (ttid < 8) S.entry[ttid] = 0xFFFFu;
-                    TEAM_A_SYNC();
-                    if (ttid == 0) {
-                        uint32_t cur = k0;
-                        T.min_[k0] = (uint8_t)((e - t0) & (C_SEG - 1));
-                        for (;;) {
-                            S.entry[cur >> 5] = (uint16_t)cur;
-                            const uint32_t t = S.jump[cur], tl = S.link[t];
-                            if (tl == C_END) { S.e_next = S.mpos[t]; S.d_next = S.xdin[t]; break; }
-                            T.min_[tl] = (uint8_t)((S.mpos[t] - t0) & (C_SEG - 1));
-                            cur = tl;
-                        }
-                        T.k0 = k0; T.e_din = e_din; T.do_parse = 1;
-                    }
-                    TEAM_A_SYNC();
-                    const uint32_t a = S.entry[twid];
-                    const uint32_t pmask = (a != 0xFFFFu) ? S.xfree[a] : 0u;
-                    if (lane == 0) T.pathmask[twid] = pmask;
-                    if (((pmask >> lane) & 1u) && inwarp) T.min_[lk] = (uint8_t)((S.mpos[ttid] - t0) & (C_SEG - 1));
-                    e = S.e_next; e_din = S.d_next;
-                }
+                const bool has_match = lz_candidates<PB_A>(S.stage.in, S.tab, T, S.a_any, b, t0, n, ttid, lane);
+                lz_chains<PB_A>(S.stage.in, T, S.fe, has_match, e, e_din, t0, limit, ttid, lane);
                 if (b) bar_arrive<PB_FULL0 + 1, 2 * P_TEAM>(); else bar_arrive<PB_FULL0, 2 * P_TEAM>();
             }
         } else {
             // =========================================================== back end: mark, merge pieces, emit
             uint32_t out_pos = 0;
-            uint32_t pd_valid = 0, pd_lit = 0, pd_start = 0, pd_off = 0, pd_end = 0;    // pending sequence (may still grow)
+            LzPending pd = {0, 0, 0, 0, 0};
             for (uint32_t ti = 0; ti < ntiles; ti++) {
                 const uint32_t t0 = ti * C_TILE, b = ti & 1;
                 PipeTile& T = S.tile[b];
-                PipeView W{S.in, T.off, S.len, T.M, T.V, S.Sel, S.Cont, S.xfree, S.xdin, S.link, S.mpos, S.longl, S.nlong};
                 if (b) bar_sync<PB_FULL0 + 1, 2 * P_TEAM>(); else bar_sync<PB_FULL0, 2 * P_TEAM>();
-                if (T.do_parse) do {
-                    const uint32_t k0 = T.k0;
-                    if (ttid < C_TILE / 32) { S.Sel[ttid] = 0; S.Cont[ttid] = 0; }
-                    TEAM_B_SYNC();
-                    if ((T.pathmask[twid] >> lane) & 1u) c_walk<2>(W, ttid, t0 + ttid * C_SEG + T.min_[ttid], ttid == k0 ? T.e_din : 0u, t0, limit);
-                    TEAM_B_SYNC();
-                    uint32_t np;
-                    {
-                        // one segment (16 positions) per thread.  segprev[j]: 1 + start of the last non-Cont piece before
-                        // segment j (0: none), the piece whose offset a Cont piece at the start of segment j continues
-                        const uint32_t sh = 16 * (ttid & 1);
-                        uint32_t w = (S.Sel[ttid >> 1] >> sh) & 0xFFFFu;
-                        const uint32_t nc = w & ~(S.Cont[ttid >> 1] >> sh);
-                        const uint32_t last = nc ? ttid * C_SEG + (31 - __clz(nc)) + 1 : 0u;
-                        uint32_t prev;
-                        uint32_t base = team_exscan_pieces<PB_B>(__popc(w), last, S.scanws, &np, &prev, twid, lane);
-                        S.segprev[ttid] = (uint16_t)prev;
-                        while (w) { const uint32_t bit = __ffs(w) - 1; w &= w - 1; S.piece[base++] = (uint16_t)(ttid * C_SEG + bit); }
-                    }
-                    TEAM_B_SYNC();
-                    if (np == 0) break;
-                    // pieces and sequences are dealt in runs of ceil(count / 256) per thread, so every warp shares the work
-                    uint32_t nh_local = 0, headmask = 0;
-                    const uint32_t ppt = (np + P_TEAM - 1) / P_TEAM;
+                if (T.do_parse) {
+                    uint32_t tile_end;
+                    const uint32_t nh = lz_heads<PB_B>(S.stage.in, T, S.be, S.scanws, pd, tile_end, t0, limit, ttid, lane);
+                    if (nh) {
+                        const LzRun R = lz_seq_run(T, S.be, pd, nh, t0, ttid);
+                        uint32_t sz = 0;
 #pragma unroll
-                    for (uint32_t k = 0; k < P_MAXPIECE / P_TEAM; k++) {
-                        const uint32_t r = ttid * ppt + k;
-                        if (k < ppt && r < np) {
-                            const uint32_t pr = S.piece[r];
-                            bool head = !((S.Cont[pr >> 5] >> (pr & 31)) & 1);
-                            if (head) {
-                                uint32_t pend, poff;
-                                if (r == 0) { pend = pd_valid ? pd_end : 0xFFFFFFFFu; poff = pd_off; }
-                                else {
-                                    const uint32_t pb = S.piece[r - 1];
-                                    pend = t0 + pb + S.len[pb];
-                                    if (!((S.Cont[pb >> 5] >> (pb & 31)) & 1)) poff = T.off[pb];
-                                    else {                      // Cont pieces start at a segment boundary (c_walk cuts there)
-                                        const uint32_t sp = S.segprev[pb / C_SEG];
-                                        poff = sp ? T.off[sp - 1] : pd_off;
-                                    }
-                                }
-                                if (pend == t0 + pr && poff == T.off[pr]) head = false;
-                            }
-                            if (head) { headmask |= 1u << k; nh_local++; }
+                        for (uint32_t k = 0; k < LZ_SPT; k++) if (k < R.cnt) sz += c_seq_size(R.lit[k], R.len[k]);
+                        uint32_t total;
+                        uint32_t o = out_pos + team_exscan1<PB_B>(sz, S.scanws, 0, &total, twid, lane);
+#pragma unroll
+                        for (uint32_t k = 0; k < LZ_SPT; k++) {
+                            if (k >= R.cnt) break;
+                            o += c_emit_seq(S.stage.in, S.be, S.nlong, dst, o, R.lit0[k], R.lit[k], R.off[k], R.len[k]);
                         }
-                    }
-                    uint32_t nh;
-                    {
-                        uint32_t hb = team_exscan1<PB_B>(nh_local, S.scanws, 1, &nh, twid, lane);
-#pragma unroll
-                        for (uint32_t k = 0; k < P_MAXPIECE / P_TEAM; k++) if (headmask & (1u << k)) S.hidx[hb++] = (uint16_t)(ttid * ppt + k);
-                    }
-                    TEAM_B_SYNC();
-                    const uint32_t lastp = S.piece[np - 1];
-                    const uint32_t tile_end = t0 + lastp + S.len[lastp];
-                    if (nh == 0) { pd_end = tile_end; break; }
-                    if (pd_valid && S.hidx[0] > 0) { const uint32_t pb = S.piece[S.hidx[0] - 1]; pd_end = t0 + pb + S.len[pb]; }
-                    const uint32_t nemit = pd_valid + nh - 1;
-                    constexpr uint32_t SPT = 1024 / P_TEAM;
-                    const uint32_t spt = (nemit + P_TEAM - 1) / P_TEAM;
-                    uint32_t sz = 0, e_lit0[SPT], e_lit[SPT], e_off[SPT], e_len[SPT], cnt = 0;
-#pragma unroll
-                    for (uint32_t k = 0; k < SPT; k++) {
-                        const uint32_t sidx = ttid * spt + k;
-                        if (k < spt && sidx < nemit) {
-                            uint32_t ls, st, of, en;
-                            if (pd_valid && sidx == 0) { ls = pd_lit; st = pd_start; of = pd_off; en = pd_end; }
-                            else {
-                                const uint32_t h = sidx - pd_valid;
-                                const uint32_t pi = S.hidx[h], pr = S.piece[pi];
-                                const uint32_t pl = S.piece[S.hidx[h + 1] - 1];
-                                st = t0 + pr; of = T.off[pr]; en = t0 + pl + S.len[pl];
-                                if (h == 0) ls = pd_valid ? pd_end : pd_lit;
-                                else { const uint32_t pp = S.piece[pi - 1]; ls = t0 + pp + S.len[pp]; }
-                            }
-                            e_lit0[k] = ls; e_lit[k] = st - ls; e_off[k] = of; e_len[k] = en - st;
-                            sz += c_seq_size(e_lit[k], e_len[k]); cnt++;
-                        }
-                    }
-                    uint32_t total;
-                    uint32_t o = out_pos + team_exscan1<PB_B>(sz, S.scanws, 0, &total, twid, lane);
-#pragma unroll
-                    for (uint32_t k = 0; k < SPT; k++) {
-                        if (k >= cnt) break;
-                        o += c_emit_seq(W, dst, o, e_lit0[k], e_lit[k], e_off[k], e_len[k]);
-                    }
-                    TEAM_B_SYNC();
-                    {
+                        team_sync<PB_B>();
                         const uint32_t nl = S.nlong;
-                        for (uint32_t s = twid; s < nl; s += P_TEAM / 32) c_long_job(W, dst, s, lane, 32u);
+                        for (uint32_t s = twid; s < nl; s += P_TEAM / 32) c_long_job(S.stage.in, S.be, dst, s, lane, 32u);
                         out_pos += total;
-                        const uint32_t pi = S.hidx[nh - 1], pr = S.piece[pi];
-                        uint32_t ls;
-                        if (nh >= 2 || pd_valid) { if (pi > 0) { const uint32_t pp = S.piece[pi - 1]; ls = t0 + pp + S.len[pp]; } else ls = pd_end; }
-                        else ls = pd_lit;
-                        pd_valid = 1; pd_lit = ls; pd_start = t0 + pr; pd_off = T.off[pr]; pd_end = tile_end;
-                        TEAM_B_SYNC();
+                        lz_next_pending(T, S.be, pd, nh, tile_end, t0);
+                        team_sync<PB_B>();
                         if (ttid == 0) S.nlong = 0;
                     }
-                } while (0);
+                }
                 if (ti + 2 < ntiles) { if (b) bar_arrive<PB_EMPTY0 + 1, 2 * P_TEAM>(); else bar_arrive<PB_EMPTY0, 2 * P_TEAM>(); }     // the front end may refill this buffer
             }
             // ---- flush the pending sequence
             uint32_t anchor = 0;
-            if (pd_valid) {
-                PipeView W{S.in, S.tile[0].off, S.len, S.tile[0].M, S.tile[0].V, S.Sel, S.Cont, S.xfree, S.xdin, S.link, S.mpos, S.longl, S.nlong};
-                anchor = pd_end;
-                TEAM_B_SYNC();                                 // S.nlong = 0 of the last tile is visible
-                if (ttid == 0) (void)c_emit_seq(W, dst, out_pos, pd_lit, pd_start - pd_lit, pd_off, pd_end - pd_start);
-                out_pos += c_seq_size(pd_start - pd_lit, pd_end - pd_start);
-                TEAM_B_SYNC();
-                const uint32_t nl = S.nlong;                            // long literal run and / or long match length of the pending sequence
-                for (uint32_t s = 0; s < nl; s++) c_long_job(W, dst, s, ttid, P_TEAM);
+            if (pd.valid) {
+                anchor = pd.end;
+                team_sync<PB_B>();                             // S.nlong = 0 of the last tile is visible
+                if (ttid == 0) (void)c_emit_seq(S.stage.in, S.be, S.nlong, dst, out_pos, pd.lit, pd.start - pd.lit, pd.off, pd.end - pd.start);
+                out_pos += c_seq_size(pd.start - pd.lit, pd.end - pd.start);
+                team_sync<PB_B>();
+                const uint32_t nl = S.nlong;                   // long literal run and / or long match length of the pending sequence
+                for (uint32_t s = 0; s < nl; s++) c_long_job(S.stage.in, S.be, dst, s, ttid, P_TEAM);
             }
             if (ttid == 0) { S.fin_anchor = anchor; S.fin_out = out_pos; }
         }
@@ -419,7 +458,7 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                     if (lit >= 15) op[1 + nf] = (uint8_t)(lit - 15 - nf * 255);
                     blk_csize[blk] = fin;
                 }
-                for (uint32_t i = tid; i < lit; i += NT) op[hl + i] = S.in[anchor + i];
+                for (uint32_t i = tid; i < lit; i += NT) op[hl + i] = S.stage.in[anchor + i];
             }
         }
     }

@@ -32,7 +32,7 @@ struct ZScratch {
     uint32_t fse[3][Z_MAXSEQ];       // (nbBits << 16) | value, per stream LL / OF / ML
 };
 
-// entropy-stage shared memory; aliases the tile arrays of the LZ77 front end (idle between tiles)
+// entropy-stage shared memory; a union with the LZ77 tile arrays (dead between tiles: ZstdSmem)
 struct ZEnt {
     uint32_t hist[256];
     uint8_t  hlen[256];
