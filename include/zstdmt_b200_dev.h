@@ -70,6 +70,13 @@ size_t   zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size);
 uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size);
 int      zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
                                   uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream);
+/* The same at a zstd level.  Levels 1-5 run the level-3 encoder above (same bytes, same workspace).  Levels 6-12 run
+ * the search class with chunk-wide hash chains and a lazy parse, each level with its own parameters; 13-22 use
+ * level 12's.  Its match window is 2 MiB (levels 6-9) or 4 MiB (10 and up), offsets may reach the whole chunk's
+ * history within that window, blocks are 16 KiB.  The workspace depends on the level; out_bound does not. */
+size_t   zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level);
+int      zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                        uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream);
 
 /* Decode.  The host walks frame + block headers (3 bytes per block, plus the two section headers of compressed
  * blocks) with zmt_zstd_scan_frame_host — exactly what the pipeline's reader thread does while it parses frames —
@@ -93,8 +100,11 @@ uint64_t zmt_device_batches(int dev);
  * zmt_prof_begin() arms it; every kernel launched by the entry points above is bracketed by two
  * events; zmt_prof_end() (after the caller synchronised the stream) sums them per kernel id. */
 enum { ZMT_K_LZ4_COMPRESS = 0, ZMT_K_XXH32, ZMT_K_LZ4_SIZES, ZMT_K_SCAN, ZMT_K_LZ4_PACK, ZMT_K_LZ4_DECODE, ZMT_K_XXH32_DEC,
-       ZMT_K_ZSTD_COMPRESS, ZMT_K_ZSTD_PACK, ZMT_K_ZSTD_DECODE, ZMT_K_LZ4_DEXEC, ZMT_K_COUNT };
-/* LZ4 decode: ZMT_K_LZ4_DECODE = pass A (token parse + literals), ZMT_K_LZ4_DEXEC = pass B (match execution) */
+       ZMT_K_ZSTD_COMPRESS, ZMT_K_ZSTD_PACK, ZMT_K_ZSTD_DECODE, ZMT_K_LZ4_DEXEC,
+       ZMT_K_ZL_HASH, ZMT_K_ZL_SORT, ZMT_K_ZL_SEARCH, ZMT_K_ZL_BLOCKS, ZMT_K_COUNT };
+/* LZ4 decode: ZMT_K_LZ4_DECODE = pass A (token parse + literals), ZMT_K_LZ4_DEXEC = pass B (match execution)
+ * zstd levels 6-22: ZMT_K_ZL_HASH = hash, ZMT_K_ZL_SORT = radix sort + prev[], ZMT_K_ZL_SEARCH = chain walk,
+ * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK) */
 void zmt_prof_begin(void);
 int  zmt_prof_end(double* ms, int* count, int max_ids);
 

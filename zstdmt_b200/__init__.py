@@ -63,6 +63,9 @@ def lib():
     L.zmt_zstdc_out_bound.restype = c_u64; L.zmt_zstdc_out_bound.argtypes = [c_u32, c_u32]
     L.zmt_zstd_compress_device.restype = ctypes.c_int
     L.zmt_zstd_compress_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_u32, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstdc_level_workspace_bytes.restype = c_sz; L.zmt_zstdc_level_workspace_bytes.argtypes = [c_u32, c_u32, ctypes.c_int]
+    L.zmt_zstd_compress_level_device.restype = ctypes.c_int
+    L.zmt_zstd_compress_level_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_u32, ctypes.c_int, c_vp, c_vp, c_vp, c_vp]
     L.zmt_zstd_blk_desc_bytes.restype = c_sz; L.zmt_zstd_blk_desc_bytes.argtypes = []
     L.zmt_zstd_scan_frame_host.restype = ctypes.c_int
     L.zmt_zstd_scan_frame_host.argtypes = [c_vp, c_sz, c_u64, c_u32, c_vp, ctypes.POINTER(c_u32), c_u32, ctypes.POINTER(c_u64), ctypes.POINTER(c_u64), ctypes.POINTER(c_u32)]
@@ -209,23 +212,27 @@ class Lz4DeviceCompressor:
 
 
 class ZstdDeviceCompressor:
-    """zmt_zstd_compress_device: same layout contract as the LZ4 twin, Zstandard frames out."""
+    """zmt_zstd_compress_level_device: same layout contract as the LZ4 twin, Zstandard frames out.  Levels 1-5 run the
+    level-3 encoder (zmt_zstd_compress_device), levels 6-22 the hash-chain class with a lazy parse."""
 
-    def __init__(self, in_bytes, chunk, device="cuda"):
+    def __init__(self, in_bytes, chunk, device="cuda", level=3):
         torch = _torch(); L = lib()
-        self.chunk, self.in_bytes = chunk, in_bytes
+        self.chunk, self.in_bytes, self.level = chunk, in_bytes, level
         self.nchunks = L.zmt_chunk_count(in_bytes, chunk)
-        self.work = torch.empty(L.zmt_zstdc_workspace_bytes(self.nchunks, chunk), dtype=torch.uint8, device=device)
+        wb = L.zmt_zstdc_level_workspace_bytes(self.nchunks, chunk, level)
+        if wb == 0:
+            raise ValueError("no workspace size for %d chunks of %d bytes at level %d" % (self.nchunks, chunk, level))
+        self.work = torch.empty(wb, dtype=torch.uint8, device=device)
         self.out = torch.empty(L.zmt_zstdc_out_bound(self.nchunks, chunk), dtype=torch.uint8, device=device)
         self.frame_off = torch.zeros(self.nchunks + 1, dtype=torch.int64, device=device)
 
     def run(self, d_in, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_zstd_compress_device(d_in.data_ptr(), self.in_bytes, self.chunk, None, self.nchunks,
-                                            self.work.data_ptr(), self.out.data_ptr(), self.frame_off.data_ptr(), s.cuda_stream)
+        rc = lib().zmt_zstd_compress_level_device(d_in.data_ptr(), self.in_bytes, self.chunk, None, self.nchunks, self.level,
+                                                  self.work.data_ptr(), self.out.data_ptr(), self.frame_off.data_ptr(), s.cuda_stream)
         if rc != 0:
-            raise RuntimeError("zmt_zstd_compress_device failed: %s" % ST_NAMES.get(rc, rc))
+            raise RuntimeError("zmt_zstd_compress_level_device failed: %s" % ST_NAMES.get(rc, rc))
         return self.out, self.frame_off
 
 

@@ -4,6 +4,7 @@
   zstdmt_b200/libzmt_datagen.so   synthetic input generator (harness/datagen.c)     [bench / test harness, no dependencies]
   zstdmt_b200/libzmt_memio.so     in-memory fn_read / fn_write drivers of the C-ABI [bench / test harness, links the product]
   oracle/liboracle.so             CPU restatement                                  [test infrastructure]
+  oracle/libzlazy_twin.so         CPU twin of the zstd level 6-12 search class     [test infrastructure]
   oracle/_ref/libzstdmt_ref.so    unmodified reference wrapper, only where the reference tree exists (oracle/Makefile REF)
 """
 import os
@@ -17,6 +18,7 @@ LIB = os.path.join(HERE, "libzstdmt_b200.so")
 HSRC = os.path.join(HERE, "harness")
 LIB_GEN = os.path.join(HERE, "libzmt_datagen.so")
 LIB_MEMIO = os.path.join(HERE, "libzmt_memio.so")
+LIB_ZLAZY = os.path.join(ROOT, "oracle", "libzlazy_twin.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -74,11 +76,17 @@ def build_harness(force=False):
             sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building libzmt_memio.so")
 
 
-def build_oracle():
+def build_oracle(force=False):
     r = subprocess.run(["make", "-C", os.path.join(ROOT, "oracle")], capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("oracle build failed")
+    # CPU twin of the zstd level 6-12 search class (shares its rule header with the kernels)
+    src, rule = os.path.join(ROOT, "oracle", "zstd_lazy_twin.c"), os.path.join(CSRC, "zstd_lazy_rule.h")
+    if force or _stale(LIB_ZLAZY, [src, rule]):
+        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_ZLAZY, src], cwd=ROOT, capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/libzlazy_twin.so")
 
 
 def build_cli():
@@ -89,7 +97,7 @@ def build_cli():
 def build_all(force=False, verbose=False):
     build_product(force=force, verbose=verbose)
     build_harness(force=force)
-    build_oracle()
+    build_oracle(force=force)
     build_cli()
 
 

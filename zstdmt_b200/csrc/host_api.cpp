@@ -36,6 +36,8 @@ extern "C" {
 size_t   zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size);
 uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size);
 int      zmt_zstd_compress_device(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, void*, void*, uint64_t*, void*);
+size_t   zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level);
+int      zmt_zstd_compress_level_device(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, int, void*, void*, uint64_t*, void*);
 size_t   zmt_zstd_blk_desc_bytes(void);
 int      zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out, uint32_t* nblocks_io,
                                   uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq);
@@ -192,17 +194,23 @@ struct StageClock {
 inline bool trace_on() { static int on = -1; if (on < 0) on = getenv("ZSTDMT_B200_TRACE") ? 1 : 0; return on == 1; }
 
 // ------------------------------------------------------------------ device codec table
+// the workspace and the compress call follow the context's level (the zstd encoders differ by level; LZ4 has one)
 struct CodecOps {
-    size_t   (*c_work)(uint32_t nchunks, uint32_t chunk);
+    size_t   (*c_work)(uint32_t nchunks, uint32_t chunk, int level);
     uint64_t (*c_bound)(uint32_t nchunks, uint32_t chunk);
-    int      (*compress)(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, void*, void*, uint64_t*, void*);
+    int      (*compress)(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, int level, void*, void*, uint64_t*, void*);
 };
 
+size_t lz4_c_work(uint32_t nchunks, uint32_t chunk, int) { return zmt_lz4c_workspace_bytes(nchunks, chunk); }
+int lz4_compress(const void* in, uint64_t n, uint32_t chunk, const uint32_t* cb, uint32_t nchunks, int, void* work, void* out, uint64_t* foff, void* st)
+{
+    return zmt_lz4_compress_device(in, n, chunk, cb, nchunks, work, out, foff, st);
+}
 
 const CodecOps* codec_ops(int codec)
 {
-    static const CodecOps lz4 = { zmt_lz4c_workspace_bytes, zmt_lz4c_out_bound, zmt_lz4_compress_device };
-    static const CodecOps zstd = { zmt_zstdc_workspace_bytes, zmt_zstdc_out_bound, zmt_zstd_compress_device };
+    static const CodecOps lz4 = { lz4_c_work, zmt_lz4c_out_bound, lz4_compress };
+    static const CodecOps zstd = { zmt_zstdc_level_workspace_bytes, zmt_zstdc_out_bound, zmt_zstd_compress_level_device };
     return codec == CODEC_LZ4 ? &lz4 : &zstd;
 }
 
@@ -430,7 +438,7 @@ size_t compress_run(Ctx* c, GenRdWr* rw)
     if (P.slots.empty()) {
         P.slots.resize(nsl);
         for (size_t i = 0; i < P.slots.size(); i++) {
-            const size_t ic = B * chunk, oc = (size_t)ops->c_bound((uint32_t)B, (uint32_t)chunk), wc = ops->c_work((uint32_t)B, (uint32_t)chunk);
+            const size_t ic = B * chunk, oc = (size_t)ops->c_bound((uint32_t)B, (uint32_t)chunk), wc = ops->c_work((uint32_t)B, (uint32_t)chunk, c->level);
             const bool okk = (i < base_slots || no_alias) ? slot_alloc(P.slots[i], c->devs[i % c->devs.size()], ic, oc, wc, B)
                                                           : slot_alloc_alias(P.slots[i], P.slots[i % base_slots], c->devs[i % c->devs.size()], ic, oc, wc, B);
             if (!okk) { ctx_release_slots(c); return E.mem; }
@@ -543,7 +551,7 @@ size_t compress_run(Ctx* c, GenRdWr* rw)
             if (Th.d[i]) ce = cudaMemcpyAsync(s->d_in + (size_t)i * chunk, s->h_in + (size_t)i * chunk, Th.d[i], cudaMemcpyHostToDevice, s->stream);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(Td.d, Th.d, (size_t)s->n * 4, cudaMemcpyHostToDevice, s->stream);
         int st = ZMT_ST_CUDA;
-        if (ce == cudaSuccess) st = ops->compress(s->d_in, 0, (uint32_t)chunk, Td.d, s->n, s->d_work, s->d_out, Td.a, s->stream);
+        if (ce == cudaSuccess) st = ops->compress(s->d_in, 0, (uint32_t)chunk, Td.d, s->n, c->level, s->d_work, s->d_out, Td.a, s->stream);
         if (s->dev >= 0 && s->dev < 64) g_dev_batches[s->dev]++;
         if (st == ZMT_ST_OK) {
             ce = cudaMemcpyAsync(Th.a, Td.a, ((size_t)s->n + 1) * 8, cudaMemcpyDeviceToHost, s->stream);
@@ -1101,19 +1109,21 @@ Ctx* ctx_new(int codec, bool comp, int threads, int level, size_t inputsize)
 }
 void ctx_delete(Ctx* c) { if (!c) return; const DeviceRestore restore_device; ctx_release_slots(c); delete c; }
 
-// Levels.  The device encoders implement one search class per codec (LZ4: the greedy single-probe parse of level 1-2;
-// zstd: the same parse + Huffman / predefined-FSE entropy stage, "level 3 (predefined FSE tables)" in BASELINE terms).
-// Higher levels are accepted — the CLI default for lz4 is 3 (programs/lz4-mt.c:19) and must keep working — and produce
-// the same stream; that is said once on stderr (ZSTDMT_B200_QUIET=1 silences it) instead of silently, and
-// ZSTDMT_B200_STRICT_LEVEL=1 turns it into the reference's own answer for a bad parameter (create returns NULL,
-// lib/lz4-mt_compress.c:103-108).
+// Levels.  LZ4 has one search class on the device: the greedy single-probe parse of levels 1-2.  zstd has two: levels 1-5
+// run the level-3 class (the LZ4 parse + Huffman / predefined-FSE entropy stage, "level 3 (predefined FSE tables)" in
+// BASELINE terms), levels 6-12 the chunk-wide hash-chain class with a lazy parse and per-level parameters, and levels
+// 13-22 that class with level 12's parameters.  A level above what its class implements is accepted — the CLI default
+// for lz4 is 3 (programs/lz4-mt.c:19) and must keep working — and produces that class's stream; that is said once per
+// codec and class on stderr (ZSTDMT_B200_QUIET=1 silences it) instead of silently, and ZSTDMT_B200_STRICT_LEVEL=1 turns
+// it into the reference's own answer for a bad parameter (create returns NULL, lib/lz4-mt_compress.c:103-108).
 bool level_ok(int codec, int level)
 {
-    const int implemented = codec == CODEC_LZ4 ? 2 : 3;
+    int implemented = 2, cls = 0;
+    if (codec != CODEC_LZ4) { implemented = level >= 6 ? 12 : 3; cls = level >= 6 ? 2 : 1; }
     if (level <= implemented) return true;
     if (getenv("ZSTDMT_B200_STRICT_LEVEL")) return false;
     static std::atomic<int> told[3];
-    if (!getenv("ZSTDMT_B200_QUIET") && told[codec].exchange(1) == 0)
+    if (!getenv("ZSTDMT_B200_QUIET") && told[cls].exchange(1) == 0)
         fprintf(stderr, "[zstdmt_b200] %s level %d requested: the device encoder implements the level-%d search class, the stream is valid but its ratio is that class's\n",
                 codec == CODEC_LZ4 ? "lz4" : "zstd", level, implemented);
     return true;

@@ -13,6 +13,8 @@
 //                               parse, scan-based emission, as two teams pipelined over 4 KiB tiles.
 //   zstd_blocks_kernel          one CTA per 64 KiB zstd match window: the same parse functions run by a single team,
 //                               sequences and literals to a scratch, entropy stage (zstd_entropy.cuh) every 4 tiles.
+//   zstd_lazy.cuh               the search class of zstd levels 6-12: chunk-wide hash chains (hash, radix sort, chain
+//                               walk) and a lazy parse per 16 KiB block, into the same entropy stage.
 //   xxh32_kernel                4 lanes per chunk (the 4 XXH32 accumulators), 8 chunks per warp.
 //   lz4_frame_sizes_kernel / lz4_frame_pack_kernel
 //                               frame size per chunk -> exclusive scan -> compaction of the block
@@ -28,6 +30,7 @@
 #include <string.h>
 #include <mutex>
 #include <vector>
+#include <cub/device/device_radix_sort.cuh>
 #include "common.cuh"
 #include "zmt_dev.h"
 #include "zstd_entropy.cuh"
@@ -344,6 +347,8 @@ zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
         if (tid == 0) blk_csize[blk] = out_pos;
     }
 }
+
+#include "zstd_lazy.cuh"
 
 // ============================================================================ XXH32 (content checksum)
 // One warp per buffer.  XXH32 is four serial accumulator chains (one per 32-bit word of every 16-byte
@@ -826,6 +831,97 @@ extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uin
 }
 
 static inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
+
+// ---------------------------------------------------------------- zstd compress, levels 6-22 (zstd_lazy.cuh)
+// chunks per group: the per-position arrays (keys, values, prev, best: 16 bytes per position) cover one group at a time
+static inline uint32_t zl_group_chunks(uint32_t nchunks, uint32_t chunk_size)
+{
+    uint32_t g = ZL_GROUP_BYTES / chunk_size;
+    if (g == 0) g = 1;
+    return g < nchunks ? g : nchunks;
+}
+static size_t zl_sort_temp_bytes(uint32_t npos)
+{
+    size_t t = 0;
+    cub::DoubleBuffer<uint32_t> k(nullptr, nullptr), v(nullptr, nullptr);
+    if (cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)npos, 0, ZL_HASHLOG) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return t;
+}
+
+extern "C" size_t zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+{
+    const size_t base = zmt_zstdc_workspace_bytes(nchunks, chunk_size);
+    if (level < ZL_MIN_LEVEL || base == 0 || nchunks == 0) return base;
+    const uint64_t npos = (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size;
+    if (npos > 0xFFFFFFFFull) return 0;
+    return base + 4 * a256(npos * 4) + a256(zl_sort_temp_bytes((uint32_t)npos));
+}
+
+extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    if (level < ZL_MIN_LEVEL) return zmt_zstd_compress_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, d_work, d_out, d_frame_off, stream_);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
+    if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
+    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
+    if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
+    const uint32_t G = zl_group_chunks(nchunks, chunk_size);
+    const uint64_t npos_max = (uint64_t)G * chunk_size;
+    if (npos_max > 0xFFFFFFFFull) return ZMT_ST_BAD_ARG;
+    const int ti = zstd_tables_init(); if (ti != ZMT_ST_OK) return ti;
+    const uint32_t nblocks = nchunks * bpc;
+    uint8_t* w = (uint8_t*)d_work;
+    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
+    uint32_t* blk_csize = (uint32_t*)w; w += a256((uint64_t)nblocks * 4);
+    uint64_t* frame_size = (uint64_t*)w; w += a256(((uint64_t)nchunks + 1) * 8);
+    ZScratch* zsc = (ZScratch*)w;
+    w = (uint8_t*)d_work + zmt_zstdc_workspace_bytes(nchunks, chunk_size);        // the level-3 layout ends here
+    uint32_t* arr[4];
+    for (int k = 0; k < 4; k++) { arr[k] = (uint32_t*)w; w += a256(npos_max * 4); }
+    void* sort_tmp = w;
+    const size_t sort_cap = zl_sort_temp_bytes((uint32_t)npos_max);
+    const ZlParams P = zl_params(level);
+    const uint32_t W = zl_window(level);
+    cudaFuncSetAttribute(zstd_lazy_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZlSmem));
+
+    for (uint32_t c0 = 0; c0 < nchunks; c0 += G) {
+        const uint32_t ng = nchunks - c0 < G ? nchunks - c0 : G;
+        uint64_t npos = (uint64_t)ng * chunk_size;
+        if (!d_chunk_bytes) { const uint64_t b = (uint64_t)c0 * chunk_size; npos = in_bytes > b ? (in_bytes - b < npos ? in_bytes - b : npos) : 0; }
+        cub::DoubleBuffer<uint32_t> K(arr[0], arr[1]), V(arr[2], arr[3]);
+        if (npos) {
+            const uint32_t np = (uint32_t)npos, g = (np + 255) / 256;
+            { ZmtProfScope ps(ZMT_K_ZL_HASH, stream);
+            zstd_lazy_hash_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, K.Current(), V.Current()); }
+            zmt_dbg_check(stream, "zstd_lazy_hash_kernel");
+            {
+                ZmtProfScope ps(ZMT_K_ZL_SORT, stream);
+                size_t tb = 0;
+                if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess || tb > sort_cap) return ZMT_ST_CUDA;
+                if (cub::DeviceRadixSort::SortPairs(sort_tmp, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
+                zstd_lazy_prev_kernel<<<g, 256, 0, stream>>>(K.Current(), V.Current(), np, V.Alternate());
+            }
+            zmt_dbg_check(stream, "zstd_lazy sort + prev");
+            { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
+            zstd_lazy_search_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, P.depth, W, V.Alternate(), K.Alternate()); }
+            zmt_dbg_check(stream, "zstd_lazy_search_kernel");
+        }
+        const uint32_t nwin = ng * bpc;
+        { ZmtProfScope ps(ZMT_K_ZL_BLOCKS, stream);
+        zstd_lazy_blocks_kernel<<<zstd_grid(nwin), 256, sizeof(ZlSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, c0, nwin, P.lazy,
+                                                                                   K.Alternate(), tmp, blk_csize, zsc); }
+        zmt_dbg_check(stream, "zstd_lazy_blocks_kernel");
+    }
+    zstd_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size);
+    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks);
+    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
+    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
+    { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
+    zstd_frame_pack_kernel<<<gridp, 256, 0, stream>>>(in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, d_frame_off, (uint8_t*)d_out, nblocks); }
+    zmt_dbg_check(stream, "zstd_frame_pack_kernel");
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
 
 // workspace: stored[] | computed[] | needs_seq[] | ticket | slot counts | first_slot | block table | progress | match records
 extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, uint64_t in_bytes)

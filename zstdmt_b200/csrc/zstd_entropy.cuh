@@ -23,7 +23,11 @@
 #define Z_HUF_MAXBITS 11
 #define Z_WARM        16u             // warm-up symbols of a speculative FSE chain chunk
 
+// litlen: literal length in bits 0-23, offset bits 16-23 in bits 24-31 (the level 6-12 class reaches 4 MiB back);
+// off: offset bits 0-15.  Eight bytes, as the level-3 encoder writes them (its offsets stay below 2^16).
 struct __align__(8) ZSeq { uint32_t litlen; uint16_t off; uint16_t mlen; };
+__device__ __forceinline__ uint32_t zseq_ll(const ZSeq& q) { return q.litlen & 0xFFFFFFu; }
+__device__ __forceinline__ uint32_t zseq_off(const ZSeq& q) { return (uint32_t)q.off | ((q.litlen >> 24) << 16); }
 
 // per-CTA scratch in global memory (L2 resident): sequence records, literal bytes, FSE (nbBits,value) pairs
 struct ZScratch {
@@ -261,7 +265,7 @@ __device__ uint32_t z_encode_block(ZEnt& Z, const ZFseShared& F, ZScratch* zs, u
                 __syncwarp();
                 for (uint32_t idx = lane; idx < nseq; idx += 32) {
                     const ZSeq q = zs->seq[idx];
-                    const uint32_t code = kk == 0 ? z_ll_code(q.litlen) : kk == 1 ? z_highbit((uint32_t)q.off + 3u) : z_ml_code((uint32_t)q.mlen - 3u);
+                    const uint32_t code = kk == 0 ? z_ll_code(zseq_ll(q)) : kk == 1 ? z_highbit(zseq_off(q) + 3u) : z_ml_code((uint32_t)q.mlen - 3u);
                     Z.codes[nseq - 1 - idx] = (uint8_t)code;
                 }
                 __syncwarp();
@@ -476,7 +480,7 @@ __device__ uint32_t z_encode_block(ZEnt& Z, const ZFseShared& F, ZScratch* zs, u
         for (uint32_t j = my_first; j < my_end; j++) {
             const uint32_t i = nseq - 1 - j;
             const ZSeq q = zs->seq[i];
-            const uint32_t llc = z_ll_code(q.litlen), mlc = z_ml_code((uint32_t)q.mlen - 3u), ofc = z_highbit((uint32_t)q.off + 3u);
+            const uint32_t llc = z_ll_code(zseq_ll(q)), mlc = z_ml_code((uint32_t)q.mlen - 3u), ofc = z_highbit(zseq_off(q) + 3u);
             b += c_ll_bits[llc] + c_ml_bits[mlc] + ofc;
             b += (zs->fse[0][i] >> 16) + (zs->fse[1][i] >> 16) + (zs->fse[2][i] >> 16);
         }
@@ -509,11 +513,11 @@ __device__ uint32_t z_encode_block(ZEnt& Z, const ZFseShared& F, ZScratch* zs, u
         for (uint32_t j = my_first; j < my_first + my_cnt; j++) {
             const uint32_t i = nseq - 1 - j;
             const ZSeq q = zs->seq[i];
-            const uint32_t llc = z_ll_code(q.litlen), mlc = z_ml_code((uint32_t)q.mlen - 3u), ofv = (uint32_t)q.off + 3u, ofc = z_highbit(ofv);
+            const uint32_t ll = zseq_ll(q), llc = z_ll_code(ll), mlc = z_ml_code((uint32_t)q.mlen - 3u), ofv = zseq_off(q) + 3u, ofc = z_highbit(ofv);
             const uint32_t fl = zs->fse[0][i], fo = zs->fse[1][i], fm = zs->fse[2][i];
             // per sequence (zstd_compress_sequences.c order): FSE OF, ML, LL state bits, then extra bits LL, ML, OF
             R.add(fo & 0xFFFF, fo >> 16); R.add(fm & 0xFFFF, fm >> 16); R.add(fl & 0xFFFF, fl >> 16);
-            R.add(q.litlen - c_ll_base[llc], c_ll_bits[llc]);
+            R.add(ll - c_ll_base[llc], c_ll_bits[llc]);
             R.add((uint32_t)q.mlen - c_ml_base[mlc], c_ml_bits[mlc]);
             R.add(ofv - (1u << ofc), ofc);
         }
