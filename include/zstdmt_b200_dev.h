@@ -8,6 +8,7 @@
  * What each call replaces in the reference (one call = the codec step of every worker
  * iteration of a whole batch of chunks):
  *   zmt_lz4_compress_device    LZ4F_compressFrame + 12-byte header, lib/lz4-mt_compress.c:280-298
+ *                              (zmt_lz4_compress_level_device: the same at a level)
  *   zmt_lz4_decompress_device  LZ4F_decompress, lib/lz4-mt_decompress.c:328-362
  *   zmt_zstd_compress_device   ZSTD_compress + 12-byte header, lib/zstd-mt_compress.c:284-302
  *   zmt_zstd_decompress_device ZSTD_decompressStream loop, lib/zstd-mt_decompress.c:442-527
@@ -52,6 +53,14 @@ size_t   zmt_lz4c_workspace_bytes(uint32_t nchunks, uint32_t chunk_size);
 uint64_t zmt_lz4c_out_bound(uint32_t nchunks, uint32_t chunk_size);
 int      zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
                                  uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream);
+/* The same at an LZ4 level.  Levels 1-9 run the encoder above (same bytes, same workspace: independent blocks, FLG 0x6C).
+ * Levels 10-12 run the high-compression class: hash chains over the whole chunk walked to a per-level depth, a lazy
+ * parse, and linked 64 KiB blocks (FLG 0x4C, 0x44 for an empty chunk) whose matches may reach up to 65535 bytes back
+ * into the chunk's earlier blocks.  Any other level returns ZMT_ST_BAD_ARG (the workspace size is then 0).  The
+ * workspace depends on the level; out_bound does not. */
+size_t   zmt_lz4c_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level);
+int      zmt_lz4_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                       uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream);
 
 /* d_in/in_bytes = the framed stream in HBM; d_frame_off[f] = offset of frame f's 12-byte header, d_frame_csize[f] =
  * its payload size; d_out_off[f..f+1] = where frame f's content goes and how much room it has;
@@ -101,10 +110,12 @@ uint64_t zmt_device_batches(int dev);
  * events; zmt_prof_end() (after the caller synchronised the stream) sums them per kernel id. */
 enum { ZMT_K_LZ4_COMPRESS = 0, ZMT_K_XXH32, ZMT_K_LZ4_SIZES, ZMT_K_SCAN, ZMT_K_LZ4_PACK, ZMT_K_LZ4_DECODE, ZMT_K_XXH32_DEC,
        ZMT_K_ZSTD_COMPRESS, ZMT_K_ZSTD_PACK, ZMT_K_ZSTD_DECODE, ZMT_K_LZ4_DEXEC,
-       ZMT_K_ZL_HASH, ZMT_K_ZL_SORT, ZMT_K_ZL_SEARCH, ZMT_K_ZL_BLOCKS, ZMT_K_COUNT };
+       ZMT_K_ZL_HASH, ZMT_K_ZL_SORT, ZMT_K_ZL_SEARCH, ZMT_K_ZL_BLOCKS, ZMT_K_L4H_BLOCKS, ZMT_K_COUNT };
 /* LZ4 decode: ZMT_K_LZ4_DECODE = pass A (token parse + literals), ZMT_K_LZ4_DEXEC = pass B (match execution)
  * zstd levels 6-22: ZMT_K_ZL_HASH = hash, ZMT_K_ZL_SORT = radix sort + prev[], ZMT_K_ZL_SEARCH = chain walk,
- * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK) */
+ * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK)
+ * LZ4 levels 10-12: hash, sort and search as zstd's (ZMT_K_ZL_HASH / SORT / SEARCH), ZMT_K_L4H_BLOCKS = lazy parse +
+ * LZ4 sequences; checksum, sizes, scan and pack as level 1's */
 void zmt_prof_begin(void);
 int  zmt_prof_end(double* ms, int* count, int max_ids);
 

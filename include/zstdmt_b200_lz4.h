@@ -78,8 +78,9 @@ typedef struct {
 
 /* compression — lib/lz4-mt_compress.c:92 (create), :312 (compress), :356-380 (stats), :382 (free).
  * `threads` (1..128) bounds the batches kept in flight per GPU; `level` 1..12 is
- * accepted, the device encoder implements the level-1 class; `inputsize` is the
- * chunk size (0 -> 4 MiB). */
+ * accepted: levels 1-9 run the level-1 class (independent blocks; 3-9 with a notice),
+ * 10-12 the high-compression class (chunk-wide hash chains, lazy parse, linked
+ * blocks); `inputsize` is the chunk size (0 -> 4 MiB). */
 typedef struct LZ4MT_CCtx_s LZ4MT_CCtx;
 LZ4MT_CCtx* LZ4MT_createCCtx(int threads, int level, int inputsize);
 size_t LZ4MT_compressCCtx(LZ4MT_CCtx* ctx, LZ4MT_RdWr_t* rdwr);

@@ -59,6 +59,9 @@ def lib():
     L.zmt_lz4c_out_bound.restype = c_u64; L.zmt_lz4c_out_bound.argtypes = [c_u32, c_u32]
     L.zmt_lz4_compress_device.restype = ctypes.c_int
     L.zmt_lz4_compress_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_u32, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_lz4c_level_workspace_bytes.restype = c_sz; L.zmt_lz4c_level_workspace_bytes.argtypes = [c_u32, c_u32, ctypes.c_int]
+    L.zmt_lz4_compress_level_device.restype = ctypes.c_int
+    L.zmt_lz4_compress_level_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_u32, ctypes.c_int, c_vp, c_vp, c_vp, c_vp]
     L.zmt_zstdc_workspace_bytes.restype = c_sz; L.zmt_zstdc_workspace_bytes.argtypes = [c_u32, c_u32]
     L.zmt_zstdc_out_bound.restype = c_u64; L.zmt_zstdc_out_bound.argtypes = [c_u32, c_u32]
     L.zmt_zstd_compress_device.restype = ctypes.c_int
@@ -191,23 +194,27 @@ def scan_frames(framed):
 
 
 class Lz4DeviceCompressor:
-    """Pre-allocated device buffers + one call per batch: zmt_lz4_compress_device."""
+    """Pre-allocated device buffers + one call per batch: zmt_lz4_compress_level_device.  Levels 1-9 run the level-1
+    encoder (zmt_lz4_compress_device, independent blocks), levels 10-12 the high-compression class with linked blocks."""
 
-    def __init__(self, in_bytes, chunk, device="cuda"):
+    def __init__(self, in_bytes, chunk, device="cuda", level=1):
         torch = _torch(); L = lib()
-        self.chunk, self.in_bytes = chunk, in_bytes
+        self.chunk, self.in_bytes, self.level = chunk, in_bytes, level
         self.nchunks = L.zmt_chunk_count(in_bytes, chunk)
-        self.work = torch.empty(L.zmt_lz4c_workspace_bytes(self.nchunks, chunk), dtype=torch.uint8, device=device)
+        wb = L.zmt_lz4c_level_workspace_bytes(self.nchunks, chunk, level)
+        if wb == 0:
+            raise ValueError("no workspace size for %d chunks of %d bytes at level %d" % (self.nchunks, chunk, level))
+        self.work = torch.empty(wb, dtype=torch.uint8, device=device)
         self.out = torch.empty(L.zmt_lz4c_out_bound(self.nchunks, chunk), dtype=torch.uint8, device=device)
         self.frame_off = torch.zeros(self.nchunks + 1, dtype=torch.int64, device=device)
 
     def run(self, d_in, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_lz4_compress_device(d_in.data_ptr(), self.in_bytes, self.chunk, None, self.nchunks,
-                                           self.work.data_ptr(), self.out.data_ptr(), self.frame_off.data_ptr(), s.cuda_stream)
+        rc = lib().zmt_lz4_compress_level_device(d_in.data_ptr(), self.in_bytes, self.chunk, None, self.nchunks, self.level,
+                                                 self.work.data_ptr(), self.out.data_ptr(), self.frame_off.data_ptr(), s.cuda_stream)
         if rc != 0:
-            raise RuntimeError("zmt_lz4_compress_device failed: %s" % ST_NAMES.get(rc, rc))
+            raise RuntimeError("zmt_lz4_compress_level_device failed: %s" % ST_NAMES.get(rc, rc))
         return self.out, self.frame_off
 
 

@@ -5,6 +5,7 @@
   zstdmt_b200/libzmt_memio.so     in-memory fn_read / fn_write drivers of the C-ABI [bench / test harness, links the product]
   oracle/liboracle.so             CPU restatement                                  [test infrastructure]
   oracle/libzlazy_twin.so         CPU twin of the zstd level 6-12 search class     [test infrastructure]
+  oracle/liblz4hc_twin.so         CPU twin of the LZ4 level 10-12 class            [test infrastructure]
   oracle/_ref/libzstdmt_ref.so    unmodified reference wrapper, only where the reference tree exists (oracle/Makefile REF)
 """
 import os
@@ -19,6 +20,7 @@ HSRC = os.path.join(HERE, "harness")
 LIB_GEN = os.path.join(HERE, "libzmt_datagen.so")
 LIB_MEMIO = os.path.join(HERE, "libzmt_memio.so")
 LIB_ZLAZY = os.path.join(ROOT, "oracle", "libzlazy_twin.so")
+LIB_L4HC = os.path.join(ROOT, "oracle", "liblz4hc_twin.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -87,6 +89,12 @@ def build_oracle(force=False):
         r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_ZLAZY, src], cwd=ROOT, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/libzlazy_twin.so")
+    # CPU twin of the LZ4 level 10-12 class (its rule header includes the zstd one)
+    src, rules = os.path.join(ROOT, "oracle", "lz4_hc_twin.c"), [os.path.join(CSRC, f) for f in ("lz4_hc_rule.h", "zstd_lazy_rule.h")]
+    if force or _stale(LIB_L4HC, [src] + rules):
+        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_L4HC, src], cwd=ROOT, capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/liblz4hc_twin.so")
 
 
 def build_cli():

@@ -194,22 +194,16 @@ struct StageClock {
 inline bool trace_on() { static int on = -1; if (on < 0) on = getenv("ZSTDMT_B200_TRACE") ? 1 : 0; return on == 1; }
 
 // ------------------------------------------------------------------ device codec table
-// the workspace and the compress call follow the context's level (the zstd encoders differ by level; LZ4 has one)
+// the workspace and the compress call follow the context's level (both codecs have more than one encoder)
 struct CodecOps {
     size_t   (*c_work)(uint32_t nchunks, uint32_t chunk, int level);
     uint64_t (*c_bound)(uint32_t nchunks, uint32_t chunk);
     int      (*compress)(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, int level, void*, void*, uint64_t*, void*);
 };
 
-size_t lz4_c_work(uint32_t nchunks, uint32_t chunk, int) { return zmt_lz4c_workspace_bytes(nchunks, chunk); }
-int lz4_compress(const void* in, uint64_t n, uint32_t chunk, const uint32_t* cb, uint32_t nchunks, int, void* work, void* out, uint64_t* foff, void* st)
-{
-    return zmt_lz4_compress_device(in, n, chunk, cb, nchunks, work, out, foff, st);
-}
-
 const CodecOps* codec_ops(int codec)
 {
-    static const CodecOps lz4 = { lz4_c_work, zmt_lz4c_out_bound, lz4_compress };
+    static const CodecOps lz4 = { zmt_lz4c_level_workspace_bytes, zmt_lz4c_out_bound, zmt_lz4_compress_level_device };
     static const CodecOps zstd = { zmt_zstdc_level_workspace_bytes, zmt_zstdc_out_bound, zmt_zstd_compress_level_device };
     return codec == CODEC_LZ4 ? &lz4 : &zstd;
 }
@@ -1109,7 +1103,8 @@ Ctx* ctx_new(int codec, bool comp, int threads, int level, size_t inputsize)
 }
 void ctx_delete(Ctx* c) { if (!c) return; const DeviceRestore restore_device; ctx_release_slots(c); delete c; }
 
-// Levels.  LZ4 has one search class on the device: the greedy single-probe parse of levels 1-2.  zstd has two: levels 1-5
+// Levels.  LZ4 has two search classes on the device: the greedy single-probe parse of levels 1-2 (levels 3-9 run it
+// too) and the high-compression class of levels 10-12 (chunk-wide hash chains, a lazy parse, linked blocks).  zstd has two: levels 1-5
 // run the level-3 class (the LZ4 parse + Huffman / predefined-FSE entropy stage, "level 3 (predefined FSE tables)" in
 // BASELINE terms), levels 6-12 the chunk-wide hash-chain class with a lazy parse and per-level parameters, and levels
 // 13-22 that class with level 12's parameters.  A level above what its class implements is accepted — the CLI default
@@ -1118,7 +1113,7 @@ void ctx_delete(Ctx* c) { if (!c) return; const DeviceRestore restore_device; ct
 // it into the reference's own answer for a bad parameter (create returns NULL, lib/lz4-mt_compress.c:103-108).
 bool level_ok(int codec, int level)
 {
-    int implemented = 2, cls = 0;
+    int implemented = level >= 10 ? 12 : 2, cls = 0;
     if (codec != CODEC_LZ4) { implemented = level >= 6 ? 12 : 3; cls = level >= 6 ? 2 : 1; }
     if (level <= implemented) return true;
     if (getenv("ZSTDMT_B200_STRICT_LEVEL")) return false;

@@ -184,8 +184,10 @@ __device__ __forceinline__ uint32_t c_seq_size(uint32_t lit, uint32_t L)
 
 // writes one LZ4 sequence at dst + o (token, lengths, offset) and returns its size.  No serial 255-runs: the 255 bytes of a
 // literal length exist only when lit >= 270 > C_LONGLIT, and the warp that copies that literal run writes them
-// (c_long_job); literal runs longer than C_LONGLIT and long match-length runs are queued as jobs in K.longl.
-__device__ __forceinline__ uint32_t c_emit_seq(const uint8_t* in, LzBack& K, uint32_t& nlong, uint8_t* dst, uint32_t o,
+// (c_long_job); literal runs longer than C_LONGLIT and long match-length runs are queued as jobs in K.longl (K: LzBack,
+// or the high-compression class's own job list).
+template <class KL>
+__device__ __forceinline__ uint32_t c_emit_seq(const uint8_t* in, KL& K, uint32_t& nlong, uint8_t* dst, uint32_t o,
                                                uint32_t lit_start, uint32_t lit, uint32_t off, uint32_t mlen)
 {
     static_assert(C_LONGLIT < 15 + 255, "literal-length 255 runs must imply the cooperative path");
@@ -208,7 +210,8 @@ __device__ __forceinline__ uint32_t c_emit_seq(const uint8_t* in, LzBack& K, uin
 
 // one job of the long list, done by `nthr` threads (thread index t): a literal run with the 255 bytes of its length
 // field, or a run of 255 bytes of a match length
-__device__ __forceinline__ void c_long_job(const uint8_t* in, const LzBack& K, uint8_t* dst, uint32_t s, uint32_t t, uint32_t nthr)
+template <class KL>
+__device__ __forceinline__ void c_long_job(const uint8_t* in, const KL& K, uint8_t* dst, uint32_t s, uint32_t t, uint32_t nthr)
 {
     const uint32_t a = K.longl[2 * s], dp = K.longl[2 * s + 1];
     if (dp & 0x80000000u) { uint8_t* q = dst + (dp & 0x7FFFFFFFu); for (uint32_t i = t; i < a; i += nthr) q[i] = 255; return; }
@@ -349,6 +352,7 @@ zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
 }
 
 #include "zstd_lazy.cuh"
+#include "lz4_hc.cuh"
 
 // ============================================================================ XXH32 (content checksum)
 // One warp per buffer.  XXH32 is four serial accumulator chains (one per 32-bit word of every 16-byte
@@ -463,12 +467,13 @@ __global__ void __launch_bounds__(1024) scan_u64_kernel(const uint64_t* __restri
 }
 
 // One CTA per (chunk, block): copies the block payload to its final place; block 0 also writes
-// the headers, the last block the end mark + checksum.
+// the headers, the last block the end mark + checksum.  indep: the FLG block-independence bit, 0x20 for the level-1
+// class's independent blocks, 0 for the linked blocks of levels 10-12.
 __global__ void __launch_bounds__(256)
 lz4_frame_pack_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes, uint32_t bpc,
                       const uint8_t* __restrict__ tmp, const uint32_t* __restrict__ blk_csize,
                       const uint32_t* __restrict__ chk, const uint64_t* __restrict__ frame_off,
-                      uint8_t* __restrict__ out, uint32_t nblocks)
+                      uint8_t* __restrict__ out, uint32_t nblocks, uint32_t indep)
 {
     for (uint32_t blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
         const uint32_t c = blk / bpc, b = blk % bpc;
@@ -487,7 +492,7 @@ lz4_frame_pack_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_
                 uint8_t h[10];
                 stg_le32(f, 0x184D2A50u); stg_le32(f + 4, 4); stg_le32(f + 8, (uint32_t)(fsz - 12));
                 stg_le32(f + 12, 0x184D2204u);
-                h[0] = cbytes ? 0x6C : 0x64; h[1] = 0x40;
+                h[0] = (uint8_t)((cbytes ? 0x4C : 0x44) | indep); h[1] = 0x40;
                 for (int i = 0; i < 8; i++) h[2 + i] = (uint8_t)(cbytes >> (8 * i));
                 const uint32_t hl = cbytes ? 10 : 2;
                 for (uint32_t i = 0; i < hl; i++) f[16 + i] = h[i];
@@ -771,7 +776,7 @@ extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint
     const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
     const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
     { ZmtProfScope ps(ZMT_K_LZ4_PACK, stream);
-    lz4_frame_pack_kernel<<<gridp, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, chk, d_frame_off, (uint8_t*)d_out, nblocks); }
+    lz4_frame_pack_kernel<<<gridp, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, chk, d_frame_off, (uint8_t*)d_out, nblocks, 0x20u); }
     zmt_dbg_check(stream, "lz4_frame_pack_kernel");
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
@@ -904,7 +909,7 @@ extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_byte
             }
             zmt_dbg_check(stream, "zstd_lazy sort + prev");
             { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
-            zstd_lazy_search_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, P.depth, W, V.Alternate(), K.Alternate()); }
+            zstd_lazy_search_kernel<ZL_BLOCK, 0, 0><<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, P.depth, W, V.Alternate(), K.Alternate()); }
             zmt_dbg_check(stream, "zstd_lazy_search_kernel");
         }
         const uint32_t nwin = ng * bpc;
@@ -920,6 +925,96 @@ extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_byte
     { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
     zstd_frame_pack_kernel<<<gridp, 256, 0, stream>>>(in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, d_frame_off, (uint8_t*)d_out, nblocks); }
     zmt_dbg_check(stream, "zstd_frame_pack_kernel");
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+// ---------------------------------------------------------------- LZ4 compress, levels 1-12 (levels 10-12: lz4_hc.cuh)
+// The level-1 layout, then the four per-position arrays (keys, values, prev, best) of one group and the sort's temp.
+extern "C" size_t zmt_lz4c_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+{
+    if (level < 1 || level > L4H_MAX_LEVEL) return 0;
+    const size_t base = zmt_lz4c_workspace_bytes(nchunks, chunk_size);
+    if (level < L4H_MIN_LEVEL || base == 0 || nchunks == 0) return base;
+    const uint64_t npos = (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size;
+    if (npos > 0xFFFFFFFFull) return 0;
+    return base + 4 * a256(npos * 4) + a256(zl_sort_temp_bytes((uint32_t)npos));
+}
+
+extern "C" int zmt_lz4_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                             uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    if (level < 1 || level > L4H_MAX_LEVEL) return ZMT_ST_BAD_ARG;
+    if (level < L4H_MIN_LEVEL) return zmt_lz4_compress_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, d_work, d_out, d_frame_off, stream_);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
+    if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
+    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
+    if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
+    const uint32_t G = zl_group_chunks(nchunks, chunk_size);
+    const uint64_t npos_max = (uint64_t)G * chunk_size;
+    if (npos_max > 0xFFFFFFFFull) return ZMT_ST_BAD_ARG;
+    const uint32_t nblocks = nchunks * bpc;
+    uint8_t* w = (uint8_t*)d_work;
+    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
+    uint32_t* blk_csize = (uint32_t*)w; w += a256((uint64_t)nblocks * 4);
+    uint32_t* chk = (uint32_t*)w; w += a256((uint64_t)nchunks * 4);
+    uint64_t* frame_size = (uint64_t*)w;
+    w = (uint8_t*)d_work + zmt_lz4c_workspace_bytes(nchunks, chunk_size);         // the level-1 layout ends here
+    uint32_t* arr[4];
+    for (int k = 0; k < 4; k++) { arr[k] = (uint32_t*)w; w += a256(npos_max * 4); }
+    void* sort_tmp = w;
+    const size_t sort_cap = zl_sort_temp_bytes((uint32_t)npos_max);
+    const L4hParams P = l4h_params(level);
+    cudaFuncSetAttribute(lz4_hc_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4hSmem));
+
+    // the content checksum only reads the input: on the side stream it runs beside the search
+    const ZmtSide side = zmt_side_stream();
+    cudaStream_t xs = side.ok ? side.stream : stream;
+    if (side.ok) { cudaEventRecord(side.fork, stream); cudaStreamWaitEvent(side.stream, side.fork, 0); }
+    { ZmtProfScope ps(ZMT_K_XXH32, xs);
+    xxh32_kernel<<<(nchunks + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, xs>>>((const uint8_t*)d_in, nullptr, nullptr, d_chunk_bytes, chunk_size, in_bytes, chk, nchunks); }
+    if (side.ok) cudaEventRecord(side.join, side.stream);
+    zmt_dbg_check(xs, "xxh32_kernel");
+
+    for (uint32_t c0 = 0; c0 < nchunks; c0 += G) {
+        const uint32_t ng = nchunks - c0 < G ? nchunks - c0 : G;
+        uint64_t npos = (uint64_t)ng * chunk_size;
+        if (!d_chunk_bytes) { const uint64_t b = (uint64_t)c0 * chunk_size; npos = in_bytes > b ? (in_bytes - b < npos ? in_bytes - b : npos) : 0; }
+        cub::DoubleBuffer<uint32_t> K(arr[0], arr[1]), V(arr[2], arr[3]);
+        if (npos) {
+            const uint32_t np = (uint32_t)npos, g = (np + 255) / 256;
+            { ZmtProfScope ps(ZMT_K_ZL_HASH, stream);
+            zstd_lazy_hash_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, L4H_MINMATCH, K.Current(), V.Current()); }
+            zmt_dbg_check(stream, "zstd_lazy_hash_kernel");
+            {
+                ZmtProfScope ps(ZMT_K_ZL_SORT, stream);
+                size_t tb = 0;
+                if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess || tb > sort_cap) return ZMT_ST_CUDA;
+                if (cub::DeviceRadixSort::SortPairs(sort_tmp, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
+                zstd_lazy_prev_kernel<<<g, 256, 0, stream>>>(K.Current(), V.Current(), np, V.Alternate());
+            }
+            zmt_dbg_check(stream, "zstd_lazy sort + prev");
+            { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
+            zstd_lazy_search_kernel<L4H_BLOCK, L4H_MFLIMIT, L4H_LASTLIT><<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np,
+                                                                                              L4H_MINMATCH, P.depth, L4H_WINDOW, V.Alternate(), K.Alternate()); }
+            zmt_dbg_check(stream, "zstd_lazy_search_kernel");
+        }
+        const uint32_t nblk = ng * bpc;
+        { ZmtProfScope ps(ZMT_K_L4H_BLOCKS, stream);
+        lz4_hc_blocks_kernel<<<zstd_grid(nblk), 256, sizeof(L4hSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, c0, nblk, P.lazy,
+                                                                                 K.Alternate(), tmp, blk_csize); }
+        zmt_dbg_check(stream, "lz4_hc_blocks_kernel");
+    }
+    if (side.ok) cudaStreamWaitEvent(stream, side.join, 0);
+    { ZmtProfScope ps(ZMT_K_LZ4_SIZES, stream);
+    lz4_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size); }
+    { ZmtProfScope ps(ZMT_K_SCAN, stream);
+    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks); }
+    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
+    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
+    { ZmtProfScope ps(ZMT_K_LZ4_PACK, stream);
+    lz4_frame_pack_kernel<<<gridp, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, chk, d_frame_off, (uint8_t*)d_out, nblocks, 0u); }
+    zmt_dbg_check(stream, "lz4_frame_pack_kernel");
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 

@@ -7,6 +7,7 @@
 //   cub::DeviceRadixSort     stable sort by key: equal keys end up next to each other in position order
 //   zstd_lazy_prev_kernel    prev[p] = the sorted neighbour with the same key (the walk stops at the chunk's start)
 //   zstd_lazy_search_kernel  one thread per position walks prev[] (input bytes through L2) and writes best[p]
+//                            (the LZ4 class of levels 10-12, lz4_hc.cuh, runs these four with its block and margins)
 //   zstd_lazy_blocks_kernel  one CTA per 64 KiB window, its four 16 KiB blocks in order: lazy parse, merge, sequences
 //                            and literals to the CTA's ZScratch, z_encode_block
 #pragma once
@@ -53,6 +54,9 @@ __device__ __forceinline__ uint32_t zl_ld32(const uint8_t* p)
     return sh ? __funnelshift_r(lo, __ldg(w + 1), sh) : lo;
 }
 
+// BLK: the parse unit (zstd: 16 KiB blocks, LZ4: 64 KiB blocks).  START: a match starts at o only if o + START <= the
+// block's end (0: o + mm, the zstd rule; LZ4: 12).  END: matches end at or before the block's end - END (zstd 0, LZ4 5).
+template <uint32_t BLK, uint32_t START, uint32_t END>
 __global__ void __launch_bounds__(256)
 zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
                         uint32_t c0, uint32_t npos, uint32_t mm, uint32_t depth, uint32_t W,
@@ -63,9 +67,9 @@ zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint3
     const uint32_t c = c0 + i / chunk_size, o = i % chunk_size;
     const uint64_t len = zmt_chunk_len(chunk_bytes, c, in_bytes, chunk_size);
     uint32_t res = 0;
-    const uint64_t bend = ((uint64_t)(o / ZL_BLOCK) + 1) * ZL_BLOCK < len ? ((uint64_t)(o / ZL_BLOCK) + 1) * ZL_BLOCK : len;
-    if ((uint64_t)o + mm <= bend) {
-        const uint32_t cap = bend - o < ZL_LCAP ? (uint32_t)(bend - o) : ZL_LCAP;
+    const uint64_t bend = ((uint64_t)(o / BLK) + 1) * BLK < len ? ((uint64_t)(o / BLK) + 1) * BLK : len;
+    if ((uint64_t)o + (START ? START : mm) <= bend) {
+        const uint32_t cap = bend - END - o < ZL_LCAP ? (uint32_t)(bend - END - o) : ZL_LCAP;
         const uint8_t* base = in + (uint64_t)c * chunk_size;
         const uint8_t* ps = base + o;
         const uint32_t cs0 = i - o;              // group-relative start of the chunk
