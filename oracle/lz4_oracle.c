@@ -61,7 +61,9 @@ uint32_t orc_xxh32(const void* data, size_t len, uint32_t seed)
 }
 
 /* --------------------------------------------------------- LZ4 block decode */
-long orc_lz4_block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t prefix)
+/* tr != NULL: one ORC_L4S_* row per sequence; token positions are counted from src - base (the frame start) */
+static long block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t prefix,
+                         orc_lz4f_trace_t* tr, size_t base)
 {
     const uint8_t* ip = src;
     const uint8_t* const iend = src + srcSize;
@@ -69,8 +71,9 @@ long orc_lz4_block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size
     uint8_t* const oend = dst + dstCap;
     if (srcSize == 0) return ORC_ERR_BLOCK;
     for (;;) {
-        size_t lit, ml, off;
+        size_t lit, ml, off, tokpos = (size_t)(ip - src), llext, mlext, mdst;
         unsigned token;
+        int64_t* row;
         if (ip >= iend) return ORC_ERR_BLOCK;
         token = *ip++;
         lit = token >> 4;
@@ -78,24 +81,41 @@ long orc_lz4_block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size
             unsigned b;
             do { if (ip >= iend) return ORC_ERR_BLOCK; b = *ip++; lit += b; } while (b == 255);
         }
+        llext = (size_t)(ip - src) - tokpos - 1;
         if (lit > (size_t)(iend - ip)) return ORC_ERR_BLOCK;
         if (lit > (size_t)(oend - op)) return ORC_ERR_DST_SMALL;
         memcpy(op, ip, lit); ip += lit; op += lit;
-        if (ip == iend) break;                      /* last sequence: literals only */
-        if ((size_t)(iend - ip) < 2) return ORC_ERR_BLOCK;
-        off = (size_t)ip[0] | ((size_t)ip[1] << 8); ip += 2;
-        if (off == 0 || off > (size_t)(op - dst) + prefix) return ORC_ERR_BLOCK;
-        ml = token & 15;
-        if (ml == 15) {
-            unsigned b;
-            do { if (ip >= iend) return ORC_ERR_BLOCK; b = *ip++; ml += b; } while (b == 255);
+        off = ml = mlext = 0; mdst = (size_t)(op - dst);
+        if (ip != iend) {
+            const uint8_t* e;
+            if ((size_t)(iend - ip) < 2) return ORC_ERR_BLOCK;
+            off = (size_t)ip[0] | ((size_t)ip[1] << 8); ip += 2;
+            if (off == 0 || off > (size_t)(op - dst) + prefix) return ORC_ERR_BLOCK;
+            ml = token & 15; e = ip;
+            if (ml == 15) {
+                unsigned b;
+                do { if (ip >= iend) return ORC_ERR_BLOCK; b = *ip++; ml += b; } while (b == 255);
+            }
+            mlext = (size_t)(ip - e);
+            ml += 4;
+            if (ml > (size_t)(oend - op)) return ORC_ERR_DST_SMALL;
+            { const uint8_t* m = op - off; size_t i; for (i = 0; i < ml; i++) op[i] = m[i]; }
+            op += ml;
         }
-        ml += 4;
-        if (ml > (size_t)(oend - op)) return ORC_ERR_DST_SMALL;
-        { const uint8_t* m = op - off; size_t i; for (i = 0; i < ml; i++) op[i] = m[i]; }
-        op += ml;
+        if (tr) {
+            if (tr->nseqs >= tr->max_seqs) return ORC_ERR_DST_SMALL;
+            row = tr->seq + tr->nseqs++ * ORC_L4S_NF;
+            row[ORC_L4S_TOKPOS] = (int64_t)(base + tokpos); row[ORC_L4S_LLEXT] = (int64_t)llext; row[ORC_L4S_MLEXT] = (int64_t)mlext;
+            row[ORC_L4S_LL] = (int64_t)lit; row[ORC_L4S_OFF] = (int64_t)off; row[ORC_L4S_ML] = (int64_t)ml; row[ORC_L4S_DST] = (int64_t)mdst;
+        }
+        if (!ml) break;                             /* last sequence: literals only; a block ending after a match is malformed */
     }
     return (long)(op - dst);
+}
+
+long orc_lz4_block_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t prefix)
+{
+    return block_decode(src, srcSize, dst, dstCap, prefix, NULL, 0);
 }
 
 /* --------------------------------- GPU compressor twin (deterministic spec)
@@ -188,8 +208,8 @@ size_t orc_lz4_block_compress_b200(const uint8_t* src, size_t n, uint8_t* dst, s
 #define LZ4F_MAGIC 0x184D2204u
 static const size_t k_blkmax[8] = { 0, 0, 0, 0, 65536, 262144, 1048576, 4194304 };
 
-int orc_lz4f_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap,
-                    size_t* outSize, size_t* consumed)
+static int lz4f_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap,
+                       size_t* outSize, size_t* consumed, orc_lz4f_trace_t* tr)
 {
     const uint8_t* ip = src;
     const uint8_t* const iend = src + srcSize;
@@ -208,23 +228,35 @@ int orc_lz4f_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dst
     if (csz) content = rd64(ip + 6);
     if (((orc_xxh32(ip + 4, hdrlen, 0) >> 8) & 0xFF) != ip[4 + hdrlen]) return ORC_ERR_HDR_CHECKSUM;
     ip += 4 + hdrlen + 1;
+    if (tr) tr->nblocks = tr->nseqs = 0;
     for (;;) {
         uint32_t bh; size_t bs;
+        int64_t* row = NULL;
         if ((size_t)(iend - ip) < 4) return ORC_ERR_TRUNCATED;
         bh = rd32(ip); ip += 4;
         if (bh == 0) break;
         bs = bh & 0x7FFFFFFFu;
         if (bs > blkmax) return ORC_ERR_BLOCK;
         if ((size_t)(iend - ip) < bs + (bchk ? 4 : 0)) return ORC_ERR_TRUNCATED;
+        if (tr) {
+            if (tr->nblocks >= tr->max_blocks) return ORC_ERR_DST_SMALL;
+            row = tr->blk + tr->nblocks++ * ORC_L4B_NF;
+            row[ORC_L4B_FOFF] = (int64_t)(ip - src); row[ORC_L4B_BSIZE] = (int64_t)bs; row[ORC_L4B_STORED] = (bh >> 31) != 0;
+            row[ORC_L4B_REGEN] = -1; row[ORC_L4B_LINKED] = !indep; row[ORC_L4B_BCHK] = bchk;
+            row[ORC_L4B_BCHK_OK] = bchk ? orc_xxh32(ip, bs, 0) == rd32(ip + bs) : -1;
+            row[ORC_L4B_SEQ_FIRST] = (int64_t)tr->nseqs; row[ORC_L4B_NSEQ] = 0; row[ORC_L4B_DST] = (int64_t)total;
+        }
         if (bh & 0x80000000u) {
             if (bs > dstCap - total) return ORC_ERR_DST_SMALL;
             memcpy(dst + total, ip, bs); total += bs;
+            if (row) row[ORC_L4B_REGEN] = (int64_t)bs;
         } else {
             size_t prefix = indep ? 0 : (total < 65536 ? total : 65536);
             size_t cap = dstCap - total < blkmax ? dstCap - total : blkmax;
-            long d = orc_lz4_block_decode(ip, bs, dst + total, cap, prefix);
+            long d = block_decode(ip, bs, dst + total, cap, prefix, tr, (size_t)(ip - src));
             if (d < 0) return (int)d;
             total += (size_t)d;
+            if (row) { row[ORC_L4B_REGEN] = d; row[ORC_L4B_NSEQ] = (int64_t)tr->nseqs - row[ORC_L4B_SEQ_FIRST]; }
         }
         if (bchk && orc_xxh32(ip, bs, 0) != rd32(ip + bs)) return ORC_ERR_BLOCK;
         ip += bs + (bchk ? 4 : 0);
@@ -238,6 +270,17 @@ int orc_lz4f_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dst
     if (outSize) *outSize = total;
     if (consumed) *consumed = (size_t)(ip - src);
     return ORC_OK;
+}
+
+int orc_lz4f_decode(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed)
+{
+    return lz4f_decode(src, srcSize, dst, dstCap, outSize, consumed, NULL);
+}
+
+int orc_lz4f_trace(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCap, size_t* outSize, size_t* consumed,
+                   orc_lz4f_trace_t* tr)
+{
+    return lz4f_decode(src, srcSize, dst, dstCap, outSize, consumed, tr);
 }
 
 size_t orc_lz4f_bound(size_t n)

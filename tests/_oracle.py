@@ -160,3 +160,61 @@ def mt_frames(framed):
     if n < 0:
         raise ValueError("orc_mt_scan failed: %d" % n)
     return [framed[int(offs[i]) + 12: int(offs[i]) + 12 + int(cs[i])] for i in range(n)]
+
+
+# ---- LZ4 frame trace (orc_lz4f_trace) ----
+# columns of Lz4Trace.blk / .seq, in the order of the ORC_L4B_* / ORC_L4S_* enums of oracle/oracle.h
+L4B_FIELDS = ("foff", "bsize", "stored", "regen", "linked", "bchk", "bchk_ok", "seq_first", "nseq", "dst")
+L4S_FIELDS = ("tokpos", "llext", "mlext", "ll", "off", "ml", "dst")
+L4B = {name: i for i, name in enumerate(L4B_FIELDS)}
+L4S = {name: i for i, name in enumerate(L4S_FIELDS)}
+
+
+class _L4Trace(ctypes.Structure):
+    _fields_ = [("max_blocks", c_sz), ("max_seqs", c_sz), ("blk", c_vp), ("seq", c_vp), ("nblocks", c_sz), ("nseqs", c_sz)]
+
+
+class Lz4Trace:
+    """What every block of one LZ4 frame contained, as int64 numpy arrays: blk[b, L4B[field]] and seq[i, L4S[field]]
+    (token position in the frame, extension byte counts, literal length, offset, match length, block-relative
+    destination of the match; offset and match length 0 for a literals-only last sequence); content: the decoded bytes."""
+
+    def __init__(self, blk, seq, content, consumed):
+        self.blk, self.seq, self.content, self.consumed = blk, seq, content, consumed
+
+    def col(self, name):
+        return self.blk[:, L4B[name]]
+
+    def s(self, name):
+        return self.seq[:, L4S[name]]
+
+    def block_seqs(self, b):
+        a = int(self.blk[b, L4B["seq_first"]])
+        return self.seq[a: a + int(self.blk[b, L4B["nseq"]])]
+
+
+def lz4f_trace(frame, out_cap):
+    """orc_lz4f_trace on one LZ4 frame (starting at its magic).  Raises on a decode error."""
+    frame = _arr(frame)
+    L = orc()
+    if not hasattr(L, "_l4t_ready"):
+        L.orc_lz4f_trace.restype = ctypes.c_int
+        L.orc_lz4f_trace.argtypes = [c_vp, c_sz, c_vp, c_sz, ctypes.POINTER(c_sz), ctypes.POINTER(c_sz), ctypes.POINTER(_L4Trace)]
+        L._l4t_ready = True
+    mb, ms = frame.size // 4 + 2, frame.size + 2                      # a block costs >= 4 header bytes, a sequence >= 1 byte
+    blk = np.empty((mb, len(L4B_FIELDS)), np.int64); seq = np.empty((ms, len(L4S_FIELDS)), np.int64)
+    out = np.empty(out_cap + 1, np.uint8)
+    t = _L4Trace(mb, ms, blk.ctypes.data, seq.ctypes.data, 0, 0)
+    got, used = c_sz(0), c_sz(0)
+    rc = L.orc_lz4f_trace(frame.ctypes.data, frame.size, out.ctypes.data, out.size, ctypes.byref(got), ctypes.byref(used), ctypes.byref(t))
+    if rc != 0:
+        raise ValueError("orc_lz4f_trace failed: %d" % rc)
+    return Lz4Trace(blk[: t.nblocks].copy(), seq[: t.nseqs].copy(), out[: got.value].copy(), used.value)
+
+
+def lz4f_decode(frame, out_cap):
+    """orc_lz4f_decode on one LZ4 frame: (rc, decoded bytes, bytes consumed)."""
+    frame = _arr(frame)
+    out = np.empty(out_cap + 1, np.uint8); got, used = c_sz(0), c_sz(0)
+    rc = orc().orc_lz4f_decode(frame.ctypes.data, frame.size, out.ctypes.data, out.size, ctypes.byref(got), ctypes.byref(used))
+    return rc, out[: got.value].copy(), used.value

@@ -37,6 +37,7 @@
 
 #define LZB_LINKED 1u         // block may copy from the previous block of its frame
 #define LZB_LAST   2u         // last block of its frame
+#define LZB_BCHK   4u         // an XXH32 of the block's stored bytes follows them (FLG.BC)
 
 struct LzBlk {
     uint32_t src;             // offset of the block data inside the LZ4F frame
@@ -77,7 +78,8 @@ __global__ void lz4_slot_counts_kernel(const uint64_t* __restrict__ out_off, uin
 __global__ void lz4_scan_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
                                        const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ first_slot, uint32_t slot_cap,
                                        LzBlk* __restrict__ tab, uint32_t* __restrict__ prog, uint32_t* __restrict__ status,
-                                       uint32_t* __restrict__ stored_chk, uint32_t* __restrict__ needs_seq, uint32_t nframes)
+                                       uint32_t* __restrict__ stored_chk, uint32_t* __restrict__ needs_seq, uint32_t* __restrict__ any_bchk,
+                                       uint32_t nframes)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
@@ -118,7 +120,7 @@ __global__ void lz4_scan_frames_kernel(const uint8_t* __restrict__ in, const uin
         // the sequential pass decodes it block after block and reports what is wrong, if anything
         if (b >= nslot || (uint64_t)b * blkmax > cap) { seq = true; }
         else {
-            LzBlk e; e.src = ip; e.csize = bh; e.flags = ((!indep && b > 0) ? LZB_LINKED : 0u) | (blklog << 8); e.nrec = 0; e.frame = f;
+            LzBlk e; e.src = ip; e.csize = bh; e.flags = ((!indep && b > 0) ? LZB_LINKED : 0u) | (bchk ? LZB_BCHK : 0u) | (blklog << 8); e.nrec = 0; e.frame = f;
             if (bs == 0) e.csize = 0;                      // a zero-sized stored block regenerates nothing (bit 31 set, size 0)
             if (bs == 0) seq = true;                       // ... and breaks the fixed block addressing
             T[b] = e;
@@ -138,6 +140,30 @@ __global__ void lz4_scan_frames_kernel(const uint8_t* __restrict__ in, const uin
     if (err) { status[f] = err; for (uint32_t s = 0; s < nslot; s++) T[s].csize = 0; return; }
     if (seq) { needs_seq[f] = 1; for (uint32_t s = 0; s < nslot; s++) T[s].csize = 0; return; }
     if (b > 0) T[b - 1].flags |= LZB_LAST;
+    if (bchk) *any_bchk = 1;
+}
+
+// ---------------------------------------------------------------- block checksums (FLG.BC), before pass A
+// One warp per slot of the two-pass path: XXH32 of the block's stored bytes against the 4 bytes that follow them; a
+// mismatch fails the frame with ZMT_ST_BLOCK, so pass A skips it.  Frames of the sequential pass are checked there,
+// block by block.  Exits at once when no frame of the batch sets FLG.BC (every frame this library writes).
+__global__ void __launch_bounds__(32 * X_WARPS)
+lz4_block_checksum_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint64_t* __restrict__ first_slot,
+                          const LzBlk* __restrict__ tab, uint32_t* __restrict__ status, const uint32_t* __restrict__ any_bchk,
+                          uint32_t nframes, uint32_t slot_cap)
+{
+    __shared__ uint4 tile[X_WARPS][2][32];
+    if (*any_bchk == 0) return;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint64_t nslots = first_slot[nframes] < slot_cap ? first_slot[nframes] : slot_cap;
+    for (uint64_t t = (uint64_t)blockIdx.x * X_WARPS + wid; t < nslots; t += (uint64_t)gridDim.x * X_WARPS) {
+        const LzBlk B = tab[t];
+        if (B.csize == 0 || !(B.flags & LZB_BCHK) || (status[B.frame] & 0xFF) != 0) continue;
+        const uint8_t* src = in + frame_off[B.frame] + 12 + B.src;
+        const uint32_t bs = B.csize & 0x7FFFFFFFu;
+        const uint32_t h = warp_xxh32(src, bs, tile[wid], lane);
+        if (lane == 0 && h != ldg_le32(src + bs)) d_fail(status, B.frame, ZMT_ST_BLOCK, lane);
+    }
 }
 
 // ---------------------------------------------------------------- pass A: token parse, literals, match records
@@ -390,8 +416,8 @@ lz4_ticket_windows_kernel(const uint64_t* __restrict__ first_slot, uint32_t nfra
 }
 
 // STAGED: every step's output window lives in shared memory as well (chains of matches that feed each other run at shared
-// memory latency) — pays when few chains are in flight (small batches, few frames); with tens of thousands of blocks the
-// extra window traffic costs more than the latency it hides, and the plain variant (all reads from global memory) is used.
+// memory latency).  zmt_lz4_decompress_device always launches the staged variant; the plain one (all reads from global
+// memory) runs only when ZSTDMT_B200_LZ4_STAGED=0 is set, for A/B measurements and tests.
 template <bool STAGED>
 __global__ void __launch_bounds__(32 * LZD_WARPS)
 lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ frame_off,
@@ -691,6 +717,11 @@ lz4_decode_frames_seq_kernel(const uint8_t* __restrict__ in, const uint8_t* __re
             W.gsrc = p + ip; W.pos = 0x40000000;            // empty window
             d = warp_decode_block(W, bs, dst + total, dcap, hist, lane);
             if (d == 0xFFFFFFFFu) { d_fail(status, f, ZMT_ST_BLOCK, lane); return; }
+        }
+        if (bchk) {
+            __syncwarp();
+            const uint32_t h = warp_xxh32(p + ip, bs, reinterpret_cast<uint4(*)[32]>(W.w), lane);      // the window is refilled per block
+            if (__shfl_sync(ZMT_FULL_MASK, h != ldg_le32(p + ip + bs), 0)) { d_fail(status, f, ZMT_ST_BLOCK, lane); return; }
         }
         ip += bs + (bchk ? 4 : 0);
         total += d;

@@ -361,18 +361,9 @@ zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
 // per warp), park each tile in a per-warp shared-memory slot, and lanes 0..3 walk the slot word by word.
 #define X_WARPS 8
 #define X_DEPTH 4
-__global__ void __launch_bounds__(32 * X_WARPS)
-xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs, const uint64_t* __restrict__ lens,
-             const uint32_t* __restrict__ lens32, uint64_t stride, uint64_t total_bytes, uint32_t* __restrict__ out, uint32_t nbuf)
+// XXH32 (seed 0) of p[0, n) by one warp; tile = the warp's 1 KiB of shared memory.  The hash is valid on lane 0.
+__device__ __forceinline__ uint32_t warp_xxh32(const uint8_t* p, uint64_t n, uint4 (*tile)[32], uint32_t lane)
 {
-    __shared__ uint4 tile[X_WARPS][2][32];
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint32_t g = blockIdx.x * X_WARPS + wid;
-    if (g >= nbuf) return;                                   // whole warp leaves together
-    uint64_t off, n;
-    if (offs) { off = offs[g]; n = lens ? lens[g] : offs[g + 1] - off; }
-    else { off = (uint64_t)g * stride; n = zmt_chunk_len(lens32, g, total_bytes, (uint32_t)stride); }
-    const uint8_t* p = base + off;
     const uint32_t j = lane & 3;
     uint32_t acc = j == 0 ? XXP1 + XXP2 : j == 1 ? XXP2 : j == 2 ? 0u : 0u - XXP1;
     const uint64_t ns = n >> 4;                              // 16-byte stripes
@@ -387,7 +378,7 @@ xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs
 #pragma unroll
             for (int d = 0; d < X_DEPTH; d++) {
                 if (t + d < nt) {
-                    uint4* slot = tile[wid][d & 1];
+                    uint4* slot = tile[d & 1];
                     slot[lane] = r[d];
                     if (t + d + X_DEPTH < nt) r[d] = __ldg(v + (t + d + X_DEPTH) * 32 + lane);
                     __syncwarp();
@@ -405,16 +396,32 @@ xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs
     else for (; s < ns; s++) acc = xxh32_round(acc, ldg_le32(p + 16 * s + 4 * j));
     const uint32_t a1 = __shfl_sync(ZMT_FULL_MASK, acc, 0), a2 = __shfl_sync(ZMT_FULL_MASK, acc, 1);
     const uint32_t a3 = __shfl_sync(ZMT_FULL_MASK, acc, 2), a4 = __shfl_sync(ZMT_FULL_MASK, acc, 3);
+    uint32_t h = 0;
     if (lane == 0) {
-        uint32_t h = n >= 16 ? rotl32(a1, 1) + rotl32(a2, 7) + rotl32(a3, 12) + rotl32(a4, 18) : XXP5;
+        h = n >= 16 ? rotl32(a1, 1) + rotl32(a2, 7) + rotl32(a3, 12) + rotl32(a4, 18) : XXP5;
         h += (uint32_t)n;
         const uint8_t* q = p + (ns << 4);
         const uint8_t* end = p + n;
         while (q + 4 <= end) { h = rotl32(h + ldg_le32(q) * XXP3, 17) * XXP4; q += 4; }
         while (q < end) { h = rotl32(h + (*q) * XXP5, 11) * XXP1; q++; }
         h ^= h >> 15; h *= XXP2; h ^= h >> 13; h *= XXP3; h ^= h >> 16;
-        out[g] = h;
     }
+    return h;
+}
+
+__global__ void __launch_bounds__(32 * X_WARPS)
+xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs, const uint64_t* __restrict__ lens,
+             const uint32_t* __restrict__ lens32, uint64_t stride, uint64_t total_bytes, uint32_t* __restrict__ out, uint32_t nbuf)
+{
+    __shared__ uint4 tile[X_WARPS][2][32];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t g = blockIdx.x * X_WARPS + wid;
+    if (g >= nbuf) return;                                   // whole warp leaves together
+    uint64_t off, n;
+    if (offs) { off = offs[g]; n = lens ? lens[g] : offs[g + 1] - off; }
+    else { off = (uint64_t)g * stride; n = zmt_chunk_len(lens32, g, total_bytes, (uint32_t)stride); }
+    const uint32_t h = warp_xxh32(base + off, n, tile[wid], lane);
+    if (lane == 0) out[g] = h;
 }
 
 // ============================================================================ frame pack
@@ -1018,7 +1025,7 @@ extern "C" int zmt_lz4_compress_level_device(const void* d_in, uint64_t in_bytes
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
-// workspace: stored[] | computed[] | needs_seq[] | ticket | slot counts | first_slot | block table | progress | match records
+// workspace: stored[] | computed[] | needs_seq[] | ticket, any-FLG.BC flag | slot counts | first_slot | block table | progress | match records
 extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, uint64_t in_bytes)
 {
     uint64_t sz = 3 * a256((uint64_t)nframes * 4) + 256 + 2 * a256(((uint64_t)nframes + 1) * 8) + a256(((uint64_t)nframes / LZX_WIN + 2) * 8);
@@ -1038,7 +1045,8 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
     uint32_t* stored = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
     uint32_t* computed = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
     uint32_t* needs_seq = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
-    unsigned long long* ticket = (unsigned long long*)w; w += 256;
+    unsigned long long* ticket = (unsigned long long*)w;
+    uint32_t* any_bchk = (uint32_t*)(ticket + 1); w += 256;
     unsigned long long* wbase = (unsigned long long*)w; w += a256(((uint64_t)nframes / LZX_WIN + 2) * 8);
     uint64_t* slot_cnt = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
     uint64_t* first_slot = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
@@ -1052,8 +1060,13 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
     lz4_slot_counts_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(d_out_off, nframes, slot_cnt);
     scan_u64_kernel<<<1, 1024, 0, stream>>>(slot_cnt, first_slot, nframes);
     lz4_ticket_windows_kernel<<<1, 256, 0, stream>>>(first_slot, nframes, wbase);
-    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, nframes);
+    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, any_bchk, nframes);
     zmt_dbg_check(stream, "lz4_scan_frames_kernel");
+    {
+        const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8), need = (nslots + X_WARPS - 1) / X_WARPS;
+        lz4_block_checksum_kernel<<<need < maxg ? need : maxg, 32 * X_WARPS, 0, stream>>>(in, d_frame_off, first_slot, tab, d_status, any_bchk, nframes, nslots);
+    }
+    zmt_dbg_check(stream, "lz4_block_checksum_kernel");
     { ZmtProfScope ps(ZMT_K_LZ4_DECODE, stream);
     lz4_parse_blocks_kernel<<<(nslots + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(
         in, in + in_bytes, d_frame_off, (uint8_t*)d_out, d_out_off, first_slot, tab, rec, (unsigned long long*)d_out_size, d_status, needs_seq, nframes, nslots); }
