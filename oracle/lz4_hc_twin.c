@@ -38,6 +38,18 @@ static int chunk_best(const uint8_t* src, size_t n, uint32_t depth, uint32_t W, 
     return 0;
 }
 
+/* best[] of one chunk of n bytes at `level` (window / block as for orc_lz4_hc_sequences) into best[0 .. n):
+ * length | offset << ZL_LEN_BITS, 0 where there is no match.  Returns 0, or -1 when memory runs out. */
+int orc_lz4_hc_best(const uint8_t* src, size_t n, int level, uint32_t window, uint32_t block, uint32_t* best)
+{
+    const L4hParams P = l4h_params(level);
+    uint32_t* b = (uint32_t*)calloc(n + 3, sizeof(uint32_t));
+    if (!b || chunk_best(src, n, P.depth, window ? window : L4H_WINDOW, block ? block : L4H_BLOCK, b)) { free(b); return -1; }
+    memcpy(best, b, sizeof(uint32_t) * n);
+    free(b);
+    return 0;
+}
+
 /* the parse of block [b0, b1): appends 3 words per sequence (literal length, offset, match length) to seq */
 static long block_parse(const uint32_t* best, size_t b0, size_t b1, uint32_t lazy, uint32_t* seq, size_t max_seqs)
 {

@@ -8,22 +8,14 @@
 
 #define NONE 0xFFFFFFFFu
 
-/* One chunk (= one frame) of n bytes at `level`.  window / block: 0 for the level's window and 16 KiB blocks; other
- * values shrink them so that small inputs reach their edges.  seq: 3 words per sequence (literal length, offset, match
- * length), all blocks back to back; blk_nseq[b]: sequences of block b.  Returns the number of sequences, or -1 when
- * max_seqs / max_blocks is too small or memory runs out. */
-long orc_zstd_lazy_sequences(const uint8_t* src, size_t n, int level, uint32_t window, uint32_t block,
-                             uint32_t* seq, size_t max_seqs, uint32_t* blk_nseq, size_t max_blocks)
+/* best[] of one chunk of n bytes (window W, blocks of B bytes); best must hold n + 3 zeroed words.  A match starts at
+ * p only if p + minMatch <= blockEnd, so the parse of a block never reads best[] of the next one. */
+static int chunk_best(const uint8_t* src, size_t n, ZlParams P, uint32_t W, uint32_t B, uint32_t* best)
 {
-    const ZlParams P = zl_params(level);
-    const uint32_t W = window ? window : zl_window(level), B = block ? block : ZL_BLOCK, mm = P.min_match;
-    const size_t nblocks = (n + B - 1) / B;
-    if (nblocks > max_blocks) return -1;
+    const uint32_t mm = P.min_match;
     uint32_t* head = (uint32_t*)malloc(sizeof(uint32_t) << ZL_HASHLOG);
     uint32_t* prev = (uint32_t*)malloc(sizeof(uint32_t) * (n + 1));
-    uint32_t* best = (uint32_t*)calloc(n + 3, sizeof(uint32_t));
-    long ns = 0;
-    if (!head || !prev || !best) { ns = -1; goto done; }
+    if (!head || !prev) { free(head); free(prev); return -1; }
     memset(head, 0xFF, sizeof(uint32_t) << ZL_HASHLOG);
     for (size_t p = 0; p + mm <= n; p++) {
         uint64_t v = 0;
@@ -31,8 +23,8 @@ long orc_zstd_lazy_sequences(const uint8_t* src, size_t n, int level, uint32_t w
         const uint32_t h = zl_hash(v, mm);
         prev[p] = head[h]; head[h] = (uint32_t)p;
     }
-    for (size_t b = 0; b < nblocks; b++) {
-        const size_t b0 = b * B, b1 = b0 + B < n ? b0 + B : n;
+    for (size_t b0 = 0; b0 < n; b0 += B) {
+        const size_t b1 = b0 + B < n ? b0 + B : n;
         for (size_t p = b0; p + mm <= b1; p++) {
             const uint32_t cap = (uint32_t)(b1 - p < ZL_LCAP ? b1 - p : ZL_LCAP);
             uint32_t bl = 0, bo = 0, q = prev[p];
@@ -43,6 +35,39 @@ long orc_zstd_lazy_sequences(const uint8_t* src, size_t n, int level, uint32_t w
             }
             best[p] = bl ? bl | (bo << ZL_LEN_BITS) : 0;
         }
+    }
+    free(head); free(prev);
+    return 0;
+}
+
+/* best[] of one chunk of n bytes at `level` (window / block as for orc_zstd_lazy_sequences) into best[0 .. n):
+ * length | offset << ZL_LEN_BITS, 0 where there is no match.  Returns 0, or -1 when memory runs out. */
+int orc_zstd_lazy_best(const uint8_t* src, size_t n, int level, uint32_t window, uint32_t block, uint32_t* best)
+{
+    const ZlParams P = zl_params(level);
+    uint32_t* b = (uint32_t*)calloc(n + 3, sizeof(uint32_t));
+    if (!b || chunk_best(src, n, P, window ? window : zl_window(level), block ? block : ZL_BLOCK, b)) { free(b); return -1; }
+    memcpy(best, b, sizeof(uint32_t) * n);
+    free(b);
+    return 0;
+}
+
+/* One chunk (= one frame) of n bytes at `level`.  window / block: 0 for the level's window and 16 KiB blocks; other
+ * values shrink them so that small inputs reach their edges.  seq: 3 words per sequence (literal length, offset, match
+ * length), all blocks back to back; blk_nseq[b]: sequences of block b.  Returns the number of sequences, or -1 when
+ * max_seqs / max_blocks is too small or memory runs out. */
+long orc_zstd_lazy_sequences(const uint8_t* src, size_t n, int level, uint32_t window, uint32_t block,
+                             uint32_t* seq, size_t max_seqs, uint32_t* blk_nseq, size_t max_blocks)
+{
+    const ZlParams P = zl_params(level);
+    const uint32_t W = window ? window : zl_window(level), B = block ? block : ZL_BLOCK;
+    const size_t nblocks = (n + B - 1) / B;
+    if (nblocks > max_blocks) return -1;
+    uint32_t* best = (uint32_t*)calloc(n + 3, sizeof(uint32_t));
+    long ns = 0;
+    if (!best || chunk_best(src, n, P, W, B, best)) { ns = -1; goto done; }
+    for (size_t b = 0; b < nblocks; b++) {
+        const size_t b0 = b * B, b1 = b0 + B < n ? b0 + B : n;
         uint32_t nb = 0, last_off = 0;
         size_t anchor = b0;
         for (size_t p = b0; p < b1;) {
@@ -63,6 +88,6 @@ long orc_zstd_lazy_sequences(const uint8_t* src, size_t n, int level, uint32_t w
         blk_nseq[b] = nb;
     }
 done:
-    free(head); free(prev); free(best);
+    free(best);
     return ns;
 }

@@ -212,8 +212,19 @@ def twin():
                                            ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
         L.orc_lz4_hc_compress.restype = ctypes.c_size_t
         L.orc_lz4_hc_compress.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t]
+        L.orc_lz4_hc_best.restype = ctypes.c_int
+        L.orc_lz4_hc_best.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_void_p]
         _twin = L
     return _twin
+
+
+def twin_best(data, level, W=0, block=0):
+    """orc_lz4_hc_best: the chunk's best[] (uint32, length | offset << LEN_BITS, 0: no match)."""
+    src = np.ascontiguousarray(data, dtype=np.uint8)
+    best = np.zeros(max(int(src.size), 1), np.uint32)
+    if twin().orc_lz4_hc_best(src.ctypes.data, src.size, level, W, block, best.ctypes.data) != 0:
+        raise RuntimeError("orc_lz4_hc_best failed")
+    return best[: src.size]
 
 
 def twin_sequences(data, level, W=0, block=0):

@@ -127,8 +127,19 @@ def twin():
         L.orc_zstd_lazy_sequences.restype = ctypes.c_long
         L.orc_zstd_lazy_sequences.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32,
                                               ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
+        L.orc_zstd_lazy_best.restype = ctypes.c_int
+        L.orc_zstd_lazy_best.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_void_p]
         _twin = L
     return _twin
+
+
+def twin_best(data, level, W=0, block=0):
+    """orc_zstd_lazy_best: the chunk's best[] (uint32, length | offset << LEN_BITS, 0: no match)."""
+    src = np.ascontiguousarray(data, dtype=np.uint8)
+    best = np.zeros(max(int(src.size), 1), np.uint32)
+    if twin().orc_zstd_lazy_best(src.ctypes.data, src.size, level, W, block, best.ctypes.data) != 0:
+        raise RuntimeError("orc_zstd_lazy_best failed")
+    return best[: src.size]
 
 
 def twin_sequences(data, level, W=0, block=0):

@@ -173,26 +173,45 @@ def _code(base, v):
     return int(np.searchsorted(base, v, side="right")) - 1
 
 
-def raw_by_bitbuf(win, a, e, mseq):
-    """True when a sub-block stored raw certainly was so because its sequence bits overflow the bit buffer: bounded from
-    below they overflow it, and bounded from above the compressed block would have been smaller than its content (the
-    other reason to store it raw).  A state transition of a predefined FSE table emits maxBitsOut or maxBitsOut - 1 bits
-    (exactly log for a count of 1 or -1); the first symbol of each stream emits none."""
-    if not len(mseq):
-        return False
-    nlit = (e - a) - int(mseq[:, 2].sum())
+def seq_bit_bounds(rows):
+    """Lower and upper bounds of the bits of a block's sequence bitstream, rows (literal length, offset, match length)
+    with explicit offsets (Offset_Value = offset + 3).  A state transition of a predefined FSE table emits maxBitsOut or
+    maxBitsOut - 1 bits (exactly log for a count of 1 or -1); the first symbol of each stream emits none."""
     lo = hi = 6 + 5 + 6 - (6 + 5 + 6)                               # final states flushed; first symbols emit nothing
-    p = a
-    for s, off, ml in mseq.tolist():
-        ll = s - p; p = s + ml
+    for ll, off, ml in rows:
         lc, mc, oc = _code(LL_BASE, ll), _code(ML_BASE, ml), (off + 3).bit_length() - 1
         extra = (int(LL_BASE[lc + 1] - LL_BASE[lc]) - 1).bit_length() + (int(ML_BASE[mc + 1] - ML_BASE[mc]) - 1).bit_length() + oc
         mx = LL_MAXB[lc] + ML_MAXB[mc] + OF_MAXB[oc]
         mn = sum(b if b == lg else b - 1 for b, lg in ((LL_MAXB[lc], 6), (ML_MAXB[mc], 6), (OF_MAXB[oc], 5)))
         lo += extra + mn; hi += extra + mx
-    lo += 6 + 5 + 6 - 17; hi += 6 + 5 + 6
-    upper = 3 + (nlit + 5) + 4 + hi // 8 + 1
-    return upper < e - a and lo // 8 + 1 + 8 > Z_BITBUF
+    return lo + 6 + 5 + 6 - 17, hi + 6 + 5 + 6
+
+
+def raw_bounds(regen, rows):
+    """(upper bound of the compressed block's size, whether its sequence bits certainly overflow the bit buffer)."""
+    nlit = regen - sum(ml for _, _, ml in rows)
+    lo, hi = seq_bit_bounds(rows)
+    return 3 + (nlit + 5) + 4 + hi // 8 + 1, lo // 8 + 1 + 8 > Z_BITBUF
+
+
+def raw_is_justified(regen, rows):
+    """A block of `regen` bytes whose parse is `rows` may be stored raw: the compressed block may not be smaller than
+    its content, or its sequence bits overflow the bit buffer."""
+    upper, overflow = raw_bounds(regen, rows)
+    return upper >= regen or overflow
+
+
+def raw_by_bitbuf(win, a, e, mseq):
+    """True when a sub-block stored raw certainly was so because its sequence bits overflow the bit buffer: bounded from
+    below they overflow it, and bounded from above the compressed block would have been smaller than its content (the
+    other reason to store it raw)."""
+    if not len(mseq):
+        return False
+    rows, p = [], a
+    for s, off, ml in mseq.tolist():
+        rows.append((s - p, off, ml)); p = s + ml
+    upper, overflow = raw_bounds(e - a, rows)
+    return upper < e - a and overflow
 
 
 def check_roundtrip(torch, framed, src):

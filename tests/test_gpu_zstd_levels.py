@@ -2,6 +2,8 @@
 written by zmt_zstd_compress_level_device is traced by the oracle (orc_zstd_trace) and checked:
   - every compressed block's sequences equal the CPU twin's (oracle/zstd_lazy_twin.c) for that block, offsets explicit;
   - blocks are raw or compressed, 16 KiB (the chunk's last one may be short), predefined modes, own Huffman tree;
+  - every raw block is raw for a reason: on the twin's parse, an upper bound of its compressed size is at least its
+    content, or a lower bound of its sequence bits overflows the entropy stage's bit buffer;
   - the Huffman lengths are _zenc.huf_lengths of the block's literal histogram;
   - the oracle, libzstd (T=1 and T>1, when oracle/_ref exists) and the GPU decoder restore the frames.
 Inputs are built here with fixed seeds; each edge case asserts from the trace that it reached its edge."""
@@ -13,7 +15,7 @@ import pytest
 import _oracle as o
 import _zlazy as zl
 import zstdmt_b200 as z
-from test_gpu_zstd_encoder import check_huffman, check_modes, check_roundtrip
+from test_gpu_zstd_encoder import check_huffman, check_modes, check_roundtrip, raw_bounds, raw_is_justified
 
 pytestmark = pytest.mark.gpu
 ZT = o.ZT
@@ -53,6 +55,7 @@ class Report:
         self.seqs = []                   # (frame, block start in the frame, traced (ll, off, ml) rows) of every compressed block
         self.types = []
         self.huf = 0
+        self.raw_bitbuf = 0              # raw blocks whose twin parse certainly overflows the bit buffer
 
     def all_seqs(self):
         return np.concatenate([s for _, _, s in self.seqs]) if self.seqs else np.zeros((0, 3), np.int64)
@@ -78,6 +81,9 @@ def check(torch, src, chunk, level, chunk_bytes=None):
         for k, b in enumerate(blocks):
             rep.types.append(int(tr.blk[b, ZT["type"]]))
             if tr.blk[b, ZT["type"]] != 2:
+                rows = [tuple(r) for r in twin[k].astype(np.int64).tolist()]
+                assert raw_is_justified(int(regen[b]), rows), ("raw block the twin's parse would compress", fi, k)
+                rep.raw_bitbuf += raw_bounds(int(regen[b]), rows)[1]
                 continue
             q = tr.block_seqs(b).astype(np.int64)
             assert (q[:, 1] == q[:, 3] + 3).all()                     # Offset_Value = offset + 3: no repeat codes
