@@ -32,6 +32,7 @@
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>
 #include "common.cuh"
+#include "host_common.h"
 #include "zmt_dev.h"
 #include "zstd_entropy.cuh"
 
@@ -246,7 +247,7 @@ static_assert(sizeof(ZstdSmem) + 1024 <= (228 * 1024) / 2, "two CTAs per SM");
 
 __global__ void __launch_bounds__(P_TEAM, 2)
 zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
-                   uint32_t bpc, uint8_t* __restrict__ tmp, uint32_t* __restrict__ blk_csize, uint32_t nblocks, uint32_t flags,
+                   uint32_t bpc, uint8_t* __restrict__ tmp, uint32_t* __restrict__ blk_csize, uint32_t nblocks,
                    ZScratch* __restrict__ zscratch)
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -271,7 +272,7 @@ zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
 
         CTA_SYNC();                                       // previous block fully consumed
         if (tid == 0) { S.nlong = 0; S.any[0] = 0; S.any[1] = 0; }
-        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, flags, tid);
+        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, tid);
 
         const uint32_t limit = n >= 5 ? n - 5 : 0;        // matches end at or before n-5
         uint32_t e = 0, e_din = 0, out_pos = 0;
@@ -601,23 +602,16 @@ static int zstd_tables_init()
     int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ZMT_ST_CUDA;
     std::lock_guard<std::mutex> guard(mu);
     if (done[dev]) return ZMT_ST_OK;
-    static const int16_t LLn[36] = { 4,3,2,2,2,2,2,2,2,2,2,2,2,1,1,1,2,2,2,2,2,2,2,2,2,3,2,1,1,1,1,1,-1,-1,-1,-1 };
-    static const int16_t MLn[53] = { 1,4,3,2,2,2,2,2,2,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,-1,-1,-1,-1,-1,-1,-1 };
-    static const int16_t OFn[29] = { 1,1,1,1,1,1,2,2,2,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,-1,-1,-1,-1,-1 };
-    static const uint32_t LLb[36] = { 0,1,2,3,4,5,6,7,8,9,10,11,12,13,14,15,16,18,20,22,24,28,32,40,48,64,128,256,512,1024,2048,4096,8192,16384,32768,65536 };
-    static const uint8_t  LLx[36] = { 0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,1,1,1,1,2,2,3,3,4,6,7,8,9,10,11,12,13,14,15,16 };
-    static const uint32_t MLb[53] = { 3,4,5,6,7,8,9,10,11,12,13,14,15,16,17,18,19,20,21,22,23,24,25,26,27,28,29,30,31,32,33,34,35,37,39,41,43,47,51,59,67,83,99,131,259,515,1027,2051,4099,8195,16387,32771,65539 };
-    static const uint8_t  MLx[53] = { 0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,1,1,1,1,2,2,3,3,4,4,5,7,8,9,10,11,12,13,14,15,16 };
     ZFseCTable t;
-    zstd_build_ctable(t, LLn, 36, 6); if (cudaMemcpyToSymbol(c_fse_ll, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
-    zstd_build_ctable(t, OFn, 29, 5); if (cudaMemcpyToSymbol(c_fse_of, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
-    zstd_build_ctable(t, MLn, 53, 6); if (cudaMemcpyToSymbol(c_fse_ml, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    zstd_build_ctable(t, ZSTD_LL_NORM, 36, 6); if (cudaMemcpyToSymbol(c_fse_ll, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    zstd_build_ctable(t, ZSTD_OF_NORM, 29, 5); if (cudaMemcpyToSymbol(c_fse_of, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    zstd_build_ctable(t, ZSTD_ML_NORM, 53, 6); if (cudaMemcpyToSymbol(c_fse_ml, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
     uint8_t llc[64], mlc[128];
-    for (int v = 0; v < 64; v++) { int c = 0; while (c + 1 < 36 && LLb[c + 1] <= (uint32_t)v) c++; llc[v] = (uint8_t)c; }
-    for (int v = 0; v < 128; v++) { int c = 0; while (c + 1 < 53 && MLb[c + 1] <= (uint32_t)v + 3) c++; mlc[v] = (uint8_t)c; }
+    for (int v = 0; v < 64; v++) { int c = 0; while (c + 1 < 36 && ZSTD_LL_BASE[c + 1] <= (uint32_t)v) c++; llc[v] = (uint8_t)c; }
+    for (int v = 0; v < 128; v++) { int c = 0; while (c + 1 < 53 && ZSTD_ML_BASE[c + 1] <= (uint32_t)v + 3) c++; mlc[v] = (uint8_t)c; }
     cudaMemcpyToSymbol(c_ll_code, llc, sizeof(llc)); cudaMemcpyToSymbol(c_ml_code, mlc, sizeof(mlc));
-    cudaMemcpyToSymbol(c_ll_base, LLb, sizeof(LLb)); cudaMemcpyToSymbol(c_ml_base, MLb, sizeof(MLb));
-    cudaMemcpyToSymbol(c_ll_bits, LLx, sizeof(LLx)); cudaMemcpyToSymbol(c_ml_bits, MLx, sizeof(MLx));
+    cudaMemcpyToSymbol(c_ll_base, ZSTD_LL_BASE, sizeof(ZSTD_LL_BASE)); cudaMemcpyToSymbol(c_ml_base, ZSTD_ML_BASE, sizeof(ZSTD_ML_BASE));
+    cudaMemcpyToSymbol(c_ll_bits, ZSTD_LL_BITS, sizeof(ZSTD_LL_BITS)); cudaMemcpyToSymbol(c_ml_bits, ZSTD_ML_BITS, sizeof(ZSTD_ML_BITS));
     if (cudaGetLastError() != cudaSuccess) return ZMT_ST_CUDA;
     if (cudaDeviceSynchronize() != cudaSuccess) return ZMT_ST_CUDA;    // the kernels run on non-blocking streams: nothing else orders the table copies before them
     done[dev] = true;
@@ -672,26 +666,14 @@ static bool zmt_dbg_check(cudaStream_t st, const char* what)
     return true;
 }
 
-static std::mutex g_dev_mu;                     // guards the per-device lazy state below (contexts may run on several host threads)
-static inline int zmt_sm_count()
-{
-    static int n[64];
-    int dev = 0; cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 132;
-    std::lock_guard<std::mutex> g(g_dev_mu);
-    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 132; }
-    return n[dev];
-}
-
 // side stream + fork / join events, one set per (device, host thread): a set must not be shared by two launch sequences
 // that interleave, and every host thread enqueues its own sequences in order
 struct ZmtSide { cudaStream_t stream = nullptr; cudaEvent_t fork = nullptr, join = nullptr; bool ok = false; };
 static ZmtSide zmt_side_stream()
 {
-    static const bool off = getenv("ZSTDMT_B200_NO_SIDE_STREAM") != nullptr;
     thread_local ZmtSide side[64];
     int dev = 0;
-    if (off || cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ZmtSide();
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ZmtSide();
     ZmtSide& s = side[dev];
     if (!s.ok && !s.stream) {
         bool ok = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
@@ -710,142 +692,13 @@ extern "C" uint32_t zmt_chunk_count(uint64_t in_bytes, uint32_t chunk_size)
     return n > 0x7FFFFFFFull ? 0 : (uint32_t)n;
 }
 
-extern "C" size_t zmt_lz4c_workspace_bytes(uint32_t nchunks, uint32_t chunk_size)
-{
-    if (chunk_size == 0) return 0;
-    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
-    const uint64_t nblocks = (uint64_t)nchunks * bpc;
-    uint64_t sz = 0;
-    sz += nblocks * ZMT_LZ4_TMP_STRIDE;                  // per-block temp slots
-    sz += ((nblocks * 4 + 255) & ~255ull);               // blk_csize
-    sz += (((uint64_t)nchunks * 4 + 255) & ~255ull);     // chk
-    sz += ((((uint64_t)nchunks + 1) * 8 + 255) & ~255ull); // frame_size
-    return (size_t)sz + 1024;
-}
+static inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
+static inline uint32_t zmt_bpc(uint32_t chunk_size) { return (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK); }   // 64 KiB blocks per chunk
 
-extern "C" uint64_t zmt_lz4c_out_bound(uint32_t nchunks, uint32_t chunk_size)
-{
-    if (chunk_size == 0) return 0;
-    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
-    return (uint64_t)nchunks * ((uint64_t)chunk_size + 12 + 15 + 8 + 4 * bpc) + 256;
-}
-
-extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
-                                       uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
-{
-    cudaStream_t stream = (cudaStream_t)stream_;
-    if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
-    if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
-    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
-    if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
-    const uint32_t nblocks = nchunks * bpc;
-    uint8_t* w = (uint8_t*)d_work;
-    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
-    uint32_t* blk_csize = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint32_t* chk = (uint32_t*)w; w += (((uint64_t)nchunks * 4 + 255) & ~255ull);
-    uint64_t* frame_size = (uint64_t*)w;
-
-    // 2 CTAs x 16 warps per SM: throughput scales ~linearly with resident warps (DESIGN.md §3)
-    cudaFuncSetAttribute(lz4_blocks_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PipeSmem));
-    const uint32_t maxc = (uint32_t)(zmt_sm_count() * 2 * 8);
-    uint32_t gridc = nblocks < maxc ? nblocks : maxc;
-    static bool occ_shown = false;
-    if (!occ_shown && getenv("ZSTDMT_B200_SHOW_OCC")) {
-        int nb = 0; occ_shown = true;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, lz4_blocks_pipe_kernel, 2 * P_TEAM, sizeof(PipeSmem));
-        fprintf(stderr, "[zstdmt_b200] lz4_blocks_pipe_kernel: %d CTAs/SM, %zu B smem\n", nb, sizeof(PipeSmem));
-    }
-    const ZmtSide side = zmt_side_stream();
-    if (side.ok) cudaEventRecord(side.fork, stream);
-    { ZmtProfScope ps(ZMT_K_LZ4_COMPRESS, stream);
-    lz4_blocks_pipe_kernel<<<gridc, 2 * P_TEAM, sizeof(PipeSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u); }
-    zmt_dbg_check(stream, "lz4 block compressor");
-    // The content checksum only reads the input.  It cannot share an SM with the compressor (two compressor CTAs hold every
-    // register of an SM), but enqueued on a side stream BEHIND the compressor's launch it fills the SMs the compressor's last,
-    // ragged wave leaves idle, instead of starting when the last CTA has retired; the pack kernel joins both.
-    if (side.ok) {
-        cudaStreamWaitEvent(side.stream, side.fork, 0);          // fork = everything before the compressor launch (the input is ready)
-        { ZmtProfScope ps(ZMT_K_XXH32, side.stream);
-        xxh32_kernel<<<(nchunks + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, side.stream>>>((const uint8_t*)d_in, nullptr, nullptr, d_chunk_bytes, chunk_size, in_bytes, chk, nchunks); }
-        cudaEventRecord(side.join, side.stream);
-        cudaStreamWaitEvent(stream, side.join, 0);
-    } else {
-        ZmtProfScope ps(ZMT_K_XXH32, stream);
-        xxh32_kernel<<<(nchunks + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_in, nullptr, nullptr, d_chunk_bytes, chunk_size, in_bytes, chk, nchunks);
-    }
-    zmt_dbg_check(stream, "xxh32_kernel");
-    { ZmtProfScope ps(ZMT_K_LZ4_SIZES, stream);
-    lz4_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size); }
-    zmt_dbg_check(stream, "lz4_frame_sizes_kernel");
-    { ZmtProfScope ps(ZMT_K_SCAN, stream);
-    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks); }
-    zmt_dbg_check(stream, "scan_u64_kernel");
-    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
-    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
-    { ZmtProfScope ps(ZMT_K_LZ4_PACK, stream);
-    lz4_frame_pack_kernel<<<gridp, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, chk, d_frame_off, (uint8_t*)d_out, nblocks, 0x20u); }
-    zmt_dbg_check(stream, "lz4_frame_pack_kernel");
-    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
-}
-
-// ---------------------------------------------------------------- zstd compress
 #define ZSTD_MAX_GRID (132u * 2u * 4u)       // the workspace holds one ZScratch per CTA of the largest grid (H100 SXM: 132 SMs)
 static inline uint32_t zstd_grid(uint32_t nblocks) { uint32_t m = (uint32_t)(zmt_sm_count() * 2 * 4); if (m > ZSTD_MAX_GRID) m = ZSTD_MAX_GRID; return nblocks < m ? nblocks : m; }
 
-extern "C" size_t zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size)
-{
-    if (chunk_size == 0) return 0;
-    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
-    const uint64_t nblocks = (uint64_t)nchunks * bpc;
-    uint64_t sz = nblocks * ZMT_LZ4_TMP_STRIDE;
-    sz += ((nblocks * 4 + 255) & ~255ull);
-    sz += ((((uint64_t)nchunks + 1) * 8 + 255) & ~255ull);
-    sz += (uint64_t)(ZSTD_MAX_GRID + 8) * ((sizeof(ZScratch) + 255) & ~255ull);    // per-CTA scratch, sized for the largest grid we launch
-    return (size_t)sz + 1024;
-}
-
-extern "C" uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size)
-{
-    if (chunk_size == 0) return 0;
-    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
-    return (uint64_t)nchunks * ((uint64_t)chunk_size + 12 + 9 + 3 + 32 * bpc) + 256;     // <= 5 blocks x 3-byte headers per 64 KiB window
-}
-
-extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
-                                        uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
-{
-    cudaStream_t stream = (cudaStream_t)stream_;
-    if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
-    if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
-    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
-    if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
-    const int ti = zstd_tables_init(); if (ti != ZMT_ST_OK) return ti;
-    const uint32_t nblocks = nchunks * bpc;
-    uint8_t* w = (uint8_t*)d_work;
-    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
-    uint32_t* blk_csize = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint64_t* frame_size = (uint64_t*)w; w += ((((uint64_t)nchunks + 1) * 8 + 255) & ~255ull);
-    ZScratch* zsc = (ZScratch*)w;
-    static_assert(sizeof(ZScratch) % 8 == 0, "scratch stride");
-    cudaFuncSetAttribute(zstd_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZstdSmem));
-    const uint32_t gridc = zstd_grid(nblocks);
-    { ZmtProfScope ps(ZMT_K_ZSTD_COMPRESS, stream);
-    zstd_blocks_kernel<<<gridc, P_TEAM, sizeof(ZstdSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, nblocks, getenv("ZSTDMT_B200_NO_TMA") ? 1u : 0u, zsc); }
-    zmt_dbg_check(stream, "zstd_blocks_kernel");
-    zstd_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size);
-    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks);
-    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
-    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
-    { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
-    zstd_frame_pack_kernel<<<gridp, 256, 0, stream>>>(in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, d_frame_off, (uint8_t*)d_out, nblocks); }
-    zmt_dbg_check(stream, "zstd_frame_pack_kernel");
-    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
-}
-
-static inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
-
-// ---------------------------------------------------------------- zstd compress, levels 6-22 (zstd_lazy.cuh)
-// chunks per group: the per-position arrays (keys, values, prev, best: 16 bytes per position) cover one group at a time
+// chunks per group of the chain classes: the per-position arrays (keys, values, prev, best: 16 bytes per position) cover one group at a time
 static inline uint32_t zl_group_chunks(uint32_t nchunks, uint32_t chunk_size)
 {
     uint32_t g = ZL_GROUP_BYTES / chunk_size;
@@ -860,169 +713,266 @@ static size_t zl_sort_temp_bytes(uint32_t npos)
     return t;
 }
 
-extern "C" size_t zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+// ---------------------------------------------------------------- encoder arguments
+// A batch as every encoder entry point checks and sees it.  The chain classes (zstd levels 6-12, LZ4 levels 10-12) run
+// group by group: G chunks, at most npos_max positions (both 0 for the other classes).
+struct ZmtBatch {
+    const uint8_t* in; uint64_t in_bytes; uint32_t chunk_size; const uint32_t* chunk_bytes; uint32_t nchunks;
+    uint32_t bpc, nblocks;
+    uint32_t G; uint64_t npos_max;
+};
+static int zmt_batch(ZmtBatch& b, const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes, uint32_t nchunks, bool chain)
 {
-    const size_t base = zmt_zstdc_workspace_bytes(nchunks, chunk_size);
-    if (level < ZL_MIN_LEVEL || base == 0 || nchunks == 0) return base;
-    const uint64_t npos = (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size;
-    if (npos > 0xFFFFFFFFull) return 0;
-    return base + 4 * a256(npos * 4) + a256(zl_sort_temp_bytes((uint32_t)npos));
-}
-
-extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
-                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
-{
-    if (level < ZL_MIN_LEVEL) return zmt_zstd_compress_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, d_work, d_out, d_frame_off, stream_);
-    cudaStream_t stream = (cudaStream_t)stream_;
     if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
     if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
-    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
+    const uint32_t bpc = zmt_bpc(chunk_size);
     if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
-    const uint32_t G = zl_group_chunks(nchunks, chunk_size);
+    const uint32_t G = chain ? zl_group_chunks(nchunks, chunk_size) : 0;
     const uint64_t npos_max = (uint64_t)G * chunk_size;
     if (npos_max > 0xFFFFFFFFull) return ZMT_ST_BAD_ARG;
-    const int ti = zstd_tables_init(); if (ti != ZMT_ST_OK) return ti;
-    const uint32_t nblocks = nchunks * bpc;
-    uint8_t* w = (uint8_t*)d_work;
-    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
-    uint32_t* blk_csize = (uint32_t*)w; w += a256((uint64_t)nblocks * 4);
-    uint64_t* frame_size = (uint64_t*)w; w += a256(((uint64_t)nchunks + 1) * 8);
-    ZScratch* zsc = (ZScratch*)w;
-    w = (uint8_t*)d_work + zmt_zstdc_workspace_bytes(nchunks, chunk_size);        // the level-3 layout ends here
-    uint32_t* arr[4];
-    for (int k = 0; k < 4; k++) { arr[k] = (uint32_t*)w; w += a256(npos_max * 4); }
-    void* sort_tmp = w;
-    const size_t sort_cap = zl_sort_temp_bytes((uint32_t)npos_max);
-    const ZlParams P = zl_params(level);
-    const uint32_t W = zl_window(level);
-    cudaFuncSetAttribute(zstd_lazy_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZlSmem));
+    b = ZmtBatch{(const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, bpc, nchunks * bpc, G, npos_max};
+    return ZMT_ST_OK;
+}
 
-    for (uint32_t c0 = 0; c0 < nchunks; c0 += G) {
-        const uint32_t ng = nchunks - c0 < G ? nchunks - c0 : G;
-        uint64_t npos = (uint64_t)ng * chunk_size;
-        if (!d_chunk_bytes) { const uint64_t b = (uint64_t)c0 * chunk_size; npos = in_bytes > b ? (in_bytes - b < npos ? in_bytes - b : npos) : 0; }
-        cub::DoubleBuffer<uint32_t> K(arr[0], arr[1]), V(arr[2], arr[3]);
+// ---------------------------------------------------------------- encoder workspaces
+// One layout function per codec places the slots from `base`; with base == nullptr it only adds up their sizes.  The
+// *_workspace_bytes functions and the launchers both call it, so the size a caller allocates is the size the launcher carves.
+// npos: the positions of one group for the chain classes, 0 for the others.
+struct ZmtCarve {
+    uint8_t* base; uint64_t off;
+    template <class T> T* take(uint64_t bytes) { T* p = base ? (T*)(base + off) : nullptr; off += bytes; return p; }
+};
+
+// chain classes: keys, values, prev and best of one group, then the radix sort's temporary storage
+struct ZlChainWs { uint32_t* arr[4]; void* sort_tmp; size_t sort_cap; };
+static void zl_chain_layout(ZmtCarve& c, uint64_t npos, ZlChainWs& ch)
+{
+    for (int k = 0; k < 4; k++) ch.arr[k] = c.take<uint32_t>(a256(npos * 4));
+    ch.sort_cap = zl_sort_temp_bytes((uint32_t)npos);
+    ch.sort_tmp = c.take<void>(a256(ch.sort_cap));
+}
+
+struct Lz4Ws { uint8_t* tmp; uint32_t* blk_csize; uint32_t* chk; uint64_t* frame_size; ZlChainWs ch; };
+static uint64_t lz4_layout(uint8_t* base, uint64_t nchunks, uint64_t nblocks, uint64_t npos, Lz4Ws& w)
+{
+    ZmtCarve c{base, 0};
+    w = Lz4Ws{};
+    w.tmp = c.take<uint8_t>(nblocks * ZMT_LZ4_TMP_STRIDE);          // per-block temp slots
+    w.blk_csize = c.take<uint32_t>(a256(nblocks * 4));
+    w.chk = c.take<uint32_t>(a256(nchunks * 4));                    // content checksum per chunk
+    w.frame_size = c.take<uint64_t>(a256((nchunks + 1) * 8));
+    if (npos) zl_chain_layout(c, npos, w.ch);
+    return c.off + 1024;
+}
+
+struct ZstdWs { uint8_t* tmp; uint32_t* blk_csize; uint64_t* frame_size; ZScratch* zsc; ZlChainWs ch; };
+static uint64_t zstd_layout(uint8_t* base, uint64_t nchunks, uint64_t nblocks, uint64_t npos, ZstdWs& w)
+{
+    static_assert(sizeof(ZScratch) % 8 == 0, "scratch stride");
+    ZmtCarve c{base, 0};
+    w = ZstdWs{};
+    w.tmp = c.take<uint8_t>(nblocks * ZMT_LZ4_TMP_STRIDE);
+    w.blk_csize = c.take<uint32_t>(a256(nblocks * 4));
+    w.frame_size = c.take<uint64_t>(a256((nchunks + 1) * 8));
+    w.zsc = c.take<ZScratch>((uint64_t)(ZSTD_MAX_GRID + 8) * a256(sizeof(ZScratch)));    // per-CTA scratch, sized for the largest grid we launch
+    if (npos) zl_chain_layout(c, npos, w.ch);
+    return c.off + 1024;
+}
+
+extern "C" size_t zmt_lz4c_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+{
+    if (level < 1 || level > L4H_MAX_LEVEL || chunk_size == 0) return 0;
+    const uint64_t npos = level >= L4H_MIN_LEVEL ? (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size : 0;
+    if (npos > 0xFFFFFFFFull) return 0;
+    Lz4Ws w;
+    return (size_t)lz4_layout(nullptr, nchunks, (uint64_t)nchunks * zmt_bpc(chunk_size), npos, w);
+}
+extern "C" size_t zmt_lz4c_workspace_bytes(uint32_t nchunks, uint32_t chunk_size) { return zmt_lz4c_level_workspace_bytes(nchunks, chunk_size, 1); }
+
+extern "C" size_t zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+{
+    if (chunk_size == 0) return 0;
+    const uint64_t npos = level >= ZL_MIN_LEVEL ? (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size : 0;
+    if (npos > 0xFFFFFFFFull) return 0;
+    ZstdWs w;
+    return (size_t)zstd_layout(nullptr, nchunks, (uint64_t)nchunks * zmt_bpc(chunk_size), npos, w);
+}
+extern "C" size_t zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size) { return zmt_zstdc_level_workspace_bytes(nchunks, chunk_size, 3); }
+
+extern "C" uint64_t zmt_lz4c_out_bound(uint32_t nchunks, uint32_t chunk_size)
+{
+    if (chunk_size == 0) return 0;
+    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
+    return (uint64_t)nchunks * ((uint64_t)chunk_size + 12 + 15 + 8 + 4 * bpc) + 256;
+}
+
+extern "C" uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size)
+{
+    if (chunk_size == 0) return 0;
+    const uint64_t bpc = ((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK;
+    return (uint64_t)nchunks * ((uint64_t)chunk_size + 12 + 9 + 3 + 32 * bpc) + 256;     // <= 5 blocks x 3-byte headers per 64 KiB window
+}
+
+// ---------------------------------------------------------------- chain search (zstd_lazy.cuh), shared by both chain classes
+// One group of G chunks at a time: hash every position, radix-sort the (hash, position) pairs, link each position to the
+// previous one with its hash (prev[]), walk the chains into best[], then run the class's block kernel over the group's
+// blocks through blocks(c0, nblk, best).
+template <uint32_t BLK, uint32_t START, uint32_t END, class Blocks>
+static int zl_chain_groups(const ZmtBatch& b, const ZlChainWs& ch, uint32_t min_match, uint32_t depth, uint32_t window, cudaStream_t stream, Blocks blocks)
+{
+    for (uint32_t c0 = 0; c0 < b.nchunks; c0 += b.G) {
+        const uint32_t ng = b.nchunks - c0 < b.G ? b.nchunks - c0 : b.G;
+        uint64_t npos = (uint64_t)ng * b.chunk_size;
+        if (!b.chunk_bytes) { const uint64_t s = (uint64_t)c0 * b.chunk_size; npos = b.in_bytes > s ? (b.in_bytes - s < npos ? b.in_bytes - s : npos) : 0; }
+        cub::DoubleBuffer<uint32_t> K(ch.arr[0], ch.arr[1]), V(ch.arr[2], ch.arr[3]);
         if (npos) {
             const uint32_t np = (uint32_t)npos, g = (np + 255) / 256;
             { ZmtProfScope ps(ZMT_K_ZL_HASH, stream);
-            zstd_lazy_hash_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, K.Current(), V.Current()); }
+            zstd_lazy_hash_kernel<<<g, 256, 0, stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, c0, np, min_match, K.Current(), V.Current()); }
             zmt_dbg_check(stream, "zstd_lazy_hash_kernel");
             {
                 ZmtProfScope ps(ZMT_K_ZL_SORT, stream);
                 size_t tb = 0;
-                if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess || tb > sort_cap) return ZMT_ST_CUDA;
-                if (cub::DeviceRadixSort::SortPairs(sort_tmp, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
+                if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess || tb > ch.sort_cap) return ZMT_ST_CUDA;
+                if (cub::DeviceRadixSort::SortPairs(ch.sort_tmp, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
                 zstd_lazy_prev_kernel<<<g, 256, 0, stream>>>(K.Current(), V.Current(), np, V.Alternate());
             }
             zmt_dbg_check(stream, "zstd_lazy sort + prev");
             { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
-            zstd_lazy_search_kernel<ZL_BLOCK, 0, 0><<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, P.min_match, P.depth, W, V.Alternate(), K.Alternate()); }
+            zstd_lazy_search_kernel<BLK, START, END><<<g, 256, 0, stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, c0, np, min_match, depth, window,
+                                                                            V.Alternate(), K.Alternate()); }
             zmt_dbg_check(stream, "zstd_lazy_search_kernel");
         }
-        const uint32_t nwin = ng * bpc;
-        { ZmtProfScope ps(ZMT_K_ZL_BLOCKS, stream);
-        zstd_lazy_blocks_kernel<<<zstd_grid(nwin), 256, sizeof(ZlSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, c0, nwin, P.lazy,
-                                                                                   K.Alternate(), tmp, blk_csize, zsc); }
-        zmt_dbg_check(stream, "zstd_lazy_blocks_kernel");
+        blocks(c0, ng * b.bpc, K.Alternate());
     }
-    zstd_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size);
-    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks);
-    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
-    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
-    { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
-    zstd_frame_pack_kernel<<<gridp, 256, 0, stream>>>(in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, d_frame_off, (uint8_t*)d_out, nblocks); }
-    zmt_dbg_check(stream, "zstd_frame_pack_kernel");
-    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+    return ZMT_ST_OK;
 }
 
 // ---------------------------------------------------------------- LZ4 compress, levels 1-12 (levels 10-12: lz4_hc.cuh)
-// The level-1 layout, then the four per-position arrays (keys, values, prev, best) of one group and the sort's temp.
-extern "C" size_t zmt_lz4c_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level)
+// frame sizes -> frame offsets -> pack; indep: the FLG block-independence bit
+static int lz4_frame_tail(const ZmtBatch& b, const Lz4Ws& w, uint8_t* out, uint64_t* frame_off, uint32_t indep, cudaStream_t stream)
 {
-    if (level < 1 || level > L4H_MAX_LEVEL) return 0;
-    const size_t base = zmt_lz4c_workspace_bytes(nchunks, chunk_size);
-    if (level < L4H_MIN_LEVEL || base == 0 || nchunks == 0) return base;
-    const uint64_t npos = (uint64_t)zl_group_chunks(nchunks, chunk_size) * chunk_size;
-    if (npos > 0xFFFFFFFFull) return 0;
-    return base + 4 * a256(npos * 4) + a256(zl_sort_temp_bytes((uint32_t)npos));
+    { ZmtProfScope ps(ZMT_K_LZ4_SIZES, stream);
+    lz4_frame_sizes_kernel<<<(b.nchunks + 255) / 256, 256, 0, stream>>>(w.blk_csize, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, b.nchunks, w.frame_size); }
+    zmt_dbg_check(stream, "lz4_frame_sizes_kernel");
+    { ZmtProfScope ps(ZMT_K_SCAN, stream);
+    scan_u64_kernel<<<1, 1024, 0, stream>>>(w.frame_size, frame_off, b.nchunks); }
+    zmt_dbg_check(stream, "scan_u64_kernel");
+    const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
+    { ZmtProfScope ps(ZMT_K_LZ4_PACK, stream);
+    lz4_frame_pack_kernel<<<b.nblocks < maxp ? b.nblocks : maxp, 256, 0, stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, w.tmp, w.blk_csize, w.chk,
+                                                                                  frame_off, out, b.nblocks, indep); }
+    zmt_dbg_check(stream, "lz4_frame_pack_kernel");
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
 extern "C" int zmt_lz4_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
 {
     if (level < 1 || level > L4H_MAX_LEVEL) return ZMT_ST_BAD_ARG;
-    if (level < L4H_MIN_LEVEL) return zmt_lz4_compress_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, d_work, d_out, d_frame_off, stream_);
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (chunk_size == 0 || nchunks == 0) return ZMT_ST_BAD_ARG;
-    if (!d_chunk_bytes && nchunks != zmt_chunk_count(in_bytes, chunk_size)) return ZMT_ST_BAD_ARG;
-    const uint32_t bpc = (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK);
-    if ((uint64_t)nchunks * bpc > 0x7FFFFFFFull) return ZMT_ST_BAD_ARG;
-    const uint32_t G = zl_group_chunks(nchunks, chunk_size);
-    const uint64_t npos_max = (uint64_t)G * chunk_size;
-    if (npos_max > 0xFFFFFFFFull) return ZMT_ST_BAD_ARG;
-    const uint32_t nblocks = nchunks * bpc;
-    uint8_t* w = (uint8_t*)d_work;
-    uint8_t* tmp = w; w += (uint64_t)nblocks * ZMT_LZ4_TMP_STRIDE;
-    uint32_t* blk_csize = (uint32_t*)w; w += a256((uint64_t)nblocks * 4);
-    uint32_t* chk = (uint32_t*)w; w += a256((uint64_t)nchunks * 4);
-    uint64_t* frame_size = (uint64_t*)w;
-    w = (uint8_t*)d_work + zmt_lz4c_workspace_bytes(nchunks, chunk_size);         // the level-1 layout ends here
-    uint32_t* arr[4];
-    for (int k = 0; k < 4; k++) { arr[k] = (uint32_t*)w; w += a256(npos_max * 4); }
-    void* sort_tmp = w;
-    const size_t sort_cap = zl_sort_temp_bytes((uint32_t)npos_max);
-    const L4hParams P = l4h_params(level);
-    cudaFuncSetAttribute(lz4_hc_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4hSmem));
+    const bool hc = level >= L4H_MIN_LEVEL;
+    ZmtBatch b;
+    const int st = zmt_batch(b, d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, hc);
+    if (st != ZMT_ST_OK) return st;
+    Lz4Ws w;
+    lz4_layout((uint8_t*)d_work, nchunks, b.nblocks, b.npos_max, w);
 
-    // the content checksum only reads the input: on the side stream it runs beside the search
+    // The content checksum only reads the input: it runs on a side stream, forked before the first encoder launch and
+    // joined before the frame tail.  Levels 1-9 enqueue it BEHIND the compressor's launch: it cannot share an SM with the
+    // compressor (two compressor CTAs hold every register of an SM), but there it fills the SMs the compressor's last,
+    // ragged wave leaves idle, instead of starting when the last CTA has retired.  Levels 10-12 run it beside the search.
     const ZmtSide side = zmt_side_stream();
-    cudaStream_t xs = side.ok ? side.stream : stream;
-    if (side.ok) { cudaEventRecord(side.fork, stream); cudaStreamWaitEvent(side.stream, side.fork, 0); }
+    const cudaStream_t xs = side.ok ? side.stream : stream;
+    if (side.ok) cudaEventRecord(side.fork, stream);
+    if (!hc) {
+        // 2 CTAs x 16 warps per SM: throughput scales ~linearly with resident warps (DESIGN.md §3)
+        cudaFuncSetAttribute(lz4_blocks_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PipeSmem));
+        const uint32_t maxc = (uint32_t)(zmt_sm_count() * 2 * 8);
+        { ZmtProfScope ps(ZMT_K_LZ4_COMPRESS, stream);
+        lz4_blocks_pipe_kernel<<<b.nblocks < maxc ? b.nblocks : maxc, 2 * P_TEAM, sizeof(PipeSmem), stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc,
+                                                                                                             w.tmp, w.blk_csize, b.nblocks); }
+        zmt_dbg_check(stream, "lz4 block compressor");
+    }
+    if (side.ok) cudaStreamWaitEvent(side.stream, side.fork, 0);
     { ZmtProfScope ps(ZMT_K_XXH32, xs);
-    xxh32_kernel<<<(nchunks + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, xs>>>((const uint8_t*)d_in, nullptr, nullptr, d_chunk_bytes, chunk_size, in_bytes, chk, nchunks); }
+    xxh32_kernel<<<(nchunks + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, xs>>>(b.in, nullptr, nullptr, b.chunk_bytes, chunk_size, in_bytes, w.chk, nchunks); }
     if (side.ok) cudaEventRecord(side.join, side.stream);
     zmt_dbg_check(xs, "xxh32_kernel");
-
-    for (uint32_t c0 = 0; c0 < nchunks; c0 += G) {
-        const uint32_t ng = nchunks - c0 < G ? nchunks - c0 : G;
-        uint64_t npos = (uint64_t)ng * chunk_size;
-        if (!d_chunk_bytes) { const uint64_t b = (uint64_t)c0 * chunk_size; npos = in_bytes > b ? (in_bytes - b < npos ? in_bytes - b : npos) : 0; }
-        cub::DoubleBuffer<uint32_t> K(arr[0], arr[1]), V(arr[2], arr[3]);
-        if (npos) {
-            const uint32_t np = (uint32_t)npos, g = (np + 255) / 256;
-            { ZmtProfScope ps(ZMT_K_ZL_HASH, stream);
-            zstd_lazy_hash_kernel<<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np, L4H_MINMATCH, K.Current(), V.Current()); }
-            zmt_dbg_check(stream, "zstd_lazy_hash_kernel");
-            {
-                ZmtProfScope ps(ZMT_K_ZL_SORT, stream);
-                size_t tb = 0;
-                if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess || tb > sort_cap) return ZMT_ST_CUDA;
-                if (cub::DeviceRadixSort::SortPairs(sort_tmp, tb, K, V, (int)np, 0, ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
-                zstd_lazy_prev_kernel<<<g, 256, 0, stream>>>(K.Current(), V.Current(), np, V.Alternate());
-            }
-            zmt_dbg_check(stream, "zstd_lazy sort + prev");
-            { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
-            zstd_lazy_search_kernel<L4H_BLOCK, L4H_MFLIMIT, L4H_LASTLIT><<<g, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, c0, np,
-                                                                                              L4H_MINMATCH, P.depth, L4H_WINDOW, V.Alternate(), K.Alternate()); }
-            zmt_dbg_check(stream, "zstd_lazy_search_kernel");
-        }
-        const uint32_t nblk = ng * bpc;
-        { ZmtProfScope ps(ZMT_K_L4H_BLOCKS, stream);
-        lz4_hc_blocks_kernel<<<zstd_grid(nblk), 256, sizeof(L4hSmem), stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, c0, nblk, P.lazy,
-                                                                                 K.Alternate(), tmp, blk_csize); }
-        zmt_dbg_check(stream, "lz4_hc_blocks_kernel");
+    if (hc) {
+        const L4hParams P = l4h_params(level);
+        cudaFuncSetAttribute(lz4_hc_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4hSmem));
+        const int cs = zl_chain_groups<L4H_BLOCK, L4H_MFLIMIT, L4H_LASTLIT>(b, w.ch, L4H_MINMATCH, P.depth, L4H_WINDOW, stream,
+            [&](uint32_t c0, uint32_t nblk, const uint32_t* best) {
+                { ZmtProfScope ps(ZMT_K_L4H_BLOCKS, stream);
+                lz4_hc_blocks_kernel<<<zstd_grid(nblk), 256, sizeof(L4hSmem), stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, c0, nblk, P.lazy,
+                                                                                         best, w.tmp, w.blk_csize); }
+                zmt_dbg_check(stream, "lz4_hc_blocks_kernel");
+            });
+        if (cs != ZMT_ST_OK) return cs;
     }
     if (side.ok) cudaStreamWaitEvent(stream, side.join, 0);
-    { ZmtProfScope ps(ZMT_K_LZ4_SIZES, stream);
-    lz4_frame_sizes_kernel<<<(nchunks + 255) / 256, 256, 0, stream>>>(blk_csize, in_bytes, chunk_size, d_chunk_bytes, bpc, nchunks, frame_size); }
-    { ZmtProfScope ps(ZMT_K_SCAN, stream);
-    scan_u64_kernel<<<1, 1024, 0, stream>>>(frame_size, d_frame_off, nchunks); }
+    return lz4_frame_tail(b, w, (uint8_t*)d_out, d_frame_off, hc ? 0u : 0x20u, stream);
+}
+
+extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                       uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    return zmt_lz4_compress_level_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, 1, d_work, d_out, d_frame_off, stream_);
+}
+
+// ---------------------------------------------------------------- zstd compress, levels 1-22 (levels 6-22: zstd_lazy.cuh)
+// frame sizes -> frame offsets -> pack
+static int zstd_frame_tail(const ZmtBatch& b, const ZstdWs& w, uint8_t* out, uint64_t* frame_off, cudaStream_t stream)
+{
+    zstd_frame_sizes_kernel<<<(b.nchunks + 255) / 256, 256, 0, stream>>>(w.blk_csize, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, b.nchunks, w.frame_size);
+    zmt_dbg_check(stream, "zstd_frame_sizes_kernel");
+    scan_u64_kernel<<<1, 1024, 0, stream>>>(w.frame_size, frame_off, b.nchunks);
+    zmt_dbg_check(stream, "scan_u64_kernel");
     const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
-    const uint32_t gridp = nblocks < maxp ? nblocks : maxp;
-    { ZmtProfScope ps(ZMT_K_LZ4_PACK, stream);
-    lz4_frame_pack_kernel<<<gridp, 256, 0, stream>>>((const uint8_t*)d_in, in_bytes, chunk_size, d_chunk_bytes, bpc, tmp, blk_csize, chk, d_frame_off, (uint8_t*)d_out, nblocks, 0u); }
-    zmt_dbg_check(stream, "lz4_frame_pack_kernel");
+    { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
+    zstd_frame_pack_kernel<<<b.nblocks < maxp ? b.nblocks : maxp, 256, 0, stream>>>(b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, w.tmp, w.blk_csize, frame_off,
+                                                                                   out, b.nblocks); }
+    zmt_dbg_check(stream, "zstd_frame_pack_kernel");
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const bool chain = level >= ZL_MIN_LEVEL;
+    ZmtBatch b;
+    int st = zmt_batch(b, d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, chain);
+    if (st == ZMT_ST_OK) st = zstd_tables_init();
+    if (st != ZMT_ST_OK) return st;
+    ZstdWs w;
+    zstd_layout((uint8_t*)d_work, nchunks, b.nblocks, b.npos_max, w);
+    if (!chain) {
+        cudaFuncSetAttribute(zstd_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZstdSmem));
+        { ZmtProfScope ps(ZMT_K_ZSTD_COMPRESS, stream);
+        zstd_blocks_kernel<<<zstd_grid(b.nblocks), P_TEAM, sizeof(ZstdSmem), stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, w.tmp, w.blk_csize,
+                                                                                       b.nblocks, w.zsc); }
+        zmt_dbg_check(stream, "zstd_blocks_kernel");
+    } else {
+        const ZlParams P = zl_params(level);
+        cudaFuncSetAttribute(zstd_lazy_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZlSmem));
+        st = zl_chain_groups<ZL_BLOCK, 0, 0>(b, w.ch, P.min_match, P.depth, zl_window(level), stream,
+            [&](uint32_t c0, uint32_t nwin, const uint32_t* best) {
+                { ZmtProfScope ps(ZMT_K_ZL_BLOCKS, stream);
+                zstd_lazy_blocks_kernel<<<zstd_grid(nwin), 256, sizeof(ZlSmem), stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, c0, nwin, P.lazy,
+                                                                                           best, w.tmp, w.blk_csize, w.zsc); }
+                zmt_dbg_check(stream, "zstd_lazy_blocks_kernel");
+            });
+        if (st != ZMT_ST_OK) return st;
+    }
+    return zstd_frame_tail(b, w, (uint8_t*)d_out, d_frame_off, stream);
+}
+
+extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                        uint32_t nchunks, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    return zmt_zstd_compress_level_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, 3, d_work, d_out, d_frame_off, stream_);
 }
 
 // workspace: stored[] | computed[] | needs_seq[] | ticket, any-FLG.BC flag | slot counts | first_slot | block table | progress | match records

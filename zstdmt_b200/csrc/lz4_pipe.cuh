@@ -91,9 +91,9 @@ __device__ __forceinline__ uint32_t team_exscan_pieces(uint32_t v, uint32_t m, u
 // Stages the n bytes at src into St.in (TMA bulk copy when 16-byte aligned), zeroes the pads and the hash table.  The
 // caller has a CTA barrier between the previous block's last reader and this call.
 template <uint32_t NT>
-__device__ __forceinline__ void lz_stage(LzStage& St, uint32_t* tab, uint64_t* mbar, const uint8_t* src, uint32_t n, uint32_t flags, uint32_t tid)
+__device__ __forceinline__ void lz_stage(LzStage& St, uint32_t* tab, uint64_t* mbar, const uint8_t* src, uint32_t n, uint32_t tid)
 {
-    const uint32_t nb16 = ((((uintptr_t)src & 15) == 0) && !(flags & 1)) ? (n & ~15u) : 0;
+    const uint32_t nb16 = (((uintptr_t)src & 15) == 0) ? (n & ~15u) : 0;
     if (tid == 0 && nb16) mbar_init(mbar, 1);
     CTA_SYNC();
     if (tid == 0 && nb16) { mbar_expect_tx(mbar, nb16); bulk_g2s(St.in, src, nb16, mbar); }
@@ -358,7 +358,7 @@ static_assert(sizeof(PipeSmem) + 1024 <= (228 * 1024) / 2, "two CTAs per SM");
 
 __global__ void __launch_bounds__(2 * P_TEAM, 2)
 lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
-                       uint32_t bpc, uint8_t* __restrict__ tmp, uint32_t* __restrict__ blk_csize, uint32_t nblocks, uint32_t flags)
+                       uint32_t bpc, uint8_t* __restrict__ tmp, uint32_t* __restrict__ blk_csize, uint32_t nblocks)
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     PipeSmem& S = *reinterpret_cast<PipeSmem*>(smem_raw);
@@ -378,7 +378,7 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
 
         CTA_SYNC();                                       // previous block fully consumed
         if (tid == 0) { S.nlong = 0; S.a_any[0] = 0; S.a_any[1] = 0; }
-        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, flags, tid);
+        lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, tid);
 
         const uint32_t limit = n >= 5 ? n - 5 : 0;        // matches end at or before n-5
         const uint32_t ntiles = (n + C_TILE - 1) / C_TILE;

@@ -33,6 +33,7 @@
 #include <mutex>
 #include <vector>
 #include "common.cuh"
+#include "host_common.h"
 #include "zmt_dev.h"
 
 extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
@@ -1314,35 +1315,18 @@ static void zd_build_dtable(ZFseDTable& T, const int16_t* norm, int nsym, int lo
     }
 }
 
-static int zd_sm_count()
-{
-    static std::mutex mu; static int n[64];
-    int dev = 0; cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 132;
-    std::lock_guard<std::mutex> g(mu);
-    if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 132; }
-    return n[dev];
-}
-
 static int zd_tables_init()
 {
     static std::mutex mu; static bool done[64];   // devices whose __constant__ copies are loaded (contexts may run on several host threads)
     int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ZMT_ST_CUDA;
     std::lock_guard<std::mutex> guard(mu);
     if (done[dev]) return ZMT_ST_OK;
-    static const int16_t LLn[36] = { 4,3,2,2,2,2,2,2,2,2,2,2,2,1,1,1,2,2,2,2,2,2,2,2,2,3,2,1,1,1,1,1,-1,-1,-1,-1 };
-    static const int16_t MLn[53] = { 1,4,3,2,2,2,2,2,2,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,-1,-1,-1,-1,-1,-1,-1 };
-    static const int16_t OFn[29] = { 1,1,1,1,1,1,2,2,2,1,1,1,1,1,1,1,1,1,1,1,1,1,1,1,-1,-1,-1,-1,-1 };
-    static const uint32_t LLb[36] = { 0,1,2,3,4,5,6,7,8,9,10,11,12,13,14,15,16,18,20,22,24,28,32,40,48,64,128,256,512,1024,2048,4096,8192,16384,32768,65536 };
-    static const uint8_t  LLx[36] = { 0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,1,1,1,1,2,2,3,3,4,6,7,8,9,10,11,12,13,14,15,16 };
-    static const uint32_t MLb[53] = { 3,4,5,6,7,8,9,10,11,12,13,14,15,16,17,18,19,20,21,22,23,24,25,26,27,28,29,30,31,32,33,34,35,37,39,41,43,47,51,59,67,83,99,131,259,515,1027,2051,4099,8195,16387,32771,65539 };
-    static const uint8_t  MLx[53] = { 0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,1,1,1,1,2,2,3,3,4,4,5,7,8,9,10,11,12,13,14,15,16 };
     ZFseDTable t;
-    zd_build_dtable(t, LLn, 36, 6); if (cudaMemcpyToSymbol(d_fse_ll, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
-    zd_build_dtable(t, OFn, 29, 5); if (cudaMemcpyToSymbol(d_fse_of, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
-    zd_build_dtable(t, MLn, 53, 6); if (cudaMemcpyToSymbol(d_fse_ml, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
-    cudaMemcpyToSymbol(d_ll_base, LLb, sizeof(LLb)); cudaMemcpyToSymbol(d_ml_base, MLb, sizeof(MLb));
-    cudaMemcpyToSymbol(d_ll_bits, LLx, sizeof(LLx)); cudaMemcpyToSymbol(d_ml_bits, MLx, sizeof(MLx));
+    zd_build_dtable(t, ZSTD_LL_NORM, 36, 6); if (cudaMemcpyToSymbol(d_fse_ll, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    zd_build_dtable(t, ZSTD_OF_NORM, 29, 5); if (cudaMemcpyToSymbol(d_fse_of, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    zd_build_dtable(t, ZSTD_ML_NORM, 53, 6); if (cudaMemcpyToSymbol(d_fse_ml, &t, sizeof(t)) != cudaSuccess) return ZMT_ST_CUDA;
+    cudaMemcpyToSymbol(d_ll_base, ZSTD_LL_BASE, sizeof(ZSTD_LL_BASE)); cudaMemcpyToSymbol(d_ml_base, ZSTD_ML_BASE, sizeof(ZSTD_ML_BASE));
+    cudaMemcpyToSymbol(d_ll_bits, ZSTD_LL_BITS, sizeof(ZSTD_LL_BITS)); cudaMemcpyToSymbol(d_ml_bits, ZSTD_ML_BITS, sizeof(ZSTD_ML_BITS));
     if (cudaGetLastError() != cudaSuccess) return ZMT_ST_CUDA;
     if (cudaDeviceSynchronize() != cudaSuccess) return ZMT_ST_CUDA;    // the kernels run on non-blocking streams: nothing else orders the table copies before them
     done[dev] = true;
@@ -1516,7 +1500,7 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
     zstd_offsets_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>((const ZBlk*)d_blocks, nblocks, d_frame_first_blk, regen, blk_out, d_out_off, d_expect,
                                                                    (unsigned long long*)d_out_size, d_status, nframes);
     if (nblocks) {
-        const uint32_t gmax = (uint32_t)(zd_sm_count() * (2048 / (32 * ZX_WARPS)));
+        const uint32_t gmax = (uint32_t)(zmt_sm_count() * (2048 / (32 * ZX_WARPS)));
         const uint32_t gneed = (nblocks + ZX_WARPS - 1) / ZX_WARPS;
         cudaMemsetAsync(xticket, 0, 8, stream);
         zstd_ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, xwbase);
