@@ -2,10 +2,6 @@
 more, 3-byte sequence counts, repeat offsets, inherited and RLE tables, every literal-section form, matches hundreds of
 blocks back; through each of the three entropy routes, through the callback API, with content checksums, and in
 batches larger than one ticket window (both decoders)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -86,26 +82,6 @@ def test_gpu_decodes_all_edge_cases_in_one_batch_through_three_routes(batch):
     assert routes["far"] == routes["tables"] == routes["literals"] == routes["dense"] == "dep"
     assert routes["far_predef"] == routes["reference_ultra"] == "self"
     assert routes["reps_predef"] == "runtime"
-
-
-def test_gpu_batch_without_fast_entropy_kernels_matches(batch, tmp_path):
-    """(c) The same batch with ZSTDMT_B200_NO_FAST_ENTROPY=1 (warp-per-block and frame-sequential kernels only; the knob is
-    read once per process, so a child process decodes it): the same bytes and the same per-frame status."""
-    srcs, frames, dec, out, st, sz = batch
-    fb = framed(frames)
-    inp, outp, stp = tmp_path / "in.bin", tmp_path / "out.npy", tmp_path / "st.npy"
-    fb.tofile(inp)
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = ("import sys; sys.path.insert(0, %r)\n"
-            "import numpy as np, torch, zstdmt_b200 as z\n"
-            "fb = np.fromfile(sys.argv[1], dtype=np.uint8)\n"
-            "dec = z.ZstdDeviceDecompressor(fb)\n"
-            "out, st = dec.run(torch.from_numpy(fb).cuda()); torch.cuda.synchronize()\n"
-            "np.save(sys.argv[2], out.cpu().numpy()); np.save(sys.argv[3], st.cpu().numpy())\n" % root)
-    env = dict(os.environ, ZSTDMT_B200_NO_FAST_ENTROPY="1")
-    subprocess.run([sys.executable, "-c", code, str(inp), str(outp), str(stp)], env=env, timeout=600, check=True)
-    assert np.array_equal(np.load(stp)[: len(frames)], st)
-    assert np.array_equal(np.load(outp), out)
 
 
 @pytest.mark.parametrize("name", CASES)

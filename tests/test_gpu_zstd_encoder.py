@@ -86,7 +86,7 @@ def check(torch, src, chunk=1 << 20, chunk_bytes=None):
 
 
 def check_modes(tr):
-    """(c) the mode rules of the default build (Z_ALWAYS_FSE_WEIGHTS=0)."""
+    """(c) the mode rules of the encoder."""
     typ, last, regen, bsize = tr.col("type"), tr.col("last"), tr.col("regen"), tr.col("bsize")
     assert set(typ.tolist()) <= {0, 2}                              # raw or compressed blocks only
     assert list(last) == [0] * (len(last) - 1) + [1]                 # only the last block is flagged last

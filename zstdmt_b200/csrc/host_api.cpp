@@ -27,27 +27,12 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <functional>
 #include <mutex>
 #include <thread>
 #include <vector>
+#include "host_common.h"
 #include "zmt_dev.h"
-
-extern "C" {
-size_t   zmt_zstdc_workspace_bytes(uint32_t nchunks, uint32_t chunk_size);
-uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size);
-int      zmt_zstd_compress_device(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, void*, void*, uint64_t*, void*);
-size_t   zmt_zstdc_level_workspace_bytes(uint32_t nchunks, uint32_t chunk_size, int level);
-int      zmt_zstd_compress_level_device(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, int, void*, void*, uint64_t*, void*);
-size_t   zmt_zstd_blk_desc_bytes(void);
-int      zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out, uint32_t* nblocks_io,
-                                  uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq);
-int      zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out, uint32_t* nblocks_io,
-                                   uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed);
-size_t   zmt_zstdd_workspace_bytes(uint32_t nframes, uint32_t nblocks, uint64_t scratch_bytes);
-int      zmt_zstd_decompress_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk, const uint64_t* d_expect,
-                                    const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status,
-                                    void* d_work, void* stream);
-}
 
 namespace {
 
@@ -187,11 +172,9 @@ struct DeviceRestore {
 };
 
 // ------------------------------------------------------------------ optional stage timing (ZSTDMT_B200_TRACE=1)
-struct StageClock {
-    double cb = 0, wait = 0, gpu = 0;       // seconds: inside callbacks / waiting for a slot or queue / CUDA sync + copies
-    static double now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-};
-inline bool trace_on() { static int on = -1; if (on < 0) on = getenv("ZSTDMT_B200_TRACE") ? 1 : 0; return on == 1; }
+inline bool trace_on() { static const bool on = getenv("ZSTDMT_B200_TRACE") != nullptr; return on; }
+// seconds on a steady clock when tracing, else 0 (the clock is not read)
+inline double trace_now() { return trace_on() ? std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count() : 0; }
 
 // ------------------------------------------------------------------ device codec table
 // the workspace and the compress call follow the context's level (both codecs have more than one encoder)
@@ -201,11 +184,11 @@ struct CodecOps {
     int      (*compress)(const void*, uint64_t, uint32_t, const uint32_t*, uint32_t, int level, void*, void*, uint64_t*, void*);
 };
 
-const CodecOps* codec_ops(int codec)
+const CodecOps& codec_ops(int codec)
 {
     static const CodecOps lz4 = { zmt_lz4c_level_workspace_bytes, zmt_lz4c_out_bound, zmt_lz4_compress_level_device };
     static const CodecOps zstd = { zmt_zstdc_level_workspace_bytes, zmt_zstdc_out_bound, zmt_zstd_compress_level_device };
-    return codec == CODEC_LZ4 ? &lz4 : &zstd;
+    return codec == CODEC_LZ4 ? lz4 : zstd;
 }
 
 // ------------------------------------------------------------------ staging slots
@@ -226,16 +209,26 @@ struct Slot {
     size_t in_used = 0, out_used = 0;
     int state = 0;               // 0 free, 1 filled, 2 submitted
     bool ok = false;
-    bool host_alias = false;     // h_in / h_out are borrowed from another slot of the same context (never pooled, never freed here)
+    bool host_alias = false;     // h_in / h_out are borrowed from another slot of the same context (never freed here)
 };
 
-// table layout (entries = tab_cap):  u64 a[cap+1] | u64 b[cap+1] | u64 c[cap+1] | u64 f[cap+1] | u32 d[cap] | u32 e[cap] | u32 g[cap+1]
-struct Tables { uint64_t *a, *b, *c, *f; uint32_t *d, *e, *g; };
+// Per-chunk / per-frame tables of a batch (entries = tab_cap).  Layout:
+//   u64 frame_off[cap+1] | u64 out_off[cap+1] | u64 out_size[cap+1] | u64 expect[cap+1] | u32 per_frame[cap] | u32 status[cap] | u32 first_blk[cap+1]
+struct Tables {
+    uint64_t* frame_off;         // compress: where each frame starts in the output (+ total); decompress: where its 12-byte header starts in the input
+    uint64_t* out_off;           // decompress: where each frame's content goes (+ total)
+    uint64_t* out_size;          // decompress: bytes each frame decoded to
+    uint64_t* expect;            // zstd decompress: content size from the frame header, ~0 when the header has none
+    uint32_t* per_frame;         // compress: bytes in the chunk; lz4 decompress: payload bytes of the frame;
+                                 // zstd decompress: frame flags of the host scan (sequential pass, checksum, no size)
+    uint32_t* status;            // decompress: ZMT_ST_* per frame
+    uint32_t* first_blk;         // zstd decompress: the frame's first block descriptor (+ total)
+};
 inline size_t tables_bytes(size_t cap) { return 4 * (cap + 1) * 8 + 2 * cap * 4 + (cap + 1) * 4 + 64; }
 inline Tables tables_at(uint8_t* base, size_t cap)
 {
-    Tables t; t.a = (uint64_t*)base; t.b = t.a + cap + 1; t.c = t.b + cap + 1; t.f = t.c + cap + 1;
-    t.d = (uint32_t*)(t.f + cap + 1); t.e = t.d + cap; t.g = t.e + cap; return t;
+    Tables t; t.frame_off = (uint64_t*)base; t.out_off = t.frame_off + cap + 1; t.out_size = t.out_off + cap + 1; t.expect = t.out_size + cap + 1;
+    t.per_frame = (uint32_t*)(t.expect + cap + 1); t.status = t.per_frame + cap; t.first_blk = t.status + cap; return t;
 }
 
 // lz4 decode block table capacity of a slot: every frame owns max(1, ceil(out / 64 KiB)) slots
@@ -260,28 +253,6 @@ void slot_free_raw(Slot& s)
     s = Slot();
 }
 
-bool slot_alloc_raw(Slot& s, int dev, size_t in_cap, size_t out_cap, size_t work_cap, size_t tab_cap)
-{
-    s.dev = dev;
-    if (cudaSetDevice(dev) != cudaSuccess) return false;
-    const ScopedAffinity bind(device_local_cpus(dev));     // first touch of the pinned rings happens on the GPU's node
-    bool ok = true;
-    ok = ok && cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming) == cudaSuccess;
-    for (int k = 0; k < 2; k++) ok = ok && cudaEventCreateWithFlags(&s.evp[k], cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void**)&s.h_in, in_cap + 64, cudaHostAllocPortable) == cudaSuccess;
-    ok = ok && cudaHostAlloc((void**)&s.h_out, out_cap + 64, cudaHostAllocPortable) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_in, in_cap + 256) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_out, out_cap + 256) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_work, work_cap + 256) == cudaSuccess;
-    s.tab_bytes = tables_bytes(tab_cap);
-    ok = ok && cudaHostAlloc((void**)&s.h_tab, s.tab_bytes, cudaHostAllocPortable) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_tab, s.tab_bytes) == cudaSuccess;
-    s.in_cap = in_cap; s.out_cap = out_cap; s.work_cap = work_cap; s.tab_cap = tab_cap; s.ok = ok;
-    if (!ok) { cudaGetLastError(); slot_free_raw(s); }
-    return ok;
-}
-
 // Process-wide pool of staging slots: pinned allocations cost ~0.1 s per context otherwise (the reference's
 // malloc'd buffers are free by comparison).  Slots go back to the pool when a context is freed and are
 // reused by the next context that needs the same device and no larger capacities.
@@ -289,74 +260,57 @@ std::mutex g_pool_mu;
 std::vector<Slot> g_pool;
 const size_t kPoolMax = 16;
 
-bool slot_alloc(Slot& s, int dev, size_t in_cap, size_t out_cap, size_t work_cap, size_t tab_cap)
+// host_owner: the slot whose pinned staging buffers this one borrows (a call over more devices than it keeps batches in
+// flight: the host ring stays 4 x 8 MiB — cache-resident for the callbacks' memcpy — while every device has its own
+// device-side buffers); nullptr: the slot gets pinned buffers of its own.
+bool slot_alloc(Slot& s, int dev, size_t in_cap, size_t out_cap, size_t work_cap, size_t tab_cap, const Slot* host_owner)
 {
+    bool ok = false;
     {
-        std::lock_guard<std::mutex> g(g_pool_mu);
-        for (size_t i = 0; i < g_pool.size(); i++) {
+        std::lock_guard<std::mutex> g(g_pool_mu);                       // a pooled slot of a previous call (device-only for a borrower)
+        for (size_t i = 0; i < g_pool.size() && !ok; i++) {
             Slot& c = g_pool[i];
-            if (c.h_in && c.dev == dev && c.in_cap >= in_cap && c.out_cap >= out_cap && c.work_cap >= work_cap && c.tab_cap == tab_cap) {
+            if ((c.h_in == nullptr) == (host_owner != nullptr) && c.dev == dev && c.in_cap >= in_cap && c.out_cap >= out_cap &&
+                c.work_cap >= work_cap && c.tab_cap == tab_cap) {
                 s = c; g_pool.erase(g_pool.begin() + (long)i);
                 s.state = 0; s.n = 0; s.in_used = s.out_used = 0;
-                return true;
+                ok = true;
             }
         }
     }
-    return slot_alloc_raw(s, dev, in_cap, out_cap, work_cap, tab_cap);
-}
-
-// A slot whose pinned staging buffers are those of `owner` (a call over more devices than it keeps batches in flight: the
-// host ring stays 4 x 8 MiB — cache-resident for the callbacks' memcpy — while every device has its own device-side buffers).
-bool slot_alloc_alias(Slot& s, const Slot& owner, int dev, size_t in_cap, size_t out_cap, size_t work_cap, size_t tab_cap)
-{
-    {
-        std::lock_guard<std::mutex> g(g_pool_mu);                       // a pooled device-only slot of a previous call
-        for (size_t i = 0; i < g_pool.size(); i++) {
-            Slot& c = g_pool[i];
-            if (!c.h_in && c.dev == dev && c.in_cap >= in_cap && c.out_cap >= out_cap && c.work_cap >= work_cap && c.tab_cap == tab_cap) {
-                s = c; g_pool.erase(g_pool.begin() + (long)i);
-                s.state = 0; s.n = 0; s.in_used = s.out_used = 0;
-                s.h_in = owner.h_in; s.h_out = owner.h_out; s.host_alias = true;
-                return true;
-            }
+    if (!ok) {
+        s.dev = dev;
+        if (cudaSetDevice(dev) != cudaSuccess) return false;
+        const ScopedAffinity bind(device_local_cpus(dev));     // first touch of the pinned buffers happens on the GPU's node
+        ok = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
+        ok = ok && cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming) == cudaSuccess;
+        for (int k = 0; k < 2; k++) ok = ok && cudaEventCreateWithFlags(&s.evp[k], cudaEventDisableTiming) == cudaSuccess;
+        if (!host_owner) {
+            ok = ok && cudaHostAlloc((void**)&s.h_in, in_cap + 64, cudaHostAllocPortable) == cudaSuccess;
+            ok = ok && cudaHostAlloc((void**)&s.h_out, out_cap + 64, cudaHostAllocPortable) == cudaSuccess;
         }
+        ok = ok && cudaMalloc((void**)&s.d_in, in_cap + 256) == cudaSuccess;
+        ok = ok && cudaMalloc((void**)&s.d_out, out_cap + 256) == cudaSuccess;
+        ok = ok && cudaMalloc((void**)&s.d_work, work_cap + 256) == cudaSuccess;
+        s.tab_bytes = tables_bytes(tab_cap);
+        ok = ok && cudaHostAlloc((void**)&s.h_tab, s.tab_bytes, cudaHostAllocPortable) == cudaSuccess;
+        ok = ok && cudaMalloc((void**)&s.d_tab, s.tab_bytes) == cudaSuccess;
+        s.in_cap = in_cap; s.out_cap = out_cap; s.work_cap = work_cap; s.tab_cap = tab_cap; s.ok = ok;
+        if (!ok) { cudaGetLastError(); slot_free_raw(s); return false; }
     }
-    s.dev = dev;
-    if (cudaSetDevice(dev) != cudaSuccess) return false;
-    bool ok = true;
-    ok = ok && cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming) == cudaSuccess;
-    for (int k = 0; k < 2; k++) ok = ok && cudaEventCreateWithFlags(&s.evp[k], cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_in, in_cap + 256) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_out, out_cap + 256) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_work, work_cap + 256) == cudaSuccess;
-    s.tab_bytes = tables_bytes(tab_cap);
-    ok = ok && cudaHostAlloc((void**)&s.h_tab, s.tab_bytes, cudaHostAllocPortable) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&s.d_tab, s.tab_bytes) == cudaSuccess;
-    s.in_cap = in_cap; s.out_cap = out_cap; s.work_cap = work_cap; s.tab_cap = tab_cap; s.ok = ok;
-    if (!ok) { cudaGetLastError(); slot_free_raw(s); return false; }
-    s.h_in = owner.h_in; s.h_out = owner.h_out; s.host_alias = true;
+    if (host_owner) { s.h_in = host_owner->h_in; s.h_out = host_owner->h_out; s.host_alias = true; }
     return true;
 }
 
 void slot_free(Slot& s)
 {
-    if (s.host_alias) {
-        // hand the borrowed buffers back (they belong to the owner slot); the device side goes to the pool as a device-only slot
-        s.h_in = nullptr; s.h_out = nullptr; s.host_alias = false;
-        if (s.ok) {
-            cudaSetDevice(s.dev);
-            if (s.stream) cudaStreamSynchronize(s.stream);
-            std::lock_guard<std::mutex> g(g_pool_mu);
-            if (g_pool.size() < kPoolMax && !getenv("ZSTDMT_B200_NO_POOL")) { g_pool.push_back(s); s = Slot(); return; }
-        }
-        slot_free_raw(s); return;
-    }
+    // borrowed buffers belong to the owner slot: the device side goes to the pool as a device-only slot
+    if (s.host_alias) { s.h_in = nullptr; s.h_out = nullptr; s.host_alias = false; }
     if (s.ok) {
         cudaSetDevice(s.dev);
         if (s.stream) cudaStreamSynchronize(s.stream);
         std::lock_guard<std::mutex> g(g_pool_mu);
-        if (g_pool.size() < kPoolMax && !getenv("ZSTDMT_B200_NO_POOL")) { g_pool.push_back(s); s = Slot(); return; }
+        if (g_pool.size() < kPoolMax) { g_pool.push_back(s); s = Slot(); return; }
     }
     slot_free_raw(s);
 }
@@ -390,7 +344,6 @@ struct Ctx {
     int codec = 0, level = 0, threads = 0;
     size_t inputsize = 0;
     size_t insize = 0, outsize = 0, frames = 0, curframe = 0;
-    bool is_comp = false;
     std::vector<int> devs;
     Pipe pipe;
     size_t lib_errcode = 0;
@@ -404,13 +357,118 @@ void ctx_release_slots(Ctx* c)
     c->pipe.slots.clear();
 }
 
+// a frame's ZMT_ST_* -> the library error of the call: a cut or overlong frame is the frame's fault, the rest the codec's
+inline size_t status_error(const ErrCodes& E, uint32_t st) { return st == ZMT_ST_TRUNCATED || st == ZMT_ST_TRAILING ? E.frame_decompress : E.library; }
+
+// ------------------------------------------------------------------ the pipeline of one call
+// reader thread  : fill    — fn_read into the free slot, in sequence order (pt_read / the read section of pt_compress)
+// calling thread : submit  — H2D, the device entry point, D2H of the tables, s.ev recorded
+// writer thread  : drain   — after s.ev: fn_write the slot's frames in order (pt_write)
+// A slot goes 0 free -> 1 filled -> 2 submitted -> 0.  Batch q + in_flight is filled only once batch q has been written
+// (slots beyond the first in_flight share their pinned buffers).  The first error any stage raises with P.fail() stops all
+// three; the call returns it.
+struct PipeOps {
+    std::function<bool(Slot&)> fill;     // false: no batch (end of input, or after P.fail)
+    std::function<int(Slot&)>  submit;   // ZMT_ST_*
+    std::function<bool(Slot&)> drain;    // false after P.fail
+    const char* name = "";               // ZSTDMT_B200_TRACE line
+    size_t batch_bytes = 0;
+    const double* scan = nullptr;        // decompress: the reader's time in the frame scan (traced only)
+};
+
+size_t run_pipeline(Ctx* c, size_t in_flight, const PipeOps& ops)
+{
+    const ErrCodes& E = *c->E;
+    Pipe& P = c->pipe;
+    const size_t N = P.slots.size();
+    P.fill_seq = P.submit_seq = P.write_seq = 0; P.reader_done = false; P.error = 0;
+    for (auto& s : P.slots) s.state = 0;
+    struct { double wait = 0, work = 0, gpu = 0; } rd, sb, wr;             // seconds, ZSTDMT_B200_TRACE only
+    const CpuSet host_cpus = common_local_cpus(c->devs);
+
+    std::thread reader([&]() {
+        const ScopedAffinity bind(host_cpus);
+        for (;;) {
+            Slot* s;
+            {
+                const double t0 = trace_now();
+                std::unique_lock<std::mutex> lk(P.mu);
+                s = &P.slots[P.fill_seq % N];
+                P.cv.wait(lk, [&] { return (s->state == 0 && P.fill_seq - P.write_seq < in_flight) || P.error; });
+                rd.wait += trace_now() - t0;
+                if (P.error) break;
+            }
+            const double t0 = trace_now();
+            const bool filled = ops.fill(*s);
+            rd.work += trace_now() - t0;
+            if (!filled) break;
+            { std::lock_guard<std::mutex> g(P.mu); s->state = 1; P.fill_seq++; }
+            P.cv.notify_all();
+        }
+        { std::lock_guard<std::mutex> g(P.mu); P.reader_done = true; }
+        P.cv.notify_all();
+    });
+
+    std::thread writer([&]() {
+        const ScopedAffinity bind(host_cpus);
+        for (;;) {
+            Slot* s;
+            {
+                const double t0 = trace_now();
+                std::unique_lock<std::mutex> lk(P.mu);
+                s = &P.slots[P.write_seq % N];
+                P.cv.wait(lk, [&] { return s->state == 2 || P.error || (P.reader_done && P.write_seq == P.fill_seq); });
+                wr.wait += trace_now() - t0;
+                if (P.error || s->state != 2) break;
+            }
+            cudaSetDevice(s->dev);
+            const double t0 = trace_now();
+            if (cudaEventSynchronize(s->ev) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); break; }
+            const double t1 = trace_now();
+            const bool drained = ops.drain(*s);
+            wr.gpu += t1 - t0; wr.work += trace_now() - t1;
+            if (!drained) break;
+            { std::lock_guard<std::mutex> g(P.mu); s->state = 0; P.write_seq++; }
+            P.cv.notify_all();
+        }
+    });
+
+    for (;;) {
+        Slot* s;
+        {
+            const double t0 = trace_now();
+            std::unique_lock<std::mutex> lk(P.mu);
+            s = &P.slots[P.submit_seq % N];
+            P.cv.wait(lk, [&] { return s->state == 1 || P.error || (P.reader_done && P.submit_seq == P.fill_seq); });
+            sb.wait += trace_now() - t0;
+            if (P.error || s->state != 1) break;
+        }
+        cudaSetDevice(s->dev);
+        const double t0 = trace_now();
+        const int st = ops.submit(*s);
+        sb.work += trace_now() - t0;
+        if (s->dev >= 0 && s->dev < 64) g_dev_batches[s->dev]++;
+        if (st != ZMT_ST_OK) { c->lib_errcode = (size_t)st; P.fail(E.library); break; }
+        { std::lock_guard<std::mutex> g(P.mu); s->state = 2; P.submit_seq++; }
+        P.cv.notify_all();
+    }
+    reader.join(); writer.join();
+    for (auto& s : P.slots) if (s.ok) { cudaSetDevice(s.dev); cudaStreamSynchronize(s.stream); }
+    if (trace_on()) {
+        char scan[48] = "";
+        if (ops.scan) snprintf(scan, sizeof(scan), " | reader scan %.3fs", *ops.scan);
+        fprintf(stderr, "[zstdmt_b200] %s: reader fill %.3fs wait %.3fs | submit enqueue %.3fs wait %.3fs | writer gpu-wait %.3fs drain %.3fs wait %.3fs"
+                " | slots %zu, batch %zu KiB%s\n", ops.name, rd.work, rd.wait, sb.work, sb.wait, wr.gpu, wr.work, wr.wait, N, ops.batch_bytes >> 10, scan);
+    }
+    return P.error;
+}
+
 // ------------------------------------------------------------------ compression
 size_t compress_run(Ctx* c, GenRdWr* rw)
 {
     const DeviceRestore restore_device;
     const ErrCodes& E = *c->E;
-    const CodecOps* ops = codec_ops(c->codec);
-    if (!ops->compress || !ops->c_work || !ops->c_bound) { c->lib_errcode = ZMT_ST_UNSUPPORTED; return E.library; }
+    const CodecOps& ops = codec_ops(c->codec);
     Pipe& P = c->pipe;
     const size_t chunk = c->inputsize;
     // Slots in flight: the call is bound by the serialised callbacks (one memcpy stream); a GPU turns a batch around in a
@@ -425,147 +483,96 @@ size_t compress_run(Ctx* c, GenRdWr* rw)
     size_t nsl = env_size("ZSTDMT_B200_SLOTS", base_slots > c->devs.size() ? base_slots : c->devs.size());
     if (nsl < 2) nsl = 2; if (nsl < c->devs.size()) nsl = c->devs.size(); if (nsl > 64) nsl = 64;
     size_t batch_bytes = env_size("ZSTDMT_B200_BATCH_MB", 8) << 20;
-    const bool no_alias = getenv("ZSTDMT_B200_NO_RING_SHARE") != nullptr;          // A/B knob: every slot its own pinned buffers
-    if (!no_alias && nsl > base_slots) nsl = (nsl + base_slots - 1) / base_slots * base_slots;   // batch q uses host buffer q % base_slots: needs base_slots | slots
+    if (nsl > base_slots) nsl = (nsl + base_slots - 1) / base_slots * base_slots;   // batch q uses host buffer q % base_slots: needs base_slots | slots
     size_t B = batch_bytes / chunk; if (B < 1) B = 1; if (B > 65536) B = 65536;
 
     if (P.slots.empty()) {
         P.slots.resize(nsl);
         for (size_t i = 0; i < P.slots.size(); i++) {
-            const size_t ic = B * chunk, oc = (size_t)ops->c_bound((uint32_t)B, (uint32_t)chunk), wc = ops->c_work((uint32_t)B, (uint32_t)chunk, c->level);
-            const bool okk = (i < base_slots || no_alias) ? slot_alloc(P.slots[i], c->devs[i % c->devs.size()], ic, oc, wc, B)
-                                                          : slot_alloc_alias(P.slots[i], P.slots[i % base_slots], c->devs[i % c->devs.size()], ic, oc, wc, B);
-            if (!okk) { ctx_release_slots(c); return E.mem; }
+            const size_t ic = B * chunk, oc = (size_t)ops.c_bound((uint32_t)B, (uint32_t)chunk), wc = ops.c_work((uint32_t)B, (uint32_t)chunk, c->level);
+            if (!slot_alloc(P.slots[i], c->devs[i % c->devs.size()], ic, oc, wc, B, i < base_slots ? nullptr : &P.slots[i % base_slots])) {
+                ctx_release_slots(c); return E.mem;
+            }
         }
     }
-    const size_t N = P.slots.size();
-    // batches in flight: slots beyond the first `base_slots` borrow their pinned buffers from slot i % base_slots, so batch q + H
-    // may only be filled once batch q has been written
-    const size_t H = (N > base_slots && !no_alias) ? base_slots : N;
-    P.fill_seq = P.submit_seq = P.write_seq = 0; P.reader_done = false; P.error = 0;
-    for (auto& s : P.slots) s.state = 0;
 
-    // ---- reader: fills slots in sequence order (pt_compress read section, lz4-mt_compress.c:255-277)
-    StageClock ck_r, ck_w, ck_s;
-    const CpuSet host_cpus = common_local_cpus(c->devs);
-    std::thread reader([&]() {
-        const ScopedAffinity bind(host_cpus);
-        size_t frames_read = 0; bool eof = false;
-        while (!eof) {
-            Slot* s;
-            {
-                const double t0 = StageClock::now();
-                std::unique_lock<std::mutex> lk(P.mu);
-                s = &P.slots[P.fill_seq % N];
-                P.cv.wait(lk, [&] { return (s->state == 0 && P.fill_seq - P.write_seq < H) || P.error; });
-                ck_r.wait += StageClock::now() - t0;
-                if (P.error) break;
-            }
-            Tables T = tables_at(s->h_tab, s->tab_cap);
-            uint32_t n = 0; size_t got_bytes = 0;
-            while (n < B) {
-                GenBuffer b; b.buf = s->h_in + (size_t)n * chunk; b.size = chunk; b.allocated = chunk;
-                const double t0 = StageClock::now();
-                int rv = rw->fn_read(rw->arg_read, &b);
-                ck_r.cb += StageClock::now() - t0;
-                if (rv != 0) { P.fail(mt_error(E, rv)); eof = true; n = 0; break; }
-                if (b.size > chunk) { P.fail(E.read_fail); eof = true; n = 0; break; }
-                if (b.size == 0 && frames_read > 0) { eof = true; break; }
-                T.d[n] = (uint32_t)b.size; got_bytes += b.size; frames_read++; n++;
-            }
-            if (n == 0) break;
-            s->n = n; s->in_used = got_bytes;
-            {
-                std::lock_guard<std::mutex> g(P.mu);
-                c->insize += got_bytes; c->frames += n;
-                s->state = 1; P.fill_seq++;
-            }
-            P.cv.notify_all();
+    size_t frames_read = 0; bool eof = false;
+    PipeOps po;
+    // pt_compress read section, lz4-mt_compress.c:255-277
+    po.fill = [&](Slot& s) -> bool {
+        if (eof) return false;
+        Tables T = tables_at(s.h_tab, s.tab_cap);
+        uint32_t n = 0; size_t got_bytes = 0;
+        while (n < B) {
+            GenBuffer b; b.buf = s.h_in + (size_t)n * chunk; b.size = chunk; b.allocated = chunk;
+            int rv = rw->fn_read(rw->arg_read, &b);
+            if (rv != 0) { P.fail(mt_error(E, rv)); return false; }
+            if (b.size > chunk) { P.fail(E.read_fail); return false; }
+            if (b.size == 0 && frames_read > 0) { eof = true; break; }
+            T.per_frame[n] = (uint32_t)b.size; got_bytes += b.size; frames_read++; n++;
         }
-        { std::lock_guard<std::mutex> g(P.mu); P.reader_done = true; }
-        P.cv.notify_all();
-    });
-
-    // ---- writer: in-order emission (pt_write, lz4-mt_compress.c:178-205)
-    std::thread writer([&]() {
-        const ScopedAffinity bind(host_cpus);
-        for (;;) {
-            Slot* s;
-            {
-                const double t0 = StageClock::now();
-                std::unique_lock<std::mutex> lk(P.mu);
-                s = &P.slots[P.write_seq % N];
-                P.cv.wait(lk, [&] { return s->state == 2 || P.error || (P.reader_done && P.write_seq == P.fill_seq); });
-                ck_w.wait += StageClock::now() - t0;
-                if (P.error || s->state != 2) break;
-            }
-            cudaSetDevice(s->dev);
-            const double tg = StageClock::now();
-            if (cudaEventSynchronize(s->ev) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); break; }
-            Tables T = tables_at(s->h_tab, s->tab_cap);
-            const uint64_t total = T.a[s->n];
-            if (total > s->out_cap) { c->lib_errcode = ZMT_ST_DST_SMALL; P.fail(E.library); break; }
-            if (cudaMemcpyAsync(s->h_out, s->d_out, total, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess ||
-                cudaStreamSynchronize(s->stream) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); break; }
-            ck_w.gpu += StageClock::now() - tg;
-            bool bad = false;
-            const double tc = StageClock::now();
-            for (uint32_t i = 0; i < s->n; i++) {
-                GenBuffer b; b.buf = s->h_out + T.a[i]; b.size = (size_t)(T.a[i + 1] - T.a[i]); b.allocated = b.size;
-                int rv = rw->fn_write(rw->arg_write, &b);
-                if (rv != 0) { P.fail(mt_error(E, rv)); bad = true; break; }
-                c->outsize += b.size; c->curframe++;
-            }
-            ck_w.cb += StageClock::now() - tc;
-            if (bad) break;
-            { std::lock_guard<std::mutex> g(P.mu); s->state = 0; P.write_seq++; }
-            P.cv.notify_all();
-        }
-    });
-
-    // ---- submit (calling thread)
-    for (;;) {
-        Slot* s;
-        {
-            const double t0 = StageClock::now();
-            std::unique_lock<std::mutex> lk(P.mu);
-            s = &P.slots[P.submit_seq % N];
-            P.cv.wait(lk, [&] { return s->state == 1 || P.error || (P.reader_done && P.submit_seq == P.fill_seq); });
-            ck_s.wait += StageClock::now() - t0;
-            if (P.error || s->state != 1) break;
-        }
-        const double ts = StageClock::now();
-        cudaSetDevice(s->dev);
-        Tables Th = tables_at(s->h_tab, s->tab_cap), Td = tables_at(s->d_tab, s->tab_cap);
+        if (n == 0) return false;
+        s.n = n; s.in_used = got_bytes;
+        c->insize += got_bytes; c->frames += n;
+        return true;
+    };
+    po.submit = [&](Slot& s) -> int {
+        Tables Th = tables_at(s.h_tab, s.tab_cap), Td = tables_at(s.d_tab, s.tab_cap);
         bool full = true;
-        for (uint32_t i = 0; i < s->n; i++) if (Th.d[i] != chunk) { full = false; break; }
+        for (uint32_t i = 0; i < s.n; i++) if (Th.per_frame[i] != chunk) { full = false; break; }
         cudaError_t ce = cudaSuccess;
-        if (full) ce = cudaMemcpyAsync(s->d_in, s->h_in, (size_t)s->n * chunk, cudaMemcpyHostToDevice, s->stream);
-        else for (uint32_t i = 0; i < s->n && ce == cudaSuccess; i++)
-            if (Th.d[i]) ce = cudaMemcpyAsync(s->d_in + (size_t)i * chunk, s->h_in + (size_t)i * chunk, Th.d[i], cudaMemcpyHostToDevice, s->stream);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(Td.d, Th.d, (size_t)s->n * 4, cudaMemcpyHostToDevice, s->stream);
-        int st = ZMT_ST_CUDA;
-        if (ce == cudaSuccess) st = ops->compress(s->d_in, 0, (uint32_t)chunk, Td.d, s->n, c->level, s->d_work, s->d_out, Td.a, s->stream);
-        if (s->dev >= 0 && s->dev < 64) g_dev_batches[s->dev]++;
-        if (st == ZMT_ST_OK) {
-            ce = cudaMemcpyAsync(Th.a, Td.a, ((size_t)s->n + 1) * 8, cudaMemcpyDeviceToHost, s->stream);
-            if (ce == cudaSuccess) ce = cudaEventRecord(s->ev, s->stream);
-            if (ce != cudaSuccess) st = ZMT_ST_CUDA;
+        if (full) ce = cudaMemcpyAsync(s.d_in, s.h_in, (size_t)s.n * chunk, cudaMemcpyHostToDevice, s.stream);
+        else for (uint32_t i = 0; i < s.n && ce == cudaSuccess; i++)
+            if (Th.per_frame[i]) ce = cudaMemcpyAsync(s.d_in + (size_t)i * chunk, s.h_in + (size_t)i * chunk, Th.per_frame[i], cudaMemcpyHostToDevice, s.stream);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(Td.per_frame, Th.per_frame, (size_t)s.n * 4, cudaMemcpyHostToDevice, s.stream);
+        if (ce != cudaSuccess) return ZMT_ST_CUDA;
+        const int st = ops.compress(s.d_in, 0, (uint32_t)chunk, Td.per_frame, s.n, c->level, s.d_work, s.d_out, Td.frame_off, s.stream);
+        if (st != ZMT_ST_OK) return st;
+        if (cudaMemcpyAsync(Th.frame_off, Td.frame_off, ((size_t)s.n + 1) * 8, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
+            cudaEventRecord(s.ev, s.stream) != cudaSuccess) return ZMT_ST_CUDA;
+        return ZMT_ST_OK;
+    };
+    // pt_write, lz4-mt_compress.c:178-205
+    po.drain = [&](Slot& s) -> bool {
+        Tables T = tables_at(s.h_tab, s.tab_cap);
+        const uint64_t total = T.frame_off[s.n];
+        if (total > s.out_cap) { c->lib_errcode = ZMT_ST_DST_SMALL; P.fail(E.library); return false; }
+        if (cudaMemcpyAsync(s.h_out, s.d_out, total, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
+            cudaStreamSynchronize(s.stream) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); return false; }
+        for (uint32_t i = 0; i < s.n; i++) {
+            GenBuffer b; b.buf = s.h_out + T.frame_off[i]; b.size = (size_t)(T.frame_off[i + 1] - T.frame_off[i]); b.allocated = b.size;
+            int rv = rw->fn_write(rw->arg_write, &b);
+            if (rv != 0) { P.fail(mt_error(E, rv)); return false; }
+            c->outsize += b.size; c->curframe++;
         }
-        if (st != ZMT_ST_OK) { c->lib_errcode = (size_t)st; P.fail(E.library); break; }
-        ck_s.gpu += StageClock::now() - ts;
-        { std::lock_guard<std::mutex> g(P.mu); s->state = 2; P.submit_seq++; }
-        P.cv.notify_all();
-    }
-    reader.join(); writer.join();
-    for (auto& s : P.slots) { cudaSetDevice(s.dev); cudaStreamSynchronize(s.stream); }
-    if (trace_on())
-        fprintf(stderr, "[zstdmt_b200] compress: reader cb %.3fs wait %.3fs | submit enqueue %.3fs wait %.3fs | writer gpu-wait %.3fs cb %.3fs wait %.3fs | slots %zu x %zu chunks\n",
-                ck_r.cb, ck_r.wait, ck_s.gpu, ck_s.wait, ck_w.gpu, ck_w.cb, ck_w.wait, N, B);
-    return P.error;
+        return true;
+    };
+    po.name = "compress"; po.batch_bytes = B * chunk;
+    return run_pipeline(c, P.slots.size() > base_slots ? base_slots : P.slots.size(), po);
 }
 
 // ------------------------------------------------------------------ decompression
+// Walks an LZ4F frame's header and block headers in p[0..n) (n >= 7): *len = the frame's length, content checksum
+// included; *bound = the most its blocks decode to (blockMaxSize per compressed block).  false: the block headers run
+// past n (*bound then covers the blocks before the cut).
+bool lz4f_walk(const uint8_t* p, size_t n, size_t* len, uint64_t* bound)
+{
+    const uint32_t flg = p[4];
+    const uint64_t blkmax = 1ull << (8 + 2 * ((p[5] >> 4) & 7));
+    size_t q = 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1;
+    *bound = 0;
+    for (;;) {
+        if (q + 4 > n) return false;
+        const uint32_t bh = rd32(p + q); q += 4;
+        if (bh == 0) break;
+        const uint32_t bs = bh & 0x7FFFFFFFu;
+        *bound += (bh & 0x80000000u) ? bs : blkmax;
+        q += (size_t)bs + ((flg & 0x10) ? 4 : 0);
+    }
+    *len = q + ((flg & 4) ? 4 : 0);
+    return true;
+}
+
 // Output size of one payload, from its own header (pt_decompress sizes the buffer from
 // LE64 @ payload+6, lz4-mt_decompress.c:329-335; zstd: frame content size).
 // Returns false if the header is unusable.
@@ -582,17 +589,10 @@ bool lz4f_out_size(const uint8_t* p, size_t n, uint64_t* out)
         *out = v; return true;
     }
     // no content-size field: bound it by walking the block headers (each block <= blockMaxSize)
-    const uint32_t id = (bd >> 4) & 7; if (id < 4) return false;
-    const uint64_t blkmax = 1ull << (8 + 2 * id);
-    size_t pos = 4 + 2 + ((flg & 1) ? 4 : 0) + 1; uint64_t total = 0;
-    while (pos + 4 <= n) {
-        const uint32_t bh = rd32(p + pos); pos += 4;
-        if (bh == 0) break;
-        const uint32_t bs = bh & 0x7FFFFFFFu;
-        total += (bh & 0x80000000u) ? bs : blkmax;
-        pos += (size_t)bs + ((flg & 0x10) ? 4 : 0);
-    }
-    *out = total; return true;
+    if (((bd >> 4) & 7) < 4) return false;
+    size_t len = 0;
+    lz4f_walk(p, n, &len, out);
+    return true;
 }
 
 // reads exactly `want` bytes unless EOF; returns 0 ok / error; *got = delivered
@@ -603,6 +603,14 @@ size_t read_some(const ErrCodes& E, GenRdWr* rw, void* dst, size_t want, size_t*
     if (rv != 0) return mt_error(E, rv);
     if (b.size > want) return E.read_fail;
     *got = b.size; return 0;
+}
+
+// Enqueues the decode of one batch of n frames on `st`: the frames' tables in Td (device), the zstd block descriptors in d_blk.
+int decode_batch(bool is_zstd, const void* d_in, size_t in_bytes, const void* d_blk, uint32_t nblk, const Tables& Td, uint32_t n,
+                 uint32_t nslots, void* d_out, void* d_work, cudaStream_t st)
+{
+    return is_zstd ? zmt_zstd_decompress_device(d_in, d_blk, nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size, Td.status, d_work, st)
+                   : zmt_lz4_decompress_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, d_work, st);
 }
 
 // ------------------------------------------------------------------ plain (unframed) single streams
@@ -667,24 +675,16 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                 if (n - pos < 7) { if (eof) return E.data_error; need_more = true; break; }
                 const uint32_t flg = s[pos + 4], bd = s[pos + 5], id = (bd >> 4) & 7;
                 if ((flg >> 6) != 1 || id < 4) { c->lib_errcode = ZMT_ST_BAD_HEADER; return E.library; }
-                const uint64_t blkmax = 1ull << (8 + 2 * id);
-                size_t q = pos + 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1;
-                uint64_t bound = 0; bool cut = false;
-                for (;;) {
-                    if (q + 4 > n) { cut = true; break; }
-                    const uint32_t bh = rd32(s + q); q += 4;
-                    if (bh == 0) break;
-                    const uint32_t bs = bh & 0x7FFFFFFFu;
-                    bound += (bh & 0x80000000u) ? bs : blkmax;
-                    q += (size_t)bs + ((flg & 0x10) ? 4 : 0);
+                size_t len = 0; uint64_t bound = 0;
+                if (!lz4f_walk(s + pos, n - pos, &len, &bound) || len > n - pos) {
+                    if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; }
+                    need_more = true; break;
                 }
-                if (!cut && (flg & 4)) q += 4;
-                if (cut || q > n) { if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; } need_more = true; break; }
                 uint64_t osz = bound;
                 if (flg & 8) { osz = rd64(s + pos + 6); if (osz > bound) { c->lib_errcode = ZMT_ST_CONTENT_SIZE; return E.library; } }    // untrusted field, bounded by the block walk
-                foff.push_back(pos); fcs.push_back((uint32_t)(q - pos)); ooff.push_back(ooff.back() + osz);
+                foff.push_back(pos); fcs.push_back((uint32_t)len); ooff.push_back(ooff.back() + osz);
                 { const uint64_t nb = (osz + 65535) / 65536; nslots += nb ? nb : 1; }
-                pos = q;
+                pos += len;
             } else {
                 if (magic < 0xFD2FB522u || magic > 0xFD2FB528u) return E.data_error;
                 uint64_t cs = 0; uint32_t fl = 0; size_t used = 0;
@@ -697,7 +697,7 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                     blocks.resize(blocks.size() * 2 + 4096 * dsz);            // block table full: grow and rescan this frame
                 }
                 if (zr == ZMT_ST_TRUNCATED && !eof) { nblk = nblk0; scratch = scr0; need_more = true; break; }
-                if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; return zr == ZMT_ST_TRUNCATED ? E.frame_decompress : E.library; }
+                if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; return status_error(E, zr); }
                 foff.push_back(pos); expect.push_back((fl & 4u) ? ~0ull : cs); fflags.push_back(fl); first_blk.push_back(nblk); ooff.push_back(ooff.back() + cs);
                 pos += used;
             }
@@ -712,8 +712,12 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
             const size_t tab_bytes = tables_bytes(nf);
             h_tab.resize(tab_bytes);
             Tables T = tables_at(h_tab.data(), nf);
-            for (uint32_t i = 0; i < nf; i++) { T.a[i] = foff[i]; T.b[i] = ooff[i]; if (is_zstd) { T.f[i] = expect[i]; T.d[i] = fflags[i]; T.g[i] = first_blk[i]; } else T.d[i] = fcs[i]; }
-            T.b[nf] = total; if (is_zstd) T.g[nf] = nblk;
+            for (uint32_t i = 0; i < nf; i++) {
+                T.frame_off[i] = foff[i]; T.out_off[i] = ooff[i];
+                T.per_frame[i] = is_zstd ? fflags[i] : fcs[i];
+                if (is_zstd) { T.expect[i] = expect[i]; T.first_blk[i] = first_blk[i]; }
+            }
+            T.out_off[nf] = total; if (is_zstd) T.first_blk[nf] = nblk;
             const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes(nf, nblk, scratch) : zmt_lz4d_workspace_bytes(nf, (uint32_t)nslots, in_bytes);
             if (!d_in.need(in_bytes + 256) || !d_out.need(total + 256) || !d_tab.need(tab_bytes) || !d_work.need(wk) || (is_zstd && !d_blk.need((size_t)nblk * dsz + 16))) return E.mem;
             Tables Td = tables_at((uint8_t*)d_tab.p, nf);
@@ -722,20 +726,19 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
             cudaMemcpyAsync((uint8_t*)d_in.p + lo, in.data() + lo, hi - lo, cudaMemcpyHostToDevice, st);
             cudaMemcpyAsync(d_tab.p, h_tab.data(), tab_bytes, cudaMemcpyHostToDevice, st);
             if (is_zstd && nblk) cudaMemcpyAsync(d_blk.p, blocks.data(), (size_t)nblk * dsz, cudaMemcpyHostToDevice, st);
-            const int rc = is_zstd ? zmt_zstd_decompress_device(d_in.p, d_blk.p, nblk, Td.g, Td.f, Td.d, nf, d_out.p, Td.b, Td.c, Td.e, d_work.p, st)
-                                   : zmt_lz4_decompress_device(d_in.p, in_bytes, Td.a, Td.d, nf, (uint32_t)nslots, d_out.p, Td.b, Td.c, Td.e, d_work.p, st);
+            const int rc = decode_batch(is_zstd, d_in.p, in_bytes, d_blk.p, nblk, Td, nf, (uint32_t)nslots, d_out.p, d_work.p, st);
             out.resize(total ? total : 1);
             std::vector<uint32_t> status(nf); std::vector<uint64_t> osz(nf);
             cudaError_t ce = cudaSuccess;
             if (rc == ZMT_ST_OK) {
                 if (total) ce = cudaMemcpyAsync(out.data(), d_out.p, total, cudaMemcpyDeviceToHost, st);
-                if (ce == cudaSuccess) ce = cudaMemcpyAsync(status.data(), Td.e, (size_t)nf * 4, cudaMemcpyDeviceToHost, st);
-                if (ce == cudaSuccess) ce = cudaMemcpyAsync(osz.data(), Td.c, (size_t)nf * 8, cudaMemcpyDeviceToHost, st);
+                if (ce == cudaSuccess) ce = cudaMemcpyAsync(status.data(), Td.status, (size_t)nf * 4, cudaMemcpyDeviceToHost, st);
+                if (ce == cudaSuccess) ce = cudaMemcpyAsync(osz.data(), Td.out_size, (size_t)nf * 8, cudaMemcpyDeviceToHost, st);
                 if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
             }
             if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library; }
             for (uint32_t i = 0; i < nf; i++) {
-                if (status[i] != ZMT_ST_OK) { c->lib_errcode = status[i]; return (status[i] == ZMT_ST_TRUNCATED || status[i] == ZMT_ST_TRAILING) ? E.frame_decompress : E.library; }
+                if (status[i] != ZMT_ST_OK) { c->lib_errcode = status[i]; return status_error(E, status[i]); }
                 // frame by frame, in pieces of at most `piece` bytes (st_decompress writes as it goes)
                 uint64_t o = 0;
                 while (o < osz[i]) {
@@ -779,7 +782,10 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     const uint32_t kBlkCap = 32768;
     // decode batches must hold enough frames to fill the GPU (one warp per 64 KiB block; a linked-block frame is a chain)
     const size_t in_cap0 = (env_size("ZSTDMT_B200_DBATCH_MB", 32) << 20), out_cap0 = in_cap0 * 2, tab_cap = 8192;
-    const uint64_t piece_bytes = (uint64_t)env_size("ZSTDMT_B200_D2H_PIECE_MB", 2) << 20;      // 0: whole slot right after the kernels
+    // The decoded bytes come over in pieces of a few MiB, one piece ahead of the one being written: what fn_write's memcpy
+    // reads was DMA-written moments ago and is still in the last-level cache, instead of a whole 64 MiB slot that was
+    // copied long before its first byte is used.
+    const uint64_t kPieceBytes = 2 << 20;
 
     // ---- stream-type sniffing on the calling thread (LZ4MT_decompressDCtx, lz4-mt_decompress.c:503-520;
     //      ZSTDCB_decompressDCtx, zstd-mt_decompress.c:721-759)
@@ -828,276 +834,200 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
         {
             // zstd scratch: 16 B per sequence + the literals: ~2x the output on text, bounded at 3x + tables (the reader closes a batch early otherwise)
             const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes((uint32_t)tab_cap, kBlkCap, 3 * (uint64_t)out_cap0) : zmt_lz4d_workspace_bytes((uint32_t)tab_cap, lz4_slot_cap(out_cap0, tab_cap), in_cap0);
-            if (!slot_alloc(P.slots[i], c->devs[i % c->devs.size()], in_cap0, out_cap0, wk, tab_cap) || (is_zstd && !slot_ensure_blocks(P.slots[i], kBlkCap))) { ctx_release_slots(c); return E.mem; }
+            if (!slot_alloc(P.slots[i], c->devs[i % c->devs.size()], in_cap0, out_cap0, wk, tab_cap, nullptr) || (is_zstd && !slot_ensure_blocks(P.slots[i], kBlkCap))) {
+                ctx_release_slots(c); return E.mem;
+            }
             P.slots[i].scr_cap = is_zstd ? 3 * (uint64_t)P.slots[i].out_cap : 0;
         }
     }
-    const size_t N = P.slots.size();
-    P.fill_seq = P.submit_seq = P.write_seq = 0; P.reader_done = false; P.error = 0;
-    for (auto& s : P.slots) s.state = 0;
 
-    StageClock rd_clk, wr_clk; double rd_scan = 0, rd_total = 0, wr_total = 0;     // ZSTDMT_B200_TRACE=1
-    const bool tr = trace_on();
-    // ---- reader (pt_read, lz4-mt_decompress.c:192-281 / zstd-mt_decompress.c:209-369)
-    const CpuSet host_cpus = common_local_cpus(c->devs);
-    std::thread reader([&]() {
-        const ScopedAffinity bind(host_cpus);
-        const double t_start = tr ? StageClock::now() : 0;
-        bool eof = false;
-        std::vector<uint8_t> carry;              // a frame that did not fit the previous slot
-        uint64_t carry_out = 0;
-        while (!eof) {
-            Slot* s;
-            {
-                std::unique_lock<std::mutex> lk(P.mu);
-                s = &P.slots[P.fill_seq % N];
-                const double t0 = tr ? StageClock::now() : 0;
-                P.cv.wait(lk, [&] { return s->state == 0 || P.error; });
-                if (tr) rd_clk.wait += StageClock::now() - t0;
-                if (P.error) break;
-            }
-            Tables T = tables_at(s->h_tab, s->tab_cap);
-            uint32_t n = 0; size_t in_used = 0; uint64_t out_used = 0; size_t stat_in = 0;
-            bool failed = false;
-            uint32_t nblk = 0; uint64_t scr = 0;                 // zstd: block descriptors + scratch demand of this batch
-            // (re)allocate the still empty slot so that one frame of these dimensions fits; takes P.mu for the swap because the
-            // writer's wait predicate reads s->state
-            auto grow = [&](size_t need_in, uint64_t need_out, uint64_t need_scr, uint32_t need_blk) -> bool {
-                if (need_in <= s->in_cap && need_out <= s->out_cap && need_scr <= s->scr_cap && need_blk <= s->blk_cap) return true;
-                const int dev = s->dev;
-                const size_t nin = need_in > s->in_cap ? need_in : s->in_cap, nout = need_out > s->out_cap ? (size_t)need_out : s->out_cap;
-                const uint64_t nscr = is_zstd ? (need_scr > 3 * (uint64_t)nout ? need_scr : 3 * (uint64_t)nout) : 0;
-                const uint32_t nb = need_blk > s->blk_cap ? need_blk : s->blk_cap;
-                const size_t tc = s->tab_cap;
-                const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes((uint32_t)tc, nb, nscr) : zmt_lz4d_workspace_bytes((uint32_t)tc, lz4_slot_cap(nout, tc), nin);
-                std::lock_guard<std::mutex> g(P.mu);
-                slot_free(*s);
-                if (!slot_alloc(*s, dev, nin, nout, wk, tc) || (is_zstd && !slot_ensure_blocks(*s, nb))) return false;
-                s->scr_cap = nscr;
-                return true;
-            };
-            // Put one whole frame (12-byte header + payload, held in `fr`) at the start of the empty slot, growing the slot
-            // (input, output, zstd block table and entropy scratch) until it fits.  Returns false after P.fail().
-            auto place_first = [&](const std::vector<uint8_t>& fr) -> bool {
-                const size_t toRead = fr.size() - 12;
-                if (!grow(fr.size(), 0, 0, 0)) { P.fail(E.mem); return false; }
-                uint64_t osz = 0; uint32_t nsq = 0;
-                if (!is_zstd) {
-                    if (!lz4f_out_size(fr.data() + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); return false; }
-                    if (!grow(fr.size(), osz, 0, 0)) { P.fail(E.mem); return false; }
+    double rd_scan = 0;
+    bool eof = false;
+    std::vector<uint8_t> carry;              // a frame that did not fit the previous slot
+    PipeOps po;
+    // pt_read, lz4-mt_decompress.c:192-281 / zstd-mt_decompress.c:209-369
+    po.fill = [&](Slot& slot) -> bool {
+        if (eof) return false;
+        Slot* s = &slot;
+        Tables T = tables_at(s->h_tab, s->tab_cap);
+        uint32_t n = 0; size_t in_used = 0; uint64_t out_used = 0; size_t stat_in = 0;
+        bool failed = false;
+        uint32_t nblk = 0; uint64_t scr = 0;                 // zstd: block descriptors + scratch demand of this batch
+        // (re)allocate the still empty slot so that one frame of these dimensions fits; takes P.mu for the swap because the
+        // writer's wait predicate reads s->state
+        auto grow = [&](size_t need_in, uint64_t need_out, uint64_t need_scr, uint32_t need_blk) -> bool {
+            if (need_in <= s->in_cap && need_out <= s->out_cap && need_scr <= s->scr_cap && need_blk <= s->blk_cap) return true;
+            const int dev = s->dev;
+            const size_t nin = need_in > s->in_cap ? need_in : s->in_cap, nout = need_out > s->out_cap ? (size_t)need_out : s->out_cap;
+            const uint64_t nscr = is_zstd ? (need_scr > 3 * (uint64_t)nout ? need_scr : 3 * (uint64_t)nout) : 0;
+            const uint32_t nb = need_blk > s->blk_cap ? need_blk : s->blk_cap;
+            const size_t tc = s->tab_cap;
+            const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes((uint32_t)tc, nb, nscr) : zmt_lz4d_workspace_bytes((uint32_t)tc, lz4_slot_cap(nout, tc), nin);
+            std::lock_guard<std::mutex> g(P.mu);
+            slot_free(*s);
+            if (!slot_alloc(*s, dev, nin, nout, wk, tc, nullptr) || (is_zstd && !slot_ensure_blocks(*s, nb))) return false;
+            s->scr_cap = nscr;
+            return true;
+        };
+        // Put one whole frame (12-byte header + payload, held in `fr`) at the start of the empty slot, growing the slot
+        // (input, output, zstd block table and entropy scratch) until it fits.  Returns false after P.fail().
+        auto place_first = [&](const std::vector<uint8_t>& fr) -> bool {
+            const size_t toRead = fr.size() - 12;
+            if (!grow(fr.size(), 0, 0, 0)) { P.fail(E.mem); return false; }
+            uint64_t osz = 0; uint32_t nsq = 0;
+            if (!is_zstd) {
+                if (!lz4f_out_size(fr.data() + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); return false; }
+                if (!grow(fr.size(), osz, 0, 0)) { P.fail(E.mem); return false; }
+                memcpy(s->h_in, fr.data(), fr.size());
+            } else {
+                for (int tries = 0;; tries++) {
                     memcpy(s->h_in, fr.data(), fr.size());
-                } else {
-                    for (int tries = 0;; tries++) {
-                        memcpy(s->h_in, fr.data(), fr.size());
-                        uint64_t cs = 0; nblk = 0; scr = 0;
-                        const int zr = zmt_zstd_scan_frame_host(s->h_in + 12, toRead, 12, 0, s->h_blk, &nblk, s->blk_cap, &scr, &cs, &nsq);
-                        if (zr == ZMT_ST_DST_SMALL && tries < 2) {          // more blocks than descriptors: every block costs >= 3 bytes
-                            if (!grow(fr.size(), 0, 0, (uint32_t)(toRead / 3 + 16))) { P.fail(E.mem); return false; }
-                            continue;
-                        }
-                        if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(zr == ZMT_ST_TRUNCATED || zr == ZMT_ST_TRAILING ? E.frame_decompress : E.library); return false; }
-                        osz = cs;
-                        if (osz <= s->out_cap && scr <= s->scr_cap) break;
-                        if (tries >= 2 || !grow(fr.size(), osz, scr, 0)) { P.fail(E.mem); return false; }
+                    uint64_t cs = 0; nblk = 0; scr = 0;
+                    const int zr = zmt_zstd_scan_frame_host(s->h_in + 12, toRead, 12, 0, s->h_blk, &nblk, s->blk_cap, &scr, &cs, &nsq);
+                    if (zr == ZMT_ST_DST_SMALL && tries < 2) {          // more blocks than descriptors: every block costs >= 3 bytes
+                        if (!grow(fr.size(), 0, 0, (uint32_t)(toRead / 3 + 16))) { P.fail(E.mem); return false; }
+                        continue;
                     }
-                }
-                T = tables_at(s->h_tab, s->tab_cap);
-                T.a[0] = 0; T.d[0] = (uint32_t)toRead; T.b[0] = 0;
-                if (is_zstd) { T.g[0] = 0; T.f[0] = (nsq & 4u) ? ~0ull : osz; T.d[0] = nsq; }      // flag 4: no content size in the header, osz is a bound
-                in_used = fr.size(); out_used = osz; n = 1;
-                return true;
-            };
-            if (!carry.empty()) {
-                if (!place_first(carry)) break;
-                carry.clear();
-            }
-            while (n < s->tab_cap) {
-                uint8_t hdr[12]; size_t pre = 0;
-                if (hdr_pending) { memcpy(hdr, first, 12); hdr_pending = false; pre = first_payload_have; }
-                else {
-                    size_t g = 0; size_t e = read_some(E, rw, hdr, 12, &g);
-                    if (e) { P.fail(e); failed = true; break; }
-                    if (g == 0) { eof = true; break; }
-                    if (g != 12) { P.fail(E.read_fail); failed = true; break; }
-                    if (rd32(hdr) != MT_MAGIC_SKIPPABLE) { P.fail(E.data_error); failed = true; break; }
-                    if (c->codec == CODEC_ZSTD) stat_in += 12;
-                }
-                if (rd32(hdr + 4) != 4) { P.fail(E.data_error); failed = true; break; }
-                if (c->codec == CODEC_LZ4) stat_in += 12;
-                const size_t toRead = rd32(hdr + 8);
-                if (toRead < pre) { P.fail(E.data_error); failed = true; break; }
-                // where to put it: the current slot if it fits behind the frames already there, else a temporary buffer
-                // (first frame of a batch that needs a bigger slot, or a frame that moves to the next batch)
-                uint8_t* dstp; bool to_tmp = false;
-                if (in_used + 12 + toRead <= s->in_cap) dstp = s->h_in + in_used;
-                else { carry.resize(12 + toRead); dstp = carry.data(); to_tmp = true; }
-                memcpy(dstp, hdr, 12);
-                if (pre) memcpy(dstp + 12, first + 12, pre);
-                const double tc0 = tr ? StageClock::now() : 0;
-                size_t g = 0; size_t e = read_some(E, rw, dstp + 12 + pre, toRead - pre, &g);
-                if (tr) rd_clk.cb += StageClock::now() - tc0;
-                if (e) { P.fail(e); failed = true; break; }
-                if (g != toRead - pre) { P.fail(E.data_error); failed = true; break; }
-                stat_in += g;
-                if (to_tmp) {
-                    if (n > 0) break;                                   // next batch starts with it
-                    if (!place_first(carry)) { failed = true; break; }
-                    carry.clear();
-                    continue;
-                }
-                uint64_t osz = 0; uint32_t nsq = 0;
-                uint32_t nblk_new = nblk; uint64_t scr_new = scr;
-                bool moves = false;                                     // does not fit behind the others: first frame of the next batch
-                if (!is_zstd) {
-                    if (!lz4f_out_size(dstp + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); failed = true; break; }
-                } else {
-                    // block table of this frame (descriptors are appended; dropped again if the frame moves to the next batch)
-                    uint64_t cs = 0;
-                    const double ts0 = tr ? StageClock::now() : 0;
-                    const int zr = zmt_zstd_scan_frame_host(dstp + 12, toRead, in_used + 12, n, s->h_blk, &nblk_new, s->blk_cap, &scr_new, &cs, &nsq);
-                    if (tr) rd_scan += StageClock::now() - ts0;
-                    if (zr == ZMT_ST_DST_SMALL) moves = true;
-                    else if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(zr == ZMT_ST_TRUNCATED || zr == ZMT_ST_TRAILING ? E.frame_decompress : E.library); failed = true; break; }
-                    else if (scr_new > s->scr_cap) moves = true;
+                    if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(status_error(E, zr)); return false; }
                     osz = cs;
+                    if (osz <= s->out_cap && scr <= s->scr_cap) break;
+                    if (tries >= 2 || !grow(fr.size(), osz, scr, 0)) { P.fail(E.mem); return false; }
                 }
-                if (!moves && osz > s->out_cap - out_used) moves = true;
-                if (moves) {
-                    carry.assign(dstp, dstp + 12 + toRead);
-                    if (n > 0) break;
-                    if (!place_first(carry)) { failed = true; break; }  // a single frame larger than the slot: grow the slot
-                    carry.clear();
-                    continue;
-                }
-                T.a[n] = in_used; T.d[n] = (uint32_t)toRead; T.b[n] = out_used;
-                if (is_zstd) { T.g[n] = nblk; T.f[n] = (nsq & 4u) ? ~0ull : osz; T.d[n] = nsq; nblk = nblk_new; scr = scr_new; }     // T.d = frame flags (sequential pass, checksum, no size)
-                in_used += 12 + toRead; out_used += osz; n++;
             }
-            if (failed) break;
-            if (n == 0) break;
-            T.b[n] = out_used;
-            if (is_zstd) { T.g[n] = nblk; s->nblk = nblk; s->scratch_used = scr; }
-            s->n = n; s->in_used = in_used; s->out_used = (size_t)out_used;
-            { uint64_t ns = 0; for (uint32_t i = 0; i < n; i++) { const uint64_t nb = (T.b[i + 1] - T.b[i] + 65535) / 65536; ns += nb ? nb : 1; } s->nslots = (uint32_t)ns; }
-            {
-                std::lock_guard<std::mutex> g(P.mu);
-                c->insize += stat_in; c->frames += n;
-                s->state = 1; P.fill_seq++;
+            T = tables_at(s->h_tab, s->tab_cap);
+            T.frame_off[0] = 0; T.per_frame[0] = (uint32_t)toRead; T.out_off[0] = 0;
+            if (is_zstd) { T.first_blk[0] = 0; T.expect[0] = (nsq & 4u) ? ~0ull : osz; T.per_frame[0] = nsq; }      // flag 4: no content size in the header, osz is a bound
+            in_used = fr.size(); out_used = osz; n = 1;
+            return true;
+        };
+        if (!carry.empty()) {
+            if (!place_first(carry)) return false;
+            carry.clear();
+        }
+        while (n < s->tab_cap) {
+            uint8_t hdr[12]; size_t pre = 0;
+            if (hdr_pending) { memcpy(hdr, first, 12); hdr_pending = false; pre = first_payload_have; }
+            else {
+                size_t g = 0; size_t e = read_some(E, rw, hdr, 12, &g);
+                if (e) { P.fail(e); failed = true; break; }
+                if (g == 0) { eof = true; break; }
+                if (g != 12) { P.fail(E.read_fail); failed = true; break; }
+                if (rd32(hdr) != MT_MAGIC_SKIPPABLE) { P.fail(E.data_error); failed = true; break; }
+                if (c->codec == CODEC_ZSTD) stat_in += 12;
             }
-            P.cv.notify_all();
-        }
-        if (tr) rd_total = StageClock::now() - t_start;
-        { std::lock_guard<std::mutex> g(P.mu); P.reader_done = true; }
-        P.cv.notify_all();
-    });
-
-    // ---- writer (pt_write, lz4-mt_decompress.c:165-187)
-    std::thread writer([&]() {
-        const ScopedAffinity bind(host_cpus);
-        const double t_start = tr ? StageClock::now() : 0;
-        for (;;) {
-            Slot* s;
-            {
-                std::unique_lock<std::mutex> lk(P.mu);
-                s = &P.slots[P.write_seq % N];
-                const double t0 = tr ? StageClock::now() : 0;
-                P.cv.wait(lk, [&] { return s->state == 2 || P.error || (P.reader_done && P.write_seq == P.fill_seq); });
-                if (tr) wr_clk.wait += StageClock::now() - t0;
-                if (P.error || s->state != 2) break;
+            if (rd32(hdr + 4) != 4) { P.fail(E.data_error); failed = true; break; }
+            if (c->codec == CODEC_LZ4) stat_in += 12;
+            const size_t toRead = rd32(hdr + 8);
+            if (toRead < pre) { P.fail(E.data_error); failed = true; break; }
+            // where to put it: the current slot if it fits behind the frames already there, else a temporary buffer
+            // (first frame of a batch that needs a bigger slot, or a frame that moves to the next batch)
+            uint8_t* dstp; bool to_tmp = false;
+            if (in_used + 12 + toRead <= s->in_cap) dstp = s->h_in + in_used;
+            else { carry.resize(12 + toRead); dstp = carry.data(); to_tmp = true; }
+            memcpy(dstp, hdr, 12);
+            if (pre) memcpy(dstp + 12, first + 12, pre);
+            size_t g = 0; size_t e = read_some(E, rw, dstp + 12 + pre, toRead - pre, &g);
+            if (e) { P.fail(e); failed = true; break; }
+            if (g != toRead - pre) { P.fail(E.data_error); failed = true; break; }
+            stat_in += g;
+            if (to_tmp) {
+                if (n > 0) break;                                   // next batch starts with it
+                if (!place_first(carry)) { failed = true; break; }
+                carry.clear();
+                continue;
             }
-            cudaSetDevice(s->dev);
-            const double tg0 = tr ? StageClock::now() : 0;
-            if (cudaEventSynchronize(s->ev) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); break; }
-            if (tr) wr_clk.gpu += StageClock::now() - tg0;
-            Tables T = tables_at(s->h_tab, s->tab_cap);
-            bool bad = false;
-            // The decoded bytes come over in pieces of a few MiB, one piece ahead of the one being written: what fn_write's
-            // memcpy reads was DMA-written moments ago and is still in the last-level cache, instead of a whole 64 MiB slot that
-            // was copied long before its first byte is used.
-            uint32_t issued = 0, ready = 0; int np_issued = 0, np_ready = 0;       // frames [0, issued) requested, [0, ready) landed
-            auto issue_piece = [&]() -> bool {
-                if (issued >= s->n) return true;
-                uint32_t j = issued; uint64_t lo = T.b[j], hi = lo;
-                while (j < s->n && hi - lo < piece_bytes) { hi = T.b[j] + T.c[j]; j++; }
-                if (hi > s->out_cap) hi = s->out_cap;
-                if (hi > lo && cudaMemcpyAsync(s->h_out + lo, s->d_out + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) return false;
-                if (cudaEventRecord(s->evp[np_issued & 1], s->stream) != cudaSuccess) return false;
-                np_issued++; issued = j;
-                return true;
-            };
-            uint32_t piece_end[2] = { 0, 0 };
-            for (uint32_t i = 0; i < s->n; i++) {
-                const uint32_t st = T.e[i];
-                if (st != ZMT_ST_OK) {
-                    c->lib_errcode = st;
-                    P.fail((st == ZMT_ST_TRUNCATED || st == ZMT_ST_TRAILING) ? E.frame_decompress : E.library);
-                    bad = true; break;
-                }
-                if (piece_bytes && i >= ready) {
-                    bool okp = true;
-                    if (np_issued == np_ready) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }
-                    if (okp && issued < s->n && np_issued == np_ready + 1) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }   // one ahead
-                    if (okp) okp = cudaEventSynchronize(s->evp[np_ready & 1]) == cudaSuccess;
-                    if (!okp) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); bad = true; break; }
-                    ready = piece_end[np_ready & 1]; np_ready++;
-                }
-                GenBuffer b; b.buf = s->h_out + T.b[i]; b.size = (size_t)T.c[i]; b.allocated = b.size;
-                const double tc0 = tr ? StageClock::now() : 0;
-                int rv = rw->fn_write(rw->arg_write, &b);
-                if (tr) wr_clk.cb += StageClock::now() - tc0;
-                if (rv != 0) { P.fail(mt_error(E, rv)); bad = true; break; }
-                c->outsize += b.size; c->curframe++;
+            uint64_t osz = 0; uint32_t nsq = 0;
+            uint32_t nblk_new = nblk; uint64_t scr_new = scr;
+            bool moves = false;                                     // does not fit behind the others: first frame of the next batch
+            if (!is_zstd) {
+                if (!lz4f_out_size(dstp + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); failed = true; break; }
+            } else {
+                // block table of this frame (descriptors are appended; dropped again if the frame moves to the next batch)
+                uint64_t cs = 0;
+                const double ts0 = trace_now();
+                const int zr = zmt_zstd_scan_frame_host(dstp + 12, toRead, in_used + 12, n, s->h_blk, &nblk_new, s->blk_cap, &scr_new, &cs, &nsq);
+                rd_scan += trace_now() - ts0;
+                if (zr == ZMT_ST_DST_SMALL) moves = true;
+                else if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(status_error(E, zr)); failed = true; break; }
+                else if (scr_new > s->scr_cap) moves = true;
+                osz = cs;
             }
-            if (bad) break;
-            { std::lock_guard<std::mutex> g(P.mu); s->state = 0; P.write_seq++; }
-            P.cv.notify_all();
+            if (!moves && osz > s->out_cap - out_used) moves = true;
+            if (moves) {
+                carry.assign(dstp, dstp + 12 + toRead);
+                if (n > 0) break;
+                if (!place_first(carry)) { failed = true; break; }  // a single frame larger than the slot: grow the slot
+                carry.clear();
+                continue;
+            }
+            T.frame_off[n] = in_used; T.per_frame[n] = (uint32_t)toRead; T.out_off[n] = out_used;
+            if (is_zstd) { T.first_blk[n] = nblk; T.expect[n] = (nsq & 4u) ? ~0ull : osz; T.per_frame[n] = nsq; nblk = nblk_new; scr = scr_new; }
+            in_used += 12 + toRead; out_used += osz; n++;
         }
-    });
-
-    // ---- submit
-    for (;;) {
-        Slot* s;
-        {
-            std::unique_lock<std::mutex> lk(P.mu);
-            s = &P.slots[P.submit_seq % N];
-            P.cv.wait(lk, [&] { return s->state == 1 || P.error || (P.reader_done && P.submit_seq == P.fill_seq); });
-            if (P.error || s->state != 1) break;
+        if (failed || n == 0) return false;
+        T.out_off[n] = out_used;
+        if (is_zstd) { T.first_blk[n] = nblk; s->nblk = nblk; s->scratch_used = scr; }
+        s->n = n; s->in_used = in_used; s->out_used = (size_t)out_used;
+        { uint64_t ns = 0; for (uint32_t i = 0; i < n; i++) { const uint64_t nb = (T.out_off[i + 1] - T.out_off[i] + 65535) / 65536; ns += nb ? nb : 1; } s->nslots = (uint32_t)ns; }
+        c->insize += stat_in; c->frames += n;
+        return true;
+    };
+    po.submit = [&](Slot& s) -> int {
+        Tables Th = tables_at(s.h_tab, s.tab_cap), Td = tables_at(s.d_tab, s.tab_cap);
+        if (cudaMemcpyAsync(s.d_in, s.h_in, s.in_used, cudaMemcpyHostToDevice, s.stream) != cudaSuccess ||
+            cudaMemcpyAsync(s.d_tab, s.h_tab, s.tab_bytes, cudaMemcpyHostToDevice, s.stream) != cudaSuccess ||
+            (is_zstd && s.nblk && cudaMemcpyAsync(s.d_blk, s.h_blk, (size_t)s.nblk * zmt_zstd_blk_desc_bytes(), cudaMemcpyHostToDevice, s.stream) != cudaSuccess))
+            return ZMT_ST_CUDA;
+        const int st = decode_batch(is_zstd, s.d_in, s.in_used, s.d_blk, s.nblk, Td, s.n, s.nslots, s.d_out, s.d_work, s.stream);
+        if (st != ZMT_ST_OK) return st;
+        if (cudaMemcpyAsync(Th.out_size, Td.out_size, (size_t)s.n * 8, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
+            cudaMemcpyAsync(Th.status, Td.status, (size_t)s.n * 4, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
+            cudaEventRecord(s.ev, s.stream) != cudaSuccess) return ZMT_ST_CUDA;
+        return ZMT_ST_OK;
+    };
+    // pt_write, lz4-mt_decompress.c:165-187
+    po.drain = [&](Slot& s) -> bool {
+        Tables T = tables_at(s.h_tab, s.tab_cap);
+        uint32_t issued = 0, ready = 0; int np_issued = 0, np_ready = 0;       // frames [0, issued) requested, [0, ready) landed
+        auto issue_piece = [&]() -> bool {
+            if (issued >= s.n) return true;
+            uint32_t j = issued; uint64_t lo = T.out_off[j], hi = lo;
+            while (j < s.n && hi - lo < kPieceBytes) { hi = T.out_off[j] + T.out_size[j]; j++; }
+            if (hi > s.out_cap) hi = s.out_cap;
+            if (hi > lo && cudaMemcpyAsync(s.h_out + lo, s.d_out + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return false;
+            if (cudaEventRecord(s.evp[np_issued & 1], s.stream) != cudaSuccess) return false;
+            np_issued++; issued = j;
+            return true;
+        };
+        uint32_t piece_end[2] = { 0, 0 };
+        for (uint32_t i = 0; i < s.n; i++) {
+            const uint32_t st = T.status[i];
+            if (st != ZMT_ST_OK) { c->lib_errcode = st; P.fail(status_error(E, st)); return false; }
+            if (i >= ready) {
+                bool okp = true;
+                if (np_issued == np_ready) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }
+                if (okp && issued < s.n && np_issued == np_ready + 1) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }   // one ahead
+                if (okp) okp = cudaEventSynchronize(s.evp[np_ready & 1]) == cudaSuccess;
+                if (!okp) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); return false; }
+                ready = piece_end[np_ready & 1]; np_ready++;
+            }
+            GenBuffer b; b.buf = s.h_out + T.out_off[i]; b.size = (size_t)T.out_size[i]; b.allocated = b.size;
+            int rv = rw->fn_write(rw->arg_write, &b);
+            if (rv != 0) { P.fail(mt_error(E, rv)); return false; }
+            c->outsize += b.size; c->curframe++;
         }
-        cudaSetDevice(s->dev);
-        Tables Th = tables_at(s->h_tab, s->tab_cap), Td = tables_at(s->d_tab, s->tab_cap);
-        cudaError_t ce = cudaMemcpyAsync(s->d_in, s->h_in, s->in_used, cudaMemcpyHostToDevice, s->stream);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(s->d_tab, s->h_tab, s->tab_bytes, cudaMemcpyHostToDevice, s->stream);
-        int st = ZMT_ST_CUDA;
-        if (ce == cudaSuccess && is_zstd && s->nblk) ce = cudaMemcpyAsync(s->d_blk, s->h_blk, (size_t)s->nblk * zmt_zstd_blk_desc_bytes(), cudaMemcpyHostToDevice, s->stream);
-        if (ce == cudaSuccess) st = is_zstd ? zmt_zstd_decompress_device(s->d_in, s->d_blk, s->nblk, Td.g, Td.f, Td.d, s->n, s->d_out, Td.b, Td.c, Td.e, s->d_work, s->stream)
-                                            : zmt_lz4_decompress_device(s->d_in, s->in_used, Td.a, Td.d, s->n, s->nslots, s->d_out, Td.b, Td.c, Td.e, s->d_work, s->stream);
-        if (s->dev >= 0 && s->dev < 64) g_dev_batches[s->dev]++;
-        if (st == ZMT_ST_OK) {
-            if (s->out_used && piece_bytes == 0) ce = cudaMemcpyAsync(s->h_out, s->d_out, s->out_used, cudaMemcpyDeviceToHost, s->stream);
-            if (ce == cudaSuccess) ce = cudaMemcpyAsync(Th.c, Td.c, (size_t)s->n * 8, cudaMemcpyDeviceToHost, s->stream);
-            if (ce == cudaSuccess) ce = cudaMemcpyAsync(Th.e, Td.e, (size_t)s->n * 4, cudaMemcpyDeviceToHost, s->stream);
-            if (ce == cudaSuccess) ce = cudaEventRecord(s->ev, s->stream);
-            if (ce != cudaSuccess) st = ZMT_ST_CUDA;
-        }
-        if (st != ZMT_ST_OK) { c->lib_errcode = (size_t)st; P.fail(E.library); break; }
-        { std::lock_guard<std::mutex> g(P.mu); s->state = 2; P.submit_seq++; }
-        P.cv.notify_all();
-    }
-    reader.join(); writer.join();
-    for (auto& s : P.slots) { if (s.ok) { cudaSetDevice(s.dev); cudaStreamSynchronize(s.stream); } }
-    if (tr)
-        fprintf(stderr, "[zstdmt_b200] decompress: reader total %.3fs cb %.3fs scan %.3fs wait %.3fs | writer gpu-wait %.3fs cb %.3fs wait %.3fs | slots %zu, batch %zu MiB\n",
-                rd_total, rd_clk.cb, rd_scan, rd_clk.wait, wr_clk.gpu, wr_clk.cb, wr_clk.wait, N, in_cap0 >> 20);
-    (void)wr_total;
-    return P.error;
+        return true;
+    };
+    po.name = "decompress"; po.batch_bytes = in_cap0; po.scan = &rd_scan;
+    return run_pipeline(c, P.slots.size(), po);
 }
 
 // ------------------------------------------------------------------ context helpers
-Ctx* ctx_new(int codec, bool comp, int threads, int level, size_t inputsize)
+Ctx* ctx_new(int codec, int threads, int level, size_t inputsize)
 {
     Ctx* c = new (std::nothrow) Ctx();
     if (!c) return nullptr;
-    c->codec = codec; c->is_comp = comp; c->threads = threads; c->level = level; c->inputsize = inputsize;
+    c->codec = codec; c->threads = threads; c->level = level; c->inputsize = inputsize;
     c->E = codec == CODEC_LZ4 ? &kErrLz4 : &kErrZstd;
     return c;
 }
@@ -1145,8 +1075,6 @@ const char* status_string(size_t st)
 
 const char* error_string(bool lz4, size_t code, size_t lib_errcode)
 {
-    static const char* none = nullptr;
-    (void)none;
     const size_t neg = 0 - code;
     // the reference returns the codec library's own message whenever its global errcode is set
     // (lz4-mt_common.c:37-38); we own the status table instead of liblz4 / libzstd
@@ -1182,7 +1110,7 @@ void* LZ4MT_createCCtx(int threads, int level, int inputsize)                   
     if (level < 1 || level > 12) return nullptr;
     if (inputsize < 0) return nullptr;
     if (!level_ok(CODEC_LZ4, level)) return nullptr;
-    return ctx_new(CODEC_LZ4, true, threads, level, inputsize ? (size_t)inputsize : (size_t)4 << 20);
+    return ctx_new(CODEC_LZ4, threads, level, inputsize ? (size_t)inputsize : (size_t)4 << 20);
 }
 size_t LZ4MT_compressCCtx(void* ctx, void* rdwr)                                       // lz4-mt_compress.c:312-353
 {
@@ -1202,7 +1130,7 @@ void* LZ4MT_createDCtx(int threads, int inputsize)                              
 {
     if (threads < 1 || threads > 128) return nullptr;
     if (inputsize < 0) return nullptr;
-    return ctx_new(CODEC_LZ4, false, threads, 0, inputsize ? (size_t)inputsize : (size_t)64 << 10);
+    return ctx_new(CODEC_LZ4, threads, 0, inputsize ? (size_t)inputsize : (size_t)64 << 10);
 }
 size_t LZ4MT_decompressDCtx(void* ctx, void* rdwr)                                     // lz4-mt_decompress.c:485-567
 {
@@ -1236,7 +1164,7 @@ void* ZSTDCB_createCCtx(int threads, int level, int inputsize)                  
         chunk = (size_t)1 << (windowLog[idx] + 1);
         if (chunk > ((size_t)1 << 30)) chunk = (size_t)1 << 30;     // keep int-sized like the reference's int inputsize
     }
-    return ctx_new(CODEC_ZSTD, true, threads, level, chunk);
+    return ctx_new(CODEC_ZSTD, threads, level, chunk);
 }
 size_t ZSTDCB_compressCCtx(void* ctx, void* rdwr)                                      // zstd-mt_compress.c:322-392
 {
@@ -1258,7 +1186,7 @@ void* ZSTDCB_createDCtx(int threads, int inputsize)                             
 {
     if (threads < 1 || threads > 128) return nullptr;
     if (inputsize < 0) return nullptr;
-    return ctx_new(CODEC_ZSTD, false, threads, 0, inputsize ? (size_t)inputsize : (size_t)512 << 10);
+    return ctx_new(CODEC_ZSTD, threads, 0, inputsize ? (size_t)inputsize : (size_t)512 << 10);
 }
 size_t ZSTDCB_decompressDCtx(void* ctx, void* rdwr)                                    // zstd-mt_decompress.c:693-843
 {

@@ -415,17 +415,15 @@ lz4_ticket_windows_kernel(const uint64_t* __restrict__ first_slot, uint32_t nfra
     if (threadIdx.x == 0) wbase[nwin] = base;
 }
 
-// STAGED: every step's output window lives in shared memory as well (chains of matches that feed each other run at shared
-// memory latency).  zmt_lz4_decompress_device always launches the staged variant; the plain one (all reads from global
-// memory) runs only when ZSTDMT_B200_LZ4_STAGED=0 is set, for A/B measurements and tests.
-template <bool STAGED>
+// Every step's output window lives in shared memory as well (chains of matches that feed each other run at shared
+// memory latency).
 __global__ void __launch_bounds__(32 * LZD_WARPS)
 lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ frame_off,
                        const uint64_t* __restrict__ first_slot, const LzBlk* __restrict__ tab, const unsigned long long* __restrict__ rec,
                        uint32_t* __restrict__ prog, const uint32_t* __restrict__ status, const uint32_t* __restrict__ needs_seq,
                        unsigned long long* __restrict__ ticket, const unsigned long long* __restrict__ wbase, uint32_t nframes, uint32_t slot_cap)
 {
-    __shared__ __align__(16) uint8_t stage[STAGED ? LZD_WARPS : 1][STAGED ? LZX_SPAN + 32 : 16];
+    __shared__ __align__(16) uint8_t stage[LZD_WARPS][LZX_SPAN + 32];
     const uint32_t lane = threadIdx.x & 31;
     if (first_slot[nframes] > slot_cap) return;             // the scan reported the undersized table per frame
     const uint32_t nwin = (nframes + LZX_WIN - 1) / LZX_WIN;
@@ -463,7 +461,7 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
             const bool publish = !(B.flags & LZB_LAST) && (tab[t + 1].flags & LZB_LINKED);     // the next block may read this one
             bool prev_done = !linked;
             uint32_t since_pub = 0;
-            uint8_t* const S = stage[STAGED ? (threadIdx.x >> 5) : 0];
+            uint8_t* const S = stage[threadIdx.x >> 5];
             // The records of the NEXT step are loaded while this one executes (one L2 round trip less on the chain of a block).
             unsigned long long rnext = lane < B.nrec ? R[lane] : 0ull;
             for (uint32_t base = 0; base < B.nrec;) {
@@ -472,7 +470,7 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                 { const unsigned long long r = lane < cnt ? rnext : 0ull; d = (uint32_t)r & 0xFFFFFFu; ml = (uint32_t)(r >> 24) & 0xFFFFFFu; off = (uint32_t)(r >> 48); }
                 const uint32_t d0 = __shfl_sync(ZMT_FULL_MASK, d, 0);
                 // ---- the step = the longest prefix of these records whose destinations fit the staging window [d0, d0 + LZX_SPAN)
-                const uint32_t nfit = STAGED ? __popc(__ballot_sync(ZMT_FULL_MASK, ml && d + ml - d0 <= LZX_SPAN)) : cnt;       // destinations are sorted: a prefix
+                const uint32_t nfit = __popc(__ballot_sync(ZMT_FULL_MASK, ml && d + ml - d0 <= LZX_SPAN));       // destinations are sorted: a prefix
                 if (nfit == 0) {
                     // one match longer than the window: straight in global memory, by the whole warp
                     const uint32_t qml = __shfl_sync(ZMT_FULL_MASK, ml, 0), qoff = __shfl_sync(ZMT_FULL_MASK, off, 0);
@@ -529,7 +527,7 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                 const bool own = indep && ml <= LZD_LONG;               // copied by its own lane
                 // own lane: the part of the source below d0 comes from global memory — its first 8 bytes are requested NOW, before
                 // the window load below stalls on its own round trip (one latency per step instead of two)
-                const int32_t nlow = !own ? 0 : !STAGED ? (int32_t)ml : sp >= (int32_t)d0 ? 0 : ((int32_t)d0 - sp < (int32_t)ml ? (int32_t)d0 - sp : (int32_t)ml);
+                const int32_t nlow = !own ? 0 : sp >= (int32_t)d0 ? 0 : ((int32_t)d0 - sp < (int32_t)ml ? (int32_t)d0 - sp : (int32_t)ml);
                 const uint8_t* mp = dst + sp;
                 uint8_t x0[8];
 #pragma unroll
@@ -539,27 +537,25 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                 //      AND to the window; a source byte at or above d0 is read from the window.  A chain of matches that feed each
                 //      other then runs at shared-memory latency instead of one L2 round trip per link.
                 const uint32_t gsh = (uint32_t)((uintptr_t)(dst + d0) & 15);
-                if (STAGED) {
-                    const uint4* ga = reinterpret_cast<const uint4*>(dst + d0 - gsh);
-                    const uint32_t nvec = (gsh + span + 15) >> 4;
-                    for (uint32_t i = lane; i < nvec; i += 32) reinterpret_cast<uint4*>(S)[i] = ga[i];
-                }
+                const uint4* ga = reinterpret_cast<const uint4*>(dst + d0 - gsh);
+                const uint32_t nvec = (gsh + span + 15) >> 4;
+                for (uint32_t i = lane; i < nvec; i += 32) reinterpret_cast<uint4*>(S)[i] = ga[i];
                 const int32_t wb = (int32_t)gsh - (int32_t)d0;          // S[wb + p] = window byte of block position p (p >= d0)
                 __syncwarp();
                 if (own) {
                     uint8_t* dp = dst + d; uint8_t* dw = S + (wb + (int32_t)d);
 #pragma unroll
-                    for (int j = 0; j < 8; j++) if (j < nlow) { dp[j] = x0[j]; if (STAGED) dw[j] = x0[j]; }
+                    for (int j = 0; j < 8; j++) if (j < nlow) { dp[j] = x0[j]; dw[j] = x0[j]; }
                     int32_t i = 8;
                     for (; i < nlow; i += 8) {                              // loads first, stores after: one L2 latency per 8 bytes, not per byte
                         uint8_t x[8];
 #pragma unroll
                         for (int j = 0; j < 8; j++) x[j] = (i + j < nlow) ? mp[i + j] : (uint8_t)0;
 #pragma unroll
-                        for (int j = 0; j < 8; j++) if (i + j < nlow) { dp[i + j] = x[j]; if (STAGED) dw[i + j] = x[j]; }
+                        for (int j = 0; j < 8; j++) if (i + j < nlow) { dp[i + j] = x[j]; dw[i + j] = x[j]; }
                     }
                     i = nlow;
-                    for (; i < (int32_t)ml; i++) { const uint8_t x = S[wb + sp + i]; dp[i] = x; dw[i] = x; }        // STAGED only (nlow == ml otherwise)
+                    for (; i < (int32_t)ml; i++) { const uint8_t x = S[wb + sp + i]; dp[i] = x; dw[i] = x; }
                 }
                 uint32_t dm = __ballot_sync(ZMT_FULL_MASK, ml && !own);      // long independent ones too: whole warp
                 if (dm) __syncwarp();
@@ -568,16 +564,15 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                     const uint32_t qd = __shfl_sync(ZMT_FULL_MASK, d, jq), qml = __shfl_sync(ZMT_FULL_MASK, ml, jq), qoff = __shfl_sync(ZMT_FULL_MASK, off, jq);
                     const int32_t qs = (int32_t)qd - (int32_t)qoff;
                     uint8_t* dp = dst + qd; uint8_t* dw = S + (wb + (int32_t)qd);
-                    if (qoff >= qml && !STAGED && qml >= 64) warp_copy_lit(dp, dst + qs, qml, lane);
-                    else if (qoff >= qml) {
-                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)i; const uint8_t x = (STAGED && q >= (int32_t)d0) ? S[wb + q] : dst[q]; dp[i] = x; if (STAGED) dw[i] = x; }
+                    if (qoff >= qml) {
+                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)i; const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i] = x; dw[i] = x; }
                     } else if (qoff >= 32) {                            // overlapping, period >= warp width: 32-byte waves
                         for (uint32_t i = 0; i < qml; i += 32) {
-                            if (i + lane < qml) { const int32_t q = qs + (int32_t)(i + lane); const uint8_t x = (STAGED && q >= (int32_t)d0) ? S[wb + q] : dst[q]; dp[i + lane] = x; if (STAGED) dw[i + lane] = x; }
+                            if (i + lane < qml) { const int32_t q = qs + (int32_t)(i + lane); const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i + lane] = x; dw[i + lane] = x; }
                             __syncwarp();
                         }
                     } else {                                            // short period: replicate the pattern
-                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)(i % qoff); const uint8_t x = (STAGED && q >= (int32_t)d0) ? S[wb + q] : dst[q]; dp[i] = x; if (STAGED) dw[i] = x; }
+                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)(i % qoff); const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i] = x; dw[i] = x; }
                     }
                     __syncwarp();
                 }

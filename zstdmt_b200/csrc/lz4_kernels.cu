@@ -1026,15 +1026,9 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
         const uint32_t need = (nslots + LZD_WARPS - 1) / LZD_WARPS;
         ZmtProfScope ps(ZMT_K_LZ4_DEXEC, stream);
         // the shared-memory step window turns a chain of matches feeding each other into SMEM round trips instead of L2 ones
-        // (DESIGN.md §3.2); ZSTDMT_B200_LZ4_STAGED=0 keeps the plain variant for A/B
-        static const char* force = getenv("ZSTDMT_B200_LZ4_STAGED");
-        const bool staged = force ? (*force == '1') : true;
-        if (staged)
-            lz4_exec_blocks_kernel<true><<<need < maxg ? need : maxg, 32 * LZD_WARPS, 0, stream>>>(
-                (uint8_t*)d_out, d_out_off, d_frame_off, first_slot, tab, rec, prog, d_status, needs_seq, ticket, wbase, nframes, nslots);
-        else
-            lz4_exec_blocks_kernel<false><<<need < maxg ? need : maxg, 32 * LZD_WARPS, 0, stream>>>(
-                (uint8_t*)d_out, d_out_off, d_frame_off, first_slot, tab, rec, prog, d_status, needs_seq, ticket, wbase, nframes, nslots);
+        // (DESIGN.md §3.2)
+        lz4_exec_blocks_kernel<<<need < maxg ? need : maxg, 32 * LZD_WARPS, 0, stream>>>(
+            (uint8_t*)d_out, d_out_off, d_frame_off, first_slot, tab, rec, prog, d_status, needs_seq, ticket, wbase, nframes, nslots);
     }
     zmt_dbg_check(stream, "lz4_exec_blocks_kernel");
     lz4_decode_frames_seq_kernel<<<(nframes + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(

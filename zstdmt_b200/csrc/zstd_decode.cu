@@ -946,12 +946,13 @@ zstd_resolve_offsets_kernel(const ZBlk* __restrict__ blocks, const uint32_t* __r
 }
 
 // ---------------------------------------------------------------- kernel 1b: frame-sequential entropy decode
-// One warp per frame that needs state across blocks: Huffman table reuse (treeless literals), Repeat_Mode sequence
-// tables, repeat offsets.  Same per-block routine, blocks in order, state in registers / this warp's shared tables.
+// One warp per frame that needs state across blocks (Huffman table reuse, Repeat_Mode sequence tables, repeat offsets)
+// and that the block-parallel kernels could not finish.  Same per-block routine, blocks in order, state in registers /
+// this warp's shared tables.
 __global__ void __launch_bounds__(32 * ZD_WARPS)
 zstd_entropy_seq_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, const uint32_t* __restrict__ frame_first_blk,
                         const uint32_t* __restrict__ frame_seq, uint8_t* __restrict__ scratch, uint32_t* __restrict__ regen,
-                        uint32_t* __restrict__ status, uint32_t nframes, uint32_t flagged_only)
+                        uint32_t* __restrict__ status, uint32_t nframes)
 {
     __shared__ ZWarpTabs tabs[ZD_WARPS];
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -959,11 +960,11 @@ zstd_entropy_seq_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
     if (f >= nframes) return;
     const uint32_t st0 = status[f];
     const bool flagged = (st0 & 0x8000u) != 0;
-    // flagged_only: frames the host scan marked were decoded block-parallel (kernel 1c); this pass then only takes the
-    // frames a block-parallel decoder flagged at run time (a repeat offset in a frame whose headers showed no state)
-    if (!flagged && (flagged_only || !(frame_seq[f] & ZF_NEEDS_SEQ))) return;
+    // frames the host scan marked were decoded block-parallel (kernel 1c); this pass only takes the frames a
+    // block-parallel decoder flagged at run time (a repeat offset in a frame whose headers showed no state)
+    if (!flagged) return;
     __syncwarp();
-    if (lane == 0 && flagged) status[f] = 0;
+    if (lane == 0) status[f] = 0;
     ZWarpTabs& W = tabs[wid];
     zd_load_predef(W, lane);
     ZFrameState fs; fs.rep[0] = 1; fs.rep[1] = 4; fs.rep[2] = 8; fs.have_tabs = false; fs.raw_offsets = false; fs.huf_ready = false;
@@ -1333,9 +1334,6 @@ static int zd_tables_init()
     return ZMT_ST_OK;
 }
 
-extern "C" int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out, uint32_t* nblocks_io,
-                                         uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed);
-
 static inline uint32_t h_rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 
 // Walk one zstd frame on the host (frame header + 3-byte block headers + the two section headers of every
@@ -1349,9 +1347,9 @@ extern "C" int zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t
 }
 
 // same, for frames whose length is not known in advance (plain .zst streams): *consumed receives the frame length
-extern "C" int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
-                                         void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
-                                         uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed)
+int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
+                              void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
+                              uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed)
 {
     *needs_seq = 0;
     ZBlk* out = (ZBlk*)blocks_out;
@@ -1477,25 +1475,19 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
     if (nblocks) {
         cudaMemsetAsync(seq_done, 0, (size_t)nblocks * 4, stream);
         cudaMemsetAsync(lit_done, 0, (size_t)nblocks * 4, stream);
-        static const bool no_fast = getenv("ZSTDMT_B200_NO_FAST_ENTROPY") != nullptr;      // A/B knob: warp-per-block entropy decode only
-        if (!no_fast) {
-            const size_t lsm = sizeof(ZLitGroup) * ZL_GROUPS * ZL_WARPS;
-            cudaFuncSetAttribute(zstd_literals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm);
-            const uint32_t per = ZL_GROUPS * ZL_WARPS;
-            zstd_literals_kernel<<<(nblocks + per - 1) / per, 32 * ZL_WARPS, lsm, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, lit_done);
-        }
-        if (!no_fast)
+        const size_t lsm = sizeof(ZLitGroup) * ZL_GROUPS * ZL_WARPS;
+        cudaFuncSetAttribute(zstd_literals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm);
+        const uint32_t per = ZL_GROUPS * ZL_WARPS;
+        zstd_literals_kernel<<<(nblocks + per - 1) / per, 32 * ZL_WARPS, lsm, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, lit_done);
         zstd_seq_predef_kernel<<<(nblocks + ZS_THREADS - 1) / ZS_THREADS, ZS_THREADS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch,
                                                                                            seq_done, seq_ml, d_status);
         zstd_entropy_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen, d_status,
                                                                                            seq_done, seq_ml, lit_done);
-        if (!no_fast) {
-            zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen,
-                                                                                               d_status, lit_done);
-            zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, scratch, d_status, nframes);
-        }
+        zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen,
+                                                                                           d_status, lit_done);
+        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, scratch, d_status, nframes);
         zstd_entropy_seq_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
-                                                                                           scratch, regen, d_status, nframes, no_fast ? 0u : 1u);
+                                                                                           scratch, regen, d_status, nframes);
     }
     zstd_offsets_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>((const ZBlk*)d_blocks, nblocks, d_frame_first_blk, regen, blk_out, d_out_off, d_expect,
                                                                    (unsigned long long*)d_out_size, d_status, nframes);

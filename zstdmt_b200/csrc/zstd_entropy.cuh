@@ -11,9 +11,6 @@
 // Every block is self-contained (own Huffman tree, predefined sequence tables, explicit offsets: no repeat
 // codes), so the decoder can give each block its own CTA.
 #pragma once
-#ifndef Z_ALWAYS_FSE_WEIGHTS
-#define Z_ALWAYS_FSE_WEIGHTS 0
-#endif
 #include "common.cuh"
 
 #define Z_MAXSEQ     4352u           // sequences per sub-block (4 tiles x 1024 + pending + slack)
@@ -389,8 +386,8 @@ __device__ uint32_t z_encode_block(ZEnt& Z, const ZFseShared& F, ZScratch* zs, u
                 const uint32_t direct = maxsym <= 128 ? 1 + (maxsym + 1) / 2 : 0xFFFFu;
                 // The FSE form is built only where it is mandatory (a symbol above 128).  Where the direct form exists it costs
                 // <= 65 bytes per block, the FSE form would save ~30 of them (0.4 % of the output on text) — and this single-thread
-                // step is a serial wait for the whole CTA.  -DZ_ALWAYS_FSE_WEIGHTS=1 builds the FSE form wherever it is smaller.
-                const uint32_t fl = (direct == 0xFFFFu || Z_ALWAYS_FSE_WEIGHTS) ? z_fse_weights(Z, maxsym, maxbits) : 0u;
+                // step is a serial wait for the whole CTA.
+                const uint32_t fl = direct == 0xFFFFu ? z_fse_weights(Z, maxsym, maxbits) : 0u;
                 Z.wdesc_len = (fl && fl < direct) ? fl : (direct != 0xFFFFu ? 0u : 0xFFFFu);       // 0: direct form, 0xFFFF: no valid form
             }
             z_lit_sync();
