@@ -100,6 +100,54 @@ int      zmt_zstd_decompress_device(const void* d_in, const void* d_blocks, uint
                                     const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out,
                                     const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream);
 
+/* ---- Frame index on the device: the tables of the two decode calls above, built on the GPU from a container-framed
+ * stream ([LE32 0x184D2A50][LE32 4][LE32 size] + payload, repeated) that is already in HBM, for callers whose stream
+ * arrives there without passing the host (GPUDirect Storage, NCCL, the device compressors).  The host reads back only
+ * the zmt_frame_index summary to size its allocations; the tables are exactly the arguments the decode calls take.
+ *
+ *   zmt_lz4_index_device   fills d_frame_off[f], d_frame_csize[f] (f < min(nframes, max_frames)) and d_out_off[0..max_frames]:
+ *                          frame f's room is its LZ4F content size, or the block bound without one, as the host pipeline
+ *                          gives it; info.nblocks = the nslots argument of zmt_lz4_decompress_device.
+ *   zmt_zstd_index_device  fills the same three plus d_frame_first_blk[0..max_frames], d_frame_scratch[0..max_frames] (scratch
+ *                          base of each frame's blocks), d_expect[f] (content size, ~0 for a frame without one: its room is
+ *                          the block bound) and d_frame_seq[f] (ZF_* flags); info.nblocks descriptors and info.scratch_bytes
+ *                          (the third argument of zmt_zstdd_workspace_bytes) are what to allocate.
+ *   zmt_zstd_blocks_device then writes the info.nblocks descriptors into d_blocks, byte for byte what zmt_zstd_scan_frame_host
+ *                          writes for the same frames.
+ * Arrays indexed 0..max_frames hold max_frames + 1 entries; entry nframes is the total.  d_work: zmt_index_workspace_bytes.
+ * Streams up to 3 * (2^32 - 1) bytes (ZMT_ST_BAD_ARG above).  Every read stays inside [d_in, d_in + in_bytes).
+ *
+ * info.status, each the decision the host pipeline takes on the same bytes; the first failure in stream order wins:
+ *   ZMT_ST_BAD_MAGIC    a container header with the wrong magic, or a length field other than 4 (bad_frame = nframes)
+ *   ZMT_ST_TRUNCATED    a container header or payload runs past in_bytes (bad_frame = nframes)
+ *   ZMT_ST_BAD_HEADER   LZ4: an unusable LZ4F header, or a content size above 255 * payload + 65536 (bad_offset = the payload)
+ *                       An LZ4 payload without the LZ4F magic gets room 0 and indexes fine; the decoder reports BAD_MAGIC.
+ *   zstd: what zmt_zstd_scan_frame_host returns for the frame (BAD_MAGIC, BAD_HEADER, UNSUPPORTED for a dictionary ID,
+ *                       BLOCK, TRUNCATED, TRAILING); bad_offset = the frame or block header the walk stopped at, or the
+ *                       first trailing byte
+ *   ZMT_ST_DST_SMALL    more than max_frames frames: nframes is the true count, bad_frame = max_frames, bad_offset its header
+ *   in_bytes == 0       ZMT_ST_OK with nframes = 0
+ * With ZMT_ST_OK, bad_frame = nframes and bad_offset = 0.  The other fields are only meaningful with ZMT_ST_OK.
+ * The calls return ZMT_ST_OK once enqueued, ZMT_ST_BAD_ARG or ZMT_ST_CUDA. */
+typedef struct {
+    uint32_t status;        /* ZMT_ST_OK or the first failure met */
+    uint32_t bad_frame;     /* frame it was met in (== nframes when the container itself is at fault) */
+    uint64_t bad_offset;    /* stream offset where the walk stopped */
+    uint32_t nframes;       /* frames in the stream, also when > max_frames (status ZMT_ST_DST_SMALL) */
+    uint32_t nblocks;       /* zstd: descriptors to allocate; lz4: block-table slots (the nslots argument) */
+    uint64_t out_bytes;     /* d_out_off[nframes] */
+    uint64_t scratch_bytes; /* zstd: third argument of zmt_zstdd_workspace_bytes */
+} zmt_frame_index;
+
+size_t zmt_index_workspace_bytes(uint32_t max_frames);
+int    zmt_lz4_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                            uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream);
+int    zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                             uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                             uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream);
+int    zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                              const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream);
+
 /* ---- multi-GPU: one LZ4MT_* / ZSTDCB_* call deals its batches round-robin over the devices named by the
  * environment variable ZSTDMT_GPUS ("all" or "0,1,..."; default: the calling thread's current device) and re-serialises
  * the frames on the host.  zmt_device_batches(dev) = batches submitted to that device since the library was loaded. */
@@ -110,12 +158,13 @@ uint64_t zmt_device_batches(int dev);
  * events; zmt_prof_end() (after the caller synchronised the stream) sums them per kernel id. */
 enum { ZMT_K_LZ4_COMPRESS = 0, ZMT_K_XXH32, ZMT_K_LZ4_SIZES, ZMT_K_SCAN, ZMT_K_LZ4_PACK, ZMT_K_LZ4_DECODE, ZMT_K_XXH32_DEC,
        ZMT_K_ZSTD_COMPRESS, ZMT_K_ZSTD_PACK, ZMT_K_ZSTD_DECODE, ZMT_K_LZ4_DEXEC,
-       ZMT_K_ZL_HASH, ZMT_K_ZL_SORT, ZMT_K_ZL_SEARCH, ZMT_K_ZL_BLOCKS, ZMT_K_L4H_BLOCKS, ZMT_K_COUNT };
+       ZMT_K_ZL_HASH, ZMT_K_ZL_SORT, ZMT_K_ZL_SEARCH, ZMT_K_ZL_BLOCKS, ZMT_K_L4H_BLOCKS, ZMT_K_FRAME_INDEX, ZMT_K_COUNT };
 /* LZ4 decode: ZMT_K_LZ4_DECODE = pass A (token parse + literals), ZMT_K_LZ4_DEXEC = pass B (match execution)
  * zstd levels 6-22: ZMT_K_ZL_HASH = hash, ZMT_K_ZL_SORT = radix sort + prev[], ZMT_K_ZL_SEARCH = chain walk,
  * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK)
  * LZ4 levels 10-12: hash, sort and search as zstd's (ZMT_K_ZL_HASH / SORT / SEARCH), ZMT_K_L4H_BLOCKS = lazy parse +
- * LZ4 sequences; checksum, sizes, scan and pack as level 1's */
+ * LZ4 sequences; checksum, sizes, scan and pack as level 1's
+ * ZMT_K_FRAME_INDEX = one index call (container walk, frame pass, scans, summary) or one zmt_zstd_blocks_device call */
 void zmt_prof_begin(void);
 int  zmt_prof_end(double* ms, int* count, int max_ids);
 

@@ -78,6 +78,13 @@ def lib():
     L.zmt_lz4d_workspace_bytes.restype = c_sz; L.zmt_lz4d_workspace_bytes.argtypes = [c_u32, c_u32, c_u64]
     L.zmt_lz4_decompress_device.restype = ctypes.c_int
     L.zmt_lz4_decompress_device.argtypes = [c_vp, c_u64, c_vp, c_vp, c_u32, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_index_workspace_bytes.restype = c_sz; L.zmt_index_workspace_bytes.argtypes = [c_u32]
+    L.zmt_lz4_index_device.restype = ctypes.c_int
+    L.zmt_lz4_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_index_device.restype = ctypes.c_int
+    L.zmt_zstd_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_blocks_device.restype = ctypes.c_int
+    L.zmt_zstd_blocks_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_vp]
     for pre, api in (("LZ4MT", "lz4"), ("ZSTDCB", "zstd"), ("ZSTDMT", "zstd")):
         getattr(L, pre + "_createCCtx").restype = c_vp; getattr(L, pre + "_createCCtx").argtypes = [ctypes.c_int] * 3
         getattr(L, pre + "_createDCtx").restype = c_vp; getattr(L, pre + "_createDCtx").argtypes = [ctypes.c_int] * 2
@@ -193,6 +200,53 @@ def scan_frames(framed):
     return np.array(offs, dtype=np.uint64), np.array(sizes, dtype=np.uint32)
 
 
+class FrameIndex(ctypes.Structure):
+    """zmt_frame_index (include/zstdmt_b200_dev.h): the summary of a device frame index."""
+    _fields_ = [("status", c_u32), ("bad_frame", c_u32), ("bad_offset", c_u64), ("nframes", c_u32), ("nblocks", c_u32),
+                ("out_bytes", c_u64), ("scratch_bytes", c_u64)]
+
+    def __repr__(self):
+        return "FrameIndex(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
+
+
+def _device_index(d_framed, max_frames, stream, zstd):
+    """Run zmt_{lz4,zstd}_index_device over a framed stream in device memory.  Only the summary struct is read back; on
+    ZMT_ST_DST_SMALL the index runs once more with the exact frame count.  Returns (summary, device tables by name)."""
+    torch = _torch(); L = lib()
+    s = stream if stream is not None else torch.cuda.current_stream()
+    dev, nbytes = d_framed.device, d_framed.numel()
+    cap = int(max_frames) if max_frames is not None else min(nbytes // 12, 1 << 16)
+    for attempt in range(2):
+        e = lambda n, dt: torch.empty(max(n, 1), dtype=dt, device=dev)
+        t = {"frame_off": e(cap, torch.int64), "frame_csize": e(cap, torch.int32), "out_off": e(cap + 1, torch.int64)}
+        if zstd:
+            t.update(first_blk=e(cap + 1, torch.int32), frame_scratch=e(cap + 1, torch.int64), expect=e(cap, torch.int64),
+                     frame_seq=e(cap, torch.int32))
+        wb = L.zmt_index_workspace_bytes(cap)
+        if wb == 0:
+            raise ValueError("no index workspace size for %d frames" % cap)
+        work = torch.empty(wb, dtype=torch.uint8, device=dev)
+        d_info = torch.zeros(ctypes.sizeof(FrameIndex), dtype=torch.uint8, device=dev)
+        p = lambda k: t[k].data_ptr()
+        if zstd:
+            rc = L.zmt_zstd_index_device(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("first_blk"), p("frame_scratch"),
+                                         p("expect"), p("frame_seq"), p("out_off"), d_info.data_ptr(), work.data_ptr(), s.cuda_stream)
+        else:
+            rc = L.zmt_lz4_index_device(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("out_off"), d_info.data_ptr(),
+                                        work.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("frame index failed: %s" % ST_NAMES.get(rc, rc))
+        s.synchronize()
+        info = FrameIndex.from_buffer_copy(d_info.cpu().numpy().tobytes())
+        if info.status == 6 and attempt == 0:                               # ZMT_ST_DST_SMALL: info.nframes is the true count
+            cap = info.nframes
+            continue
+        break
+    if info.status != 0:
+        raise ValueError("framed stream rejected: %s in frame %d at offset %d" % (ST_NAMES.get(info.status, info.status), info.bad_frame, info.bad_offset))
+    return info, t
+
+
 class Lz4DeviceCompressor:
     """Pre-allocated device buffers + one call per batch: zmt_lz4_compress_level_device.  Levels 1-9 run the level-1
     encoder (zmt_lz4_compress_device, independent blocks), levels 10-12 the high-compression class with linked blocks."""
@@ -262,6 +316,24 @@ class Lz4DeviceDecompressor:
         self.in_bytes_cap = int((np.asarray(frame_off, dtype=np.int64) + 12 + np.asarray(frame_csize, dtype=np.int64)).max()) if self.n else 0
         self.work = torch.empty(L.zmt_lz4d_workspace_bytes(self.n, self.nslots, self.in_bytes_cap), dtype=torch.uint8, device=device)
 
+    @classmethod
+    def from_device(cls, d_framed, max_frames=None, stream=None):
+        """A decoder for a framed stream that is already in device memory: the frame tables are built on the GPU
+        (zmt_lz4_index_device) and only the summary comes back to the host, as .index_info.  run(d_framed) decodes.
+        max_frames sizes the first attempt (default: up to 65536 frames); a larger stream is indexed once more at its
+        exact count.  Raises ValueError naming the status, frame and offset of a stream the index rejects."""
+        torch = _torch(); L = lib()
+        info, t = _device_index(d_framed, max_frames, stream, zstd=False)
+        self = cls.__new__(cls)
+        self.index_info, self.n, self.nslots, self.out_total = info, info.nframes, max(info.nblocks, 1), info.out_bytes
+        self.d_off, self.d_cs, self.d_out_off = t["frame_off"], t["frame_csize"], t["out_off"]
+        self.out = torch.empty(max(self.out_total, 1), dtype=torch.uint8, device=d_framed.device)
+        self.out_size = torch.zeros(max(self.n, 1), dtype=torch.int64, device=d_framed.device)
+        self.status = torch.zeros(max(self.n, 1), dtype=torch.int32, device=d_framed.device)
+        self.in_bytes_cap = d_framed.numel()
+        self.work = torch.empty(L.zmt_lz4d_workspace_bytes(self.n, self.nslots, self.in_bytes_cap), dtype=torch.uint8, device=d_framed.device)
+        return self
+
     def run(self, d_framed, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
@@ -274,8 +346,9 @@ class Lz4DeviceDecompressor:
 
 
 class ZstdDeviceDecompressor:
-    """zmt_zstd_decompress_device.  The block table is built on the host from the framed bytes
-    (zmt_zstd_scan_frame_host: frame + block headers only), as the host pipeline does while reading."""
+    """zmt_zstd_decompress_device.  The constructor builds the block table on the host from the framed bytes
+    (zmt_zstd_scan_frame_host: frame + block headers only), as the host pipeline does while reading; from_device builds
+    it on the GPU from a stream already in device memory."""
 
     def __init__(self, framed_host, device="cuda"):
         torch = _torch(); L = lib()
@@ -301,6 +374,7 @@ class ZstdDeviceDecompressor:
         self.scan_ok = all(rc == 0 for rc in self.scan_status)
         oo = np.zeros(self.n + 1, dtype=np.int64); oo[1:] = np.cumsum(expect[: self.n].astype(np.int64))
         self.out_total = int(oo[-1])
+        expect[: self.n][(fseq[: self.n] & 4) != 0] = ~np.uint64(0)     # ZF_NO_SIZE: the room is a bound, not a size to check
         self.d_blocks = torch.from_numpy(blocks[: max(1, self.nblk) * dsz].copy()).to(device)
         self.d_first = torch.from_numpy(first.astype(np.int32)).to(device)
         self.d_expect = torch.from_numpy(expect.astype(np.int64)).to(device)
@@ -311,6 +385,30 @@ class ZstdDeviceDecompressor:
         self.out_size = torch.zeros(max(self.n, 1), dtype=torch.int64, device=device)
         self.status = torch.zeros(max(self.n, 1), dtype=torch.int32, device=device)
         self.work = torch.empty(L.zmt_zstdd_workspace_bytes(self.n, self.nblk, scr.value), dtype=torch.uint8, device=device)
+
+    @classmethod
+    def from_device(cls, d_framed, max_frames=None, stream=None):
+        """A decoder for a framed stream that is already in device memory: the frame tables and the block table are built
+        on the GPU (zmt_zstd_index_device, zmt_zstd_blocks_device) and only the summary comes back to the host, as
+        .index_info.  run(d_framed) decodes.  max_frames and the errors as Lz4DeviceDecompressor.from_device."""
+        torch = _torch(); L = lib()
+        s = stream if stream is not None else torch.cuda.current_stream()
+        info, t = _device_index(d_framed, max_frames, s, zstd=True)
+        dev = d_framed.device
+        self = cls.__new__(cls)
+        self.index_info, self.n, self.nblk, self.out_total = info, info.nframes, info.nblocks, info.out_bytes
+        self.d_first, self.d_expect, self.d_fseq, self.d_out_off = t["first_blk"], t["expect"], t["frame_seq"], t["out_off"]
+        self.d_blocks = torch.empty(max(1, self.nblk) * L.zmt_zstd_blk_desc_bytes(), dtype=torch.uint8, device=dev)
+        rc = L.zmt_zstd_blocks_device(d_framed.data_ptr(), self.n, t["frame_off"].data_ptr(), t["frame_csize"].data_ptr(), self.d_first.data_ptr(),
+                                      t["frame_scratch"].data_ptr(), self.d_blocks.data_ptr(), self.nblk, s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("zmt_zstd_blocks_device failed: %s" % ST_NAMES.get(rc, rc))
+        self.d_frame_off, self.d_frame_csize, self.d_frame_scratch = t["frame_off"], t["frame_csize"], t["frame_scratch"]
+        self.out = torch.empty(max(self.out_total, 1), dtype=torch.uint8, device=dev)
+        self.out_size = torch.zeros(max(self.n, 1), dtype=torch.int64, device=dev)
+        self.status = torch.zeros(max(self.n, 1), dtype=torch.int32, device=dev)
+        self.work = torch.empty(L.zmt_zstdd_workspace_bytes(self.n, self.nblk, info.scratch_bytes), dtype=torch.uint8, device=dev)
+        return self
 
     def run(self, d_framed, stream=None):
         torch = _torch()

@@ -1,0 +1,201 @@
+// frame_format.h — the header formats the decoders read, in one place for the host and the device.
+//
+// The host pipeline (host_api.cpp, zmt_zstd_scan_frame_host in zstd_decode.cu) and the device frame index
+// (frame_index.cu) both call these walkers, so the block table the zstd decoder takes and the room the LZ4 decoder
+// gets per frame are defined once.  Every read stays inside [p, p + n): the fields come from outside the program.
+#pragma once
+#include <stddef.h>
+#include <stdint.h>
+#include "zmt_dev.h"
+
+#ifdef __CUDACC__
+#define ZMT_HD __host__ __device__ __forceinline__
+#else
+#define ZMT_HD inline
+#endif
+
+#define ZMT_CONTAINER_MAGIC 0x184D2A50u      // [LE32 magic][LE32 4][LE32 payload size] before every frame
+#define ZMT_LZ4F_MAGIC      0x184D2204u
+#define ZMT_ZSTD_MAGIC      0xFD2FB528u
+
+ZMT_HD uint32_t zf_rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
+ZMT_HD uint64_t zf_rd64(const uint8_t* p) { return (uint64_t)zf_rd32(p) | ((uint64_t)zf_rd32(p + 4) << 32); }
+
+// ---------------------------------------------------------------- LZ4F
+// Walks an LZ4F frame's header and block headers in p[0..n) (n >= 7): *len = the frame's length, content checksum
+// included; *bound = the most its blocks decode to (blockMaxSize per compressed block).  false: the block headers run
+// past n (*bound then covers the blocks before the cut).
+ZMT_HD bool lz4f_walk(const uint8_t* p, size_t n, size_t* len, uint64_t* bound)
+{
+    const uint32_t flg = p[4];
+    const uint64_t blkmax = 1ull << (8 + 2 * ((p[5] >> 4) & 7));
+    size_t q = 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1;
+    *bound = 0;
+    for (;;) {
+        if (q + 4 > n) return false;
+        const uint32_t bh = zf_rd32(p + q); q += 4;
+        if (bh == 0) break;
+        const uint32_t bs = bh & 0x7FFFFFFFu;
+        *bound += (bh & 0x80000000u) ? bs : blkmax;
+        q += (size_t)bs + ((flg & 0x10) ? 4 : 0);
+    }
+    *len = q + ((flg & 4) ? 4 : 0);
+    return true;
+}
+
+// The room one LZ4 payload of n bytes gets in the output, from its own header (pt_decompress sizes the buffer from
+// LE64 @ payload+6, lz4-mt_decompress.c:329-335).  Returns false if the header is unusable (ZMT_ST_BAD_HEADER).
+// A payload without the LZ4F magic gets room 0: the decoder reports its precise status.
+ZMT_HD bool lz4f_out_size(const uint8_t* p, size_t n, uint64_t* out)
+{
+    if (n < 7 || zf_rd32(p) != ZMT_LZ4F_MAGIC) { *out = 0; return true; }
+    const uint32_t flg = p[4], bd = p[5];
+    if (flg & 0x08) {
+        if (n < 15) return false;
+        // untrusted field: LZ4 cannot expand by more than 255x, anything larger is a corrupt header (the reference
+        // fails its malloc there); without this bound a huge value would wrap the running output offsets
+        const uint64_t v = zf_rd64(p + 6);
+        if (v > (uint64_t)n * 255 + 65536) return false;
+        *out = v; return true;
+    }
+    // no content-size field: bound it by walking the block headers (each block <= blockMaxSize)
+    if (((bd >> 4) & 7) < 4) return false;
+    size_t len = 0;
+    lz4f_walk(p, n, &len, out);
+    return true;
+}
+
+// LZ4 decoder block-table slots a frame with this much room takes (the nslots argument sums them)
+ZMT_HD uint64_t lz4_frame_slots(uint64_t room) { const uint64_t nb = (room + 65535) / 65536; return nb ? nb : 1; }
+
+// ---------------------------------------------------------------- zstd block descriptors (the zstd decoder's block table)
+#define ZB_RAW 0u
+#define ZB_RLE 1u
+#define ZB_CMP 2u
+struct ZBlk {
+    uint64_t comp_off;      // offset of the block CONTENT (after its 3-byte header) in the input buffer
+    uint32_t comp_size;     // content bytes (1 for RLE)
+    uint32_t frame;         // frame index in the batch
+    uint32_t type;          // ZB_*
+    uint32_t regen_hint;    // raw / RLE: regenerated size; compressed: literal bytes (regenerated)
+    uint32_t nseq;          // compressed: number of sequences
+    uint32_t first;         // 1 if first block of its frame
+    uint64_t seq_off;       // scratch offsets (bytes) for this block's sequence records / literals
+    uint64_t lit_off;
+    // blocks whose tables come from an earlier block of the frame (treeless literals, Repeat_Mode sequence tables): index of
+    // the block whose section header DESCRIBES the table in use (ZB_SELF / ZB_PREDEF / ZB_NONE otherwise) — found by the
+    // frame walk, so that every block can be entropy-decoded on its own
+    uint32_t huf_src, ll_src, of_src, ml_src;
+};
+#define ZB_SELF   0xFFFFFFFFu
+#define ZB_PREDEF 0xFFFFFFFEu
+#define ZB_NONE   0xFFFFFFFDu
+struct ZDSeq { uint32_t ll; uint32_t off; uint32_t ml; uint32_t pad; };
+
+// per-frame flags (the d_frame_seq[] argument of zmt_zstd_decompress_device)
+#define ZF_NEEDS_SEQ 1u     // blocks depend on earlier blocks: frame-sequential entropy pass
+#define ZF_CHECKSUM  2u     // 4-byte content checksum (low 32 bits of XXH64) follows the last block
+#define ZF_NO_SIZE   4u     // no Frame_Content_Size: the reported size is an upper bound (128 KiB per compressed block)
+
+// Walks one zstd frame in frame[0..n) (frame header + 3-byte block headers + the two section headers of every
+// compressed block).  `base_off` = offset of the frame's first byte in the decoder's input buffer.
+// W = true writes one descriptor per accepted block at blocks_out[*nblocks_io++] (below index max_blocks); W = false
+// only counts them.  Either way *nblocks_io advances by the block count, *scratch_used by the entropy scratch the
+// blocks take (their seq_off / lit_off), *flags receives the ZF_* bits and, on success, *content_size the frame content
+// size (the block bound without a content-size field).  *end = the frame's length on success, else the offset of the
+// header element the walk stopped at.  Bytes behind the frame are the caller's business.  Returns ZMT_ST_*.
+template <bool W>
+ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
+                           uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size,
+                           uint32_t* flags, size_t* end)
+{
+    *flags = 0; *end = 0;
+    if (n < 6 || zf_rd32(frame) != ZMT_ZSTD_MAGIC) return n < 6 ? ZMT_ST_TRUNCATED : ZMT_ST_BAD_MAGIC;
+    const uint32_t fhd = frame[4], fcs = fhd >> 6, single = (fhd >> 5) & 1, did = fhd & 3;
+    if (fhd & 0x08) return ZMT_ST_BAD_HEADER;
+    const bool has_chk = (fhd & 0x04) != 0;                          // XXH64 content checksum after the last block (verified on the device)
+    if (did) return ZMT_ST_UNSUPPORTED;                               // dictionaries: not on the reference path
+    size_t pos = 5 + (single ? 0 : 1);
+    const size_t fl = fcs == 0 ? (single ? 1 : 0) : fcs == 1 ? 2 : fcs == 2 ? 4 : 8;
+    if (n < pos + fl) return ZMT_ST_TRUNCATED;
+    uint64_t cs = 0;
+    if (fl == 1) cs = frame[pos]; else if (fl == 2) cs = (uint64_t)(frame[pos] | (frame[pos + 1] << 8)) + 256;
+    else if (fl == 4) cs = zf_rd32(frame + pos); else if (fl == 8) cs = zf_rd64(frame + pos);
+    pos += fl;
+    const bool no_size = fl == 0;                                     // streamed frame: size from the blocks (bound: 128 KiB per compressed block)
+    uint64_t bound = 0;
+    if (has_chk) *flags |= ZF_CHECKSUM;
+    if (no_size) *flags |= ZF_NO_SIZE;
+    bool first = true;
+    uint32_t last_huf = ZB_NONE, cur_src[3] = { ZB_NONE, ZB_NONE, ZB_NONE };     // block that last described the Huffman tree / each sequence table
+    for (;;) {
+        *end = pos;
+        if (n - pos < 3) return ZMT_ST_TRUNCATED;
+        const uint32_t bh = frame[pos] | (frame[pos + 1] << 8) | ((uint32_t)frame[pos + 2] << 16); pos += 3;
+        const uint32_t last = bh & 1, type = (bh >> 1) & 3, bs = bh >> 3;
+        if (type == 3 || bs > 128 * 1024) return ZMT_ST_BLOCK;
+        if (*nblocks_io >= max_blocks) return ZMT_ST_DST_SMALL;
+        ZBlk B = ZBlk();                                              // no padding: every byte is zeroed
+        B.frame = frame_idx; B.type = type; B.first = first ? 1 : 0; B.comp_off = base_off + pos;
+        bound += type == ZB_CMP ? 128 * 1024 : bs;
+        if (type == ZB_RAW) { if (n - pos < bs) return ZMT_ST_TRUNCATED; B.comp_size = bs; B.regen_hint = bs; pos += bs; }
+        else if (type == ZB_RLE) { if (n - pos < 1) return ZMT_ST_TRUNCATED; B.comp_size = 1; B.regen_hint = bs; pos += 1; }
+        else {
+            if (n - pos < bs || bs < 2) return ZMT_ST_TRUNCATED;
+            const uint8_t* s = frame + pos;
+            const uint32_t b0 = s[0], lt = b0 & 3, sf = (b0 >> 2) & 3;
+            uint32_t lregen, lcomp, lhdr;
+            if (lt < 2) {
+                if (sf == 0 || sf == 2) { lregen = b0 >> 3; lhdr = 1; }
+                else if (sf == 1) { if (bs < 2) return ZMT_ST_BLOCK; lregen = (b0 >> 4) | ((uint32_t)s[1] << 4); lhdr = 2; }
+                else { if (bs < 3) return ZMT_ST_BLOCK; lregen = (b0 >> 4) | ((uint32_t)s[1] << 4) | ((uint32_t)s[2] << 12); lhdr = 3; }
+                lcomp = lt == 0 ? lregen : 1;
+            } else {
+                if (bs < 5) return ZMT_ST_BLOCK;
+                if (sf < 2) { const uint32_t v = s[0] | (s[1] << 8) | ((uint32_t)s[2] << 16); lregen = (v >> 4) & 0x3FF; lcomp = (v >> 14) & 0x3FF; lhdr = 3; }
+                else if (sf == 2) { const uint32_t v = zf_rd32(s); lregen = (v >> 4) & 0x3FFF; lcomp = (v >> 18) & 0x3FFF; lhdr = 4; }
+                else { const uint64_t v = (uint64_t)zf_rd32(s) | ((uint64_t)s[4] << 32); lregen = (uint32_t)((v >> 4) & 0x3FFFF); lcomp = (uint32_t)((v >> 22) & 0x3FFFF); lhdr = 5; }
+            }
+            if ((uint64_t)lhdr + lcomp + 1 > bs) return ZMT_ST_BLOCK;
+            const uint8_t* q = s + lhdr + lcomp; const uint32_t qn = bs - lhdr - lcomp;
+            uint32_t nseq; const uint32_t q0 = q[0];
+            if (q0 == 0) nseq = 0; else if (q0 < 128) nseq = q0;
+            else if (q0 < 255) { if (qn < 2) return ZMT_ST_BLOCK; nseq = ((q0 - 128) << 8) + q[1]; }
+            else { if (qn < 3) return ZMT_ST_BLOCK; nseq = q[1] + (q[2] << 8) + 0x7F00; }
+            // state across blocks visible in the headers: treeless literals, FSE-coded weights are fine block-parallel,
+            // any non-predefined sequence table mode may be followed by Repeat_Mode -> frame-sequential pass
+            {
+                const uint32_t used = q0 == 0 ? 1u : q0 < 128 ? 1u : q0 < 255 ? 2u : 3u;
+                if (lt == 3) *flags |= ZF_NEEDS_SEQ;
+                if (nseq && qn > used && q[used] != 0) *flags |= ZF_NEEDS_SEQ;
+                const uint32_t me = *nblocks_io;
+                B.huf_src = ZB_SELF;
+                if (lt == 2) last_huf = me; else if (lt == 3) B.huf_src = last_huf;
+                B.ll_src = B.of_src = B.ml_src = ZB_SELF;
+                if (nseq && qn > used) {
+                    uint32_t src[3];
+#pragma unroll
+                    for (uint32_t t = 0; t < 3; t++) {
+                        const uint32_t mode = (q[used] >> (6 - 2 * t)) & 3;
+                        if (mode == 0) cur_src[t] = ZB_PREDEF; else if (mode != 3) cur_src[t] = me;
+                        src[t] = (mode == 3) ? cur_src[t] : (mode == 0 ? ZB_PREDEF : ZB_SELF);
+                    }
+                    B.ll_src = src[0]; B.of_src = src[1]; B.ml_src = src[2];
+                }
+            }
+            B.comp_size = bs; B.regen_hint = lregen; B.nseq = nseq;
+            B.seq_off = *scratch_used; *scratch_used += (((uint64_t)nseq * sizeof(ZDSeq)) + 15) & ~15ull;
+            B.lit_off = *scratch_used; *scratch_used += ((uint64_t)lregen + 15) & ~15ull;
+            pos += bs;
+        }
+        if (W) blocks_out[*nblocks_io] = B;
+        (*nblocks_io)++;
+        first = false;
+        if (last) break;
+    }
+    *end = pos;
+    if (has_chk) { if (n - pos < 4) return ZMT_ST_TRUNCATED; pos += 4; }
+    *content_size = no_size ? bound : cs;
+    *end = pos;
+    return ZMT_ST_OK;
+}

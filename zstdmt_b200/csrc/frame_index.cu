@@ -1,0 +1,223 @@
+// frame_index.cu — the decoders' tables, built on the GPU from a container-framed stream that is already in HBM.
+//
+// zmt_lz4_decompress_device and zmt_zstd_decompress_device take per-frame tables (and, for zstd, a block table) that the
+// host pipeline builds while its reader walks the headers.  A caller whose stream reaches HBM some other way (GPUDirect
+// Storage, NCCL, our own device compressor) builds them here instead, and the host learns only a summary to size its
+// allocations with:
+//   zidx_walk_kernel          one thread follows the chain of 12-byte container headers (one dependent load per frame)
+//   zidx_lz4_frames_kernel    one thread per frame: the LZ4F room rule (lz4f_out_size) and the block-table slot count
+//   zidx_zstd_frames_kernel   one thread per frame: the counting walk of zstd_frame_walk (blocks, scratch, content size, flags)
+//   cub::DeviceScan           exclusive sums in place: output offsets, first block, scratch bases, slots
+//   zidx_summary_kernel       one thread: the first failure in stream order and the totals (zmt_frame_index)
+//   zidx_zstd_blocks_kernel   one thread per frame: the writing walk of zstd_frame_walk fills the ZBlk table
+// The header formats live in frame_format.h, shared with the host walkers, so both sources of tables agree byte for byte.
+#include <stdint.h>
+#include <cub/device/device_scan.cuh>
+#include "frame_format.h"
+
+extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
+
+namespace {
+
+constexpr uint32_t kThreads = 128;
+constexpr uint64_t kMaxIndexBytes = 3ull * 0xFFFFFFFFull;     // frames (>= 12 B), zstd blocks (>= 3 B) and LZ4 slots then fit in 32 bits
+
+struct IdxCtl {
+    uint32_t nframes;       // container headers accepted
+    uint32_t cstatus;       // ZMT_ST_* of the container walk
+    uint32_t first_bad;     // lowest frame index whose per-frame pass failed (~0: none)
+    uint32_t pad;
+    uint64_t coff;          // stream offset where the container walk stopped
+    uint64_t max_off;       // offset of frame max_frames' header (the first one not stored)
+};
+
+__host__ __device__ inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
+
+struct IdxWork { IdxCtl* ctl; uint32_t* fstat; uint64_t* fstop; uint64_t* slots; void* tmp; size_t tmp_bytes; };
+
+// workspace: ctl | per-frame status | per-frame stop offset | LZ4 slots (max_frames + 1) | cub scan storage
+size_t scan_tmp_bytes(uint32_t max_frames)
+{
+    size_t t64 = 0, t32 = 0;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, t64, (uint64_t*)nullptr, (int)max_frames + 1) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, t32, (uint32_t*)nullptr, (int)max_frames + 1) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return t64 > t32 ? t64 : t32;
+}
+
+IdxWork carve(void* d_work, uint32_t max_frames, size_t tmp_bytes)
+{
+    uint8_t* w = (uint8_t*)d_work;
+    IdxWork k;
+    k.ctl = (IdxCtl*)w; w += 256;
+    k.fstat = (uint32_t*)w; w += a256((uint64_t)max_frames * 4);
+    k.fstop = (uint64_t*)w; w += a256((uint64_t)max_frames * 8);
+    k.slots = (uint64_t*)w; w += a256(((uint64_t)max_frames + 1) * 8);
+    k.tmp = w; k.tmp_bytes = tmp_bytes;
+    return k;
+}
+
+__global__ void zidx_walk_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t max_frames, uint64_t* __restrict__ frame_off,
+                                 uint32_t* __restrict__ frame_csize, IdxCtl* __restrict__ ctl)
+{
+    uint64_t pos = 0, max_off = 0;
+    uint32_t n = 0, st = ZMT_ST_OK;
+    while (pos < in_bytes) {
+        if (in_bytes - pos < 12) { st = ZMT_ST_TRUNCATED; break; }
+        const uint8_t* h = in + pos;
+        if (zf_rd32(h) != ZMT_CONTAINER_MAGIC || zf_rd32(h + 4) != 4) { st = ZMT_ST_BAD_MAGIC; break; }
+        const uint32_t cs = zf_rd32(h + 8);
+        if (in_bytes - pos - 12 < cs) { st = ZMT_ST_TRUNCATED; break; }
+        if (n < max_frames) { frame_off[n] = pos; frame_csize[n] = cs; }
+        else if (n == max_frames) max_off = pos;
+        n++; pos += 12 + (uint64_t)cs;
+    }
+    ctl->nframes = n; ctl->cstatus = st; ctl->first_bad = 0xFFFFFFFFu; ctl->coff = pos; ctl->max_off = max_off;
+}
+
+__device__ __forceinline__ void zidx_fail(IdxWork k, uint32_t f, uint32_t st, uint64_t at)
+{
+    k.fstat[f] = st; k.fstop[f] = at;
+    atomicMin(&k.ctl->first_bad, f);
+}
+
+// f in [0, max_frames]: the entries behind the stored frames are zeroed, so the scans over max_frames + 1 entries leave
+// the totals at index min(nframes, max_frames)
+__global__ void __launch_bounds__(kThreads)
+zidx_lz4_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
+                       uint64_t* __restrict__ out_off, IdxWork k, uint32_t max_frames)
+{
+    const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+    if (f > max_frames) return;
+    const uint32_t stored = min(k.ctl->nframes, max_frames);
+    uint64_t room = 0, slots = 0;
+    if (f < stored) {
+        const uint64_t p = frame_off[f] + 12;
+        if (lz4f_out_size(in + p, frame_csize[f], &room)) slots = lz4_frame_slots(room);
+        else { room = 0; zidx_fail(k, f, ZMT_ST_BAD_HEADER, p); }
+    }
+    out_off[f] = room; k.slots[f] = slots;
+}
+
+__global__ void __launch_bounds__(kThreads)
+zidx_zstd_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
+                        uint32_t* __restrict__ first_blk, uint64_t* __restrict__ frame_scratch, uint64_t* __restrict__ expect,
+                        uint32_t* __restrict__ frame_seq, uint64_t* __restrict__ out_off, IdxWork k, uint32_t max_frames)
+{
+    const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+    if (f > max_frames) return;
+    const uint32_t stored = min(k.ctl->nframes, max_frames);
+    uint32_t nb = 0, flags = 0; uint64_t scr = 0, cs = 0;
+    if (f < stored) {
+        const uint64_t p = frame_off[f] + 12;
+        const uint32_t n = frame_csize[f];
+        size_t end = 0;
+        int r = zstd_frame_walk<false>(in + p, n, p, f, nullptr, &nb, 0xFFFFFFFFu, &scr, &cs, &flags, &end);
+        if (r == ZMT_ST_OK && end != n) r = ZMT_ST_TRAILING;
+        if (r != ZMT_ST_OK) { nb = 0; scr = 0; cs = 0; flags = 0; zidx_fail(k, f, (uint32_t)r, p + end); }
+    }
+    first_blk[f] = nb; frame_scratch[f] = scr; out_off[f] = cs;
+    if (f < max_frames) { expect[f] = (flags & ZF_NO_SIZE) ? ~0ull : cs; frame_seq[f] = flags; }
+}
+
+__global__ void zidx_summary_kernel(IdxWork k, uint32_t max_frames, const uint64_t* __restrict__ out_off, const uint32_t* __restrict__ first_blk,
+                                    const uint64_t* __restrict__ frame_scratch, zmt_frame_index* __restrict__ info)
+{
+    const IdxCtl c = *k.ctl;
+    const uint32_t stored = min(c.nframes, max_frames);
+    zmt_frame_index r;
+    r.status = c.cstatus; r.bad_frame = c.nframes; r.bad_offset = c.cstatus == ZMT_ST_OK ? 0 : c.coff;
+    if (c.nframes > max_frames) { r.status = ZMT_ST_DST_SMALL; r.bad_frame = max_frames; r.bad_offset = c.max_off; }
+    if (c.first_bad < stored) { r.status = k.fstat[c.first_bad]; r.bad_frame = c.first_bad; r.bad_offset = k.fstop[c.first_bad]; }
+    r.nframes = c.nframes;
+    r.out_bytes = out_off[stored];
+    if (first_blk) { r.nblocks = first_blk[stored]; r.scratch_bytes = frame_scratch[stored]; }
+    else { r.nblocks = (uint32_t)k.slots[stored]; r.scratch_bytes = 0; }
+    *info = r;
+}
+
+__global__ void __launch_bounds__(kThreads)
+zidx_zstd_blocks_kernel(const uint8_t* __restrict__ in, uint32_t nframes, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
+                        const uint32_t* __restrict__ first_blk, const uint64_t* __restrict__ frame_scratch, ZBlk* __restrict__ blocks, uint32_t nblocks)
+{
+    const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+    if (f >= nframes) return;
+    const uint64_t p = frame_off[f] + 12;
+    uint32_t nb = first_blk[f], flags = 0;
+    const uint32_t lim = min(first_blk[f + 1], nblocks);
+    uint64_t scr = frame_scratch[f], cs = 0;
+    size_t end = 0;
+    zstd_frame_walk<true>(in + p, frame_csize[f], p, f, blocks, &nb, lim, &scr, &cs, &flags, &end);
+}
+
+// The common part of both index calls: container walk, per-frame pass, scans, summary.
+template <typename FramePass>
+int index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize, uint64_t* d_out_off,
+                 uint32_t* d_first_blk, uint64_t* d_frame_scratch, zmt_frame_index* d_info, void* d_work, cudaStream_t stream, FramePass pass)
+{
+    if (in_bytes > kMaxIndexBytes || max_frames >= 0x7FFFFFFFu || !d_info || !d_work || !d_out_off || (max_frames && (!d_frame_off || !d_frame_csize)))
+        return ZMT_ST_BAD_ARG;
+    const size_t tb = scan_tmp_bytes(max_frames);
+    if (!tb) return ZMT_ST_CUDA;
+    const IdxWork k = carve(d_work, max_frames, tb);
+    const int nitems = (int)max_frames + 1;
+    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    zidx_walk_kernel<<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k.ctl);
+    pass((max_frames + kThreads) / kThreads, k);
+    size_t t = k.tmp_bytes;
+    bool ok = cub::DeviceScan::ExclusiveSum(k.tmp, t, d_out_off, nitems, stream) == cudaSuccess;
+    if (d_first_blk) {
+        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, d_first_blk, nitems, stream) == cudaSuccess;
+        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, d_frame_scratch, nitems, stream) == cudaSuccess;
+    } else {
+        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, k.slots, nitems, stream) == cudaSuccess;
+    }
+    zidx_summary_kernel<<<1, 1, 0, stream>>>(k, max_frames, d_out_off, d_first_blk, d_frame_scratch, d_info);
+    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
+    return ok && cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+}  // namespace
+
+extern "C" size_t zmt_index_workspace_bytes(uint32_t max_frames)
+{
+    if (max_frames >= 0x7FFFFFFFu) return 0;
+    const size_t tb = scan_tmp_bytes(max_frames);
+    if (!tb) return 0;
+    return 256 + a256((uint64_t)max_frames * 4) + a256((uint64_t)max_frames * 8) + a256(((uint64_t)max_frames + 1) * 8) + tb;
+}
+
+extern "C" int zmt_lz4_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                    uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, nullptr, nullptr, d_info, d_work, stream,
+                        [&](uint32_t grid, IdxWork k) {
+                            zidx_lz4_frames_kernel<<<grid, kThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, d_frame_csize, d_out_off, k, max_frames);
+                        });
+}
+
+extern "C" int zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                     uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                     uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!d_frame_first_blk || !d_frame_scratch || (max_frames && (!d_expect || !d_frame_seq))) return ZMT_ST_BAD_ARG;
+    return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, d_frame_first_blk, d_frame_scratch, d_info, d_work, stream,
+                        [&](uint32_t grid, IdxWork k) {
+                            zidx_zstd_frames_kernel<<<grid, kThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, d_frame_csize, d_frame_first_blk,
+                                                                                 d_frame_scratch, d_expect, d_frame_seq, d_out_off, k, max_frames);
+                        });
+}
+
+extern "C" int zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                      const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (nframes == 0 || nblocks == 0) return ZMT_ST_OK;
+    if (!d_in || !d_frame_off || !d_frame_csize || !d_frame_first_blk || !d_frame_scratch || !d_blocks) return ZMT_ST_BAD_ARG;
+    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    zidx_zstd_blocks_kernel<<<(nframes + kThreads - 1) / kThreads, kThreads, 0, stream>>>((const uint8_t*)d_in, nframes, d_frame_off, d_frame_csize,
+                                                                                         d_frame_first_blk, d_frame_scratch, (ZBlk*)d_blocks, nblocks);
+    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}

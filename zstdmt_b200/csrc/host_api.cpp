@@ -31,6 +31,7 @@
 #include <mutex>
 #include <thread>
 #include <vector>
+#include "frame_format.h"
 #include "host_common.h"
 #include "zmt_dev.h"
 
@@ -552,49 +553,6 @@ size_t compress_run(Ctx* c, GenRdWr* rw)
 }
 
 // ------------------------------------------------------------------ decompression
-// Walks an LZ4F frame's header and block headers in p[0..n) (n >= 7): *len = the frame's length, content checksum
-// included; *bound = the most its blocks decode to (blockMaxSize per compressed block).  false: the block headers run
-// past n (*bound then covers the blocks before the cut).
-bool lz4f_walk(const uint8_t* p, size_t n, size_t* len, uint64_t* bound)
-{
-    const uint32_t flg = p[4];
-    const uint64_t blkmax = 1ull << (8 + 2 * ((p[5] >> 4) & 7));
-    size_t q = 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1;
-    *bound = 0;
-    for (;;) {
-        if (q + 4 > n) return false;
-        const uint32_t bh = rd32(p + q); q += 4;
-        if (bh == 0) break;
-        const uint32_t bs = bh & 0x7FFFFFFFu;
-        *bound += (bh & 0x80000000u) ? bs : blkmax;
-        q += (size_t)bs + ((flg & 0x10) ? 4 : 0);
-    }
-    *len = q + ((flg & 4) ? 4 : 0);
-    return true;
-}
-
-// Output size of one payload, from its own header (pt_decompress sizes the buffer from
-// LE64 @ payload+6, lz4-mt_decompress.c:329-335; zstd: frame content size).
-// Returns false if the header is unusable.
-bool lz4f_out_size(const uint8_t* p, size_t n, uint64_t* out)
-{
-    if (n < 7 || rd32(p) != LZ4F_MAGIC) { *out = 0; return true; }     // the device decoder reports the precise status
-    const uint32_t flg = p[4], bd = p[5];
-    if (flg & 0x08) {
-        if (n < 15) return false;
-        // untrusted field: LZ4 cannot expand by more than 255x, anything larger is a corrupt header (the reference
-        // fails its malloc there); without this bound a huge value would wrap the running output offsets
-        const uint64_t v = rd64(p + 6);
-        if (v > (uint64_t)n * 255 + 65536) return false;
-        *out = v; return true;
-    }
-    // no content-size field: bound it by walking the block headers (each block <= blockMaxSize)
-    if (((bd >> 4) & 7) < 4) return false;
-    size_t len = 0;
-    lz4f_walk(p, n, &len, out);
-    return true;
-}
-
 // reads exactly `want` bytes unless EOF; returns 0 ok / error; *got = delivered
 size_t read_some(const ErrCodes& E, GenRdWr* rw, void* dst, size_t want, size_t* got)
 {
@@ -683,7 +641,7 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                 uint64_t osz = bound;
                 if (flg & 8) { osz = rd64(s + pos + 6); if (osz > bound) { c->lib_errcode = ZMT_ST_CONTENT_SIZE; return E.library; } }    // untrusted field, bounded by the block walk
                 foff.push_back(pos); fcs.push_back((uint32_t)len); ooff.push_back(ooff.back() + osz);
-                { const uint64_t nb = (osz + 65535) / 65536; nslots += nb ? nb : 1; }
+                nslots += lz4_frame_slots(osz);
                 pos += len;
             } else {
                 if (magic < 0xFD2FB522u || magic > 0xFD2FB528u) return E.data_error;
@@ -968,7 +926,7 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
         T.out_off[n] = out_used;
         if (is_zstd) { T.first_blk[n] = nblk; s->nblk = nblk; s->scratch_used = scr; }
         s->n = n; s->in_used = in_used; s->out_used = (size_t)out_used;
-        { uint64_t ns = 0; for (uint32_t i = 0; i < n; i++) { const uint64_t nb = (T.out_off[i + 1] - T.out_off[i] + 65535) / 65536; ns += nb ? nb : 1; } s->nslots = (uint32_t)ns; }
+        { uint64_t ns = 0; for (uint32_t i = 0; i < n; i++) ns += lz4_frame_slots(T.out_off[i + 1] - T.out_off[i]); s->nslots = (uint32_t)ns; }
         c->insize += stat_in; c->frames += n;
         return true;
     };

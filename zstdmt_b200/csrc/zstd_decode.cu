@@ -33,39 +33,11 @@
 #include <mutex>
 #include <vector>
 #include "common.cuh"
+#include "frame_format.h"
 #include "host_common.h"
 #include "zmt_dev.h"
 
 extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
-
-// ---------------------------------------------------------------- block descriptors (host-built)
-#define ZB_RAW 0u
-#define ZB_RLE 1u
-#define ZB_CMP 2u
-struct ZBlk {
-    uint64_t comp_off;      // offset of the block CONTENT (after its 3-byte header) in the input buffer
-    uint32_t comp_size;     // content bytes (1 for RLE)
-    uint32_t frame;         // frame index in the batch
-    uint32_t type;          // ZB_*
-    uint32_t regen_hint;    // raw / RLE: regenerated size; compressed: literal bytes (regenerated)
-    uint32_t nseq;          // compressed: number of sequences
-    uint32_t first;         // 1 if first block of its frame
-    uint64_t seq_off;       // scratch offsets (bytes) for this block's sequence records / literals
-    uint64_t lit_off;
-    // blocks whose tables come from an earlier block of the frame (treeless literals, Repeat_Mode sequence tables): index of
-    // the block whose section header DESCRIBES the table in use (ZB_SELF / ZB_PREDEF / ZB_NONE otherwise) — found by the
-    // host scan, so that every block can be entropy-decoded on its own
-    uint32_t huf_src, ll_src, of_src, ml_src;
-};
-#define ZB_SELF   0xFFFFFFFFu
-#define ZB_PREDEF 0xFFFFFFFEu
-#define ZB_NONE   0xFFFFFFFDu
-struct ZDSeq { uint32_t ll; uint32_t off; uint32_t ml; uint32_t pad; };
-
-// per-frame flags (the d_frame_seq[] argument; produced by zmt_zstd_scan_frame_host)
-#define ZF_NEEDS_SEQ 1u     // blocks depend on earlier blocks: frame-sequential entropy pass
-#define ZF_CHECKSUM  2u     // 4-byte content checksum (low 32 bits of XXH64) follows the last block
-#define ZF_NO_SIZE   4u     // no Frame_Content_Size: the reported size is an upper bound (128 KiB per compressed block)
 
 // ---------------------------------------------------------------- predefined FSE decode tables
 struct ZFseDTable { uint8_t sym[64]; uint8_t nb[64]; uint16_t base[64]; uint32_t log; };
@@ -1334,11 +1306,9 @@ static int zd_tables_init()
     return ZMT_ST_OK;
 }
 
-static inline uint32_t h_rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
-
 // Walk one zstd frame on the host (frame header + 3-byte block headers + the two section headers of every
-// compressed block).  `base_off` = offset of the frame's first byte inside the batch input buffer.
-// Appends block descriptors (scratch offsets assigned from *scratch_used).  Returns ZMT_ST_*.
+// compressed block; zstd_frame_walk in frame_format.h).  `base_off` = offset of the frame's first byte inside the batch
+// input buffer.  Appends block descriptors (scratch offsets assigned from *scratch_used).  Returns ZMT_ST_*.
 extern "C" int zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
                                         void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
                                         uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq)
@@ -1351,92 +1321,12 @@ int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off,
                               void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
                               uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed)
 {
-    *needs_seq = 0;
-    ZBlk* out = (ZBlk*)blocks_out;
-    if (n < 6 || h_rd32(frame) != 0xFD2FB528u) return n < 6 ? ZMT_ST_TRUNCATED : ZMT_ST_BAD_MAGIC;
-    const uint32_t fhd = frame[4], fcs = fhd >> 6, single = (fhd >> 5) & 1, did = fhd & 3;
-    if (fhd & 0x08) return ZMT_ST_BAD_HEADER;
-    const bool has_chk = (fhd & 0x04) != 0;                          // XXH64 content checksum after the last block (verified on the device)
-    if (did) return ZMT_ST_UNSUPPORTED;                               // dictionaries: not on the reference path
-    size_t pos = 5 + (single ? 0 : 1);
-    const size_t fl = fcs == 0 ? (single ? 1 : 0) : fcs == 1 ? 2 : fcs == 2 ? 4 : 8;
-    if (n < pos + fl) return ZMT_ST_TRUNCATED;
-    uint64_t cs = 0;
-    if (fl == 1) cs = frame[pos]; else if (fl == 2) cs = (uint64_t)(frame[pos] | (frame[pos + 1] << 8)) + 256;
-    else if (fl == 4) cs = h_rd32(frame + pos); else if (fl == 8) cs = (uint64_t)h_rd32(frame + pos) | ((uint64_t)h_rd32(frame + pos + 4) << 32);
-    pos += fl;
-    const bool no_size = fl == 0;                                     // streamed frame: size from the blocks (bound: 128 KiB per compressed block)
-    uint64_t bound = 0;
-    if (has_chk) *needs_seq |= ZF_CHECKSUM;
-    if (no_size) *needs_seq |= ZF_NO_SIZE;
-    bool first = true;
-    uint32_t last_huf = ZB_NONE, cur_src[3] = { ZB_NONE, ZB_NONE, ZB_NONE };     // block that last described the Huffman tree / each sequence table
-    for (;;) {
-        if (n - pos < 3) return ZMT_ST_TRUNCATED;
-        const uint32_t bh = frame[pos] | (frame[pos + 1] << 8) | ((uint32_t)frame[pos + 2] << 16); pos += 3;
-        const uint32_t last = bh & 1, type = (bh >> 1) & 3, bs = bh >> 3;
-        if (type == 3 || bs > 128 * 1024) return ZMT_ST_BLOCK;
-        if (*nblocks_io >= max_blocks) return ZMT_ST_DST_SMALL;
-        ZBlk& B = out[*nblocks_io];
-        memset(&B, 0, sizeof(B));
-        B.frame = frame_idx; B.type = type; B.first = first ? 1 : 0; B.comp_off = base_off + pos;
-        bound += type == ZB_CMP ? 128 * 1024 : bs;
-        if (type == ZB_RAW) { if (n - pos < bs) return ZMT_ST_TRUNCATED; B.comp_size = bs; B.regen_hint = bs; pos += bs; }
-        else if (type == ZB_RLE) { if (n - pos < 1) return ZMT_ST_TRUNCATED; B.comp_size = 1; B.regen_hint = bs; pos += 1; }
-        else {
-            if (n - pos < bs || bs < 2) return ZMT_ST_TRUNCATED;
-            const uint8_t* s = frame + pos;
-            const uint32_t b0 = s[0], lt = b0 & 3, sf = (b0 >> 2) & 3;
-            uint32_t lregen, lcomp, lhdr;
-            if (lt < 2) {
-                if (sf == 0 || sf == 2) { lregen = b0 >> 3; lhdr = 1; }
-                else if (sf == 1) { if (bs < 2) return ZMT_ST_BLOCK; lregen = (b0 >> 4) | ((uint32_t)s[1] << 4); lhdr = 2; }
-                else { if (bs < 3) return ZMT_ST_BLOCK; lregen = (b0 >> 4) | ((uint32_t)s[1] << 4) | ((uint32_t)s[2] << 12); lhdr = 3; }
-                lcomp = lt == 0 ? lregen : 1;
-            } else {
-                if (bs < 5) return ZMT_ST_BLOCK;
-                if (sf < 2) { const uint32_t v = s[0] | (s[1] << 8) | ((uint32_t)s[2] << 16); lregen = (v >> 4) & 0x3FF; lcomp = (v >> 14) & 0x3FF; lhdr = 3; }
-                else if (sf == 2) { const uint32_t v = h_rd32(s); lregen = (v >> 4) & 0x3FFF; lcomp = (v >> 18) & 0x3FFF; lhdr = 4; }
-                else { const uint64_t v = (uint64_t)h_rd32(s) | ((uint64_t)s[4] << 32); lregen = (uint32_t)((v >> 4) & 0x3FFFF); lcomp = (uint32_t)((v >> 22) & 0x3FFFF); lhdr = 5; }
-            }
-            if ((uint64_t)lhdr + lcomp + 1 > bs) return ZMT_ST_BLOCK;
-            const uint8_t* q = s + lhdr + lcomp; const uint32_t qn = bs - lhdr - lcomp;
-            uint32_t nseq; const uint32_t q0 = q[0];
-            if (q0 == 0) nseq = 0; else if (q0 < 128) nseq = q0;
-            else if (q0 < 255) { if (qn < 2) return ZMT_ST_BLOCK; nseq = ((q0 - 128) << 8) + q[1]; }
-            else { if (qn < 3) return ZMT_ST_BLOCK; nseq = q[1] + (q[2] << 8) + 0x7F00; }
-            // state across blocks visible in the headers: treeless literals, FSE-coded weights are fine block-parallel,
-            // any non-predefined sequence table mode may be followed by Repeat_Mode -> frame-sequential pass
-            {
-                const uint32_t used = q0 == 0 ? 1u : q0 < 128 ? 1u : q0 < 255 ? 2u : 3u;
-                if (lt == 3) *needs_seq |= ZF_NEEDS_SEQ;
-                if (nseq && qn > used && q[used] != 0) *needs_seq |= ZF_NEEDS_SEQ;
-                const uint32_t me = *nblocks_io;
-                B.huf_src = ZB_SELF;
-                if (lt == 2) last_huf = me; else if (lt == 3) B.huf_src = last_huf;
-                B.ll_src = B.of_src = B.ml_src = ZB_SELF;
-                if (nseq && qn > used) {
-                    uint32_t* const dst3[3] = { &B.ll_src, &B.of_src, &B.ml_src };
-                    for (uint32_t t = 0; t < 3; t++) {
-                        const uint32_t mode = (q[used] >> (6 - 2 * t)) & 3;
-                        if (mode == 0) cur_src[t] = ZB_PREDEF; else if (mode != 3) cur_src[t] = me;
-                        *dst3[t] = (mode == 3) ? cur_src[t] : (mode == 0 ? ZB_PREDEF : ZB_SELF);
-                    }
-                }
-            }
-            B.comp_size = bs; B.regen_hint = lregen; B.nseq = nseq;
-            B.seq_off = *scratch_used; *scratch_used += (((uint64_t)nseq * sizeof(ZDSeq)) + 15) & ~15ull;
-            B.lit_off = *scratch_used; *scratch_used += ((uint64_t)lregen + 15) & ~15ull;
-            pos += bs;
-        }
-        (*nblocks_io)++;
-        first = false;
-        if (last) break;
-    }
-    if (has_chk) { if (n - pos < 4) return ZMT_ST_TRUNCATED; pos += 4; }
-    *content_size = no_size ? bound : cs;
-    if (consumed) { *consumed = pos; return ZMT_ST_OK; }
-    return pos == n ? ZMT_ST_OK : ZMT_ST_TRAILING;
+    size_t end = 0;
+    const int r = zstd_frame_walk<true>(frame, n, base_off, frame_idx, (ZBlk*)blocks_out, nblocks_io, max_blocks, scratch_used, content_size,
+                                        needs_seq, &end);
+    if (r != ZMT_ST_OK) return r;
+    if (consumed) { *consumed = end; return ZMT_ST_OK; }
+    return end == n ? ZMT_ST_OK : ZMT_ST_TRAILING;
 }
 
 extern "C" size_t zmt_zstd_blk_desc_bytes(void) { return sizeof(ZBlk); }
