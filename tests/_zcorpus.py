@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import _oracle as o
+import _zxmodel as zx
 
 c_sz, c_vp, c_int = ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int
 
@@ -471,8 +472,280 @@ def _reached_literals(tr):
                 and ((lt == 0) & (sf == 3)).any() and ((lt == 1) & (sf == 3)).any() and (tr.col("type") == 1).any())
 
 
+# ---------------------------------------------------------------------------------------------------- GPU schedule edges
+# The x_* cases state edges of the execute pass (zx_block) and of the lane-per-block sequence reader, as events of the
+# models in _zxmodel.py.  Each execute case is written twice from the same parse: at level 1 with raw literals (predefined
+# tables: the lane sequence decoder) and at level 19 (Huffman literals, described tables: the dependent-block route).
+class Plan:
+    """A parse written block by block: every block of `bsize` bytes is an explicit list of block-relative rows (ll, off,
+    ml), then one pad match (or literals) that fills it exactly.  off may be a (lo, hi) range: a fresh offset from it that
+    is none of the repeat offsets libzstd would code it as.  raw() and rle() add a block of random literals (stored raw)
+    and one of a single byte (an RLE block).  The repeat-offset history is followed as libzstd keeps it (raw and RLE blocks
+    leave it unchanged), and dictated offsets that it would code as repeats are counted in `reps`.
+    omit: labels of blocks written as pad only — how a test checks that a case's predicate depends on its edge blocks."""
+    omit = frozenset()
+
+    def __init__(self, seed, bsize=4096, alpha=b"abcd"):
+        self.rng, self.bsize, self.alpha = np.random.default_rng(seed), bsize, alpha
+        self.seqs, self.alphas, self.pos, self.carry, self.carry_random = [], [], 0, 0, False
+        self.hist, self.reps = [1, 4, 8], 0
+
+    def _is_rep(self, ll, off):
+        h = self.hist
+        return off in (h[1], h[2]) or (off == h[0] if ll else off == h[0] - 1)
+
+    def fresh(self, at, ll, lo, hi):
+        """An offset in [lo, min(hi, at)] that is no repeat offset for a sequence with ll literals at position at."""
+        hi = min(hi, at)
+        assert lo <= hi, (lo, hi, at)
+        while True:
+            off = int(self.rng.integers(lo, hi + 1))
+            if not self._is_rep(self.carry + ll, off):
+                return off
+
+    def _put(self, ll, off, ml, at, track=True):
+        if isinstance(off, tuple):
+            off = self.fresh(at, ll, *off)
+        assert 0 < off <= at, (off, at)
+        if track:
+            if self._is_rep(self.carry + ll, off):
+                self.reps += 1
+            else:
+                self.hist = [off] + self.hist[:2]
+        self.seqs.append((self.carry + ll, off, ml)); self.alphas.append(RANDOM if self.carry_random else self.alpha)
+        self.carry, self.carry_random = 0, False
+
+    def block(self, rows, tail=0, label=None):
+        if label is not None and label in Plan.omit:
+            rows = [(8, (16, 64), 8)]
+        p = 0
+        for ll, off, ml in rows:
+            self._put(ll, off, ml, self.pos + p + ll); p += ll + ml
+        rest = self.bsize - p - tail
+        assert rest >= 0, (label, p, tail)
+        if rest >= 4:
+            self._put(1, (64, 4000), rest - 1, self.pos + p + 1)
+        else:
+            tail += rest
+        self.carry += tail; self.pos += self.bsize
+        return self
+
+    def seed(self):
+        return self.block([(256, (16, 200), 40)], label=None)
+
+    def raw(self):
+        self.carry += self.bsize; self.pos += self.bsize; self.carry_random = True
+        return self
+
+    def rle(self):
+        self._put(1, 1, self.bsize - 1, self.pos + 1, track=False); self.pos += self.bsize
+        return self
+
+    def build(self, params):
+        seqs = np.array(self.seqs, np.int64).reshape(-1, 3)
+        src = build_from_seqs(seqs, self.carry, self.alphas + [RANDOM], self.rng)
+        return src, seqs, {**params, P_MAXBLOCK: self.bsize}
+
+
+LANE_ROUTE = {P_LEVEL: 1, P_LITMODE: 2}
+DEP_ROUTE = {P_LEVEL: 19}
+
+
+def _x_steps(P):
+    """Steps ended by the 32-sequence cap, by the span at exactly 2048 bytes and at 2049, a single sequence of 2048
+    bytes; lone steps (first sequence above the span): ll > 2048 with a match in its own literals, ml > 2048 at offsets
+    >= ml, 33, 32, 31, 3, 2 and 1, first and last in their block, read by the next step."""
+    P.seed().block([(0, (64, 300), 40)] * 3)
+    P.block([(2, (16, 2000), 10)] * 34, label="cap")
+    P.block([(28, (64, 2000), 100)] * 16 + [(1, (64, 2000), 10)], label="span_2048")
+    P.block([(28, (64, 2000), 100)] * 15 + [(20, (64, 2000), 106), (0, (64, 2000), 3)], label="span_2049")
+    P.block([(48, (64, 200), 2000), (5, (2000, 4000), 10)], label="single_2048")
+    P.block([(2100, 50, 20), (3, 1000, 20)], label="lone_lits")
+    P.block([(5, (3000, 8000), 2500), (2, 40, 16)], label="lone_straight")
+    for off in (33, 32, 31, 3, 2, 1):
+        P.block([(5, off, 2100), (3, (100, 1500), 10)], label="lone_off_%d" % off)
+    P.block([(10, (64, 2000), 100), (5, (64, 2000), P.bsize - 115)], label="lone_last")
+    return P
+
+
+def _x_lits(P):
+    """Literal runs copied by their lane (0, 1, 7, 8, 9, 31, 32) and by the warp (33, 100, 300); a match reading a
+    warp-copied run of its own step back through the window; blocks ending with 0, 1 and 40 literals."""
+    P.seed()
+    rows = [(n, (64, 2000), 12) for n in (0, 1, 7, 8, 9, 31, 32)] + [(33, (64, 2000), 40), (100, (64, 2000), 80), (300, (64, 2000), 200)]
+    P.block(rows + [(120, (64, 2000), 30), (2, 100, 20)], label="runs")
+    P.block([(5, (64, 2000), 30)] * 4, tail=1, label="trail_1")
+    P.block([(5, (64, 2000), 30)] * 4, tail=40, label="trail_40")
+    P.block([(5, (64, 2000), 30)] * 4, label="trail_0")
+    return P
+
+
+def _x_matches(P):
+    """Own-lane matches with off == ml (ml 3-32) against in-order ones with off == ml - 1; independent matches of 32 and
+    33 bytes; own-lane sources split at the step start at every nlow from 0 to ml (ml 3-32); sources ending at an earlier
+    destination's start or one byte into it, starting at its end or one byte before; in-order matches reading an earlier
+    in-order match of the step, an own-lane match reading one of an earlier step; a chain of 31 dependent matches."""
+    P.seed().block([(0, (64, 300), 40)] * 3)
+    P.block([(ml, ml, ml) for ml in range(3, 33)], label="off_eq_ml")
+    P.block([(ml, ml - 1, ml) for ml in range(3, 33)], label="off_ml_minus_1")
+    P.block([(40, 40, 32), (45, 41, 33)], label="indep_32_33")
+    pairs = [(ml, k) for ml in range(3, 33) for k in range(ml + 1)]
+    for g in range(0, len(pairs), 31):
+        rows, mp = [(40, (100, 2000), 8)], 48                       # lane 0: 40 literals at the step start
+        for ml, k in pairs[g: g + 31]:
+            mp += 1
+            rows.append((1, mp + k, ml)); mp += ml                  # source starts k bytes below the step start
+        P.block(rows, label="nlow")
+    rows = []
+    for ll_j, off_i in ((12, 38), (12, 37), (12, 20), (12, 21)):    # 10-byte destination d, then 20 literals and 8 bytes
+        rows += [(ll_j, (200, 2000), 10), (20, off_i, 8)]          # from d - 8, d - 7, d + 10 (its end), d + 9
+    for t in range(6):                                              # the same one byte into 40-byte destinations, which
+        rows += [(12, (200, 2000), 40), (20 + t, 67 + t, 8)]        # the in-order pass writes after the own-lane copies
+    P.block(rows, label="dep_edges")
+    P.block([(3, 2, 20), (1, 10, 5), (1, (64, 2000), 2030), (2, 2057, 10)], label="inorder_reads")
+    P.block([(8, (64, 2000), 4)] + [(1, 5 + i % 4, 4) for i in range(31)], label="chain")
+    return P
+
+
+def _x_cross(P):
+    """Sources 1, 2 and 3 or more blocks back and sources straddling the block start, in the first and in later steps,
+    for own-lane, in-order and lone matches, across raw and RLE blocks."""
+    P.seed().block([(3, (64, 300), 60)] * 4).block([(3, (64, 300), 60)] * 4).block([(3, (64, 300), 60)] * 4)
+
+    def reach(p):
+        """Rows starting at block position p whose sources start at the given block positions (negative: earlier
+        blocks): own-lane straddling, 2 and 4 blocks back; in-order 1 block back, straddling, 2 and 4 blocks back."""
+        b, rows = P.bsize, []
+        for ll, sp, ml in ((4, -6, 16), (4, -b - 100, 16), (4, -3 * b - 50, 16), (4, -400, 100), (2, -5, 40),
+                           (4, -b - 300, 60), (4, -3 * b - 700, 60)):
+            rows.append((ll, p + ll - sp, ml)); p += ll + ml
+        return rows, p
+
+    first, p = reach(0)
+    later, _ = reach(p + 1901)                                      # after a 1901-byte sequence: a later step
+    P.raw().block(first + [(1, (64, 2000), 1900)] + later, label="after_raw")
+    P.rle().block(reach(0)[0], label="after_rle")
+    P.block([(5, 105, 2100)], label="lone_straddle")
+    P.raw().block([(5, P.bsize + 500, 2100)], label="lone_back2")
+    P.rle().block([(5, 3 * P.bsize + 200, 2100)], label="lone_back3")
+    return P
+
+
+def _x_case(build, params):
+    def gen():
+        P = build(Plan(1000 + sum(map(ord, build.__name__))))
+        if params is LANE_ROUTE:
+            assert P.reps == 0, (build.__name__, "dictated offsets libzstd would write as repeat offsets", P.reps)
+        return P.build(params)
+    return gen
+
+
+X_EVENTS = {
+    "x_steps": ["step_cap", "step_span_2048", "step_span_2049", "step_single_2048", "lone_reads_own_literals",
+                "lone_straight_long", "lone_off_33", "lone_off_32", "lone_off_31", "lone_off_3", "lone_off_2", "lone_off_1",
+                "lone_first", "lone_last", "lone_read_next", "lone_chunk32", "lone_modulo"],
+    "x_lits": ["lit_lane_%d" % n for n in (0, 1, 7, 8, 9, 31, 32)] + ["lit_warp_33", "lit_warp_long", "reads_warp_literals",
+                                                                     "trailing_0", "trailing_1", "trailing_ge33"],
+    "x_matches": ["own_off_eq_ml_%d" % m for m in range(3, 33)] + ["inorder_off_ml_minus_1_%d" % m for m in range(3, 33)]
+                 + ["nlow_%d_%d" % (m, k) for m in range(3, 33) for k in range(m + 1)]
+                 + ["indep_own_32", "indep_inorder_33", "dep_src_end_at_dest", "dep_src_end_one_into_dest",
+                    "dep_src_start_at_dest_end", "dep_src_start_one_before_dest_end", "dep_src_end_one_into_inorder_dest",
+                    "inorder_reads_inorder",
+                    "own_reads_earlier_inorder", "dep_chain_31", "inorder_modulo", "inorder_straight"],
+    "x_cross": ["cross_%s_back%d" % (p, k) for p in ("own", "inorder", "lone") for k in (1, 2, 3)]
+               + ["cross_%s_straddle" % p for p in ("own", "inorder", "lone")]
+               + ["cross_first_step", "cross_later_step", "cross_over_raw", "cross_over_rle"],
+}
+
+
+def lane_route(tr):
+    """Every sequence section on the predefined tables, raw or RLE literals, no repeat Offset_Value: the lane decoder."""
+    return bool((tr.col("modes")[tr.col("nseq") > 0] == 0).all() and not (tr.col("lit_type") >= 2).any()
+                and not (tr.seq[:, 1] <= 3).any())
+
+
+def dep_route(tr):
+    """Some block with a table that is not predefined or treeless literals (the frame the host scan flags), and some
+    Huffman-coded literals."""
+    return bool((((tr.col("nseq") > 0) & (tr.col("modes") != 0)) | (tr.col("lit_type") == 3)).any() and (tr.col("lit_type") == 2).any())
+
+
+def _reached_exec(kind, route):
+    def pred(tr):
+        ev = zx.exec_frame(tr)[1]
+        return route(tr) and all(ev[e] > 0 for e in X_EVENTS[kind])
+    return pred
+
+
+def _x_budget():
+    """Predefined-table blocks (level 1, raw literals, windowLog 27) whose sequences put the lane reader's bit budget at
+    its edges: extra bits (offset + match + literal length) of 40 and 41 with every symbol's state transition at full
+    width, at every bit phase of the refill, so that a sequence with 40 extra bits after a refill of 57 valid bits
+    leaves no bit; the largest sum a block allows (offset code 24, 16 + 15 extra bits = 55); blocks with one and two
+    sequences, whose bit streams are a few bytes."""
+    rng = np.random.default_rng(4242)
+    params = {**LANE_ROUTE, P_WINDOWLOG: 27}
+    seqs, hist, p = [], [1, 4, 8], 0
+
+    def put(ll, off, ml):
+        nonlocal p
+        while off in hist or (ll == 0 and off == hist[0] - 1):
+            off -= 1
+        assert 0 < off <= p + ll
+        seqs.append((ll, off, ml)); hist[:] = [off] + hist[:2]; p += ll + ml
+
+    def in_code(base, c):
+        return int(rng.integers(base[c], base[c + 1]))
+    lb = list(zx.LL_BASE) + [1 << 17]; mb = list(zx.ML_BASE) + [1 << 17]
+    while p < 1100 * 1024:                                  # history: about 16 sequences of 3-13 KiB per 128 KiB block
+        ll = int(rng.integers(20, 3000)); put(ll, int(rng.integers(16, max(17, min(p + ll, 60000)))), int(rng.integers(3000, 10000)))
+    # (offset code, ML code, LL code): every symbol has a count of 1 or -1 in its predefined table (17 state bits)
+    kinds = {40: [(16, 48, 31), (18, 47, 30), (14, 49, 32)], 41: [(17, 48, 30), (19, 47, 30), (15, 49, 32)]}
+    for i in range(240):
+        ofc, mc, lc = kinds[40 + i % 2][int(rng.integers(0, 3))]
+        ll, ml = in_code(lb, lc), in_code(mb, mc)
+        put(ll, int(rng.integers(1 << ofc, 2 << ofc)) - 3, ml)
+        for _ in range(int(rng.integers(0, 3))):             # jitter: the next one starts at another bit phase
+            ll = int(rng.integers(1, 700)); put(ll, int(rng.integers(16, min(p + ll, 60000))), int(rng.integers(400, 3000)))
+    for _ in range(3):
+        put(4, int(rng.integers(100, 5000)), 8)
+    # one byte up to a block boundary beyond 17 MiB (RLE blocks).  libzstd may end a block early where it splits a
+    # sequence, so the boundaries are read from a frame of the parse so far followed by a shorter run.
+    probe = np.array(seqs + [(1, 1, 2 * MiB)], np.int64)
+    tp = o.zstd_trace(compress(build_from_seqs(probe, 0, b"ETAOINSHRD", np.random.default_rng(0)), params, probe))
+    phase = int(zx.block_starts(tp)[-2]) % (1 << 17)
+    run_end = (17 << 20) + (phase - (17 << 20)) % (1 << 17)
+    put(1, 1, run_end - p - 1)
+    ll, ml = 32768 + 1000, 65539 + 2000                      # LL code 34 (15 bits), ML code 52 (16 bits), offset code 24
+    if "s1_55" in Plan.omit:
+        ll, ml = 1000, 65539 + 2000 + 32768
+    put(ll, p + ll - int(rng.integers(1000, 500000)), ml)   # 16.5-17 MiB back: into the history
+    put(10, int(rng.integers(300, 90000)), (1 << 17) - ll - ml - 10)                         # the block's 2nd sequence
+    put(5, int(rng.integers(300, 90000)), (1 << 17) - 5)                                     # a block of one sequence
+    seqs = np.array(seqs, np.int64)
+    src = build_from_seqs(seqs, 64, b"ETAOINSHRD", rng)
+    return src, seqs, params
+
+
+BUDGET_EVENTS = (["s1_%d_phase%d" % (s, r) for s in (40, 41) for r in range(8)] + ["slack_0", "s1_55", "second_refill",
+                 "short_stream", "refill_aligned", "refill_funnel", "refill_bytes"] + ["section_mod8_%d" % r for r in range(8)])
+
+
+def _reached_budget(tr):
+    lanes, ev = zx.lane_frame(tr.frame)
+    slack = [s["slack"] for r in lanes.values() for s in r["seqs"]]
+    nblk = int(((tr.col("type") == 2) & (tr.col("nseq") > 0)).sum())
+    return lane_route(tr) and len(lanes) == nblk and min(slack) == 0 and all(ev[e] > 0 for e in BUDGET_EVENTS)
+
+
+X_CASES = {}
+for _k, _b in (("x_steps", _x_steps), ("x_lits", _x_lits), ("x_matches", _x_matches), ("x_cross", _x_cross)):
+    X_CASES[_k + "_l1"] = (_x_case(_b, LANE_ROUTE), _reached_exec(_k, lane_route))
+    X_CASES[_k + "_l19"] = (_x_case(_b, DEP_ROUTE), _reached_exec(_k, dep_route))
+X_CASES["x_budget"] = (_x_budget, _reached_budget)
+
 CASES = {
-    "dense": (_dense, lambda tr: bool(((tr.col("nseq") >= 0x7F00) & (tr.col("nseq_bytes") == 3)).any())),
+    "dense":(_dense, lambda tr: bool(((tr.col("nseq") >= 0x7F00) & (tr.col("nseq_bytes") == 3)).any())),
     "far": (_far, lambda tr: of_codes(tr).max() >= 25),
     "far_predef": (_far_predef, lambda tr: any(m == 0 and (of_codes(tr)[seq_blocks(tr) == b] >= 25).any()
                                                for b, m in enumerate(tr.col("modes")))),
@@ -482,6 +755,7 @@ CASES = {
     "literals": (_literals, _reached_literals),
     "deep": (_deep, lambda tr: match_block_distance(tr).max() >= 100),
     "reference_ultra": (_reference_ultra, lambda tr: of_codes(tr).max() >= 25),
+    **X_CASES,
 }
 
 
@@ -495,4 +769,8 @@ def case(name):
 
 @functools.lru_cache(maxsize=None)
 def trace(name):
-    return o.zstd_trace(case(name)[1])
+    """The oracle's block trace of a case, with the frame itself as trace.frame."""
+    frame = case(name)[1]
+    tr = o.zstd_trace(frame)
+    tr.frame = frame
+    return tr
