@@ -148,6 +148,43 @@ int    zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_f
 int    zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
                               const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream);
 
+/* ---- LZ4F frames of any size in bounded memory ----
+ * An LZ4F frame of any size, decoded as a chain of segments, each a run of whole blocks (what LZ4F_decompress does
+ * through two fixed buffers when the reference streams a plain .lz4 file, lib/lz4-mt_decompress.c:391-483).  Frame f of
+ * a zmt_lz4_decompress_segments_device batch is then a segment whose bytes start at d_in + d_frame_off[f] + 12:
+ *   - the first segment starts with the frame header, a later one with a block header (no LZ4F header);
+ *   - the last segment ends with the end mark and the content checksum, an earlier one right behind a block;
+ *   - its content goes to d_out + d_out_off[f]; in a linked-block frame the last `history` bytes the frame decoded so
+ *     far (up to 64 KiB) must lie directly below, in place before the call.
+ * Between segments, d_seg[f] carries the frame's state on the device.  The caller zeroes it before the first segment
+ * and sets `flags` and `history` for every segment; the device owns the other fields: the first segment records FLG,
+ * BD and the content size from the header, every segment folds its bytes into the running XXH32 and advances
+ * `produced`.  The content checksum and the content size are checked on the last segment only.  d_out_size[f] is the
+ * segment's decoded size.  zmt_lz4f_segment_host finds a segment's end.  A frame with FIRST | LAST is a whole frame. */
+#define ZMT_SEG_FIRST 1u
+#define ZMT_SEG_LAST  2u
+typedef struct {
+    uint64_t history;         /* in: decoded bytes of the frame directly below d_out + d_out_off[f] (0 for the first segment) */
+    uint64_t produced;        /* device: content bytes of the frame's segments so far */
+    uint64_t content_size;    /* device: the header's content size, ~0 without one */
+    uint32_t flags;           /* in: ZMT_SEG_* */
+    uint8_t  flg, bd;         /* device: the frame's FLG / BD bytes */
+    uint16_t pending_len;     /* device: bytes in pending[] */
+    uint32_t acc[4];          /* device: XXH32 accumulators */
+    uint8_t  pending[16];     /* device: content bytes not yet folded into acc[] */
+} zmt_lz4_segment;
+int      zmt_lz4_decompress_segments_device(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                            uint32_t nframes, uint32_t nslots, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size,
+                                            uint32_t* d_status, zmt_lz4_segment* d_seg, void* d_work, void* stream);
+/* Host walk of one segment: seg[0..n) holds the segment's bytes as far as they are known, its first block header at
+ * seg[start] (start = the header length for the first segment, else 0); flg / bd are the frame's FLG / BD bytes.  The
+ * segment runs to the first block boundary at or past seg + max_in, or to where its blocks reach max_out bytes of room,
+ * or to the frame's end, and holds at least one block or the end mark.  *end = its length, *room = the output room it
+ * needs (blockMaxSize per compressed block), *last = 1 if it ends the frame.  Returns ZMT_ST_OK, or ZMT_ST_TRUNCATED when
+ * the segment's bytes are not all in seg[0..n) yet (read on). */
+int      zmt_lz4f_segment_host(const uint8_t* seg, size_t n, size_t start, uint32_t flg, uint32_t bd, size_t max_in, uint64_t max_out,
+                               size_t* end, uint64_t* room, uint32_t* last);
+
 /* ---- multi-GPU: one LZ4MT_* / ZSTDCB_* call deals its batches round-robin over the devices named by the
  * environment variable ZSTDMT_GPUS ("all" or "0,1,..."; default: the calling thread's current device) and re-serialises
  * the frames on the host.  zmt_device_batches(dev) = batches submitted to that device since the library was loaded. */

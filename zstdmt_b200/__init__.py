@@ -78,6 +78,10 @@ def lib():
     L.zmt_lz4d_workspace_bytes.restype = c_sz; L.zmt_lz4d_workspace_bytes.argtypes = [c_u32, c_u32, c_u64]
     L.zmt_lz4_decompress_device.restype = ctypes.c_int
     L.zmt_lz4_decompress_device.argtypes = [c_vp, c_u64, c_vp, c_vp, c_u32, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_lz4_decompress_segments_device.restype = ctypes.c_int
+    L.zmt_lz4_decompress_segments_device.argtypes = [c_vp, c_u64, c_vp, c_vp, c_u32, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_lz4f_segment_host.restype = ctypes.c_int
+    L.zmt_lz4f_segment_host.argtypes = [c_vp, c_sz, c_sz, c_u32, c_u32, c_sz, c_u64, ctypes.POINTER(c_sz), ctypes.POINTER(c_u64), ctypes.POINTER(c_u32)]
     L.zmt_index_workspace_bytes.restype = c_sz; L.zmt_index_workspace_bytes.argtypes = [c_u32]
     L.zmt_lz4_index_device.restype = ctypes.c_int
     L.zmt_lz4_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
@@ -343,6 +347,71 @@ class Lz4DeviceDecompressor:
         if rc != 0:
             raise RuntimeError("zmt_lz4_decompress_device failed: %s" % ST_NAMES.get(rc, rc))
         return self.out, self.status
+
+
+SEG_FIRST, SEG_LAST = 1, 2
+
+
+class Lz4Segment(ctypes.Structure):
+    """zmt_lz4_segment (include/zstdmt_b200_dev.h): the state of an LZ4F frame decoded as a chain of segments."""
+    _fields_ = [("history", c_u64), ("produced", c_u64), ("content_size", c_u64), ("flags", c_u32), ("flg", ctypes.c_uint8),
+                ("bd", ctypes.c_uint8), ("pending_len", ctypes.c_uint16), ("acc", c_u32 * 4), ("pending", ctypes.c_uint8 * 16)]
+
+
+def lz4f_segment(seg_bytes, start, flg, bd, max_in, max_out):
+    """zmt_lz4f_segment_host: (status, end, room, last) of the segment whose bytes begin seg_bytes (first block header at start)."""
+    b = np.ascontiguousarray(seg_bytes, dtype=np.uint8)
+    end, room, last = c_sz(0), c_u64(0), c_u32(0)
+    rc = lib().zmt_lz4f_segment_host(b.ctypes.data, b.size, start, flg, bd, max_in, max_out, ctypes.byref(end), ctypes.byref(room), ctypes.byref(last))
+    return rc, end.value, room.value, last.value
+
+
+def lz4_decode_segments(frame, cuts, device="cuda"):
+    """Decodes one LZ4F frame (host bytes) through zmt_lz4_decompress_segments_device as the chain of segments that ends
+    at the frame offsets `cuts` (block boundaries, increasing; the frame's length is appended).  Each segment's output
+    goes 64 KiB above the start of a fresh buffer, with the frame's last 64 KiB of content copied below it first.
+    Returns (content, status): the decoded bytes (numpy) and the ZMT_ST_* of the first failing segment, or 0."""
+    torch = _torch(); L = lib()
+    fb = np.ascontiguousarray(frame, dtype=np.uint8)
+    flg, bd = int(fb[4]), int(fb[5])
+    H = 65536
+    seg = torch.zeros(ctypes.sizeof(Lz4Segment), dtype=torch.uint8, device=device)
+    ends = [int(c) for c in cuts] + [fb.size]
+    parts, prev, hist = [], 0, torch.zeros(0, dtype=torch.uint8, device=device)
+    for k, end in enumerate(ends):
+        first, last = k == 0, k == len(ends) - 1
+        rc, e2, room, is_last = lz4f_segment(fb[prev:], (7 + (8 if flg & 8 else 0) + (4 if flg & 1 else 0)) if first else 0, flg, bd,
+                                             end - prev, 1 << 62)
+        if rc != 0 or e2 != end - prev or bool(is_last) != last:
+            raise ValueError("cut %d is not a block boundary (walk: rc %d end %d last %d)" % (end, rc, prev + e2, is_last))
+        d_in = torch.zeros(12 + (end - prev) + 256, dtype=torch.uint8, device=device)
+        d_in[12:12 + end - prev] = torch.from_numpy(fb[prev:end].copy()).to(device)
+        out = torch.zeros(H + room + 256, dtype=torch.uint8, device=device)
+        if hist.numel():
+            out[H - hist.numel():H] = hist
+        foff = torch.zeros(1, dtype=torch.int64, device=device)
+        fcs = torch.tensor([end - prev], dtype=torch.int32, device=device)
+        ooff = torch.tensor([H, H + room], dtype=torch.int64, device=device)
+        osz = torch.zeros(1, dtype=torch.int64, device=device)
+        st = torch.zeros(1, dtype=torch.int32, device=device)
+        nslots = max(1, (room + 65535) // 65536)
+        work = torch.empty(L.zmt_lz4d_workspace_bytes(1, nslots, 12 + end - prev), dtype=torch.uint8, device=device)
+        rec = Lz4Segment.from_buffer_copy(bytes(seg.cpu().numpy()))
+        rec.history, rec.flags = hist.numel(), (SEG_FIRST if first else 0) | (SEG_LAST if last else 0)
+        seg.copy_(torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8))
+        s = torch.cuda.current_stream()
+        rc = L.zmt_lz4_decompress_segments_device(d_in.data_ptr(), d_in.numel(), foff.data_ptr(), fcs.data_ptr(), 1, nslots, out.data_ptr(),
+                                                  ooff.data_ptr(), osz.data_ptr(), st.data_ptr(), seg.data_ptr(), work.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("zmt_lz4_decompress_segments_device failed: %s" % ST_NAMES.get(rc, rc))
+        torch.cuda.synchronize()
+        if int(st.item()) != 0:
+            return np.concatenate(parts) if parts else np.zeros(0, np.uint8), int(st.item())
+        n = int(osz.item())
+        parts.append(out[H:H + n].cpu().numpy())
+        hist = torch.cat([hist, out[H:H + n]])[-H:].clone()
+        prev = end
+    return np.concatenate(parts) if parts else np.zeros(0, np.uint8), 0
 
 
 class ZstdDeviceDecompressor:

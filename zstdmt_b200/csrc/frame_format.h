@@ -22,25 +22,46 @@ ZMT_HD uint32_t zf_rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p
 ZMT_HD uint64_t zf_rd64(const uint8_t* p) { return (uint64_t)zf_rd32(p) | ((uint64_t)zf_rd32(p + 4) << 32); }
 
 // ---------------------------------------------------------------- LZ4F
+// Bytes of an LZ4F frame header with this FLG byte: magic, FLG, BD, [content size], [dictionary ID], header checksum.
+ZMT_HD size_t lz4f_header_len(uint32_t flg) { return 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1; }
+
+// A block walk that can stop at a block boundary and resume there (a frame decoded as a chain of segments).
+struct Lz4fWalk {
+    size_t   pos;               // offset in the frame of the next block header (start: lz4f_header_len)
+    uint64_t bound;             // the most the blocks walked so far decode to (blockMaxSize per compressed block)
+    uint32_t nblk;              // blocks walked so far
+    uint32_t done;              // 1: the end mark was met; pos = the frame's length, content checksum included
+};
+
+// Walks block headers of the LZ4F frame p[0..n) with FLG / BD from w->pos on, and stops at the first block boundary at
+// or past pos_stop or where the bound reaches bound_stop, or at the frame's end (w->done).  Returns false if a block
+// header lies past n ("need more bytes"); w then stands behind the last header read, whose block may itself run past n.
+// Only headers are read: a caller that cuts the frame at w->pos checks that w->pos <= n.
+ZMT_HD bool lz4f_walk_blocks(const uint8_t* p, size_t n, uint32_t flg, uint32_t bd, Lz4fWalk* w, size_t pos_stop, uint64_t bound_stop)
+{
+    const uint64_t blkmax = 1ull << (8 + 2 * ((bd >> 4) & 7));
+    for (;;) {
+        if (w->pos >= pos_stop || w->bound >= bound_stop) return true;
+        if (w->pos + 4 > n) return false;
+        const uint32_t bh = zf_rd32(p + w->pos); w->pos += 4;
+        if (bh == 0) { w->pos += (flg & 4) ? 4 : 0; w->done = 1; return true; }
+        const uint32_t bs = bh & 0x7FFFFFFFu;
+        w->bound += (bh & 0x80000000u) ? bs : blkmax;
+        w->pos += (size_t)bs + ((flg & 0x10) ? 4 : 0);
+        w->nblk++;
+    }
+}
+
 // Walks an LZ4F frame's header and block headers in p[0..n) (n >= 7): *len = the frame's length, content checksum
 // included; *bound = the most its blocks decode to (blockMaxSize per compressed block).  false: the block headers run
 // past n (*bound then covers the blocks before the cut).
 ZMT_HD bool lz4f_walk(const uint8_t* p, size_t n, size_t* len, uint64_t* bound)
 {
-    const uint32_t flg = p[4];
-    const uint64_t blkmax = 1ull << (8 + 2 * ((p[5] >> 4) & 7));
-    size_t q = 4 + 2 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0) + 1;
-    *bound = 0;
-    for (;;) {
-        if (q + 4 > n) return false;
-        const uint32_t bh = zf_rd32(p + q); q += 4;
-        if (bh == 0) break;
-        const uint32_t bs = bh & 0x7FFFFFFFu;
-        *bound += (bh & 0x80000000u) ? bs : blkmax;
-        q += (size_t)bs + ((flg & 0x10) ? 4 : 0);
-    }
-    *len = q + ((flg & 4) ? 4 : 0);
-    return true;
+    Lz4fWalk w; w.pos = lz4f_header_len(p[4]); w.bound = 0; w.nblk = 0; w.done = 0;
+    const bool ok = lz4f_walk_blocks(p, n, p[4], p[5], &w, ~(size_t)0, ~0ull);
+    *bound = w.bound;
+    if (ok) *len = w.pos;
+    return ok;
 }
 
 // The room one LZ4 payload of n bytes gets in the output, from its own header (pt_decompress sizes the buffer from

@@ -591,6 +591,102 @@ struct DevBuf {
     }
 };
 
+// Appends one read of up to `piece` bytes to `in`; sets eof on an empty read.
+size_t read_piece(Ctx* c, GenRdWr* rw, std::vector<uint8_t>& in, size_t piece, bool& eof)
+{
+    const size_t old = in.size();
+    in.resize(old + piece);
+    size_t got = 0;
+    const size_t e = read_some(*c->E, rw, in.data() + old, piece, &got);
+    in.resize(old + got);
+    if (e) return e;
+    c->insize += got;
+    if (got == 0) eof = true;
+    return 0;
+}
+
+// One LZ4F frame that reaches a batch of input (or four of output) before its end, at in[12 + pos], decoded as a chain of
+// segments of whole blocks (zmt_lz4_decompress_segments_device): each segment is read, decoded and written before the
+// next one is read, and its input dropped.  The device keeps the frame's state between segments (zmt_lz4_segment: XXH32,
+// content size) in d_seg and, for linked blocks, the last 64 KiB of content in d_hist; the segment's output goes to
+// d_out + 64 KiB with the history copied directly below.  Memory stays O(batch) whatever the frame's size.  One stream
+// synchronisation per segment: status, size and the output room come back together, and the history of the next segment
+// is saved behind them.  On return the frame has been consumed (pos = 0, in holds what follows it).
+size_t decode_lz4_segments(Ctx* c, GenRdWr* rw, std::vector<uint8_t>& in, size_t& pos, bool& eof, size_t batch, size_t piece,
+                           cudaStream_t st, DevBuf& d_in, DevBuf& d_out, DevBuf& d_tab, DevBuf& d_work, DevBuf& d_seg, DevBuf& d_hist,
+                           std::vector<uint8_t>& out)
+{
+    const ErrCodes& E = *c->E;
+    const uint32_t flg = in[12 + pos + 4], bd = in[12 + pos + 5];
+    const bool linked = !(flg & 0x20);
+    const uint64_t H = 65536;                               // the history's room below each segment's output
+    if (!d_seg.need(sizeof(zmt_lz4_segment)) || !d_hist.need(H)) return E.mem;
+    cudaMemsetAsync(d_seg.p, 0, sizeof(zmt_lz4_segment), st);
+    uint64_t produced = 0;
+    bool first = true;
+    for (;;) {
+        // ---- the next segment: whole blocks up to a batch of input / four of output room
+        size_t end = 0; uint64_t room = 0; uint32_t last = 0;
+        for (;;) {
+            const int r = zmt_lz4f_segment_host(in.data() + 12 + pos, in.size() - 12 - pos, first ? lz4f_header_len(flg) : 0, flg, bd,
+                                                batch, 4 * (uint64_t)batch, &end, &room, &last);
+            if (r == ZMT_ST_OK) break;
+            if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; }
+            const size_t goal = 12 + pos + batch + piece;
+            do { const size_t e = read_piece(c, rw, in, piece, eof); if (e) return e; } while (!eof && in.size() < goal);
+        }
+        // ---- decode it: a batch of one frame, its bytes at d_in + 12
+        const uint64_t hlen = linked ? (produced < H ? produced : H) : 0;
+        const size_t tab_bytes = tables_bytes(1);
+        std::vector<uint8_t> h_tab(tab_bytes);
+        Tables T = tables_at(h_tab.data(), 1);
+        T.frame_off[0] = 0; T.per_frame[0] = (uint32_t)end; T.out_off[0] = H; T.out_off[1] = H + room;
+        const uint32_t nslots = (uint32_t)lz4_frame_slots(room);
+        const size_t wk = zmt_lz4d_workspace_bytes(1, nslots, 12 + end);
+        if (!d_in.need(12 + end + 256) || !d_out.need(H + room + 256) || !d_tab.need(tab_bytes) || !d_work.need(wk)) return E.mem;
+        Tables Td = tables_at((uint8_t*)d_tab.p, 1);
+        const uint32_t flags = (first ? ZMT_SEG_FIRST : 0u) | (last ? ZMT_SEG_LAST : 0u);
+        zmt_lz4_segment* ds = (zmt_lz4_segment*)d_seg.p;
+        cudaError_t ce = cudaMemcpyAsync((uint8_t*)d_in.p + 12, in.data() + 12 + pos, end, cudaMemcpyHostToDevice, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_tab.p, h_tab.data(), tab_bytes, cudaMemcpyHostToDevice, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->history, &hlen, sizeof(hlen), cudaMemcpyHostToDevice, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->flags, &flags, sizeof(flags), cudaMemcpyHostToDevice, st);
+        if (ce == cudaSuccess && hlen) ce = cudaMemcpyAsync((uint8_t*)d_out.p + H - hlen, d_hist.p, hlen, cudaMemcpyDeviceToDevice, st);
+        const int rc = ce == cudaSuccess ? zmt_lz4_decompress_segments_device(d_in.p, 12 + end, Td.frame_off, Td.per_frame, 1, nslots, d_out.p, Td.out_off,
+                                                                               Td.out_size, Td.status, ds, d_work.p, st) : ZMT_ST_CUDA;
+        // status, size and the whole output room (the segment's content is at most `room` bytes) in one round trip;
+        // d_out is read back before the next segment is queued on the stream
+        uint32_t status = 0; uint64_t osz = 0;
+        out.resize(room ? room : 1);
+        if (rc == ZMT_ST_OK) {
+            ce = cudaMemcpyAsync(&status, Td.status, 4, cudaMemcpyDeviceToHost, st);
+            if (ce == cudaSuccess) ce = cudaMemcpyAsync(&osz, Td.out_size, 8, cudaMemcpyDeviceToHost, st);
+            if (ce == cudaSuccess && room) ce = cudaMemcpyAsync(out.data(), (uint8_t*)d_out.p + H, room, cudaMemcpyDeviceToHost, st);
+            if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        }
+        if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library; }
+        if (status != ZMT_ST_OK) { c->lib_errcode = status; return status_error(E, status); }
+        if (osz > room) { c->lib_errcode = ZMT_ST_DST_SMALL; return E.library; }
+        // ---- the history of the next segment: the last 64 KiB of [history | this segment], contiguous below H + osz; queued
+        //      behind this segment, ahead of the next one (a reallocation of d_out in between synchronises in cudaFree)
+        const uint64_t hnext = linked ? (hlen + osz < H ? hlen + osz : H) : 0;
+        if (hnext && !last && cudaMemcpyAsync(d_hist.p, (uint8_t*)d_out.p + H + osz - hnext, hnext, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+            cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library;
+        }
+        for (uint64_t o = 0; o < osz;) {
+            GenBuffer b; b.buf = out.data() + o; b.size = (size_t)((osz - o) < piece ? (osz - o) : piece); b.allocated = b.size;
+            const size_t want = b.size;
+            const int rv = rw->fn_write(rw->arg_write, &b);
+            if (rv != 0) return mt_error(E, rv);
+            c->outsize += b.size; o += want;
+        }
+        produced += osz;
+        in.erase(in.begin() + 12, in.begin() + 12 + (long)(pos + end));       // drop the decoded segment
+        pos = 0; first = false;
+        if (last) return 0;
+    }
+}
+
 size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_t have)
 {
     const ErrCodes& E = *c->E;
@@ -604,7 +700,7 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
     size_t pos = 0;                                         // parse position inside in[12..]
     const std::vector<int> devs = env_devices();
     if (devs.empty() || cudaSetDevice(devs[0]) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
-    DevBuf d_in, d_out, d_tab, d_blk, d_work;
+    DevBuf d_in, d_out, d_tab, d_blk, d_work, d_seg, d_hist;         // d_seg, d_hist: LZ4F frames decoded in segments
     cudaStream_t st = nullptr;
     if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
     struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{st};
@@ -617,7 +713,7 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
         foff.clear(); ooff.assign(1, 0); expect.clear(); fcs.clear(); first_blk.assign(1, 0); fflags.clear();
         uint32_t nblk = 0; uint64_t scratch = 0, nslots = 0;
         const size_t batch_start = pos;
-        bool need_more = false;
+        bool need_more = false, segmented = false;
         while (!need_more) {
             const uint8_t* s = in.data() + 12; const size_t n = in.size() - 12;
             if (pos >= n) { need_more = !eof; break; }
@@ -633,6 +729,17 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                 if (n - pos < 7) { if (eof) return E.data_error; need_more = true; break; }
                 const uint32_t flg = s[pos + 4], bd = s[pos + 5], id = (bd >> 4) & 7;
                 if ((flg >> 6) != 1 || id < 4) { c->lib_errcode = ZMT_ST_BAD_HEADER; return E.library; }
+                {
+                    // a frame whose blocks reach a batch of input or four of output before its end: decoded in segments,
+                    // after the frames in front of it
+                    Lz4fWalk w; w.pos = lz4f_header_len(flg); w.bound = 0; w.nblk = 0; w.done = 0;
+                    if (lz4f_walk_blocks(s + pos, n - pos, flg, bd, &w, kPlainBatch, 4 * (uint64_t)kPlainBatch) && !w.done) {
+                        if (!foff.empty()) break;
+                        const size_t e = decode_lz4_segments(c, rw, in, pos, eof, kPlainBatch, piece, st, d_in, d_out, d_tab, d_work, d_seg, d_hist, out);
+                        if (e) return e;
+                        segmented = true; break;
+                    }
+                }
                 size_t len = 0; uint64_t bound = 0;
                 if (!lz4f_walk(s + pos, n - pos, &len, &bound) || len > n - pos) {
                     if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; }
@@ -662,6 +769,7 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
         }
         const uint32_t nf = (uint32_t)foff.size();
         if (nf == 0) {
+            if (segmented) continue;                                          // a segmented frame was decoded and consumed
             if (!need_more) break;                                            // EOF, everything consumed
         } else {
             // ---- decode this batch
@@ -715,17 +823,9 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
             // ---- read ahead: at least one more piece, up to a batch beyond the parse position
             size_t goal = in.size() + piece;
             if (goal < 12 + pos + kPlainBatch) goal = 12 + pos + kPlainBatch;
-            if (in.size() - 12 - pos >= kPlainBatch) goal = in.size() + (in.size() - 12 - pos) / 2;     // one frame larger than a batch: read ahead geometrically
-            while (!eof && in.size() < goal) {
-                const size_t old = in.size();
-                in.resize(old + piece);
-                size_t got = 0;
-                const size_t e = read_some(E, rw, in.data() + old, piece, &got);
-                in.resize(old + got);
-                if (e) return e;
-                c->insize += got;
-                if (got == 0) eof = true;
-            }
+            // one zstd frame larger than a batch: read ahead geometrically (an LZ4 frame that large is decoded in segments)
+            if (is_zstd && in.size() - 12 - pos >= kPlainBatch) goal = in.size() + (in.size() - 12 - pos) / 2;
+            while (!eof && in.size() < goal) { const size_t e = read_piece(c, rw, in, piece, eof); if (e) return e; }
         } else if (eof && pos >= in.size() - 12) break;
     }
     return 0;

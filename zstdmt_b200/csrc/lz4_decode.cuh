@@ -38,6 +38,7 @@
 #define LZB_LINKED 1u         // block may copy from the previous block of its frame
 #define LZB_LAST   2u         // last block of its frame
 #define LZB_BCHK   4u         // an XXH32 of the block's stored bytes follows them (FLG.BC)
+#define LZB_HIST   8u         // block 0 of a segment: may copy from the segment's history (in place before the launch)
 
 struct LzBlk {
     uint32_t src;             // offset of the block data inside the LZ4F frame
@@ -79,7 +80,7 @@ __global__ void lz4_scan_frames_kernel(const uint8_t* __restrict__ in, const uin
                                        const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ first_slot, uint32_t slot_cap,
                                        LzBlk* __restrict__ tab, uint32_t* __restrict__ prog, uint32_t* __restrict__ status,
                                        uint32_t* __restrict__ stored_chk, uint32_t* __restrict__ needs_seq, uint32_t* __restrict__ any_bchk,
-                                       uint32_t nframes)
+                                       zmt_lz4_segment* __restrict__ seg, uint32_t nframes)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
@@ -91,43 +92,53 @@ __global__ void lz4_scan_frames_kernel(const uint8_t* __restrict__ in, const uin
     const uint8_t* p = in + frame_off[f] + 12;              // LZ4F frame (after the skippable header)
     const uint32_t fs = frame_csize[f];
     const uint64_t cap = out_off[f + 1] - out_off[f];
-    uint32_t err = 0;
-    if (fs < 7 + 4) err = ZMT_ST_TRUNCATED;
-    else if (ldg_le32(p) != 0x184D2204u) err = ZMT_ST_BAD_MAGIC;
-    if (err) { status[f] = err; return; }
-    const uint32_t flg = p[4], bd = p[5];
+    // a segment of a longer frame (zmt_lz4_segment): a later one has no header, an earlier one no end mark
+    const uint32_t sflags = seg ? seg[f].flags : (ZMT_SEG_FIRST | ZMT_SEG_LAST);
+    const bool head = (sflags & ZMT_SEG_FIRST) != 0, tail = (sflags & ZMT_SEG_LAST) != 0;
+    uint32_t err = 0, flg, bd, ip;
+    if (head) {
+        if (fs < 7 + (tail ? 4u : 0u)) err = ZMT_ST_TRUNCATED;
+        else if (ldg_le32(p) != 0x184D2204u) err = ZMT_ST_BAD_MAGIC;
+        if (err) { status[f] = err; return; }
+        flg = p[4]; bd = p[5];
+    } else { flg = seg[f].flg; bd = seg[f].bd; }
     if ((flg >> 6) != 1 || (flg & 2) || (bd & 0x8F) || ((bd >> 4) & 7) < 4) { status[f] = ZMT_ST_BAD_HEADER; return; }
     const uint32_t indep = (flg >> 5) & 1, bchk = (flg >> 4) & 1, csz = (flg >> 3) & 1, cchk = (flg >> 2) & 1, did = flg & 1;
     const uint32_t blklog = 8 + 2 * ((bd >> 4) & 7), blkmax = 1u << blklog;
     const uint32_t hl = 2 + (csz ? 8 : 0) + (did ? 4 : 0);
-    if (fs < 4 + hl + 1 + 4) { status[f] = ZMT_ST_TRUNCATED; return; }
-    {
+    if (head) {
+        if (fs < 4 + hl + 1 + (tail ? 4u : 0u)) { status[f] = ZMT_ST_TRUNCATED; return; }
         uint8_t h[14];
         for (uint32_t i = 0; i < hl; i++) h[i] = p[4 + i];
         if (((xxh32_small(h, hl, 0) >> 8) & 0xFF) != p[4 + hl]) { status[f] = ZMT_ST_HDR_CHECKSUM; return; }
-    }
-    uint32_t ip = 4 + hl + 1, b = 0;
+        if (seg) { seg[f].flg = (uint8_t)flg; seg[f].bd = (uint8_t)bd; seg[f].content_size = csz ? ldg_le64(p + 6) : ~0ull; }
+        ip = 4 + hl + 1;
+    } else ip = 0;
+    const bool hist = seg && !head && !indep && seg[f].history > 0;     // block 0 may copy from the frame's earlier segments
+    uint32_t b = 0;
     bool seq = false;
     for (;;) {
+        if (!tail && ip == fs) break;                       // a segment that does not end the frame ends behind a block
         if (fs - ip < 4) { err = ZMT_ST_TRUNCATED; break; }
         const uint32_t bh = ldg_le32(p + ip);
-        if (bh == 0) break;
+        if (bh == 0) { if (!tail) err = ZMT_ST_BAD_ARG; break; }
         ip += 4;
         const uint32_t bs = bh & 0x7FFFFFFFu;
         if (bs > blkmax) { err = ZMT_ST_BLOCK; break; }
-        if (fs - ip < bs + (bchk ? 4 : 0) || fs - ip - bs - (bchk ? 4 : 0) < 4) { err = ZMT_ST_TRUNCATED; break; }
+        if (fs - ip < bs + (bchk ? 4 : 0) || (tail && fs - ip - bs - (bchk ? 4 : 0) < 4)) { err = ZMT_ST_TRUNCATED; break; }
         // a block beyond the slots, or one that would start past the room: partial blocks or an overlong frame —
         // the sequential pass decodes it block after block and reports what is wrong, if anything
         if (b >= nslot || (uint64_t)b * blkmax > cap) { seq = true; }
         else {
-            LzBlk e; e.src = ip; e.csize = bh; e.flags = ((!indep && b > 0) ? LZB_LINKED : 0u) | (bchk ? LZB_BCHK : 0u) | (blklog << 8); e.nrec = 0; e.frame = f;
+            const uint32_t link = !indep && b > 0 ? LZB_LINKED : (hist && b == 0 ? LZB_HIST : 0u);
+            LzBlk e; e.src = ip; e.csize = bh; e.flags = link | (bchk ? LZB_BCHK : 0u) | (blklog << 8); e.nrec = 0; e.frame = f;
             if (bs == 0) e.csize = 0;                      // a zero-sized stored block regenerates nothing (bit 31 set, size 0)
             if (bs == 0) seq = true;                       // ... and breaks the fixed block addressing
             T[b] = e;
         }
         ip += bs + (bchk ? 4 : 0); b++;
     }
-    if (!err) {
+    if (!err && tail) {
         ip += 4;
         uint32_t has_chk = 0, chkv = 0;
         if (cchk) {
@@ -343,7 +354,8 @@ __global__ void __launch_bounds__(32 * LZD_WARPS)
 lz4_parse_blocks_kernel(const uint8_t* __restrict__ in, const uint8_t* __restrict__ in_end, const uint64_t* __restrict__ frame_off,
                         uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ first_slot,
                         LzBlk* __restrict__ tab, unsigned long long* __restrict__ rec, unsigned long long* __restrict__ out_size,
-                        uint32_t* __restrict__ status, uint32_t* __restrict__ needs_seq, uint32_t nframes, uint32_t slot_cap)
+                        uint32_t* __restrict__ status, uint32_t* __restrict__ needs_seq, const zmt_lz4_segment* __restrict__ seg,
+                        uint32_t nframes, uint32_t slot_cap)
 {
     __shared__ __align__(16) uint8_t win[LZD_WARPS][LZD_WIN];
     __shared__ __align__(16) uint8_t jt[LZD_WARPS][LZD_NJ];
@@ -370,7 +382,8 @@ lz4_parse_blocks_kernel(const uint8_t* __restrict__ in, const uint8_t* __restric
         d = bs;
     } else {
         const uint32_t dcap = room < blkmax ? (uint32_t)room : blkmax;
-        const uint32_t hist = (B.flags & LZB_LINKED) ? (boff < 65536 ? (uint32_t)boff : 65536u) : 0u;
+        const uint32_t hist = (B.flags & LZB_LINKED) ? (boff < 65536 ? (uint32_t)boff : 65536u)
+                            : (B.flags & LZB_HIST) ? (seg[f].history < 65536 ? (uint32_t)seg[f].history : 65536u) : 0u;
         d = lzd_parse_block(win[wid], jt[wid], src, in_end, bs, dst, dcap, hist, rec + (abs_src + 2) / 3, &nrec, lane);
         if (d == LZD_ERR) { d_fail(status, f, ZMT_ST_BLOCK, lane); return; }
     }
@@ -674,7 +687,7 @@ __global__ void __launch_bounds__(32 * LZD_WARPS)
 lz4_decode_frames_seq_kernel(const uint8_t* __restrict__ in, const uint8_t* __restrict__ in_end, const uint64_t* __restrict__ frame_off,
                              const uint32_t* __restrict__ frame_csize, uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off,
                              unsigned long long* __restrict__ out_size, uint32_t* __restrict__ status, const uint32_t* __restrict__ needs_seq,
-                             uint32_t nframes)
+                             const zmt_lz4_segment* __restrict__ seg, uint32_t nframes)
 {
     __shared__ __align__(16) uint8_t win[LZD_WARPS][D_WIN];
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -684,17 +697,20 @@ lz4_decode_frames_seq_kernel(const uint8_t* __restrict__ in, const uint8_t* __re
     const uint32_t fs = frame_csize[f];
     uint8_t* dst = out + out_off[f];
     const uint64_t cap = out_off[f + 1] - out_off[f];
-    const uint32_t flg = p[4], bd = p[5];
+    const bool head = !seg || (seg[f].flags & ZMT_SEG_FIRST);          // the scan recorded FLG / BD of a segmented frame
+    const uint32_t flg = seg ? seg[f].flg : p[4], bd = seg ? seg[f].bd : p[5];
     const uint32_t indep = (flg >> 5) & 1, bchk = (flg >> 4) & 1, csz = (flg >> 3) & 1, did = flg & 1;
     const uint32_t blkmax = 1u << (8 + 2 * ((bd >> 4) & 7));
     const uint32_t hl = 2 + (csz ? 8 : 0) + (did ? 4 : 0);
+    const uint64_t h0 = seg && !head ? seg[f].history : 0;              // history below dst (earlier segments)
     __syncwarp();
     if (lane == 0) { status[f] &= ~0xFFu; out_size[f] = 0; }           // pass A may have reported an error for a mis-addressed block
     __syncwarp();
     DWin W; W.w = win[wid]; W.in_end = in_end;
-    uint32_t ip = 4 + hl + 1;
+    uint32_t ip = head ? 4 + hl + 1 : 0;
     uint64_t total = 0;
     for (;;) {
+        if (ip == fs) break;                                // a segment that does not end the frame ends behind a block
         const uint32_t bh = ldg_le32(p + ip);               // block walk already bounds-checked by the scan
         if (bh == 0) break;
         ip += 4;
@@ -708,7 +724,7 @@ lz4_decode_frames_seq_kernel(const uint8_t* __restrict__ in, const uint8_t* __re
         } else {
             const uint64_t room = cap - total;
             const uint32_t dcap = room < blkmax ? (uint32_t)room : blkmax;
-            const uint64_t hist = indep ? 0 : (total < 65536 ? total : 65536);
+            const uint64_t hist = indep ? 0 : (total + h0 < 65536 ? total + h0 : 65536);
             W.gsrc = p + ip; W.pos = 0x40000000;            // empty window
             d = warp_decode_block(W, bs, dst + total, dcap, hist, lane);
             if (d == 0xFFFFFFFFu) { d_fail(status, f, ZMT_ST_BLOCK, lane); return; }
@@ -723,21 +739,23 @@ lz4_decode_frames_seq_kernel(const uint8_t* __restrict__ in, const uint8_t* __re
         __syncwarp();
     }
     if (lane == 0) out_size[f] = total;
-    (void)fs;
 }
 
-// content-size check + comparison of the recomputed XXH32 with the stored content checksum
+// content-size check + comparison of the recomputed XXH32 with the stored content checksum (a segmented frame: on its
+// last segment, against the frame's total; only the last segment sets ZMT_ST_HAS_CHK)
 __global__ void lz4_verify_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
                                   uint32_t* __restrict__ status, const unsigned long long* __restrict__ out_size,
-                                  const uint32_t* __restrict__ stored_chk, const uint32_t* __restrict__ computed, uint32_t nframes)
+                                  const uint32_t* __restrict__ stored_chk, const uint32_t* __restrict__ computed,
+                                  const zmt_lz4_segment* __restrict__ seg, uint32_t nframes)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
     uint32_t st = status[f];
     if ((st & 0xFF) == ZMT_ST_OK) {
         const uint8_t* p = in + frame_off[f] + 12;
-        if (frame_csize[f] >= 15 && (p[4] & 0x08) && ldg_le64(p + 6) != out_size[f]) st = ZMT_ST_CONTENT_SIZE;
-        else if ((st & ZMT_ST_HAS_CHK) && stored_chk[f] != computed[f]) st = ZMT_ST_CONTENT_CHECKSUM;
+        if (seg) { if ((seg[f].flags & ZMT_SEG_LAST) && (seg[f].flg & 0x08) && seg[f].content_size != seg[f].produced) st = ZMT_ST_CONTENT_SIZE; }
+        else if (frame_csize[f] >= 15 && (p[4] & 0x08) && ldg_le64(p + 6) != out_size[f]) st = ZMT_ST_CONTENT_SIZE;
+        if ((st & 0xFF) == ZMT_ST_OK && (st & ZMT_ST_HAS_CHK) && stored_chk[f] != computed[f]) st = ZMT_ST_CONTENT_CHECKSUM;
     }
     status[f] = st & 0xFF;
 }

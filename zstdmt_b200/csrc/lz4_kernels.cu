@@ -32,6 +32,7 @@
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>
 #include "common.cuh"
+#include "frame_format.h"
 #include "host_common.h"
 #include "zmt_dev.h"
 #include "zstd_entropy.cuh"
@@ -362,12 +363,13 @@ zstd_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t c
 // per warp), park each tile in a per-warp shared-memory slot, and lanes 0..3 walk the slot word by word.
 #define X_WARPS 8
 #define X_DEPTH 4
-// XXH32 (seed 0) of p[0, n) by one warp; tile = the warp's 1 KiB of shared memory.  The hash is valid on lane 0.
-__device__ __forceinline__ uint32_t warp_xxh32(const uint8_t* p, uint64_t n, uint4 (*tile)[32], uint32_t lane)
+// XXH32 accumulator j (seed 0) before the first stripe
+__device__ __forceinline__ uint32_t xxh32_acc0(uint32_t j) { return j == 0 ? XXP1 + XXP2 : j == 1 ? XXP2 : j == 2 ? 0u : 0u - XXP1; }
+
+// Folds the ns 16-byte stripes at p into the accumulators: lane l carries accumulator l & 3 in and out.
+__device__ __forceinline__ uint32_t warp_xxh32_stripes(const uint8_t* p, uint64_t ns, uint4 (*tile)[32], uint32_t lane, uint32_t acc)
 {
     const uint32_t j = lane & 3;
-    uint32_t acc = j == 0 ? XXP1 + XXP2 : j == 1 ? XXP2 : j == 2 ? 0u : 0u - XXP1;
-    const uint64_t ns = n >> 4;                              // 16-byte stripes
     uint64_t s = 0;
     if (((uintptr_t)p & 15) == 0) {
         const uint4* v = reinterpret_cast<const uint4*>(p);
@@ -395,6 +397,14 @@ __device__ __forceinline__ uint32_t warp_xxh32(const uint8_t* p, uint64_t n, uin
     // remaining stripes (and unaligned buffers): the 4 chain lanes read global memory directly
     if (((uintptr_t)p & 3) == 0) { const uint32_t* w = reinterpret_cast<const uint32_t*>(p) + j; for (; s < ns; s++) acc = xxh32_round(acc, __ldg(w + 4 * s)); }
     else for (; s < ns; s++) acc = xxh32_round(acc, ldg_le32(p + 16 * s + 4 * j));
+    return acc;
+}
+
+// XXH32 (seed 0) of p[0, n) by one warp; tile = the warp's 1 KiB of shared memory.  The hash is valid on lane 0.
+__device__ __forceinline__ uint32_t warp_xxh32(const uint8_t* p, uint64_t n, uint4 (*tile)[32], uint32_t lane)
+{
+    const uint64_t ns = n >> 4;                              // 16-byte stripes
+    const uint32_t acc = warp_xxh32_stripes(p, ns, tile, lane, xxh32_acc0(lane & 3));
     const uint32_t a1 = __shfl_sync(ZMT_FULL_MASK, acc, 0), a2 = __shfl_sync(ZMT_FULL_MASK, acc, 1);
     const uint32_t a3 = __shfl_sync(ZMT_FULL_MASK, acc, 2), a4 = __shfl_sync(ZMT_FULL_MASK, acc, 3);
     uint32_t h = 0;
@@ -423,6 +433,54 @@ xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs
     else { off = (uint64_t)g * stride; n = zmt_chunk_len(lens32, g, total_bytes, (uint32_t)stride); }
     const uint32_t h = warp_xxh32(base + off, n, tile[wid], lane);
     if (lane == 0) out[g] = h;
+}
+
+// Segments of LZ4F frames (zmt_lz4_segment): one warp per segment folds its decoded bytes into the frame's running
+// XXH32 — the bytes pending from the previous segment are topped up to a stripe first, what is left behind the last
+// whole stripe waits for the next segment — and advances `produced`.  The last segment finalises the hash into out[f].
+__global__ void __launch_bounds__(32 * X_WARPS)
+lz4_segment_xxh32_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ offs, const unsigned long long* __restrict__ lens,
+                         const uint32_t* __restrict__ status, zmt_lz4_segment* __restrict__ seg, uint32_t* __restrict__ out, uint32_t nbuf)
+{
+    __shared__ uint4 tile[X_WARPS][2][32];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t f = blockIdx.x * X_WARPS + wid;
+    if (f >= nbuf || (status[f] & 0xFF) != 0) return;       // a failed segment ends the frame: its state no longer matters
+    zmt_lz4_segment& S = seg[f];
+    const bool first = (S.flags & ZMT_SEG_FIRST) != 0;
+    const uint8_t* p = base + offs[f];
+    const uint64_t n = lens[f];
+    uint8_t pend[16];
+    uint32_t pl = first ? 0u : S.pending_len;
+    for (uint32_t i = 0; i < 16; i++) pend[i] = i < pl ? S.pending[i] : (uint8_t)0;
+    uint32_t acc = first ? xxh32_acc0(lane & 3) : S.acc[lane & 3];
+    uint64_t k = 0;                                          // bytes of this segment that top up the pending stripe
+    if (pl) {
+        k = n < 16 - pl ? n : 16 - pl;
+        for (uint32_t i = 0; i < (uint32_t)k; i++) pend[pl + i] = p[i];
+        pl += (uint32_t)k;
+        if (pl == 16) { acc = xxh32_round(acc, (uint32_t)pend[4 * (lane & 3)] | ((uint32_t)pend[4 * (lane & 3) + 1] << 8) |
+                                                ((uint32_t)pend[4 * (lane & 3) + 2] << 16) | ((uint32_t)pend[4 * (lane & 3) + 3] << 24)); pl = 0; }
+    }
+    const uint64_t ns = (n - k) >> 4;
+    acc = warp_xxh32_stripes(p + k, ns, tile[wid], lane, acc);
+    const uint64_t t0 = k + (ns << 4);                       // the tail behind the last whole stripe
+    if (t0 < n) { for (uint32_t i = 0; i < (uint32_t)(n - t0); i++) pend[i] = p[t0 + i]; pl = (uint32_t)(n - t0); }
+    const uint64_t total = (first ? 0 : S.produced) + n;
+    const uint32_t a1 = __shfl_sync(ZMT_FULL_MASK, acc, 0), a2 = __shfl_sync(ZMT_FULL_MASK, acc, 1);
+    const uint32_t a3 = __shfl_sync(ZMT_FULL_MASK, acc, 2), a4 = __shfl_sync(ZMT_FULL_MASK, acc, 3);
+    if (lane != 0) return;
+    S.acc[0] = a1; S.acc[1] = a2; S.acc[2] = a3; S.acc[3] = a4;
+    for (uint32_t i = 0; i < 16; i++) S.pending[i] = pend[i];
+    S.pending_len = (uint16_t)pl; S.produced = total;
+    if (!(S.flags & ZMT_SEG_LAST)) return;
+    uint32_t h = total >= 16 ? rotl32(a1, 1) + rotl32(a2, 7) + rotl32(a3, 12) + rotl32(a4, 18) : XXP5;
+    h += (uint32_t)total;
+    uint32_t i = 0;
+    for (; i + 4 <= pl; i += 4) h = rotl32(h + ((uint32_t)pend[i] | ((uint32_t)pend[i + 1] << 8) | ((uint32_t)pend[i + 2] << 16) | ((uint32_t)pend[i + 3] << 24)) * XXP3, 17) * XXP4;
+    for (; i < pl; i++) h = rotl32(h + pend[i] * XXP5, 11) * XXP1;
+    h ^= h >> 15; h *= XXP2; h ^= h >> 13; h *= XXP3; h ^= h >> 16;
+    out[f] = h;
 }
 
 // ============================================================================ frame pack
@@ -984,9 +1042,10 @@ extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, ui
     return (size_t)sz + 1024;
 }
 
-extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, uint32_t nframes,
-                                         uint32_t nslots, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size,
-                                         uint32_t* d_status, void* d_work, void* stream_)
+// seg = nullptr: whole frames (zmt_lz4_decompress_device); else every frame of the batch is a segment
+static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, uint32_t nframes,
+                                 uint32_t nslots, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size,
+                                 uint32_t* d_status, zmt_lz4_segment* seg, void* d_work, void* stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0) return ZMT_ST_OK;
@@ -1010,7 +1069,7 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
     lz4_slot_counts_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(d_out_off, nframes, slot_cnt);
     scan_u64_kernel<<<1, 1024, 0, stream>>>(slot_cnt, first_slot, nframes);
     lz4_ticket_windows_kernel<<<1, 256, 0, stream>>>(first_slot, nframes, wbase);
-    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, any_bchk, nframes);
+    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, any_bchk, seg, nframes);
     zmt_dbg_check(stream, "lz4_scan_frames_kernel");
     {
         const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8), need = (nslots + X_WARPS - 1) / X_WARPS;
@@ -1019,7 +1078,7 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
     zmt_dbg_check(stream, "lz4_block_checksum_kernel");
     { ZmtProfScope ps(ZMT_K_LZ4_DECODE, stream);
     lz4_parse_blocks_kernel<<<(nslots + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(
-        in, in + in_bytes, d_frame_off, (uint8_t*)d_out, d_out_off, first_slot, tab, rec, (unsigned long long*)d_out_size, d_status, needs_seq, nframes, nslots); }
+        in, in + in_bytes, d_frame_off, (uint8_t*)d_out, d_out_off, first_slot, tab, rec, (unsigned long long*)d_out_size, d_status, needs_seq, seg, nframes, nslots); }
     zmt_dbg_check(stream, "lz4_parse_blocks_kernel");
     {
         const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8);
@@ -1032,11 +1091,38 @@ extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, co
     }
     zmt_dbg_check(stream, "lz4_exec_blocks_kernel");
     lz4_decode_frames_seq_kernel<<<(nframes + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(
-        in, in + in_bytes, d_frame_off, d_frame_csize, (uint8_t*)d_out, d_out_off, (unsigned long long*)d_out_size, d_status, needs_seq, nframes);
+        in, in + in_bytes, d_frame_off, d_frame_csize, (uint8_t*)d_out, d_out_off, (unsigned long long*)d_out_size, d_status, needs_seq, seg, nframes);
     zmt_dbg_check(stream, "lz4_decode_frames_seq_kernel");
     { ZmtProfScope ps(ZMT_K_XXH32_DEC, stream);
-    xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off, d_out_size, nullptr, 0, 0, computed, nframes); }
+    if (seg) lz4_segment_xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off,
+                                                                                                     (const unsigned long long*)d_out_size, d_status, seg, computed, nframes);
+    else xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off, d_out_size, nullptr, 0, 0, computed, nframes); }
     lz4_verify_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(in, d_frame_off, d_frame_csize, d_status,
-                                                                (const unsigned long long*)d_out_size, stored, computed, nframes);
+                                                                (const unsigned long long*)d_out_size, stored, computed, seg, nframes);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+extern "C" int zmt_lz4_decompress_device(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, uint32_t nframes,
+                                         uint32_t nslots, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size,
+                                         uint32_t* d_status, void* d_work, void* stream)
+{
+    return lz4_decompress_launch(d_in, in_bytes, d_frame_off, d_frame_csize, nframes, nslots, d_out, d_out_off, d_out_size, d_status, nullptr, d_work, stream);
+}
+
+extern "C" int zmt_lz4_decompress_segments_device(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                                  uint32_t nframes, uint32_t nslots, void* d_out, const uint64_t* d_out_off, uint64_t* d_out_size,
+                                                  uint32_t* d_status, zmt_lz4_segment* d_seg, void* d_work, void* stream)
+{
+    if (!d_seg && nframes) return ZMT_ST_BAD_ARG;
+    return lz4_decompress_launch(d_in, in_bytes, d_frame_off, d_frame_csize, nframes, nslots, d_out, d_out_off, d_out_size, d_status, d_seg, d_work, stream);
+}
+
+extern "C" int zmt_lz4f_segment_host(const uint8_t* seg, size_t n, size_t start, uint32_t flg, uint32_t bd, size_t max_in, uint64_t max_out,
+                                     size_t* end, uint64_t* room, uint32_t* last)
+{
+    Lz4fWalk w; w.pos = start; w.bound = 0; w.nblk = 0; w.done = 0;
+    const size_t stop = max_in > start ? max_in : start + 1;                  // at least one block (or the end mark)
+    if (!lz4f_walk_blocks(seg, n, flg, bd, &w, stop, max_out > 0 ? max_out : 1) || w.pos > n) return ZMT_ST_TRUNCATED;
+    *end = w.pos; *room = w.bound; *last = w.done;
+    return ZMT_ST_OK;
 }
