@@ -43,17 +43,11 @@ typedef int (gen_rw_fn)(void* arg, GenBuffer* b);
 struct GenRdWr { gen_rw_fn* fn_read; void* arg_read; gen_rw_fn* fn_write; void* arg_write; };
 
 enum { CODEC_LZ4 = 1, CODEC_ZSTD = 2 };
-#define MT_MAGIC_SKIPPABLE 0x184D2A50u
-#define LZ4F_MAGIC         0x184D2204u
-#define ZSTD_MAGIC         0xFD2FB528u
 
 // error numbering differs between the codecs (lz4-mt.h:41-53 vs zstd-mt.h:41-54)
 struct ErrCodes { size_t mem, read_fail, write_fail, data_error, frame_compress, frame_decompress, param, library, canceled, init_missing; };
 const ErrCodes kErrLz4  = { (size_t)-1, (size_t)-2, (size_t)-3, (size_t)-4, (size_t)-5, (size_t)-6, (size_t)-7, (size_t)-8, (size_t)-9, (size_t)-7 };
 const ErrCodes kErrZstd = { (size_t)-1, (size_t)-3, (size_t)-4, (size_t)-5, (size_t)-6, (size_t)-7, (size_t)-8, (size_t)-9, (size_t)-10, (size_t)-2 };
-
-inline uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
-inline uint64_t rd64(const uint8_t* p) { return (uint64_t)rd32(p) | ((uint64_t)rd32(p + 4) << 32); }
 
 // callback return -> library error (mt_error, lz4-mt_compress.c:161-173: write failures also map to read_fail)
 inline size_t mt_error(const ErrCodes& E, int rv)
@@ -192,27 +186,7 @@ const CodecOps& codec_ops(int codec)
     return codec == CODEC_LZ4 ? lz4 : zstd;
 }
 
-// ------------------------------------------------------------------ staging slots
-struct Slot {
-    int dev = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev = nullptr, evp[2] = { nullptr, nullptr };       // evp: decompress writer, output pieces in flight
-    uint8_t *h_in = nullptr, *h_out = nullptr, *d_in = nullptr, *d_out = nullptr, *d_work = nullptr;
-    size_t in_cap = 0, out_cap = 0, work_cap = 0, tab_cap = 0;   // tab_cap: entries in the tables below
-    // tables: pinned host mirror + device copy, one allocation each
-    uint8_t *h_tab = nullptr, *d_tab = nullptr; size_t tab_bytes = 0;
-    // batch contents
-    uint32_t n = 0;              // chunks / frames in this batch
-    uint32_t nslots = 1;         // lz4 decompress: block-table slots of this batch (sum over frames of max(1, ceil(out / 64 KiB)))
-    uint64_t scr_cap = 0;        // zstd decompress: entropy scratch bytes the workspace was sized for
-    // zstd decompress: block descriptors built by the reader (pinned) + device copy, scratch demand of the batch
-    uint8_t *h_blk = nullptr, *d_blk = nullptr; uint32_t blk_cap = 0, nblk = 0; uint64_t scratch_used = 0;
-    size_t in_used = 0, out_used = 0;
-    int state = 0;               // 0 free, 1 filled, 2 submitted
-    bool ok = false;
-    bool host_alias = false;     // h_in / h_out are borrowed from another slot of the same context (never freed here)
-};
-
+// ------------------------------------------------------------------ batch tables
 // Per-chunk / per-frame tables of a batch (entries = tab_cap).  Layout:
 //   u64 frame_off[cap+1] | u64 out_off[cap+1] | u64 out_size[cap+1] | u64 expect[cap+1] | u32 per_frame[cap] | u32 status[cap] | u32 first_blk[cap+1]
 struct Tables {
@@ -234,6 +208,83 @@ inline Tables tables_at(uint8_t* base, size_t cap)
 
 // lz4 decode block table capacity of a slot: every frame owns max(1, ceil(out / 64 KiB)) slots
 inline uint32_t lz4_slot_cap(size_t out_cap, size_t tab_cap) { return (uint32_t)(out_cap / 65536 + tab_cap + 1); }
+
+// The frames of one decode batch, in the order the decoder takes them, with the totals its workspace is sized from.
+// Every host decode batch is built here (a container slot, a batch of plain frames, one segment of an LZ4F frame) and
+// packed into a Tables view just before it is copied to the device.
+struct FrameList {
+    std::vector<uint64_t> in_off;     // where each frame starts in the batch input (LZ4: its 12-byte header)
+    std::vector<uint64_t> out_off;    // where each frame's content goes, + the end of the last one
+    std::vector<uint64_t> expect;     // zstd: the content size from the header, ~0 without one
+    std::vector<uint32_t> per_frame;  // LZ4: payload bytes; zstd: ZF_* flags of the frame walk
+    std::vector<uint32_t> first_blk;  // zstd: each frame's first block descriptor, + the total
+    uint32_t nblk = 0;                // zstd: block descriptors of the batch
+    uint64_t scratch = 0;             // zstd: entropy scratch bytes of the batch
+    uint64_t nslots = 0;              // LZ4: block-table slots of the batch (lz4_frame_slots per frame)
+
+    FrameList() { clear(); }
+    uint32_t n() const { return (uint32_t)in_off.size(); }
+    uint64_t out_end() const { return out_off.back(); }
+    // an empty batch whose output starts at out_at
+    void clear(uint64_t out_at = 0)
+    {
+        in_off.clear(); expect.clear(); per_frame.clear();
+        out_off.assign(1, out_at); first_blk.assign(1, 0);
+        nblk = 0; scratch = 0; nslots = 0;
+    }
+    // one frame at `at` with `room` bytes of output; zstd: its descriptors end at blk_to and the batch's scratch at scr_to
+    void push(uint64_t at, uint32_t pf, uint64_t room, uint64_t exp = 0, uint32_t blk_to = 0, uint64_t scr_to = 0)
+    {
+        in_off.push_back(at); per_frame.push_back(pf); expect.push_back(exp);
+        out_off.push_back(out_end() + room); first_blk.push_back(blk_to);
+        nblk = blk_to; scratch = scr_to; nslots += lz4_frame_slots(room);
+    }
+    void pack(const Tables& T) const
+    {
+        const size_t k = n();
+        memcpy(T.frame_off, in_off.data(), k * 8); memcpy(T.out_off, out_off.data(), (k + 1) * 8); memcpy(T.expect, expect.data(), k * 8);
+        memcpy(T.per_frame, per_frame.data(), k * 4); memcpy(T.first_blk, first_blk.data(), (k + 1) * 4);
+    }
+};
+
+// The zstd block-table rule of a decode batch.  Walks the zstd frame f[0..n), at base_off in the batch input, as the
+// next frame of `fl`: its descriptors go to blk[fl.nblk, cap), and *w gets the batch's block and scratch totals with it,
+// the frame's room (its content size, or the block bound with ZF_NO_SIZE), its flags and its length.  When the table is
+// full (ZMT_ST_DST_SMALL) and `count` is set, a counting walk fills *w instead and returns the frame's own status if that
+// is not OK: the caller grows the table, or carries the frame to the next batch, and walks once more.  A frame that fits
+// is walked once.
+struct ZWalk { uint32_t nblk = 0, flags = 0; uint64_t scratch = 0, room = 0; size_t end = 0; };
+int zstd_blocks(const FrameList& fl, const uint8_t* f, size_t n, uint64_t base_off, void* blk, uint32_t cap, bool count, ZWalk& w)
+{
+    w.nblk = fl.nblk; w.scratch = fl.scratch;
+    int r = zstd_frame_walk<true>(f, n, base_off, fl.n(), (ZBlk*)blk, &w.nblk, cap, &w.scratch, &w.room, &w.flags, &w.end);
+    if (r != ZMT_ST_DST_SMALL || !count) return r;
+    w.nblk = fl.nblk; w.scratch = fl.scratch;
+    r = zstd_frame_walk<false>(f, n, base_off, fl.n(), nullptr, &w.nblk, 0xFFFFFFFFu, &w.scratch, &w.room, &w.flags, &w.end);
+    return r == ZMT_ST_OK ? ZMT_ST_DST_SMALL : r;
+}
+inline uint64_t zstd_expect(const ZWalk& w) { return (w.flags & ZF_NO_SIZE) ? ~0ull : w.room; }
+
+// ------------------------------------------------------------------ staging slots
+struct Slot {
+    int dev = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev = nullptr, evp[2] = { nullptr, nullptr };       // evp: decompress writer, output pieces in flight
+    uint8_t *h_in = nullptr, *h_out = nullptr, *d_in = nullptr, *d_out = nullptr, *d_work = nullptr;
+    size_t in_cap = 0, out_cap = 0, work_cap = 0, tab_cap = 0;   // tab_cap: entries in the tables below
+    // tables: pinned host mirror + device copy, one allocation each
+    uint8_t *h_tab = nullptr, *d_tab = nullptr; size_t tab_bytes = 0;
+    // batch contents
+    uint32_t n = 0;              // compress: chunks in this batch
+    FrameList frames;            // decompress: frames in this batch
+    uint64_t scr_cap = 0;        // zstd decompress: entropy scratch bytes the workspace was sized for
+    // zstd decompress: block descriptors built by the reader (pinned) + device copy
+    uint8_t *h_blk = nullptr, *d_blk = nullptr; uint32_t blk_cap = 0;
+    size_t in_used = 0;
+    int state = 0;               // 0 free, 1 filled, 2 submitted
+    bool ok = false;
+    bool host_alias = false;     // h_in / h_out are borrowed from another slot of the same context (never freed here)
+};
 
 void slot_free_raw(Slot& s)
 {
@@ -274,7 +325,7 @@ bool slot_alloc(Slot& s, int dev, size_t in_cap, size_t out_cap, size_t work_cap
             if ((c.h_in == nullptr) == (host_owner != nullptr) && c.dev == dev && c.in_cap >= in_cap && c.out_cap >= out_cap &&
                 c.work_cap >= work_cap && c.tab_cap == tab_cap) {
                 s = c; g_pool.erase(g_pool.begin() + (long)i);
-                s.state = 0; s.n = 0; s.in_used = s.out_used = 0;
+                s.state = 0; s.n = 0; s.in_used = 0; s.frames.clear();
                 ok = true;
             }
         }
@@ -358,8 +409,13 @@ void ctx_release_slots(Ctx* c)
     c->pipe.slots.clear();
 }
 
-// a frame's ZMT_ST_* -> the library error of the call: a cut or overlong frame is the frame's fault, the rest the codec's
-inline size_t status_error(const ErrCodes& E, uint32_t st) { return st == ZMT_ST_TRUNCATED || st == ZMT_ST_TRAILING ? E.frame_decompress : E.library; }
+// a frame's ZMT_ST_* -> the library error of the call, the status kept for *_getErrorString: a cut or overlong frame is the
+// frame's fault, the rest the codec's
+inline size_t frame_error(Ctx* c, uint32_t st)
+{
+    c->lib_errcode = st;
+    return st == ZMT_ST_TRUNCATED || st == ZMT_ST_TRAILING ? c->E->frame_decompress : c->E->library;
+}
 
 // ------------------------------------------------------------------ the pipeline of one call
 // reader thread  : fill    — fn_read into the free slot, in sequence order (pt_read / the read section of pt_compress)
@@ -563,22 +619,28 @@ size_t read_some(const ErrCodes& E, GenRdWr* rw, void* dst, size_t want, size_t*
     *got = b.size; return 0;
 }
 
-// Enqueues the decode of one batch of n frames on `st`: the frames' tables in Td (device), the zstd block descriptors in d_blk.
-int decode_batch(bool is_zstd, const void* d_in, size_t in_bytes, const void* d_blk, uint32_t nblk, const Tables& Td, uint32_t n,
-                 uint32_t nslots, void* d_out, void* d_work, cudaStream_t st)
+// One decode step on `st`: the batch's tables (packed into h_tab, `cap` entries; the device copy at d_tab) and, for zstd,
+// its block descriptors go to the device, the batch is decoded (with `seg`: as one segment of an LZ4F frame), and its
+// status and sizes come back into h_tab.  The batch's input must be in place on the stream before.  Returns ZMT_ST_*.
+int decode_step(bool is_zstd, const FrameList& fl, uint8_t* h_tab, uint8_t* d_tab, size_t cap, const void* h_blk, void* d_blk,
+                const void* d_in, size_t in_bytes, void* d_out, void* d_work, zmt_lz4_segment* seg, cudaStream_t st)
 {
-    return is_zstd ? zmt_zstd_decompress_device(d_in, d_blk, nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size, Td.status, d_work, st)
-                   : zmt_lz4_decompress_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, d_work, st);
+    const Tables Th = tables_at(h_tab, cap), Td = tables_at(d_tab, cap);
+    const uint32_t n = fl.n(), nslots = (uint32_t)fl.nslots;
+    fl.pack(Th);
+    if (cudaMemcpyAsync(d_tab, h_tab, tables_bytes(cap), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        (is_zstd && fl.nblk && cudaMemcpyAsync(d_blk, h_blk, (size_t)fl.nblk * sizeof(ZBlk), cudaMemcpyHostToDevice, st) != cudaSuccess))
+        return ZMT_ST_CUDA;
+    const int r = is_zstd ? zmt_zstd_decompress_device(d_in, d_blk, fl.nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size, Td.status, d_work, st)
+                : seg ? zmt_lz4_decompress_segments_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, seg, d_work, st)
+                      : zmt_lz4_decompress_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, d_work, st);
+    if (r != ZMT_ST_OK) return r;
+    if (cudaMemcpyAsync(Th.out_size, Td.out_size, (size_t)n * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(Th.status, Td.status, (size_t)n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return ZMT_ST_CUDA;
+    return ZMT_ST_OK;
 }
 
 // ------------------------------------------------------------------ plain (unframed) single streams
-// What the reference routes to st_decompress (lz4-mt_decompress.c:391-483, zstd-mt_decompress.c:552-687): an ordinary
-// .lz4 / .zst file, i.e. codec frames back to back without the 12-byte size headers.  Frame lengths are only known after
-// walking the block headers, so the host reads ahead, cuts the bytes it holds into complete frames, and decodes them in
-// batches of at most ~kPlainBatch input bytes with the same GPU kernels; the consumed bytes are dropped before the next
-// read, so memory is bounded by the batch size or by the largest single frame, whichever is larger (the reference streams
-// through two fixed buffers; a frame here must fit in host and device memory as a whole).  `first`/`have` = the bytes
-// already consumed by the stream-type sniffing.
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
     ~DevBuf() { if (p) cudaFree(p); }
@@ -591,242 +653,232 @@ struct DevBuf {
     }
 };
 
-// Appends one read of up to `piece` bytes to `in`; sets eof on an empty read.
-size_t read_piece(Ctx* c, GenRdWr* rw, std::vector<uint8_t>& in, size_t piece, bool& eof)
-{
-    const size_t old = in.size();
-    in.resize(old + piece);
-    size_t got = 0;
-    const size_t e = read_some(*c->E, rw, in.data() + old, piece, &got);
-    in.resize(old + got);
-    if (e) return e;
-    c->insize += got;
-    if (got == 0) eof = true;
-    return 0;
-}
+// What the reference routes to st_decompress (lz4-mt_decompress.c:391-483, zstd-mt_decompress.c:552-687): an ordinary
+// .lz4 / .zst file, i.e. codec frames back to back without the 12-byte size headers.  Frame lengths are only known after
+// walking the block headers, so the host reads ahead, cuts the bytes it holds into complete frames, and decodes them in
+// batches of at most ~`batch` input bytes with the same GPU kernels; the consumed bytes are dropped before the next read.
+// An LZ4F frame larger than a batch is decoded in segments (lz4_segments), so LZ4 memory is O(batch + 64 KiB); a zstd
+// frame must fit in host and device memory as a whole.  Single-threaded: a batch's frames are written before the next read.
+struct PlainStream {
+    Ctx* c; GenRdWr* rw;
+    const bool is_zstd;
+    const size_t batch, piece;              // input bytes per batch (ZSTDMT_B200_PLAIN_MB); bytes per fn_read and per fn_write
+    std::vector<uint8_t> in;                // 12 pad bytes (the LZ4 kernel addresses a frame as base + off + 12), then the bytes held
+    size_t pos = 0;                         // parse position inside in[12..]
+    bool eof = false;
+    cudaStream_t st = nullptr;
+    DevBuf d_in, d_out, d_tab, d_blk, d_work, d_seg, d_hist;         // d_seg, d_hist: LZ4F frames decoded in segments
+    std::vector<uint8_t> h_tab, out;        // the batch's tables (status and sizes come back here) and decoded bytes
+    std::vector<ZBlk> blocks;               // zstd: the batch's block table
+    FrameList fl;
 
-// One LZ4F frame that reaches a batch of input (or four of output) before its end, at in[12 + pos], decoded as a chain of
-// segments of whole blocks (zmt_lz4_decompress_segments_device): each segment is read, decoded and written before the
-// next one is read, and its input dropped.  The device keeps the frame's state between segments (zmt_lz4_segment: XXH32,
-// content size) in d_seg and, for linked blocks, the last 64 KiB of content in d_hist; the segment's output goes to
-// d_out + 64 KiB with the history copied directly below.  Memory stays O(batch) whatever the frame's size.  One stream
-// synchronisation per segment: status, size and the output room come back together, and the history of the next segment
-// is saved behind them.  On return the frame has been consumed (pos = 0, in holds what follows it).
-size_t decode_lz4_segments(Ctx* c, GenRdWr* rw, std::vector<uint8_t>& in, size_t& pos, bool& eof, size_t batch, size_t piece,
-                           cudaStream_t st, DevBuf& d_in, DevBuf& d_out, DevBuf& d_tab, DevBuf& d_work, DevBuf& d_seg, DevBuf& d_hist,
-                           std::vector<uint8_t>& out)
-{
-    const ErrCodes& E = *c->E;
-    const uint32_t flg = in[12 + pos + 4], bd = in[12 + pos + 5];
-    const bool linked = !(flg & 0x20);
-    const uint64_t H = 65536;                               // the history's room below each segment's output
-    if (!d_seg.need(sizeof(zmt_lz4_segment)) || !d_hist.need(H)) return E.mem;
-    cudaMemsetAsync(d_seg.p, 0, sizeof(zmt_lz4_segment), st);
-    uint64_t produced = 0;
-    bool first = true;
-    for (;;) {
-        // ---- the next segment: whole blocks up to a batch of input / four of output room
-        size_t end = 0; uint64_t room = 0; uint32_t last = 0;
-        for (;;) {
-            const int r = zmt_lz4f_segment_host(in.data() + 12 + pos, in.size() - 12 - pos, first ? lz4f_header_len(flg) : 0, flg, bd,
-                                                batch, 4 * (uint64_t)batch, &end, &room, &last);
-            if (r == ZMT_ST_OK) break;
-            if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; }
-            const size_t goal = 12 + pos + batch + piece;
-            do { const size_t e = read_piece(c, rw, in, piece, eof); if (e) return e; } while (!eof && in.size() < goal);
-        }
-        // ---- decode it: a batch of one frame, its bytes at d_in + 12
-        const uint64_t hlen = linked ? (produced < H ? produced : H) : 0;
-        const size_t tab_bytes = tables_bytes(1);
-        std::vector<uint8_t> h_tab(tab_bytes);
-        Tables T = tables_at(h_tab.data(), 1);
-        T.frame_off[0] = 0; T.per_frame[0] = (uint32_t)end; T.out_off[0] = H; T.out_off[1] = H + room;
-        const uint32_t nslots = (uint32_t)lz4_frame_slots(room);
-        const size_t wk = zmt_lz4d_workspace_bytes(1, nslots, 12 + end);
-        if (!d_in.need(12 + end + 256) || !d_out.need(H + room + 256) || !d_tab.need(tab_bytes) || !d_work.need(wk)) return E.mem;
-        Tables Td = tables_at((uint8_t*)d_tab.p, 1);
-        const uint32_t flags = (first ? ZMT_SEG_FIRST : 0u) | (last ? ZMT_SEG_LAST : 0u);
-        zmt_lz4_segment* ds = (zmt_lz4_segment*)d_seg.p;
-        cudaError_t ce = cudaMemcpyAsync((uint8_t*)d_in.p + 12, in.data() + 12 + pos, end, cudaMemcpyHostToDevice, st);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_tab.p, h_tab.data(), tab_bytes, cudaMemcpyHostToDevice, st);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->history, &hlen, sizeof(hlen), cudaMemcpyHostToDevice, st);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->flags, &flags, sizeof(flags), cudaMemcpyHostToDevice, st);
-        if (ce == cudaSuccess && hlen) ce = cudaMemcpyAsync((uint8_t*)d_out.p + H - hlen, d_hist.p, hlen, cudaMemcpyDeviceToDevice, st);
-        const int rc = ce == cudaSuccess ? zmt_lz4_decompress_segments_device(d_in.p, 12 + end, Td.frame_off, Td.per_frame, 1, nslots, d_out.p, Td.out_off,
-                                                                               Td.out_size, Td.status, ds, d_work.p, st) : ZMT_ST_CUDA;
-        // status, size and the whole output room (the segment's content is at most `room` bytes) in one round trip;
-        // d_out is read back before the next segment is queued on the stream
-        uint32_t status = 0; uint64_t osz = 0;
-        out.resize(room ? room : 1);
-        if (rc == ZMT_ST_OK) {
-            ce = cudaMemcpyAsync(&status, Td.status, 4, cudaMemcpyDeviceToHost, st);
-            if (ce == cudaSuccess) ce = cudaMemcpyAsync(&osz, Td.out_size, 8, cudaMemcpyDeviceToHost, st);
-            if (ce == cudaSuccess && room) ce = cudaMemcpyAsync(out.data(), (uint8_t*)d_out.p + H, room, cudaMemcpyDeviceToHost, st);
-            if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-        }
-        if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library; }
-        if (status != ZMT_ST_OK) { c->lib_errcode = status; return status_error(E, status); }
-        if (osz > room) { c->lib_errcode = ZMT_ST_DST_SMALL; return E.library; }
-        // ---- the history of the next segment: the last 64 KiB of [history | this segment], contiguous below H + osz; queued
-        //      behind this segment, ahead of the next one (a reallocation of d_out in between synchronises in cudaFree)
-        const uint64_t hnext = linked ? (hlen + osz < H ? hlen + osz : H) : 0;
-        if (hnext && !last && cudaMemcpyAsync(d_hist.p, (uint8_t*)d_out.p + H + osz - hnext, hnext, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-            cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library;
-        }
-        for (uint64_t o = 0; o < osz;) {
-            GenBuffer b; b.buf = out.data() + o; b.size = (size_t)((osz - o) < piece ? (osz - o) : piece); b.allocated = b.size;
+    // `first`/`have` = the bytes already consumed by the stream-type sniffing
+    PlainStream(Ctx* c_, GenRdWr* rw_, const uint8_t* first, size_t have)
+        : c(c_), rw(rw_), is_zstd(c_->codec == CODEC_ZSTD), batch(env_size("ZSTDMT_B200_PLAIN_MB", 64) << 20),
+          piece(c_->inputsize < (64u << 10) ? (size_t)1 << 20 : c_->inputsize), in(12, 0)
+    {
+        in.insert(in.end(), first, first + have);
+    }
+    ~PlainStream() { if (st) cudaStreamDestroy(st); }
+
+    // Appends reads of up to `piece` bytes to `in`, at least one, until it holds `goal` bytes or the input ends.
+    size_t read_to(size_t goal)
+    {
+        do {
+            const size_t old = in.size();
+            in.resize(old + piece);
+            size_t got = 0;
+            const size_t e = read_some(*c->E, rw, in.data() + old, piece, &got);
+            in.resize(old + got);
+            if (e) return e;
+            c->insize += got;
+            if (got == 0) eof = true;
+        } while (!eof && in.size() < goal);
+        return 0;
+    }
+
+    // Writes p[0..size) to fn_write in pieces of at most `piece` bytes (st_decompress writes as it goes).
+    size_t write(const uint8_t* p, uint64_t size)
+    {
+        for (uint64_t o = 0; o < size;) {
+            GenBuffer b; b.buf = (void*)(p + o); b.size = (size_t)(size - o < piece ? size - o : piece); b.allocated = b.size;
             const size_t want = b.size;
             const int rv = rw->fn_write(rw->arg_write, &b);
-            if (rv != 0) return mt_error(E, rv);
+            if (rv != 0) return mt_error(*c->E, rv);
             c->outsize += b.size; o += want;
         }
-        produced += osz;
-        in.erase(in.begin() + 12, in.begin() + 12 + (long)(pos + end));       // drop the decoded segment
-        pos = 0; first = false;
-        if (last) return 0;
+        return 0;
     }
-}
+
+    // Decodes the batch `fl`: src[0 .. in_bytes - lo) goes to d_in + lo (the device addresses the frames at their offsets in
+    // the batch input), the decode step runs, and the output room [out_off[0], out_end) comes back into `out` with the
+    // status and sizes (in h_tab), in one stream synchronisation.
+    size_t decode(const uint8_t* src, size_t lo, size_t in_bytes, zmt_lz4_segment* seg)
+    {
+        const uint32_t nf = fl.n();
+        const uint64_t out_at = fl.out_off[0], room = fl.out_end() - out_at;
+        const size_t tab_bytes = tables_bytes(nf);
+        const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes(nf, fl.nblk, fl.scratch) : zmt_lz4d_workspace_bytes(nf, (uint32_t)fl.nslots, in_bytes);
+        if (!d_in.need(in_bytes + 256) || !d_out.need(fl.out_end() + 256) || !d_tab.need(tab_bytes) || !d_work.need(wk) ||
+            (is_zstd && !d_blk.need((size_t)fl.nblk * sizeof(ZBlk) + 16))) return c->E->mem;
+        h_tab.resize(tab_bytes);
+        out.resize(room ? room : 1);
+        cudaError_t ce = cudaMemcpyAsync((uint8_t*)d_in.p + lo, src, in_bytes - lo, cudaMemcpyHostToDevice, st);
+        const int rc = ce == cudaSuccess ? decode_step(is_zstd, fl, h_tab.data(), (uint8_t*)d_tab.p, nf, blocks.data(), d_blk.p, d_in.p, in_bytes,
+                                                       d_out.p, d_work.p, seg, st) : ZMT_ST_CUDA;
+        if (rc == ZMT_ST_OK && room) ce = cudaMemcpyAsync(out.data(), (uint8_t*)d_out.p + out_at, room, cudaMemcpyDeviceToHost, st);
+        if (rc == ZMT_ST_OK && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
+        return 0;
+    }
+
+    // One LZ4F frame that reaches a batch of input (or four of output) before its end, at in[12 + pos], decoded as a chain
+    // of segments of whole blocks (zmt_lz4_decompress_segments_device): each segment is read, decoded and written before
+    // the next one is read, and its input dropped.  The device keeps the frame's state between segments (zmt_lz4_segment:
+    // XXH32, content size) in d_seg and, for linked blocks, the last 64 KiB of content in d_hist; the segment's output goes
+    // to d_out + 64 KiB with the history copied directly below.  Memory stays O(batch) whatever the frame's size.  One
+    // stream synchronisation per segment: status, size and the output room come back together, and the history of the
+    // next segment is saved behind them.  On return the frame has been consumed (pos = 0, in holds what follows it).
+    size_t lz4_segments()
+    {
+        const uint32_t flg = in[12 + pos + 4], bd = in[12 + pos + 5];
+        const bool linked = !(flg & 0x20);
+        const uint64_t H = 65536;                               // the history's room below each segment's output
+        if (!d_seg.need(sizeof(zmt_lz4_segment)) || !d_hist.need(H)) return c->E->mem;
+        if (cudaMemsetAsync(d_seg.p, 0, sizeof(zmt_lz4_segment), st) != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
+        zmt_lz4_segment* ds = (zmt_lz4_segment*)d_seg.p;
+        uint64_t produced = 0;
+        for (bool first = true;; first = false) {
+            // ---- the next segment: whole blocks up to a batch of input / four of output room
+            size_t end = 0; uint64_t room = 0; uint32_t last = 0;
+            while (zmt_lz4f_segment_host(in.data() + 12 + pos, in.size() - 12 - pos, first ? lz4f_header_len(flg) : 0, flg, bd,
+                                         batch, 4 * (uint64_t)batch, &end, &room, &last) != ZMT_ST_OK) {
+                if (eof) return frame_error(c, ZMT_ST_TRUNCATED);
+                const size_t e = read_to(12 + pos + batch + piece);
+                if (e) return e;
+            }
+            // ---- decode it: a batch of one frame, its bytes at d_in + 12, its output at d_out + H above `hlen` bytes of history
+            const uint64_t hlen = linked ? (produced < H ? produced : H) : 0;
+            const uint32_t flags = (first ? ZMT_SEG_FIRST : 0u) | (last ? ZMT_SEG_LAST : 0u);
+            if (!d_out.need(H + room + 256)) return c->E->mem;
+            cudaError_t ce = cudaMemcpyAsync(&ds->history, &hlen, sizeof(hlen), cudaMemcpyHostToDevice, st);
+            if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->flags, &flags, sizeof(flags), cudaMemcpyHostToDevice, st);
+            if (ce == cudaSuccess && hlen) ce = cudaMemcpyAsync((uint8_t*)d_out.p + H - hlen, d_hist.p, hlen, cudaMemcpyDeviceToDevice, st);
+            if (ce != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
+            fl.clear(H); fl.push(0, (uint32_t)end, room);
+            const size_t e = decode(in.data() + 12 + pos, 12, 12 + end, ds);
+            if (e) return e;
+            const Tables T = tables_at(h_tab.data(), 1);
+            if (T.status[0] != ZMT_ST_OK) return frame_error(c, T.status[0]);
+            const uint64_t osz = T.out_size[0];
+            if (osz > room) return frame_error(c, ZMT_ST_DST_SMALL);
+            // ---- the history of the next segment: the last 64 KiB of [history | this segment], contiguous below H + osz; queued
+            //      behind this segment, ahead of the next one (a reallocation of d_out in between synchronises in cudaFree)
+            const uint64_t hnext = linked ? (hlen + osz < H ? hlen + osz : H) : 0;
+            if (hnext && !last && cudaMemcpyAsync(d_hist.p, (uint8_t*)d_out.p + H + osz - hnext, hnext, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+                cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA);
+            }
+            const size_t we = write(out.data(), osz);
+            if (we) return we;
+            produced += osz;
+            in.erase(in.begin() + 12, in.begin() + 12 + (long)(pos + end));       // drop the decoded segment
+            pos = 0;
+            if (last) return 0;
+        }
+    }
+};
 
 size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_t have)
 {
     const ErrCodes& E = *c->E;
-    const bool is_zstd = c->codec == CODEC_ZSTD;
-    const size_t kPlainBatch = env_size("ZSTDMT_B200_PLAIN_MB", 64) << 20;
-    const size_t piece = c->inputsize < (64u << 10) ? (size_t)1 << 20 : c->inputsize;
-    const size_t dsz = zmt_zstd_blk_desc_bytes();
-    std::vector<uint8_t> in(12, 0);                         // 12 pad bytes: the LZ4 kernel addresses a frame as base + off + 12
-    in.insert(in.end(), first, first + have);
-    bool eof = false;
-    size_t pos = 0;                                         // parse position inside in[12..]
+    PlainStream S(c, rw, first, have);
+    std::vector<uint8_t>& in = S.in;
+    size_t& pos = S.pos;
+    FrameList& fl = S.fl;
     const std::vector<int> devs = env_devices();
-    if (devs.empty() || cudaSetDevice(devs[0]) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
-    DevBuf d_in, d_out, d_tab, d_blk, d_work, d_seg, d_hist;         // d_seg, d_hist: LZ4F frames decoded in segments
-    cudaStream_t st = nullptr;
-    if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
-    struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{st};
-    std::vector<uint8_t> out, blocks, h_tab;
-    std::vector<uint64_t> foff, ooff, expect; std::vector<uint32_t> fcs, first_blk, fflags;
+    if (devs.empty() || cudaSetDevice(devs[0]) != cudaSuccess) return frame_error(c, ZMT_ST_CUDA);
+    if (cudaStreamCreateWithFlags(&S.st, cudaStreamNonBlocking) != cudaSuccess) return frame_error(c, ZMT_ST_CUDA);
     c->insize = have;
 
     for (;;) {
         // ---- cut complete frames out of what we hold, up to one batch
-        foff.clear(); ooff.assign(1, 0); expect.clear(); fcs.clear(); first_blk.assign(1, 0); fflags.clear();
-        uint32_t nblk = 0; uint64_t scratch = 0, nslots = 0;
+        fl.clear();
         const size_t batch_start = pos;
         bool need_more = false, segmented = false;
         while (!need_more) {
             const uint8_t* s = in.data() + 12; const size_t n = in.size() - 12;
-            if (pos >= n) { need_more = !eof; break; }
-            if (!foff.empty() && pos - batch_start >= kPlainBatch) break;
-            if (n - pos < 4) { if (eof) return E.data_error; need_more = true; break; }
-            const uint32_t magic = rd32(s + pos);
-            if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {          // skippable frame: magic, LE32 size, payload
-                if (n - pos < 8 || n - pos - 8 < rd32(s + pos + 4)) { if (eof) return E.data_error; need_more = true; break; }
-                pos += 8 + (size_t)rd32(s + pos + 4); continue;
+            if (pos >= n) { need_more = !S.eof; break; }
+            if (fl.n() && pos - batch_start >= S.batch) break;
+            if (n - pos < 4) { if (S.eof) return E.data_error; need_more = true; break; }
+            const uint32_t magic = zf_rd32(s + pos);
+            if ((magic & 0xFFFFFFF0u) == ZMT_CONTAINER_MAGIC) {    // skippable frame: magic, LE32 size, payload
+                if (n - pos < 8 || n - pos - 8 < zf_rd32(s + pos + 4)) { if (S.eof) return E.data_error; need_more = true; break; }
+                pos += 8 + (size_t)zf_rd32(s + pos + 4); continue;
             }
-            if (!is_zstd) {
-                if (magic != LZ4F_MAGIC) return E.data_error;
-                if (n - pos < 7) { if (eof) return E.data_error; need_more = true; break; }
+            if (!S.is_zstd) {
+                if (magic != ZMT_LZ4F_MAGIC) return E.data_error;
+                if (n - pos < 7) { if (S.eof) return E.data_error; need_more = true; break; }
                 const uint32_t flg = s[pos + 4], bd = s[pos + 5], id = (bd >> 4) & 7;
-                if ((flg >> 6) != 1 || id < 4) { c->lib_errcode = ZMT_ST_BAD_HEADER; return E.library; }
+                if ((flg >> 6) != 1 || id < 4) return frame_error(c, ZMT_ST_BAD_HEADER);
                 {
                     // a frame whose blocks reach a batch of input or four of output before its end: decoded in segments,
                     // after the frames in front of it
                     Lz4fWalk w; w.pos = lz4f_header_len(flg); w.bound = 0; w.nblk = 0; w.done = 0;
-                    if (lz4f_walk_blocks(s + pos, n - pos, flg, bd, &w, kPlainBatch, 4 * (uint64_t)kPlainBatch) && !w.done) {
-                        if (!foff.empty()) break;
-                        const size_t e = decode_lz4_segments(c, rw, in, pos, eof, kPlainBatch, piece, st, d_in, d_out, d_tab, d_work, d_seg, d_hist, out);
+                    if (lz4f_walk_blocks(s + pos, n - pos, flg, bd, &w, S.batch, 4 * (uint64_t)S.batch) && !w.done) {
+                        if (fl.n()) break;
+                        const size_t e = S.lz4_segments();
                         if (e) return e;
                         segmented = true; break;
                     }
                 }
                 size_t len = 0; uint64_t bound = 0;
                 if (!lz4f_walk(s + pos, n - pos, &len, &bound) || len > n - pos) {
-                    if (eof) { c->lib_errcode = ZMT_ST_TRUNCATED; return E.frame_decompress; }
+                    if (S.eof) return frame_error(c, ZMT_ST_TRUNCATED);
                     need_more = true; break;
                 }
                 uint64_t osz = bound;
-                if (flg & 8) { osz = rd64(s + pos + 6); if (osz > bound) { c->lib_errcode = ZMT_ST_CONTENT_SIZE; return E.library; } }    // untrusted field, bounded by the block walk
-                foff.push_back(pos); fcs.push_back((uint32_t)len); ooff.push_back(ooff.back() + osz);
-                nslots += lz4_frame_slots(osz);
+                if (flg & 8) { osz = zf_rd64(s + pos + 6); if (osz > bound) return frame_error(c, ZMT_ST_CONTENT_SIZE); }    // untrusted field, bounded by the block walk
+                fl.push(pos, (uint32_t)len, osz);
                 pos += len;
             } else {
-                if (magic < 0xFD2FB522u || magic > 0xFD2FB528u) return E.data_error;
-                uint64_t cs = 0; uint32_t fl = 0; size_t used = 0;
-                const uint32_t nblk0 = nblk; const uint64_t scr0 = scratch;
-                int zr;
-                for (;;) {
-                    nblk = nblk0; scratch = scr0;
-                    zr = zmt_zstd_scan_frame_host2(s + pos, n - pos, 12 + pos, (uint32_t)foff.size(), blocks.data(), &nblk, (uint32_t)(blocks.size() / dsz), &scratch, &cs, &fl, &used);
-                    if (zr != ZMT_ST_DST_SMALL) break;
-                    blocks.resize(blocks.size() * 2 + 4096 * dsz);            // block table full: grow and rescan this frame
+                if (magic < 0xFD2FB522u || magic > ZMT_ZSTD_MAGIC) return E.data_error;
+                ZWalk w;
+                int zr = zstd_blocks(fl, s + pos, n - pos, 12 + pos, S.blocks.data(), (uint32_t)S.blocks.size(), true, w);
+                if (zr == ZMT_ST_DST_SMALL) {                     // block table full: grow it and walk once more
+                    S.blocks.resize(w.nblk > 2 * S.blocks.size() + 4096 ? w.nblk : 2 * S.blocks.size() + 4096);
+                    zr = zstd_blocks(fl, s + pos, n - pos, 12 + pos, S.blocks.data(), (uint32_t)S.blocks.size(), false, w);
                 }
-                if (zr == ZMT_ST_TRUNCATED && !eof) { nblk = nblk0; scratch = scr0; need_more = true; break; }
-                if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; return status_error(E, zr); }
-                foff.push_back(pos); expect.push_back((fl & 4u) ? ~0ull : cs); fflags.push_back(fl); first_blk.push_back(nblk); ooff.push_back(ooff.back() + cs);
-                pos += used;
+                if (zr == ZMT_ST_TRUNCATED && !S.eof) { need_more = true; break; }
+                if (zr != ZMT_ST_OK) return frame_error(c, zr);
+                fl.push(pos, w.flags, w.room, zstd_expect(w), w.nblk, w.scratch);
+                pos += w.end;
             }
         }
-        const uint32_t nf = (uint32_t)foff.size();
-        if (nf == 0) {
-            if (segmented) continue;                                          // a segmented frame was decoded and consumed
+        if (segmented) continue;                                              // a segmented frame was decoded and consumed
+        if (fl.n() == 0) {
             if (!need_more) break;                                            // EOF, everything consumed
         } else {
-            // ---- decode this batch
-            const uint64_t total = ooff.back();
-            const size_t in_bytes = pos + 12;                                   // frames address the buffer from its 12-byte pad
-            const size_t tab_bytes = tables_bytes(nf);
-            h_tab.resize(tab_bytes);
-            Tables T = tables_at(h_tab.data(), nf);
-            for (uint32_t i = 0; i < nf; i++) {
-                T.frame_off[i] = foff[i]; T.out_off[i] = ooff[i];
-                T.per_frame[i] = is_zstd ? fflags[i] : fcs[i];
-                if (is_zstd) { T.expect[i] = expect[i]; T.first_blk[i] = first_blk[i]; }
+            // ---- decode this batch (only its bytes travel) and write it frame by frame
+            const size_t e = S.decode(in.data() + 12 + batch_start, 12 + batch_start, 12 + pos, nullptr);
+            if (e) return e;
+            const Tables T = tables_at(S.h_tab.data(), fl.n());
+            for (uint32_t i = 0; i < fl.n(); i++) {
+                if (T.status[i] != ZMT_ST_OK) return frame_error(c, T.status[i]);
+                const size_t we = S.write(S.out.data() + T.out_off[i], T.out_size[i]);
+                if (we) return we;
             }
-            T.out_off[nf] = total; if (is_zstd) T.first_blk[nf] = nblk;
-            const size_t wk = is_zstd ? zmt_zstdd_workspace_bytes(nf, nblk, scratch) : zmt_lz4d_workspace_bytes(nf, (uint32_t)nslots, in_bytes);
-            if (!d_in.need(in_bytes + 256) || !d_out.need(total + 256) || !d_tab.need(tab_bytes) || !d_work.need(wk) || (is_zstd && !d_blk.need((size_t)nblk * dsz + 16))) return E.mem;
-            Tables Td = tables_at((uint8_t*)d_tab.p, nf);
-            // only the bytes of this batch travel (the device addresses them at their buffer offsets)
-            const size_t lo = 12 + batch_start, hi = in_bytes;
-            cudaMemcpyAsync((uint8_t*)d_in.p + lo, in.data() + lo, hi - lo, cudaMemcpyHostToDevice, st);
-            cudaMemcpyAsync(d_tab.p, h_tab.data(), tab_bytes, cudaMemcpyHostToDevice, st);
-            if (is_zstd && nblk) cudaMemcpyAsync(d_blk.p, blocks.data(), (size_t)nblk * dsz, cudaMemcpyHostToDevice, st);
-            const int rc = decode_batch(is_zstd, d_in.p, in_bytes, d_blk.p, nblk, Td, nf, (uint32_t)nslots, d_out.p, d_work.p, st);
-            out.resize(total ? total : 1);
-            std::vector<uint32_t> status(nf); std::vector<uint64_t> osz(nf);
-            cudaError_t ce = cudaSuccess;
-            if (rc == ZMT_ST_OK) {
-                if (total) ce = cudaMemcpyAsync(out.data(), d_out.p, total, cudaMemcpyDeviceToHost, st);
-                if (ce == cudaSuccess) ce = cudaMemcpyAsync(status.data(), Td.status, (size_t)nf * 4, cudaMemcpyDeviceToHost, st);
-                if (ce == cudaSuccess) ce = cudaMemcpyAsync(osz.data(), Td.out_size, (size_t)nf * 8, cudaMemcpyDeviceToHost, st);
-                if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-            }
-            if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); c->lib_errcode = ZMT_ST_CUDA; return E.library; }
-            for (uint32_t i = 0; i < nf; i++) {
-                if (status[i] != ZMT_ST_OK) { c->lib_errcode = status[i]; return status_error(E, status[i]); }
-                // frame by frame, in pieces of at most `piece` bytes (st_decompress writes as it goes)
-                uint64_t o = 0;
-                while (o < osz[i]) {
-                    GenBuffer b; b.buf = out.data() + ooff[i] + o; b.size = (size_t)((osz[i] - o) < piece ? (osz[i] - o) : piece); b.allocated = b.size;
-                    const size_t want = b.size;
-                    const int rv = rw->fn_write(rw->arg_write, &b);
-                    if (rv != 0) return mt_error(E, rv);
-                    c->outsize += b.size; o += want;
-                }
-            }
-            // drop what has been decoded
-            in.erase(in.begin() + 12, in.begin() + 12 + (long)pos);
+            in.erase(in.begin() + 12, in.begin() + 12 + (long)pos);         // drop what has been decoded
             pos = 0;
         }
         if (need_more) {
             // ---- read ahead: at least one more piece, up to a batch beyond the parse position
-            size_t goal = in.size() + piece;
-            if (goal < 12 + pos + kPlainBatch) goal = 12 + pos + kPlainBatch;
+            size_t goal = in.size() + S.piece;
+            if (goal < 12 + pos + S.batch) goal = 12 + pos + S.batch;
             // one zstd frame larger than a batch: read ahead geometrically (an LZ4 frame that large is decoded in segments)
-            if (is_zstd && in.size() - 12 - pos >= kPlainBatch) goal = in.size() + (in.size() - 12 - pos) / 2;
-            while (!eof && in.size() < goal) { const size_t e = read_piece(c, rw, in, piece, eof); if (e) return e; }
-        } else if (eof && pos >= in.size() - 12) break;
+            if (S.is_zstd && in.size() - 12 - pos >= S.batch) goal = in.size() + (in.size() - 12 - pos) / 2;
+            const size_t e = S.read_to(goal);
+            if (e) return e;
+        } else if (S.eof && pos >= in.size() - 12) break;
     }
     return 0;
 }
@@ -853,8 +905,8 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     if (c->codec == CODEC_LZ4) {
         size_t e = read_some(E, rw, first, 4, &got); if (e) return e;
         if (got != 4) return E.data_error;
-        if (rd32(first) != MT_MAGIC_SKIPPABLE) {
-            if (rd32(first) != LZ4F_MAGIC) return E.data_error;
+        if (zf_rd32(first) != ZMT_CONTAINER_MAGIC) {
+            if (zf_rd32(first) != ZMT_LZ4F_MAGIC) return E.data_error;
             return decompress_single_stream(c, rw, first, 4);          // plain .lz4 stream (st_decompress, lz4-mt_decompress.c:512-520)
         }
         e = read_some(E, rw, first + 4, 8, &got); if (e) return e;
@@ -863,8 +915,8 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     } else {
         size_t e = read_some(E, rw, first, 16, &got); if (e) return e;
         have = got;
-        auto is_zstd = [](const uint8_t* p) { uint32_t m = rd32(p); return m >= 0xFD2FB522u && m <= 0xFD2FB528u; };
-        auto is_skip = [](const uint8_t* p) { return rd32(p) == MT_MAGIC_SKIPPABLE && rd32(p + 4) == 4; };
+        auto is_zstd = [](const uint8_t* p) { uint32_t m = zf_rd32(p); return m >= 0xFD2FB522u && m <= ZMT_ZSTD_MAGIC; };
+        auto is_skip = [](const uint8_t* p) { return zf_rd32(p) == ZMT_CONTAINER_MAGIC && zf_rd32(p + 4) == 4; };
         if (have < 16) {
             if (have < 4 || !is_zstd(first)) return E.data_error;
             if (have == 9) return 0;                                   // empty file (zstd-mt_decompress.c:735-740)
@@ -872,7 +924,7 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
         }
         c->insize += 16;
         if (is_skip(first) && is_zstd(first + 12)) { hdr_pending = true; first_payload_have = 4; }          // pzstd style
-        else if (is_zstd(first) && rd32(first + 9) == MT_MAGIC_SKIPPABLE) {                                    // zstdmt style: 9-byte empty frame + 12-byte header
+        else if (is_zstd(first) && zf_rd32(first + 9) == ZMT_CONTAINER_MAGIC) {                                    // zstdmt style: 9-byte empty frame + 12-byte header
             // (only the magic can be tested here, as IsZstd_Skippable does, zstd-mt_decompress.c:156-159: 7 of the header's 12
             //  bytes are in hand; the size field is checked with the assembled header.  Round 1 read its 4 bytes past the buffer.)
             uint8_t tmp[12]; memcpy(tmp, first + 9, 7);
@@ -885,7 +937,7 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
 
     if (P.slots.empty()) {
         c->devs = env_devices();
-        if (c->devs.empty()) { c->lib_errcode = ZMT_ST_CUDA; return E.library; }
+        if (c->devs.empty()) return frame_error(c, ZMT_ST_CUDA);
         const size_t base_slots = c->threads >= 4 ? 4 : c->threads >= 3 ? 3 : 2;       // see compress_run
         P.slots.resize(base_slots > c->devs.size() ? base_slots : c->devs.size());
         for (size_t i = 0; i < P.slots.size(); i++)
@@ -907,10 +959,10 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     po.fill = [&](Slot& slot) -> bool {
         if (eof) return false;
         Slot* s = &slot;
-        Tables T = tables_at(s->h_tab, s->tab_cap);
-        uint32_t n = 0; size_t in_used = 0; uint64_t out_used = 0; size_t stat_in = 0;
+        FrameList& fl = s->frames;           // the slot is reallocated in place by grow(), only while the list is empty
+        fl.clear();
+        size_t in_used = 0, stat_in = 0;
         bool failed = false;
-        uint32_t nblk = 0; uint64_t scr = 0;                 // zstd: block descriptors + scratch demand of this batch
         // (re)allocate the still empty slot so that one frame of these dimensions fits; takes P.mu for the swap because the
         // writer's wait predicate reads s->state
         auto grow = [&](size_t need_in, uint64_t need_out, uint64_t need_scr, uint32_t need_blk) -> bool {
@@ -927,42 +979,41 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
             s->scr_cap = nscr;
             return true;
         };
+        // the zstd payload p[0..len) at `at` in the slot's input, as the next frame: the block-table rule, and the payload
+        // must hold the frame and nothing else
+        auto zstd_payload = [&](const uint8_t* p, size_t len, uint64_t at, bool count, ZWalk& w) -> int {
+            const int zr = zstd_blocks(fl, p, len, at + 12, s->h_blk, s->blk_cap, count, w);
+            return zr == ZMT_ST_OK && w.end != len ? ZMT_ST_TRAILING : zr;
+        };
         // Put one whole frame (12-byte header + payload, held in `fr`) at the start of the empty slot, growing the slot
-        // (input, output, zstd block table and entropy scratch) until it fits.  Returns false after P.fail().
+        // (input, output, zstd block table and entropy scratch) so that it fits.  Returns false after P.fail().
         auto place_first = [&](const std::vector<uint8_t>& fr) -> bool {
-            const size_t toRead = fr.size() - 12;
+            const size_t len = fr.size() - 12;
             if (!grow(fr.size(), 0, 0, 0)) { P.fail(E.mem); return false; }
-            uint64_t osz = 0; uint32_t nsq = 0;
+            uint64_t room = 0; ZWalk w;
             if (!is_zstd) {
-                if (!lz4f_out_size(fr.data() + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); return false; }
-                if (!grow(fr.size(), osz, 0, 0)) { P.fail(E.mem); return false; }
-                memcpy(s->h_in, fr.data(), fr.size());
+                if (!lz4f_out_size(fr.data() + 12, len, &room)) { P.fail(frame_error(c, ZMT_ST_BAD_HEADER)); return false; }
+                if (!grow(fr.size(), room, 0, 0)) { P.fail(E.mem); return false; }
             } else {
-                for (int tries = 0;; tries++) {
-                    memcpy(s->h_in, fr.data(), fr.size());
-                    uint64_t cs = 0; nblk = 0; scr = 0;
-                    const int zr = zmt_zstd_scan_frame_host(s->h_in + 12, toRead, 12, 0, s->h_blk, &nblk, s->blk_cap, &scr, &cs, &nsq);
-                    if (zr == ZMT_ST_DST_SMALL && tries < 2) {          // more blocks than descriptors: every block costs >= 3 bytes
-                        if (!grow(fr.size(), 0, 0, (uint32_t)(toRead / 3 + 16))) { P.fail(E.mem); return false; }
-                        continue;
-                    }
-                    if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(status_error(E, zr)); return false; }
-                    osz = cs;
-                    if (osz <= s->out_cap && scr <= s->scr_cap) break;
-                    if (tries >= 2 || !grow(fr.size(), osz, scr, 0)) { P.fail(E.mem); return false; }
+                int zr = zstd_payload(fr.data() + 12, len, 0, true, w);
+                if (zr == ZMT_ST_DST_SMALL || (zr == ZMT_ST_OK && (w.room > s->out_cap || w.scratch > s->scr_cap))) {
+                    // more blocks than descriptors (every block costs >= 3 bytes), output or scratch: grow, walk once more
+                    if (!grow(fr.size(), w.room, w.scratch, zr == ZMT_ST_DST_SMALL ? (uint32_t)(len / 3 + 16) : 0)) { P.fail(E.mem); return false; }
+                    zr = zstd_payload(fr.data() + 12, len, 0, false, w);
                 }
+                if (zr != ZMT_ST_OK) { P.fail(frame_error(c, zr)); return false; }
+                room = w.room;
             }
-            T = tables_at(s->h_tab, s->tab_cap);
-            T.frame_off[0] = 0; T.per_frame[0] = (uint32_t)toRead; T.out_off[0] = 0;
-            if (is_zstd) { T.first_blk[0] = 0; T.expect[0] = (nsq & 4u) ? ~0ull : osz; T.per_frame[0] = nsq; }      // flag 4: no content size in the header, osz is a bound
-            in_used = fr.size(); out_used = osz; n = 1;
+            memcpy(s->h_in, fr.data(), fr.size());
+            fl.push(0, is_zstd ? w.flags : (uint32_t)len, room, zstd_expect(w), w.nblk, w.scratch);
+            in_used = fr.size();
             return true;
         };
         if (!carry.empty()) {
             if (!place_first(carry)) return false;
             carry.clear();
         }
-        while (n < s->tab_cap) {
+        while (fl.n() < s->tab_cap) {
             uint8_t hdr[12]; size_t pre = 0;
             if (hdr_pending) { memcpy(hdr, first, 12); hdr_pending = false; pre = first_payload_have; }
             else {
@@ -970,12 +1021,12 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
                 if (e) { P.fail(e); failed = true; break; }
                 if (g == 0) { eof = true; break; }
                 if (g != 12) { P.fail(E.read_fail); failed = true; break; }
-                if (rd32(hdr) != MT_MAGIC_SKIPPABLE) { P.fail(E.data_error); failed = true; break; }
+                if (zf_rd32(hdr) != ZMT_CONTAINER_MAGIC) { P.fail(E.data_error); failed = true; break; }
                 if (c->codec == CODEC_ZSTD) stat_in += 12;
             }
-            if (rd32(hdr + 4) != 4) { P.fail(E.data_error); failed = true; break; }
+            if (zf_rd32(hdr + 4) != 4) { P.fail(E.data_error); failed = true; break; }
             if (c->codec == CODEC_LZ4) stat_in += 12;
-            const size_t toRead = rd32(hdr + 8);
+            const size_t toRead = zf_rd32(hdr + 8);
             if (toRead < pre) { P.fail(E.data_error); failed = true; break; }
             // where to put it: the current slot if it fits behind the frames already there, else a temporary buffer
             // (first frame of a batch that needs a bigger slot, or a frame that moves to the next batch)
@@ -989,68 +1040,56 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
             if (g != toRead - pre) { P.fail(E.data_error); failed = true; break; }
             stat_in += g;
             if (to_tmp) {
-                if (n > 0) break;                                   // next batch starts with it
+                if (fl.n() > 0) break;                              // next batch starts with it
                 if (!place_first(carry)) { failed = true; break; }
                 carry.clear();
                 continue;
             }
-            uint64_t osz = 0; uint32_t nsq = 0;
-            uint32_t nblk_new = nblk; uint64_t scr_new = scr;
+            uint64_t room = 0; ZWalk w;
             bool moves = false;                                     // does not fit behind the others: first frame of the next batch
             if (!is_zstd) {
-                if (!lz4f_out_size(dstp + 12, toRead, &osz)) { c->lib_errcode = ZMT_ST_BAD_HEADER; P.fail(E.library); failed = true; break; }
+                if (!lz4f_out_size(dstp + 12, toRead, &room)) { P.fail(frame_error(c, ZMT_ST_BAD_HEADER)); failed = true; break; }
             } else {
                 // block table of this frame (descriptors are appended; dropped again if the frame moves to the next batch)
-                uint64_t cs = 0;
                 const double ts0 = trace_now();
-                const int zr = zmt_zstd_scan_frame_host(dstp + 12, toRead, in_used + 12, n, s->h_blk, &nblk_new, s->blk_cap, &scr_new, &cs, &nsq);
+                const int zr = zstd_payload(dstp + 12, toRead, in_used, false, w);
                 rd_scan += trace_now() - ts0;
                 if (zr == ZMT_ST_DST_SMALL) moves = true;
-                else if (zr != ZMT_ST_OK) { c->lib_errcode = (size_t)zr; P.fail(status_error(E, zr)); failed = true; break; }
-                else if (scr_new > s->scr_cap) moves = true;
-                osz = cs;
+                else if (zr != ZMT_ST_OK) { P.fail(frame_error(c, zr)); failed = true; break; }
+                else if (w.scratch > s->scr_cap) moves = true;
+                room = w.room;
             }
-            if (!moves && osz > s->out_cap - out_used) moves = true;
+            if (!moves && room > s->out_cap - fl.out_end()) moves = true;
             if (moves) {
                 carry.assign(dstp, dstp + 12 + toRead);
-                if (n > 0) break;
+                if (fl.n() > 0) break;
                 if (!place_first(carry)) { failed = true; break; }  // a single frame larger than the slot: grow the slot
                 carry.clear();
                 continue;
             }
-            T.frame_off[n] = in_used; T.per_frame[n] = (uint32_t)toRead; T.out_off[n] = out_used;
-            if (is_zstd) { T.first_blk[n] = nblk; T.expect[n] = (nsq & 4u) ? ~0ull : osz; T.per_frame[n] = nsq; nblk = nblk_new; scr = scr_new; }
-            in_used += 12 + toRead; out_used += osz; n++;
+            fl.push(in_used, is_zstd ? w.flags : (uint32_t)toRead, room, zstd_expect(w), w.nblk, w.scratch);
+            in_used += 12 + toRead;
         }
-        if (failed || n == 0) return false;
-        T.out_off[n] = out_used;
-        if (is_zstd) { T.first_blk[n] = nblk; s->nblk = nblk; s->scratch_used = scr; }
-        s->n = n; s->in_used = in_used; s->out_used = (size_t)out_used;
-        { uint64_t ns = 0; for (uint32_t i = 0; i < n; i++) ns += lz4_frame_slots(T.out_off[i + 1] - T.out_off[i]); s->nslots = (uint32_t)ns; }
-        c->insize += stat_in; c->frames += n;
+        if (failed || fl.n() == 0) return false;
+        s->in_used = in_used;
+        c->insize += stat_in; c->frames += fl.n();
         return true;
     };
     po.submit = [&](Slot& s) -> int {
-        Tables Th = tables_at(s.h_tab, s.tab_cap), Td = tables_at(s.d_tab, s.tab_cap);
-        if (cudaMemcpyAsync(s.d_in, s.h_in, s.in_used, cudaMemcpyHostToDevice, s.stream) != cudaSuccess ||
-            cudaMemcpyAsync(s.d_tab, s.h_tab, s.tab_bytes, cudaMemcpyHostToDevice, s.stream) != cudaSuccess ||
-            (is_zstd && s.nblk && cudaMemcpyAsync(s.d_blk, s.h_blk, (size_t)s.nblk * zmt_zstd_blk_desc_bytes(), cudaMemcpyHostToDevice, s.stream) != cudaSuccess))
-            return ZMT_ST_CUDA;
-        const int st = decode_batch(is_zstd, s.d_in, s.in_used, s.d_blk, s.nblk, Td, s.n, s.nslots, s.d_out, s.d_work, s.stream);
+        if (cudaMemcpyAsync(s.d_in, s.h_in, s.in_used, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) return ZMT_ST_CUDA;
+        const int st = decode_step(is_zstd, s.frames, s.h_tab, s.d_tab, s.tab_cap, s.h_blk, s.d_blk, s.d_in, s.in_used, s.d_out, s.d_work, nullptr, s.stream);
         if (st != ZMT_ST_OK) return st;
-        if (cudaMemcpyAsync(Th.out_size, Td.out_size, (size_t)s.n * 8, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
-            cudaMemcpyAsync(Th.status, Td.status, (size_t)s.n * 4, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess ||
-            cudaEventRecord(s.ev, s.stream) != cudaSuccess) return ZMT_ST_CUDA;
-        return ZMT_ST_OK;
+        return cudaEventRecord(s.ev, s.stream) == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
     };
     // pt_write, lz4-mt_decompress.c:165-187
     po.drain = [&](Slot& s) -> bool {
-        Tables T = tables_at(s.h_tab, s.tab_cap);
+        const Tables T = tables_at(s.h_tab, s.tab_cap);
+        const uint32_t n = s.frames.n();
         uint32_t issued = 0, ready = 0; int np_issued = 0, np_ready = 0;       // frames [0, issued) requested, [0, ready) landed
         auto issue_piece = [&]() -> bool {
-            if (issued >= s.n) return true;
+            if (issued >= n) return true;
             uint32_t j = issued; uint64_t lo = T.out_off[j], hi = lo;
-            while (j < s.n && hi - lo < kPieceBytes) { hi = T.out_off[j] + T.out_size[j]; j++; }
+            while (j < n && hi - lo < kPieceBytes) { hi = T.out_off[j] + T.out_size[j]; j++; }
             if (hi > s.out_cap) hi = s.out_cap;
             if (hi > lo && cudaMemcpyAsync(s.h_out + lo, s.d_out + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return false;
             if (cudaEventRecord(s.evp[np_issued & 1], s.stream) != cudaSuccess) return false;
@@ -1058,15 +1097,15 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
             return true;
         };
         uint32_t piece_end[2] = { 0, 0 };
-        for (uint32_t i = 0; i < s.n; i++) {
+        for (uint32_t i = 0; i < n; i++) {
             const uint32_t st = T.status[i];
-            if (st != ZMT_ST_OK) { c->lib_errcode = st; P.fail(status_error(E, st)); return false; }
+            if (st != ZMT_ST_OK) { P.fail(frame_error(c, st)); return false; }
             if (i >= ready) {
                 bool okp = true;
                 if (np_issued == np_ready) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }
-                if (okp && issued < s.n && np_issued == np_ready + 1) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }   // one ahead
+                if (okp && issued < n && np_issued == np_ready + 1) { okp = issue_piece(); piece_end[(np_issued - 1) & 1] = issued; }   // one ahead
                 if (okp) okp = cudaEventSynchronize(s.evp[np_ready & 1]) == cudaSuccess;
-                if (!okp) { c->lib_errcode = ZMT_ST_CUDA; P.fail(E.library); return false; }
+                if (!okp) { P.fail(frame_error(c, ZMT_ST_CUDA)); return false; }
                 ready = piece_end[np_ready & 1]; np_ready++;
             }
             GenBuffer b; b.buf = s.h_out + T.out_off[i]; b.size = (size_t)T.out_size[i]; b.allocated = b.size;

@@ -5,12 +5,6 @@
 #include <stdint.h>
 #include <mutex>
 
-// zmt_zstd_scan_frame_host for frames whose length is not known in advance (plain .zst streams): *consumed receives the
-// frame's length, and bytes behind the frame are not an error.  Internal to the library, not exported.
-__attribute__((visibility("hidden")))
-int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out, uint32_t* nblocks_io,
-                              uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed);
-
 // SM count of the current device, cached per device (contexts may run on several host threads)
 static inline int zmt_sm_count()
 {

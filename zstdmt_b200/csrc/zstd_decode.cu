@@ -1313,19 +1313,10 @@ extern "C" int zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t
                                         void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
                                         uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq)
 {
-    return zmt_zstd_scan_frame_host2(frame, n, base_off, frame_idx, blocks_out, nblocks_io, max_blocks, scratch_used, content_size, needs_seq, nullptr);
-}
-
-// same, for frames whose length is not known in advance (plain .zst streams): *consumed receives the frame length
-int zmt_zstd_scan_frame_host2(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
-                              void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
-                              uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, size_t* consumed)
-{
     size_t end = 0;
     const int r = zstd_frame_walk<true>(frame, n, base_off, frame_idx, (ZBlk*)blocks_out, nblocks_io, max_blocks, scratch_used, content_size,
                                         needs_seq, &end);
     if (r != ZMT_ST_OK) return r;
-    if (consumed) { *consumed = end; return ZMT_ST_OK; }
     return end == n ? ZMT_ST_OK : ZMT_ST_TRAILING;
 }
 
