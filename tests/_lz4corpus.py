@@ -24,7 +24,8 @@ import pytest
 import _oracle as o
 import _zcorpus as zc
 
-# lz4_decode.cuh
+# lz4_decode.cuh, and match_exec.cuh for what pass B shares with the zstd execute pass (MX_STEP, MX_OWN, MX_SPAN); the
+# model's own numbers: test_lz4_decode_corpus.py compares them with the source
 LZD_WIN = 512           # compressed bytes pass A stages per step
 LZD_NJ = 256            # token positions pass A's jump table covers per step; a step ends at the first token beyond
 LZD_SEQS = 32           # sequences per pass-A step, match records per pass-B step (one per lane)

@@ -1,4 +1,4 @@
-"""Models of two zstd decoder kernels (zstdmt_b200/csrc/zstd_decode.cu), so that the edges of their GPU schedules can be
+"""Models of two zstd decoder kernels (zstdmt_b200/csrc/zstd_decode.cu; the execute pass shares match_exec.cuh), so that the edges of their GPU schedules can be
 named on the oracle's block trace (orc_zstd_trace) and on the frame's bytes.
 
 exec_steps(trace, b) restates zx_block, the execute pass ("kernel 3"), on one compressed block: how its sequences are cut
@@ -31,28 +31,34 @@ CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
 
 
 def kernel_constants():
-    """The same constants as zstd_decode.cu states them (a regex per constant; a missing match is an error)."""
-    s = open(os.path.join(CSRC, "zstd_decode.cu")).read()
+    """The same constants as the source states them.  Each use site is found by a regex (a missing match is an error)
+    and must name its constant; the value is the constant's #define in match_exec.cuh (what the execute pass shares
+    with the LZ4 decoder) or zstd_decode.cu."""
+    from _searchcorpus import kernel_constant
+    files = ("match_exec.cuh", "zstd_decode.cu")
+    src = {f: open(os.path.join(CSRC, f)).read() for f in files}
 
-    def one(pat):
-        m = re.findall(pat, s)
-        assert m, "pattern not found in zstd_decode.cu: " + pat
-        assert len(set(m)) == 1, (pat, m)
-        v = m[0]
-        return tuple(int(x) for x in v) if isinstance(v, tuple) else int(v)
-    cap = one(r"uint32_t cnt = B\.nseq - base < (\d+) \? B\.nseq - base : (\d+);")
+    def one(f, pat):
+        m = re.findall(pat, src[f])
+        assert m, "pattern not found in %s: %s" % (f, pat)
+        m = {tuple(int(x) if x.isdigit() else kernel_constant(x, files) for x in (v if isinstance(v, tuple) else (v,))) for v in m}
+        assert len(m) == 1, (pat, m)
+        v = m.pop()
+        return v if len(v) > 1 else v[0]
+    z, x = "zstd_decode.cu", "match_exec.cuh"
+    cap = one(z, r"uint32_t cnt = B\.nseq - base < (\w+) \? B\.nseq - base : (\w+);")
     assert cap[0] == cap[1], cap
     return {
-        "ZX_SPAN": one(r"#define\s+ZX_SPAN\s+(\d+)u?\b"),
+        "ZX_SPAN": one(z, r"lane < cnt && it <= (\w+)\)"),
         "STEP_CAP": cap[0],
-        "LANE_LIT": one(r"if \(lane < lim && ll <= (\d+)\)"),
-        "LANE_LIT_WARP": one(r"__ballot_sync\(0xFFFFFFFFu, lane < lim && ll > (\d+)\)"),
-        "OWN_ML": one(r"if \(indep && ml <= (\d+)\)"),
-        "OWN_ML_BALLOT": one(r"act && !\(indep && ml <= (\d+)\)"),
-        "CHUNK": one(r"else if \(qoff >= (\d+)\)"),
-        "REFILL_AT": one(r"if \(ofc \+ \(mx >> 24\) \+ \(lx >> 24\) > (\d+)\) R\.refill\(\);"),
-        "OFC_MAX": one(r"if \(ofc > (\d+)\) return;"),
-        "INACTIVE": int(re.search(r"e_end = act \? \(int32_t\)\(my_mp \+ ml\) : (0x[0-9A-Fa-f]+)", s).group(1), 16),
+        "LANE_LIT": one(z, r"if \(lane < lim && ll <= (\w+)\)"),
+        "LANE_LIT_WARP": one(z, r"__ballot_sync\(0xFFFFFFFFu, lane < lim && ll > (\w+)\)"),
+        "OWN_ML": one(z, r"if \(indep && ml <= (\w+)\)"),
+        "OWN_ML_BALLOT": one(z, r"act && !\(indep && ml <= (\w+)\)"),
+        "CHUNK": one(x, r"else if \(off >= (\w+)\)"),
+        "REFILL_AT": one(z, r"if \(ofc \+ \(mx >> 24\) \+ \(lx >> 24\) > (\d+)\) R\.refill\(\);"),
+        "OFC_MAX": one(z, r"if \(ofc > (\d+)\) return;"),
+        "INACTIVE": one(x, r"e_end = act \? \(int32_t\)\(dst \+ ml\) : (\w+),"),
     }
 
 

@@ -13,7 +13,7 @@ from test_zstd_decode_corpus import ZF_NEEDS_SEQ, expected_flags, host_scan
 pytestmark = pytest.mark.gpu
 CASES = list(zc.CASES)
 ZMT_ST_CONTENT_CHECKSUM = 7
-TICKET_WIN = 16384                                   # ZX_WIN / LZX_WIN: frames per ticket window of the execute passes
+TICKET_WIN = 16384                                   # MX_TICKET_WIN (match_exec.cuh): frames per ticket window of the execute passes
 
 
 @pytest.fixture(scope="module")

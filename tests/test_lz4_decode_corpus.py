@@ -6,6 +6,8 @@ import pytest
 
 import _lz4corpus as lc
 import _oracle as o
+import _zxmodel as zx
+from _searchcorpus import kernel_constant
 
 CASES = list(lc.CASES)
 S, B = o.L4S, o.L4B
@@ -279,6 +281,38 @@ def test_own_lane_sources_never_straddle_d0():
             for _, _, recs, steps in _steps_b(name, lay):
                 for kind, d0, _, rs in steps:
                     assert all(nl in (0, recs[j][1]) for j, _, own, nl in rs if own)
+
+
+def test_model_constants_match_the_kernel():
+    """The models' constants are the ones the source states: pass B's step cap, span and own-lane limit are
+    match_exec.cuh's (shared with the zstd execute pass), pass A's are lz4_decode.cuh's.  A change in either fails here
+    instead of the model quietly following the code."""
+    files = ("match_exec.cuh", "lz4_decode.cuh")
+    got = {n: kernel_constant(n, files) for n in ("MX_STEP", "MX_SPAN", "MX_OWN", "MX_INACTIVE", "LZD_WIN", "LZD_NJ", "LZD_LONGLIT")}
+    assert got == {"MX_STEP": lc.LZD_SEQS, "MX_SPAN": lc.LZX_SPAN, "MX_OWN": lc.LZD_LONG, "MX_INACTIVE": zx.INACTIVE,
+                   "LZD_WIN": lc.LZD_WIN, "LZD_NJ": lc.LZD_NJ, "LZD_LONGLIT": lc.LZD_LONGLIT}
+    assert (lc.LZD_SEQS, lc.LZX_SPAN, lc.LZD_LONG) == (zx.STEP_CAP, zx.ZX_SPAN, zx.OWN_ML)
+
+
+def test_dependency_search_agrees_with_the_overlap_on_every_step():
+    """steps_b states dependence as the pairwise overlap with the step's earlier destinations; the kernel finds it by a
+    lower-bound search over the lanes (mx_independent, restated as _zxmodel.kernel_dependent).  The two agree on every
+    record of every step of the corpus, with the inactive lanes the kernel pads with."""
+    n = 0
+    for name in CASES:
+        for lay in lc.LAYOUTS:
+            for _, _, recs, steps in _steps_b(name, lay):
+                for kind, _, _, rs in steps:
+                    if kind != "step":
+                        continue
+                    pad = [zx.INACTIVE] * (lc.LZD_SEQS - len(rs))
+                    d_beg = [recs[j][0] for j, *_ in rs] + pad
+                    e_end = [recs[j][0] + recs[j][1] for j, *_ in rs] + pad
+                    for lane, (j, dep, _, _) in enumerate(rs):
+                        d, ml, off = recs[j]
+                        assert zx.kernel_dependent(lane, d - off, ml, d_beg, e_end) == dep, (name, lay, j)
+                        n += 1
+    assert n
 
 
 def test_block_ending_with_a_match_is_rejected():

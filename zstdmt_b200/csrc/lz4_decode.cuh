@@ -21,16 +21,17 @@
 //                            match of the same step) in order by the whole warp.  A match that reaches into the
 //                            previous block of a linked-block frame (what liblz4 emits for the reference,
 //                            lz4-mt_compress.c:141-146) waits on that block's published progress counter; the
-//                            previous block always holds a lower ticket, so the wait cannot deadlock.
+//                            previous block always holds a lower ticket, so the wait cannot deadlock.  Ticket order,
+//                            dependency test and copies are shared with the zstd decoder (match_exec.cuh).
 //   lz4_decode_frames_seq_kernel   fallback, one warp per flagged frame, blocks in order: frames whose non-last
 //                            blocks do not regenerate exactly blockMaxSize bytes (LZ4F_compressUpdate + flush
 //                            streams), where the output position of a block is not known before decoding.
 #pragma once
+#include "match_exec.cuh"
 
 #define LZD_WARPS 8
 #define LZD_WIN   512u        // compressed bytes staged per step and warp (one 16-byte load per lane)
 #define LZD_NJ    256u        // token-start candidates examined per step
-#define LZD_LONG  32u         // matches longer than this are copied by the whole warp
 #define LZD_LONGLIT 16u       // literal runs longer than this are copied by the whole warp (pass A: few lanes hold long runs)
 #define LZD_ERR   0xFFFFFFFFu
 #define LZD_DONE  0xFFFFFFFFu // progress value of a finished block
@@ -396,71 +397,24 @@ lz4_parse_blocks_kernel(const uint8_t* __restrict__ in, const uint8_t* __restric
 }
 
 // ---------------------------------------------------------------- pass B: match execution
-// Ticket order.  Blocks of a linked-block frame form a dependency chain (the first matches of a block usually read the
-// tail of the previous one), so tickets must not put the blocks of one frame on neighbouring warps: within a window of
-// LZX_WIN frames the order is block-index-major — block 0 of every frame of the window, then block 1 of every frame, ... —
-// which keeps as many independent chains in flight as there are frames in the window, and by the time block b+1 of a
-// frame comes up its block b has long finished.  (f, b-1) still always holds a lower ticket than (f, b): no deadlock.
-// A window whose frames have very different block counts would mostly hand out empty tickets; it falls back to
-// frame-major order (flag in the top bit of its base).
-#define LZX_WIN 16384u
-#define LZX_SPAN 2048u        // bytes of output a step may span: staged in shared memory
-__global__ void __launch_bounds__(256)
-lz4_ticket_windows_kernel(const uint64_t* __restrict__ first_slot, uint32_t nframes, unsigned long long* __restrict__ wbase)
-{
-    __shared__ uint32_t red[256];
-    const uint32_t nwin = (nframes + LZX_WIN - 1) / LZX_WIN;
-    unsigned long long base = 0;
-    for (uint32_t w = 0; w < nwin; w++) {
-        const uint32_t f0 = w * LZX_WIN, f1 = f0 + LZX_WIN < nframes ? f0 + LZX_WIN : nframes;
-        uint32_t mx = 0;
-        for (uint32_t f = f0 + threadIdx.x; f < f1; f += 256) { const uint32_t c = (uint32_t)(first_slot[f + 1] - first_slot[f]); mx = c > mx ? c : mx; }
-        red[threadIdx.x] = mx;
-        __syncthreads();
-        for (uint32_t d = 128; d > 0; d >>= 1) { if (threadIdx.x < d && red[threadIdx.x + d] > red[threadIdx.x]) red[threadIdx.x] = red[threadIdx.x + d]; __syncthreads(); }
-        mx = red[0];
-        __syncthreads();
-        const unsigned long long real = first_slot[f1] - first_slot[f0], grid = (unsigned long long)(f1 - f0) * mx;
-        const bool frame_major = grid > 8 * real + 65536;
-        if (threadIdx.x == 0) wbase[w] = base | (frame_major ? (1ull << 63) : 0ull);
-        base += frame_major ? real : grid;
-    }
-    if (threadIdx.x == 0) wbase[nwin] = base;
-}
-
-// Every step's output window lives in shared memory as well (chains of matches that feed each other run at shared
-// memory latency).
+// Tickets, the dependency test and the copies are match_exec.cuh's.  Every step's output window lives in shared memory
+// as well as in global memory (MxWin).
 __global__ void __launch_bounds__(32 * LZD_WARPS)
 lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ frame_off,
                        const uint64_t* __restrict__ first_slot, const LzBlk* __restrict__ tab, const unsigned long long* __restrict__ rec,
                        uint32_t* __restrict__ prog, const uint32_t* __restrict__ status, const uint32_t* __restrict__ needs_seq,
                        unsigned long long* __restrict__ ticket, const unsigned long long* __restrict__ wbase, uint32_t nframes, uint32_t slot_cap)
 {
-    __shared__ __align__(16) uint8_t stage[LZD_WARPS][LZX_SPAN + 32];
+    __shared__ __align__(16) uint8_t stage[LZD_WARPS][MX_SPAN + 32];
     const uint32_t lane = threadIdx.x & 31;
     if (first_slot[nframes] > slot_cap) return;             // the scan reported the undersized table per frame
-    const uint32_t nwin = (nframes + LZX_WIN - 1) / LZX_WIN;
-    const unsigned long long ntickets = wbase[nwin] & ~(1ull << 63);
+    const MxTickets T = mx_tickets(wbase, nframes);
     volatile uint32_t* vprog = prog;
     for (;;) {
-        unsigned long long tk = 0;
-        if (lane == 0) tk = atomicAdd(ticket, 1ull);
-        tk = __shfl_sync(ZMT_FULL_MASK, tk, 0);
-        if (tk >= ntickets) break;
-        // ticket -> window (binary search over the window bases) -> (frame, block) -> slot
-        uint32_t lo = 0, hi = nwin;
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if ((wbase[mid] & ~(1ull << 63)) <= tk) lo = mid; else hi = mid; }
-        const unsigned long long wb = wbase[lo];
-        const unsigned long long tl = tk - (wb & ~(1ull << 63));
-        const uint32_t f0 = lo * LZX_WIN, wn = (f0 + LZX_WIN < nframes ? LZX_WIN : nframes - f0);
+        const unsigned long long tk = mx_take_ticket(ticket, lane);
+        if (tk >= T.count) break;
         uint64_t t;
-        if (wb >> 63) t = first_slot[f0] + tl;                          // frame-major window
-        else {
-            const uint32_t fb = (uint32_t)(tl / wn), ff = f0 + (uint32_t)(tl % wn);
-            const uint64_t s0 = first_slot[ff];
-            if (fb >= first_slot[ff + 1] - s0) continue;                // this frame has fewer blocks
-            t = s0 + fb;
-        }
+        if (!mx_ticket_unit(T, tk, first_slot, t)) continue;
         const LzBlk B = tab[t];
         if (B.csize == 0) continue;                         // empty slot: nobody waits on it
         const uint32_t f = B.frame;
@@ -474,16 +428,16 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
             const bool publish = !(B.flags & LZB_LAST) && (tab[t + 1].flags & LZB_LINKED);     // the next block may read this one
             bool prev_done = !linked;
             uint32_t since_pub = 0;
-            uint8_t* const S = stage[threadIdx.x >> 5];
+            MxWin W; W.dst = dst; W.S = stage[threadIdx.x >> 5];
             // The records of the NEXT step are loaded while this one executes (one L2 round trip less on the chain of a block).
             unsigned long long rnext = lane < B.nrec ? R[lane] : 0ull;
             for (uint32_t base = 0; base < B.nrec;) {
-                const uint32_t cnt = B.nrec - base < 32 ? B.nrec - base : 32;
+                const uint32_t cnt = B.nrec - base < MX_STEP ? B.nrec - base : MX_STEP;
                 uint32_t d = 0, ml = 0, off = 0;
                 { const unsigned long long r = lane < cnt ? rnext : 0ull; d = (uint32_t)r & 0xFFFFFFu; ml = (uint32_t)(r >> 24) & 0xFFFFFFu; off = (uint32_t)(r >> 48); }
                 const uint32_t d0 = __shfl_sync(ZMT_FULL_MASK, d, 0);
-                // ---- the step = the longest prefix of these records whose destinations fit the staging window [d0, d0 + LZX_SPAN)
-                const uint32_t nfit = __popc(__ballot_sync(ZMT_FULL_MASK, ml && d + ml - d0 <= LZX_SPAN));       // destinations are sorted: a prefix
+                // ---- the step = the longest prefix of these records whose destinations fit the staging window [d0, d0 + MX_SPAN)
+                const uint32_t nfit = __popc(__ballot_sync(ZMT_FULL_MASK, ml && d + ml - d0 <= MX_SPAN));       // destinations are sorted: a prefix
                 if (nfit == 0) {
                     // one match longer than the window: straight in global memory, by the whole warp
                     const uint32_t qml = __shfl_sync(ZMT_FULL_MASK, ml, 0), qoff = __shfl_sync(ZMT_FULL_MASK, off, 0);
@@ -497,11 +451,8 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                         if (pv == LZD_DONE) prev_done = true;
                     }
                     uint8_t* dp = dst + d0;
-                    const uint8_t* m = dp - qoff;
-                    if (qoff >= qml) warp_copy_lit(dp, m, qml, lane);
-                    else if (qoff >= 32) { for (uint32_t i = 0; i < qml; i += 32) { if (i + lane < qml) dp[i + lane] = m[i + lane]; __syncwarp(); } }
-                    else { for (uint32_t i = lane; i < qml; i += 32) dp[i] = m[i % qoff]; }
-                    __syncwarp();
+                    if (qoff >= qml) { warp_copy_lit(dp, dp - qoff, qml, lane); __syncwarp(); }     // disjoint and long: the 16-byte copier
+                    else mx_warp_match_global(dp, qml, qoff, lane);
                     base += 1;
                     rnext = base + lane < B.nrec ? R[base + lane] : 0ull;
                     continue;
@@ -524,70 +475,34 @@ lz4_exec_blocks_kernel(uint8_t* __restrict__ out, const uint64_t* __restrict__ o
                         if (pv == LZD_DONE) prev_done = true;
                     }
                 }
-                // Which matches must wait for an earlier match of this very step?  Only the destinations [d_j, e_j) of matches
-                // j < k matter (sorted, disjoint): a = first j whose destination ends above my source start (binary search over
-                // the lanes by shuffle); my source touches a destination of the step iff that j lies before me and starts below
-                // my source end.  A match that overlaps its own destination (offset < length) takes the ordered path too.
-                const int32_t e_end = ml ? (int32_t)(d + ml) : 0x7FFFFFFF, d_beg = ml ? (int32_t)d : 0x7FFFFFFF;
-                uint32_t a = 0;
-#pragma unroll
-                for (uint32_t stp = 16; stp > 0; stp >>= 1) {
-                    const int32_t v = __shfl_sync(ZMT_FULL_MASK, e_end, (a + stp - 1) & 31);
-                    if (v <= sp) a += stp;                                  // e_j <= sp: destination j lies entirely below my source
-                }
-                const int32_t da = __shfl_sync(ZMT_FULL_MASK, d_beg, a & 31);
-                const bool indep = ml && off >= ml && !(a < lane && da < sp + (int32_t)ml);
-                const bool own = indep && ml <= LZD_LONG;               // copied by its own lane
+                const bool own = mx_independent(lane, ml != 0, d, ml, off) && ml <= MX_OWN;      // copied by its own lane
                 // own lane: the part of the source below d0 comes from global memory — its first 8 bytes are requested NOW, before
                 // the window load below stalls on its own round trip (one latency per step instead of two)
-                const int32_t nlow = !own ? 0 : sp >= (int32_t)d0 ? 0 : ((int32_t)d0 - sp < (int32_t)ml ? (int32_t)d0 - sp : (int32_t)ml);
+                W.lo = (int32_t)d0;
+                const int32_t nlow = own ? mx_nlow(W, sp, ml) : 0;
                 const uint8_t* mp = dst + sp;
                 uint8_t x0[8];
 #pragma unroll
                 for (int j = 0; j < 8; j++) x0[j] = (j < nlow) ? mp[j] : (uint8_t)0;
                 // ---- stage the window: output bytes [d0, d0 + span) as they stand (the literals pass A placed; match bytes are
-                //      still undefined) with aligned 16-byte loads.  Every match of the step writes its bytes to global memory
-                //      AND to the window; a source byte at or above d0 is read from the window.  A chain of matches that feed each
-                //      other then runs at shared-memory latency instead of one L2 round trip per link.
+                //      still undefined) with aligned 16-byte loads
                 const uint32_t gsh = (uint32_t)((uintptr_t)(dst + d0) & 15);
                 const uint4* ga = reinterpret_cast<const uint4*>(dst + d0 - gsh);
                 const uint32_t nvec = (gsh + span + 15) >> 4;
-                for (uint32_t i = lane; i < nvec; i += 32) reinterpret_cast<uint4*>(S)[i] = ga[i];
-                const int32_t wb = (int32_t)gsh - (int32_t)d0;          // S[wb + p] = window byte of block position p (p >= d0)
+                for (uint32_t i = lane; i < nvec; i += 32) reinterpret_cast<uint4*>(W.S)[i] = ga[i];
+                W.wb = (int32_t)gsh - (int32_t)d0;
                 __syncwarp();
                 if (own) {
-                    uint8_t* dp = dst + d; uint8_t* dw = S + (wb + (int32_t)d);
+                    uint8_t* dp = dst + d; uint8_t* dw = W.S + (W.wb + (int32_t)d);
 #pragma unroll
                     for (int j = 0; j < 8; j++) if (j < nlow) { dp[j] = x0[j]; dw[j] = x0[j]; }
-                    int32_t i = 8;
-                    for (; i < nlow; i += 8) {                              // loads first, stores after: one L2 latency per 8 bytes, not per byte
-                        uint8_t x[8];
-#pragma unroll
-                        for (int j = 0; j < 8; j++) x[j] = (i + j < nlow) ? mp[i + j] : (uint8_t)0;
-#pragma unroll
-                        for (int j = 0; j < 8; j++) if (i + j < nlow) { dp[i + j] = x[j]; dw[i + j] = x[j]; }
-                    }
-                    i = nlow;
-                    for (; i < (int32_t)ml; i++) { const uint8_t x = S[wb + sp + i]; dp[i] = x; dw[i] = x; }
+                    mx_own_match(W, d, ml, off, nlow, 8);
                 }
                 uint32_t dm = __ballot_sync(ZMT_FULL_MASK, ml && !own);      // long independent ones too: whole warp
                 if (dm) __syncwarp();
                 while (dm) {                                            // in order: may read matches of this very step, or themselves
                     const int jq = __ffs(dm) - 1; dm &= dm - 1;
-                    const uint32_t qd = __shfl_sync(ZMT_FULL_MASK, d, jq), qml = __shfl_sync(ZMT_FULL_MASK, ml, jq), qoff = __shfl_sync(ZMT_FULL_MASK, off, jq);
-                    const int32_t qs = (int32_t)qd - (int32_t)qoff;
-                    uint8_t* dp = dst + qd; uint8_t* dw = S + (wb + (int32_t)qd);
-                    if (qoff >= qml) {
-                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)i; const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i] = x; dw[i] = x; }
-                    } else if (qoff >= 32) {                            // overlapping, period >= warp width: 32-byte waves
-                        for (uint32_t i = 0; i < qml; i += 32) {
-                            if (i + lane < qml) { const int32_t q = qs + (int32_t)(i + lane); const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i + lane] = x; dw[i + lane] = x; }
-                            __syncwarp();
-                        }
-                    } else {                                            // short period: replicate the pattern
-                        for (uint32_t i = lane; i < qml; i += 32) { const int32_t q = qs + (int32_t)(i % qoff); const uint8_t x = q >= (int32_t)d0 ? S[wb + q] : dst[q]; dp[i] = x; dw[i] = x; }
-                    }
-                    __syncwarp();
+                    mx_warp_match(W, __shfl_sync(ZMT_FULL_MASK, d, jq), __shfl_sync(ZMT_FULL_MASK, ml, jq), __shfl_sync(ZMT_FULL_MASK, off, jq), lane);
                 }
                 __syncwarp();
                 base += nfit;
@@ -667,16 +582,8 @@ __device__ uint32_t warp_decode_block(DWin& W, uint32_t srcSize, uint8_t* dst, u
         ml += 4;
         if (ml > dstCap - op) return 0xFFFFFFFFu;
         __syncwarp();                                      // literals (and earlier matches) visible to all lanes
-        uint8_t* d = dst + op;
-        const uint8_t* m = d - off;
-        if (off >= ml) { for (uint32_t i = lane; i < ml; i += 32) d[i] = m[i]; }
-        else if (off >= 32) {                              // overlapping, period >= warp width: 32-byte waves
-            for (uint32_t i = 0; i < ml; i += 32) { if (i + lane < ml) d[i + lane] = m[i + lane]; __syncwarp(); }
-        } else {                                           // short period: replicate the pattern
-            for (uint32_t i = lane; i < ml; i += 32) d[i] = m[i % off];
-        }
+        mx_warp_match_global(dst + op, ml, off, lane);
         op += ml;
-        __syncwarp();
     }
     return op;
 }

@@ -21,6 +21,8 @@
 //                               payloads + LZ4F header/end-mark/checksum + skippable header.
 //   lz4_decode.cuh              the LZ4F decoder: frame scan, pass A (token parse + literals + match records), pass B (match
 //                               execution by ticket, step window in SMEM), sequential fallback for partial-block frames.
+//   match_exec.cuh              what pass B shares with the zstd execute pass (zstd_decode.cu): ticket order, step
+//                               constants, dependency test, window copies.
 //
 // The compressor's match/parse rule is deterministic and restated on the CPU in
 // oracle/lz4_oracle.c:orc_lz4_block_compress_b200 (tests compare bit-exact).
@@ -1036,7 +1038,7 @@ extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uin
 // workspace: stored[] | computed[] | needs_seq[] | ticket, any-FLG.BC flag | slot counts | first_slot | block table | progress | match records
 extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, uint64_t in_bytes)
 {
-    uint64_t sz = 3 * a256((uint64_t)nframes * 4) + 256 + 2 * a256(((uint64_t)nframes + 1) * 8) + a256(((uint64_t)nframes / LZX_WIN + 2) * 8);
+    uint64_t sz = 3 * a256((uint64_t)nframes * 4) + 256 + 2 * a256(((uint64_t)nframes + 1) * 8) + ticket_table_bytes(nframes);
     sz += a256((uint64_t)nslots * sizeof(LzBlk)) + a256((uint64_t)nslots * 4);
     sz += a256((in_bytes / 3 + 8) * 8);
     return (size_t)sz + 1024;
@@ -1056,7 +1058,7 @@ static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint
     uint32_t* needs_seq = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
     unsigned long long* ticket = (unsigned long long*)w;
     uint32_t* any_bchk = (uint32_t*)(ticket + 1); w += 256;
-    unsigned long long* wbase = (unsigned long long*)w; w += a256(((uint64_t)nframes / LZX_WIN + 2) * 8);
+    unsigned long long* wbase = (unsigned long long*)w; w += ticket_table_bytes(nframes);
     uint64_t* slot_cnt = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
     uint64_t* first_slot = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
     LzBlk* tab = (LzBlk*)w; w += a256((uint64_t)nslots * sizeof(LzBlk));
@@ -1068,7 +1070,7 @@ static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint
     const uint8_t* in = (const uint8_t*)d_in;
     lz4_slot_counts_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(d_out_off, nframes, slot_cnt);
     scan_u64_kernel<<<1, 1024, 0, stream>>>(slot_cnt, first_slot, nframes);
-    lz4_ticket_windows_kernel<<<1, 256, 0, stream>>>(first_slot, nframes, wbase);
+    ticket_windows_kernel<<<1, 256, 0, stream>>>(first_slot, nframes, wbase);
     lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, any_bchk, seg, nframes);
     zmt_dbg_check(stream, "lz4_scan_frames_kernel");
     {

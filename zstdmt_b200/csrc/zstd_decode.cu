@@ -17,7 +17,8 @@
 //                            content-size check against the frame header
 //   zstd_execute_kernel      one warp per block, blocks by ticket (block-index-major): up to 32 sequences per step, written to
 //                            global memory and to a window in SMEM; a match that reaches below the block's own output waits for
-//                            the `done` flags of the blocks it reads from
+//                            the `done` flags of the blocks it reads from.  Ticket order, dependency test and match copies
+//                            are match_exec.cuh's, shared with the LZ4 decoder
 //   zstd_checksum_kernel     one warp per frame with a content checksum: XXH64 of the regenerated frame
 // Host side (zmt_zstd_scan_frame_host): walks frame + block headers (3 bytes per block + the two section headers), sizes the
 // scratch, names per block the block whose header describes each table it uses, flags per frame (state, checksum, no size).
@@ -35,6 +36,7 @@
 #include "common.cuh"
 #include "frame_format.h"
 #include "host_common.h"
+#include "match_exec.cuh"
 #include "zmt_dev.h"
 
 extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
@@ -971,10 +973,9 @@ __global__ void zstd_offsets_kernel(const ZBlk* __restrict__ blocks, uint32_t nb
 
 // ---------------------------------------------------------------- kernel 3: sequence execution
 #define ZX_WARPS 8
-#define ZX_SPAN 2048u          // bytes a step of the execute pass may regenerate: staged in shared memory
-// One block, one warp.  Blocks are handed out by a ticket counter (see the kernel below), so every block this one may wait
-// for — lower indices of the same frame — is held by a warp that is already running: the wait cannot deadlock whatever
-// order the hardware schedules CTAs in.
+#define ZX_LANE_LIT 32u        // a literal run up to this length is copied by its own lane, a longer one by the whole warp
+// One block, one warp.  Blocks are handed out in match_exec.cuh's ticket order, so every block this one may wait for —
+// lower indices of the same frame — is held by a warp that is already running.
 __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, const uint8_t* __restrict__ scratch,
                          const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                          uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, uint8_t* S)
@@ -996,13 +997,13 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
         uint32_t waited_to = b;                              // blocks [waited_to, b) are known complete
         const uint64_t blk_abs = blk_out[b];                 // absolute output address of this block
         const uint64_t blk_in_frame = blk_abs - frame_base;
-        // Up to 32 sequences per step: one coalesced load of the records, positions from two warp scans.  Everything the step
-        // regenerates — at most ZX_SPAN bytes, else the step is cut shorter — is written to global memory AND to a window in
-        // shared memory: every lane copies its own literal run (literals come from the scratch, no ordering among them), then
-        // the matches run; a source byte at or above the step's first output byte is read from the window, so a chain of
-        // matches feeding each other runs at shared-memory latency instead of one L2 round trip per link.
+        // Up to MX_STEP sequences per step: one coalesced load of the records, positions from two warp scans.  Everything the
+        // step regenerates — at most MX_SPAN bytes, else the step is cut shorter — goes to global memory and to the step
+        // window (MxWin): every lane copies its own literal run (literals come from the scratch, no ordering among them),
+        // then the matches run.
+        MxWin W; W.dst = dst; W.S = S;
         for (uint32_t base = 0; base < B.nseq;) {
-            uint32_t cnt = B.nseq - base < 32 ? B.nseq - base : 32;
+            uint32_t cnt = B.nseq - base < MX_STEP ? B.nseq - base : MX_STEP;
             uint32_t ll = 0, off = 0, ml = 0;
             if (lane < cnt) { const ZDSeq q = seqs[base + lane]; ll = q.ll; off = q.off; ml = q.ml; }
             uint32_t it = ll + ml, il = ll;                  // inclusive scans: output bytes, literal bytes
@@ -1012,7 +1013,7 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
                 const uint32_t a = __shfl_up_sync(0xFFFFFFFFu, it, d), c = __shfl_up_sync(0xFFFFFFFFu, il, d);
                 if (lane >= (uint32_t)d) { it = (it + a) | ((it | a) & 0x40000000u); il += c; }
             }
-            const uint32_t nfit = __popc(__ballot_sync(0xFFFFFFFFu, lane < cnt && it <= ZX_SPAN));      // sorted: a prefix
+            const uint32_t nfit = __popc(__ballot_sync(0xFFFFFFFFu, lane < cnt && it <= MX_SPAN));      // sorted: a prefix
             if (nfit == 0) {
                 // the first sequence alone is larger than the window: straight in global memory, by the whole warp
                 const uint32_t qll = __shfl_sync(0xFFFFFFFFu, ll, 0), qoff = __shfl_sync(0xFFFFFFFFu, off, 0), qml = __shfl_sync(0xFFFFFFFFu, ml, 0);
@@ -1030,12 +1031,7 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
                     if (waited) __threadfence();
                 }
                 __syncwarp();
-                uint8_t* d = dst + mp;
-                const uint8_t* m = d - qoff;
-                if (qoff >= qml) { for (uint32_t k = lane; k < qml; k += 32) d[k] = m[k]; }
-                else if (qoff >= 32) { for (uint32_t k = 0; k < qml; k += 32) { if (k + lane < qml) d[k + lane] = m[k + lane]; __syncwarp(); } }
-                else { for (uint32_t k = lane; k < qml; k += 32) d[k] = m[k % qoff]; }
-                __syncwarp();
+                mx_warp_match_global(dst + mp, qml, qoff, lane);
                 op += qll + qml; lp += qll; base += 1;
                 continue;
             }
@@ -1045,23 +1041,13 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
             const bool mybad = lane < cnt && ((uint64_t)my_op + ll + ml > rg || (uint64_t)my_lp + ll > B.regen_hint || off == 0 || (uint64_t)off > blk_in_frame + my_mp);
             const uint32_t badmask = __ballot_sync(0xFFFFFFFFu, mybad);
             const uint32_t lim = badmask ? (uint32_t)(__ffs(badmask) - 1) : cnt;      // sequences of this step that are executed
-            const int32_t wb = -(int32_t)op;                                           // S[wb + p] = window byte of block position p (op <= p < op + ZX_SPAN)
-            if (lane < lim && ll <= 32) {
-                // loads first, stores after, 8 bytes at a time: a byte-wise load -> store loop pays one L2 latency per byte
-                const uint8_t* ls = lit + my_lp; uint8_t* d = dst + my_op; uint8_t* dw = S + (wb + (int32_t)my_op);
-                for (uint32_t k = 0; k < ll; k += 8) {
-                    uint8_t x[8];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) x[j] = (k + j < ll) ? ls[k + j] : (uint8_t)0;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) if (k + j < ll) { d[k + j] = x[j]; dw[k + j] = x[j]; }
-                }
-            }
-            uint32_t longmask = __ballot_sync(0xFFFFFFFFu, lane < lim && ll > 32);
+            W.lo = (int32_t)op; W.wb = -(int32_t)op;                                   // the window starts at the step's first output byte
+            if (lane < lim && ll <= ZX_LANE_LIT) mx_lane_copy(dst + my_op, S + (W.wb + (int32_t)my_op), lit + my_lp, 0, ll);
+            uint32_t longmask = __ballot_sync(0xFFFFFFFFu, lane < lim && ll > ZX_LANE_LIT);
             while (longmask) {                                // long literal runs: the whole warp copies
                 const int jl = __ffs(longmask) - 1; longmask &= longmask - 1;
                 const uint32_t o = __shfl_sync(0xFFFFFFFFu, my_op, jl), l0 = __shfl_sync(0xFFFFFFFFu, my_lp, jl), n = __shfl_sync(0xFFFFFFFFu, ll, jl);
-                for (uint32_t k = lane; k < n; k += 32) { const uint8_t x = lit[l0 + k]; dst[o + k] = x; S[wb + (int32_t)(o + k)] = x; }
+                for (uint32_t k = lane; k < n; k += 32) { const uint8_t x = lit[l0 + k]; dst[o + k] = x; S[W.wb + (int32_t)(o + k)] = x; }
             }
             // ---- matches.  Any source below this block: wait (once per step) for the earlier blocks it touches.
             {
@@ -1080,50 +1066,14 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
                 }
             }
             __syncwarp();                                                   // this step's literals are in place (global and window)
-            // (the destinations [my_mp, my_mp + ml) of a step are sorted and disjoint: a match is independent iff its source
-            //  touches no destination of an earlier match of the step — binary search over the lanes by shuffle, as in
-            //  lz4_exec_blocks_kernel — and does not overlap its own destination; independent matches run lane-parallel)
             const bool act = lane < lim && ml != 0;
-            const int32_t sp = (int32_t)my_mp - (int32_t)off;               // block-relative source start (negative: earlier blocks)
-            const int32_t e_end = act ? (int32_t)(my_mp + ml) : 0x7FFFFFFF, d_beg = act ? (int32_t)my_mp : 0x7FFFFFFF;
-            uint32_t a = 0;
-#pragma unroll
-            for (uint32_t stp = 16; stp > 0; stp >>= 1) {
-                const int32_t v = __shfl_sync(0xFFFFFFFFu, e_end, (a + stp - 1) & 31);
-                if (v <= sp) a += stp;
-            }
-            const int32_t da = __shfl_sync(0xFFFFFFFFu, d_beg, a & 31);
-            const bool indep = act && off >= ml && !(a < lane && da < sp + (int32_t)ml);
-            if (indep && ml <= 32) {
-                uint8_t* d = dst + my_mp; uint8_t* dw = S + (wb + (int32_t)my_mp);
-                const int32_t nlow = sp >= (int32_t)op ? 0 : ((int32_t)op - sp < (int32_t)ml ? (int32_t)op - sp : (int32_t)ml);
-                const uint8_t* m = dst + sp;
-                int32_t k = 0;
-                for (; k < nlow; k += 8) {
-                    uint8_t x[8];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) x[j] = (k + j < nlow) ? m[k + j] : (uint8_t)0;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) if (k + j < nlow) { d[k + j] = x[j]; dw[k + j] = x[j]; }
-                }
-                k = nlow;
-                for (; k < (int32_t)ml; k++) { const uint8_t x = S[wb + sp + k]; d[k] = x; dw[k] = x; }
-            }
-            uint32_t dm = __ballot_sync(0xFFFFFFFFu, act && !(indep && ml <= 32));       // long independent ones and the dependent ones: in order, whole warp
+            const bool indep = mx_independent(lane, act, my_mp, ml, off);
+            if (indep && ml <= MX_OWN) mx_own_match(W, my_mp, ml, off, mx_nlow(W, (int32_t)my_mp - (int32_t)off, ml), 0);
+            uint32_t dm = __ballot_sync(0xFFFFFFFFu, act && !(indep && ml <= MX_OWN));   // long independent ones and the dependent ones: in order, whole warp
             if (dm) __syncwarp();
             while (dm) {
                 const int jq = __ffs(dm) - 1; dm &= dm - 1;
-                const uint32_t qoff = __shfl_sync(0xFFFFFFFFu, off, jq), qml = __shfl_sync(0xFFFFFFFFu, ml, jq), mp = __shfl_sync(0xFFFFFFFFu, my_mp, jq);
-                const int32_t qs = (int32_t)mp - (int32_t)qoff;
-                uint8_t* d = dst + mp; uint8_t* dw = S + (wb + (int32_t)mp);
-                if (qoff >= qml) { for (uint32_t k = lane; k < qml; k += 32) { const int32_t q = qs + (int32_t)k; const uint8_t x = q >= (int32_t)op ? S[wb + q] : dst[q]; d[k] = x; dw[k] = x; } }
-                else if (qoff >= 32) {
-                    for (uint32_t k = 0; k < qml; k += 32) {
-                        if (k + lane < qml) { const int32_t q = qs + (int32_t)(k + lane); const uint8_t x = q >= (int32_t)op ? S[wb + q] : dst[q]; d[k + lane] = x; dw[k + lane] = x; }
-                        __syncwarp();
-                    }
-                } else { for (uint32_t k = lane; k < qml; k += 32) { const int32_t q = qs + (int32_t)(k % qoff); const uint8_t x = q >= (int32_t)op ? S[wb + q] : dst[q]; d[k] = x; dw[k] = x; } }
-                __syncwarp();
+                mx_warp_match(W, __shfl_sync(0xFFFFFFFFu, my_mp, jq), __shfl_sync(0xFFFFFFFFu, ml, jq), __shfl_sync(0xFFFFFFFFu, off, jq), lane);
             }
             __syncwarp();
             if (badmask) { bad = true; break; }
@@ -1142,62 +1092,20 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
     if (lane == 0) { __threadfence(); vdone[b] = 1; }
 }
 
-// Ticket order, as in lz4_exec_blocks_kernel: within a window of ZX_WIN frames block-index-major (block 0 of every frame,
-// then block 1, ...), so that the blocks of one frame — a dependency chain wherever matches reach below their block — are
-// not handed to neighbouring warps, and as many independent chains are in flight as there are frames.  Block (f, b-1)
-// always holds a lower ticket than (f, b).  Windows with very ragged block counts fall back to frame-major order.
-#define ZX_WIN 16384u
-__global__ void __launch_bounds__(256)
-zstd_ticket_windows_kernel(const uint32_t* __restrict__ frame_first_blk, uint32_t nframes, unsigned long long* __restrict__ wbase)
-{
-    __shared__ uint32_t red[256];
-    const uint32_t nwin = (nframes + ZX_WIN - 1) / ZX_WIN;
-    unsigned long long base = 0;
-    for (uint32_t w = 0; w < nwin; w++) {
-        const uint32_t f0 = w * ZX_WIN, f1 = f0 + ZX_WIN < nframes ? f0 + ZX_WIN : nframes;
-        uint32_t mx = 0;
-        for (uint32_t f = f0 + threadIdx.x; f < f1; f += 256) { const uint32_t c = frame_first_blk[f + 1] - frame_first_blk[f]; mx = c > mx ? c : mx; }
-        red[threadIdx.x] = mx;
-        __syncthreads();
-        for (uint32_t d = 128; d > 0; d >>= 1) { if (threadIdx.x < d && red[threadIdx.x + d] > red[threadIdx.x]) red[threadIdx.x] = red[threadIdx.x + d]; __syncthreads(); }
-        mx = red[0];
-        __syncthreads();
-        const unsigned long long real = frame_first_blk[f1] - frame_first_blk[f0], grid = (unsigned long long)(f1 - f0) * mx;
-        const bool frame_major = grid > 8 * real + 65536;
-        if (threadIdx.x == 0) wbase[w] = base | (frame_major ? (1ull << 63) : 0ull);
-        base += frame_major ? real : grid;
-    }
-    if (threadIdx.x == 0) wbase[nwin] = base;
-}
-
 __global__ void __launch_bounds__(32 * ZX_WARPS)
 zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, uint32_t nblocks, const uint8_t* __restrict__ scratch,
                     const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                     uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, unsigned long long* __restrict__ ticket,
                     const uint32_t* __restrict__ frame_first_blk, const unsigned long long* __restrict__ wbase, uint32_t nframes)
 {
-    __shared__ __align__(16) uint8_t stage[ZX_WARPS][ZX_SPAN];
+    __shared__ __align__(16) uint8_t stage[ZX_WARPS][MX_SPAN];
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t nwin = (nframes + ZX_WIN - 1) / ZX_WIN;
-    const unsigned long long ntickets = wbase[nwin] & ~(1ull << 63);
+    const MxTickets T = mx_tickets(wbase, nframes);
     for (;;) {
-        unsigned long long tk = 0;
-        if (lane == 0) tk = atomicAdd(ticket, 1ull);
-        tk = __shfl_sync(0xFFFFFFFFu, tk, 0);
-        if (tk >= ntickets) return;
-        uint32_t lo = 0, hi = nwin;
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if ((wbase[mid] & ~(1ull << 63)) <= tk) lo = mid; else hi = mid; }
-        const unsigned long long wb = wbase[lo];
-        const unsigned long long tl = tk - (wb & ~(1ull << 63));
-        const uint32_t f0 = lo * ZX_WIN, wn = (f0 + ZX_WIN < nframes ? ZX_WIN : nframes - f0);
+        const unsigned long long tk = mx_take_ticket(ticket, lane);
+        if (tk >= T.count) return;
         uint32_t b;
-        if (wb >> 63) b = frame_first_blk[f0] + (uint32_t)tl;
-        else {
-            const uint32_t fb = (uint32_t)(tl / wn), ff = f0 + (uint32_t)(tl % wn);
-            const uint32_t s0 = frame_first_blk[ff];
-            if (fb >= frame_first_blk[ff + 1] - s0) continue;
-            b = s0 + fb;
-        }
+        if (!mx_ticket_unit(T, tk, frame_first_blk, b)) continue;
         if (b >= nblocks) continue;
         zx_block(b, lane, in, blocks, scratch, regen, blk_out, out_off, out, done, status, stage[threadIdx.x >> 5]);
         __syncwarp();
@@ -1326,7 +1234,7 @@ extern "C" size_t zmt_zstd_blk_desc_bytes(void) { return sizeof(ZBlk); }
 extern "C" size_t zmt_zstdd_workspace_bytes(uint32_t nframes, uint32_t nblocks, uint64_t scratch_bytes)
 {
     return (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) * 2 + (((uint64_t)nblocks * 8 + 255) & ~255ull) + (((uint64_t)nframes * 8 + 255) & ~255ull)
-           + 256 + (size_t)((((uint64_t)nframes / ZX_WIN + 2) * 8 + 255) & ~255ull) + 3 * (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) + scratch_bytes + 1024;
+           + 256 + ticket_table_bytes(nframes) + 3 * (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) + scratch_bytes + 1024;
 }
 
 // d_blocks: nblocks descriptors (device copy of what zmt_zstd_scan_frame_host produced); d_frame_first_blk: nframes+1;
@@ -1344,7 +1252,7 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
     uint64_t* blk_out = (uint64_t*)w; w += (((uint64_t)nblocks * 8 + 255) & ~255ull);
     w += (((uint64_t)nframes * 8 + 255) & ~255ull);
     unsigned long long* xticket = (unsigned long long*)w; w += 256;
-    unsigned long long* xwbase = (unsigned long long*)w; w += (((uint64_t)nframes / ZX_WIN + 2) * 8 + 255) & ~255ull;
+    unsigned long long* xwbase = (unsigned long long*)w; w += ticket_table_bytes(nframes);
     uint32_t* seq_done = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
     uint32_t* seq_ml = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
     uint32_t* lit_done = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
@@ -1376,7 +1284,7 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
         const uint32_t gmax = (uint32_t)(zmt_sm_count() * (2048 / (32 * ZX_WARPS)));
         const uint32_t gneed = (nblocks + ZX_WARPS - 1) / ZX_WARPS;
         cudaMemsetAsync(xticket, 0, 8, stream);
-        zstd_ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, xwbase);
+        ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, xwbase);
         zstd_execute_kernel<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, scratch, regen, blk_out,
                                                                                      d_out_off, (uint8_t*)d_out, done, d_status, xticket, d_frame_first_blk, xwbase, nframes);
         zstd_checksum_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
