@@ -43,16 +43,23 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_product(force=False, verbose=False):
+def build_product(force=False, verbose=False, defines=(), out_dir=None):
+    """The product library; with `defines` (e.g. ["ZMT_PHASE_PROBE"]) an instrumented variant, built as
+    out_dir/libzstdmt_b200.so (out_dir is required then, so a variant never replaces the product)."""
+    if defines and not out_dir:
+        raise ValueError("a library built with extra defines goes to its own out_dir")
+    lib = os.path.join(out_dir, "libzstdmt_b200.so") if out_dir else LIB
     srcs = _sources()
     deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
-    if not force and not _stale(LIB, deps):
-        return LIB
+    if not force and not _stale(lib, deps):
+        return lib
+    if out_dir:
+        os.makedirs(out_dir, exist_ok=True)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not os.path.exists(nvcc):
         nvcc = "nvcc"
-    tmp = LIB + ".tmp.%d" % os.getpid()         # link under a scratch name, then rename: readers never see a half-written library
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + srcs + ["-lpthread"]
+    tmp = lib + ".tmp.%d" % os.getpid()         # link under a scratch name, then rename: readers never see a half-written library
+    cmd = [nvcc] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + srcs + ["-lpthread"]
     r = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True)
     if verbose or r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)
@@ -60,8 +67,8 @@ def build_product(force=False, verbose=False):
         if os.path.exists(tmp):
             os.remove(tmp)
         raise RuntimeError("nvcc failed building libzstdmt_b200.so")
-    os.replace(tmp, LIB)
-    return LIB
+    os.replace(tmp, lib)
+    return lib
 
 
 def build_harness(force=False):

@@ -705,6 +705,16 @@ extern "C" int zmt_prof_end(double* ms, int* count, int max_ids)
     return ZMT_K_COUNT < max_ids ? ZMT_K_COUNT : max_ids;
 }
 
+#ifdef ZMT_PHASE_PROBE
+// out[team * ZMT_NPHASE + phase] = cycles summed since the last call (lz4_pipe.cuh); clears the counters.  0 = ok.
+extern "C" int zmt_phase_probe_take(unsigned long long* out)
+{
+    static const unsigned long long zero[2 * ZMT_NPHASE] = {};
+    if (cudaMemcpyFromSymbol(out, zmt_phase_cycles, sizeof(zero)) != cudaSuccess) return 1;
+    return cudaMemcpyToSymbol(zmt_phase_cycles, zero, sizeof(zero)) != cudaSuccess;
+}
+#endif
+
 // begin / end marks for code outside this file (zstd_decode.cu): same records as ZmtProfScope
 static cudaEvent_t g_mark_a[ZMT_K_COUNT];
 extern "C" void zmt_prof_mark(int id, void* stream, int end)

@@ -43,6 +43,33 @@ __device__ __forceinline__ void bar_arrive()
 template <uint32_t BARID>
 __device__ __forceinline__ void team_sync() { bar_sync<BARID, P_TEAM>(); }
 
+// Per-phase cycle probe of lz4_blocks_pipe_kernel, built only with -DZMT_PHASE_PROBE (tools/lz4_phase_probe.py): thread 0
+// of each team adds the clock64() cycles since its previous mark to the counter of the phase that mark closes.  The rows
+// are those of DESIGN.md §3.4; a phase index means, for team A / team B:
+//   0 staging            1 EMPTY wait / FULL wait      2 candidate rounds / marking walk    3 walk 0 / piece list
+//   4 walk 1 / head detection    5 path resolution / emission + long jobs    6 FULL arrive / EMPTY arrive
+//   7 final sync + last literals (team B: with the flush of the pending sequence)
+// Without the define the marks are empty and the kernels compile as if they were not there.
+#ifdef ZMT_PHASE_PROBE
+#define ZMT_NPHASE 8
+__device__ unsigned long long zmt_phase_cycles[2][ZMT_NPHASE];
+__device__ __forceinline__ void zmt_phase_mark(uint32_t team, uint32_t ttid, int ph)     // ph < 0: start the clock
+{
+    __shared__ long long last[2];
+    if (ttid == 0) {
+        const long long now = clock64();
+        if (ph >= 0) atomicAdd(&zmt_phase_cycles[team][ph], (unsigned long long)(now - last[team]));
+        last[team] = now;
+    }
+}
+#define ZMT_PHASE(team, ttid, ph) zmt_phase_mark((team), (ttid), (ph))
+// inside the team functions: only the LZ4 pipeline's teams (the Zstandard encoder runs them with barrier id 0)
+#define ZMT_PHASE_TEAM(BARID, ttid, ph) do { if constexpr ((BARID) != 0) zmt_phase_mark((BARID) == PB_B, (ttid), (ph)); } while (0)
+#else
+#define ZMT_PHASE(team, ttid, ph) ((void)0)
+#define ZMT_PHASE_TEAM(BARID, ttid, ph) ((void)0)
+#endif
+
 // exclusive scan over one team (8 warps); one team barrier; `ws` = two 8-word halves used alternately
 template <uint32_t BARID>
 __device__ __forceinline__ uint32_t team_exscan1(uint32_t v, uint32_t* ws, uint32_t parity, uint32_t* total, uint32_t twid, uint32_t lane)
@@ -124,30 +151,40 @@ __device__ __forceinline__ bool lz_candidates(const uint8_t* in, uint32_t* tab, 
         const uint32_t rel = r * C_ROUND + 4 * ttid, i = t0 + rel;
         const uint32_t* w = reinterpret_cast<const uint32_t*>(in) + (i >> 2);
         const uint32_t w0 = w[-1], w1 = w[0], w2 = w[1];
-        uint32_t hreg[4], tv[4], o[4], m4 = 0;
-        // the four table reads, then the four window reads, are issued together: no position waits on another
+        uint32_t h[4], tv[4], x[4], o[4], m4 = 0;
+        // The round is straight-line code from the first table read to the offset store: the four table reads, then
+        // the four verifying reads, issued unconditionally so that none waits on another position's compare (an empty
+        // slot, t = 0, reads the word below the block, pad0, and is masked out), and the candidate is chosen by selects.
 #pragma unroll
         for (uint32_t k = 0; k < 4; k++) {
-            hreg[k] = (__funnelshift_r(w1, w2, 8 * k) * 2654435761u) >> (32 - C_HASHLOG);
-            tv[k] = tab[hreg[k]];
+            h[k] = (__funnelshift_r(w1, w2, 8 * k) * 2654435761u) >> (32 - C_HASHLOG);
+            tv[k] = tab[h[k]];
         }
 #pragma unroll
         for (uint32_t k = 0; k < 4; k++) {
+            const int32_t a = (int32_t)(tv[k] - 1);                     // -1 for an empty slot
+            const uint32_t* q = reinterpret_cast<const uint32_t*>(in) + (a >> 2);
+            x[k] = __funnelshift_r(q[0], q[1], 8u * (uint32_t)a);      // the shift counts modulo 32
+        }
+        // i is a multiple of 4, so i + k >= d fails only in the block's first quad, for d > k
+        const bool first = (i == 0);
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
             const uint32_t ik = i + k;
-            const bool ok = (ik + 12 <= n);
             const uint32_t v = __funnelshift_r(w1, w2, 8 * k), pv = __funnelshift_r(w0, w1, 8 * k);
             const uint32_t t = tv[k];
-            const bool hit = t && lds32u(in, t ? t - 1 : 0) == v;
-            o[k] = 0;
-            if (ok) {
-                // short-period candidates d = 1..4: v(i-d) is a byte-shift of the window
-                if (ik >= 1 && __funnelshift_r(pv, v, 24) == v) o[k] = 1;
-                else if (ik >= 2 && __funnelshift_r(pv, v, 16) == v) o[k] = 2;
-                else if (ik >= 3 && __funnelshift_r(pv, v, 8) == v) o[k] = 3;
-                else if (ik >= 4 && pv == v) o[k] = 4;
-                else if (hit) o[k] = ik - (t - 1);
-            }
-            if (!ok) hreg[k] = 0xFFFFFFFFu;
+            const bool hit = (t != 0) & (x[k] == v);
+            // short-period candidates d = 1..4: v(i-d) is a byte-shift of the window; the smallest d wins, then the table
+            const bool e1 = (__funnelshift_r(pv, v, 24) == v) & !(first & (k < 1));
+            const bool e2 = (__funnelshift_r(pv, v, 16) == v) & !(first & (k < 2));
+            const bool e3 = (__funnelshift_r(pv, v, 8) == v) & !(first & (k < 3));
+            const bool e4 = (pv == v) & !first;
+            uint32_t of = hit ? ik - (t - 1) : 0u;
+            of = e4 ? 4u : of;
+            of = e3 ? 3u : of;
+            of = e2 ? 2u : of;
+            of = e1 ? 1u : of;
+            o[k] = (ik + 12 <= n) ? of : 0u;                            // LZ4 MFLIMIT: only the block's last quads fail
             m4 |= (uint32_t)(o[k] != 0) << k;
         }
         *reinterpret_cast<uint2*>(&T.off[rel]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
@@ -159,12 +196,15 @@ __device__ __forceinline__ bool lz_candidates(const uint8_t* in, uint32_t* tab, 
         anyM |= mw;
         team_sync<BARID>();
         if (r == 0 && ttid == 0) any[b ^ 1] = 0;
+        // inserts: positions past the MFLIMIT are not inserted, and a later eligible position of the quad with the same
+        // hash wins anyway.  A skipped insert is a max with 0, a no-op: ptxas puts a branch region around every
+        // predicated shared atomic, even a predicated red.shared.
 #pragma unroll
         for (uint32_t k = 0; k < 4; k++) {
-            bool last = hreg[k] != 0xFFFFFFFFu;     // a later position of the quad with the same hash wins anyway
+            uint32_t val = (i + k + 12 <= n) ? i + k + 1 : 0u;
 #pragma unroll
-            for (uint32_t k2 = k + 1; k2 < 4; k2++) last &= hreg[k2] != hreg[k];
-            if (last) atomicMax(&tab[hreg[k]], i + k + 1);
+            for (uint32_t k2 = k + 1; k2 < 4; k2++) val = (h[k2] == h[k] && i + k2 + 12 <= n) ? 0u : val;
+            atomicMax(&tab[h[k]], val);
         }
         team_sync<BARID>();
     }
@@ -193,8 +233,10 @@ __device__ __forceinline__ bool lz_chains(const uint8_t* in, PipeTile& T, LzFron
     if (alive) c_walk<0>(in, T, F, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
     else F.link[ttid] = (uint16_t)ttid;                 // dead: self link, never reached
     team_sync<BARID>();
+    ZMT_PHASE_TEAM(BARID, ttid, 3);
     if (alive) c_walk<1>(in, T, F, ttid, F.xfree[ttid], F.xdin[ttid], t0, limit);
     team_sync<BARID>();
+    ZMT_PHASE_TEAM(BARID, ttid, 4);
     // Which chains lie on the true path (entry k0, follow the links).  Links only go forward.  Each warp resolves its
     // own 32 chains with shuffles (pointer doubling on lane indices: terminal chain + bitmask of the lanes on the way),
     // one thread then hops from warp to warp (<= 8 hops), and each warp reads its path mask back: 2 barriers, not 18.
@@ -247,6 +289,7 @@ __device__ __forceinline__ uint32_t lz_heads(const uint8_t* in, PipeTile& T, LzB
     team_sync<BARID>();
     if ((T.pathmask[twid] >> lane) & 1u) c_walk<2>(in, T, K, ttid, t0 + ttid * C_SEG + T.min_[ttid], ttid == k0 ? T.e_din : 0u, t0, limit);
     team_sync<BARID>();
+    ZMT_PHASE_TEAM(BARID, ttid, 2);
     uint32_t np;
     {
         // one segment (16 positions) per thread.  segprev[j]: 1 + start of the last non-Cont piece before
@@ -261,6 +304,7 @@ __device__ __forceinline__ uint32_t lz_heads(const uint8_t* in, PipeTile& T, LzB
         while (w) { const uint32_t bit = __ffs(w) - 1; w &= w - 1; K.piece[base++] = (uint16_t)(ttid * C_SEG + bit); }
     }
     team_sync<BARID>();
+    ZMT_PHASE_TEAM(BARID, ttid, 3);
     if (np == 0) return 0;
     // pieces are dealt in runs of ceil(np / 256) per thread, so every warp shares the work
     uint32_t nh_local = 0, headmask = 0;
@@ -365,6 +409,7 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
     constexpr uint32_t NT = 2 * P_TEAM;
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     const uint32_t team = tid >> 8, ttid = tid & (P_TEAM - 1), twid = ttid >> 5;
+    ZMT_PHASE(team, ttid, -1);
 
     for (uint32_t blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
         const uint32_t chunk = blk / bpc, bic = blk % bpc;
@@ -379,6 +424,7 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
         CTA_SYNC();                                       // previous block fully consumed
         if (tid == 0) { S.nlong = 0; S.a_any[0] = 0; S.a_any[1] = 0; }
         lz_stage<NT>(S.stage, S.tab, &S.mbar, in + cbase + boff, n, tid);
+        ZMT_PHASE(team, ttid, 0);
 
         const uint32_t limit = n >= 5 ? n - 5 : 0;        // matches end at or before n-5
         const uint32_t ntiles = (n + C_TILE - 1) / C_TILE;
@@ -390,9 +436,13 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                 const uint32_t t0 = ti * C_TILE, b = ti & 1;
                 PipeTile& T = S.tile[b];
                 if (ti >= 2) { if (b) bar_sync<PB_EMPTY0 + 1, 2 * P_TEAM>(); else bar_sync<PB_EMPTY0, 2 * P_TEAM>(); }               // back end released this buffer (tile ti-2)
+                ZMT_PHASE(0, ttid, 1);
                 const bool has_match = lz_candidates<PB_A>(S.stage.in, S.tab, T, S.a_any, b, t0, n, ttid, lane);
+                ZMT_PHASE(0, ttid, 2);
                 lz_chains<PB_A>(S.stage.in, T, S.fe, has_match, e, e_din, t0, limit, ttid, lane);
+                ZMT_PHASE(0, ttid, 5);
                 if (b) bar_arrive<PB_FULL0 + 1, 2 * P_TEAM>(); else bar_arrive<PB_FULL0, 2 * P_TEAM>();
+                ZMT_PHASE(0, ttid, 6);
             }
         } else {
             // =========================================================== back end: mark, merge pieces, emit
@@ -402,9 +452,11 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                 const uint32_t t0 = ti * C_TILE, b = ti & 1;
                 PipeTile& T = S.tile[b];
                 if (b) bar_sync<PB_FULL0 + 1, 2 * P_TEAM>(); else bar_sync<PB_FULL0, 2 * P_TEAM>();
+                ZMT_PHASE(1, ttid, 1);
                 if (T.do_parse) {
                     uint32_t tile_end;
                     const uint32_t nh = lz_heads<PB_B>(S.stage.in, T, S.be, S.scanws, pd, tile_end, t0, limit, ttid, lane);
+                    ZMT_PHASE(1, ttid, 4);
                     if (nh) {
                         const LzRun R = lz_seq_run(T, S.be, pd, nh, t0, ttid);
                         uint32_t sz = 0;
@@ -426,7 +478,9 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                         if (ttid == 0) S.nlong = 0;
                     }
                 }
+                ZMT_PHASE(1, ttid, 5);
                 if (ti + 2 < ntiles) { if (b) bar_arrive<PB_EMPTY0 + 1, 2 * P_TEAM>(); else bar_arrive<PB_EMPTY0, 2 * P_TEAM>(); }     // the front end may refill this buffer
+                ZMT_PHASE(1, ttid, 6);
             }
             // ---- flush the pending sequence
             uint32_t anchor = 0;
@@ -461,5 +515,6 @@ lz4_blocks_pipe_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32
                 for (uint32_t i = tid; i < lit; i += NT) op[hl + i] = S.stage.in[anchor + i];
             }
         }
+        ZMT_PHASE(team, ttid, 7);
     }
 }
