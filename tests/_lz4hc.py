@@ -1,5 +1,5 @@
 """The LZ4 high-compression class of levels 10-12 (zstdmt_b200/csrc/lz4_hc_rule.h) restated in Python, and the
-binding of its C twin (oracle/lz4_hc_twin.c, built into oracle/liblz4hc_twin.so).
+binding of its C twin (oracle/chain_twin.c, built into oracle/libchain_twin.so).
 
 The restatement keeps the chains as a dict of position lists and finds best[] by brute force over them; it is slow and
 meant for inputs of up to about 100 KiB.  Both give, per block, the merged sequences as (literal length, offset, match
@@ -206,7 +206,7 @@ _twin = None
 def twin():
     global _twin
     if _twin is None:
-        L = ctypes.CDLL(os.path.join(ROOT, "oracle", "liblz4hc_twin.so"))
+        L = ctypes.CDLL(os.path.join(ROOT, "oracle", "libchain_twin.so"))
         L.orc_lz4_hc_sequences.restype = ctypes.c_long
         L.orc_lz4_hc_sequences.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32,
                                            ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]

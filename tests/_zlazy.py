@@ -1,5 +1,5 @@
 """The zstd search class of levels 6-12 (zstdmt_b200/csrc/zstd_lazy_rule.h) restated in Python, and the binding of its
-C twin (oracle/zstd_lazy_twin.c, built into oracle/libzlazy_twin.so).
+C twin (oracle/chain_twin.c, built into oracle/libchain_twin.so).
 
 The restatement keeps the chains as a dict of position lists and finds best[] by brute force over them; it is slow and
 meant for inputs of up to about 100 KiB.  Both return, per block, the merged sequences as (literal length, offset,
@@ -123,7 +123,7 @@ _twin = None
 def twin():
     global _twin
     if _twin is None:
-        L = ctypes.CDLL(os.path.join(ROOT, "oracle", "libzlazy_twin.so"))
+        L = ctypes.CDLL(os.path.join(ROOT, "oracle", "libchain_twin.so"))
         L.orc_zstd_lazy_sequences.restype = ctypes.c_long
         L.orc_zstd_lazy_sequences.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32,
                                               ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]

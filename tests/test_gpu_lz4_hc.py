@@ -1,5 +1,5 @@
 """The LZ4 high-compression class of levels 10-12 (lz4_hc.cuh) held byte for byte to its CPU twin (pytest -m gpu).
-Every stream written by zmt_lz4_compress_level_device must equal oracle/lz4_hc_twin.c's, keep the class's frame layout
+Every stream written by zmt_lz4_compress_level_device must equal oracle/chain_twin.c's, keep the class's frame layout
 (tests/_lz4hc.py:check_structure) and be restored by zmt_lz4_decompress_device, LZ4MT_decompressDCtx, the oracle and,
 when oracle/_ref exists, liblz4 (T=1 and T>1).  Inputs are built here with fixed seeds; each edge case asserts from the
 parsed stream that it reached its edge."""

@@ -1,6 +1,6 @@
 """The zstd search class of levels 6-12 (zstd_lazy.cuh) held block by block to its rule (pytest -m gpu).  Every frame
 written by zmt_zstd_compress_level_device is traced by the oracle (orc_zstd_trace) and checked:
-  - every compressed block's sequences equal the CPU twin's (oracle/zstd_lazy_twin.c) for that block, offsets explicit;
+  - every compressed block's sequences equal the CPU twin's (oracle/chain_twin.c) for that block, offsets explicit;
   - blocks are raw or compressed, 16 KiB (the chunk's last one may be short), predefined modes, own Huffman tree;
   - every raw block is raw for a reason: on the twin's parse, an upper bound of its compressed size is at least its
     content, or a lower bound of its sequence bits overflows the entropy stage's bit buffer;

@@ -1,4 +1,4 @@
-"""The CPU twin of the LZ4 level 10-12 class (oracle/lz4_hc_twin.c) against the rule restated in Python
+"""The CPU twin of the LZ4 level 10-12 class (oracle/chain_twin.c) against the rule restated in Python
 (tests/_lz4hc.py), the frames it writes, and the LZ4 level table of LZ4MT_createCCtx.  No GPU involved."""
 import os
 import subprocess

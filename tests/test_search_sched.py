@@ -59,8 +59,9 @@ def test_every_named_event_is_reached():
 
 
 def test_model_constants_and_capacities_match_the_kernels():
-    """The model's long-job threshold is the kernels' C_LONGLIT, and the dense case's bounds fit L4H_MAXSEQ and
-    L4H_MAXLONG as lz4_hc.cuh defines them."""
+    """The model's range and quarter are the kernels' ZL_RANGE and L4H_Q, its long-job threshold is their C_LONGLIT,
+    and the dense case's bounds fit L4H_MAXSEQ and L4H_MAXLONG as lz4_hc.cuh defines them."""
+    assert (ss.RANGE, ss.QUARTER) == (sc.kernel_constant("ZL_RANGE", ("zstd_lazy.cuh",)), sc.kernel_constant("L4H_Q"))
     assert ss.LONGLIT == sc.kernel_constant("C_LONGLIT")
     assert (sc.MAXSEQ, sc.MAXLONG) == (ss.QUARTER // 4 + 2, ss.QUARTER // 33 + ss.QUARTER // 1290 + 8)
 

@@ -1,4 +1,4 @@
-"""The CPU twin of the zstd level 6-12 search class (oracle/zstd_lazy_twin.c) against the rule restated in Python
+"""The CPU twin of the zstd level 6-12 search class (oracle/chain_twin.c) against the rule restated in Python
 (tests/_zlazy.py), and the level table of ZSTDCB_createCCtx.  No GPU involved."""
 import os
 import subprocess

@@ -4,8 +4,9 @@
   zstdmt_b200/libzmt_datagen.so   synthetic input generator (harness/datagen.c)     [bench / test harness, no dependencies]
   zstdmt_b200/libzmt_memio.so     in-memory fn_read / fn_write drivers of the C-ABI [bench / test harness, links the product]
   oracle/liboracle.so             CPU restatement                                  [test infrastructure]
-  oracle/libzlazy_twin.so         CPU twin of the zstd level 6-12 search class     [test infrastructure]
-  oracle/liblz4hc_twin.so         CPU twin of the LZ4 level 10-12 class            [test infrastructure]
+  oracle/libchain_twin.so         CPU twin of the chain-search encoders            [test infrastructure]
+  oracle/libzlazy_twin.so,        links to libchain_twin.so under the per-class names that test trees and tools
+  oracle/liblz4hc_twin.so           load the zstd level 6-12 and LZ4 level 10-12 twins by
   oracle/_ref/libzstdmt_ref.so    unmodified reference wrapper, only where the reference tree exists (oracle/Makefile REF)
 """
 import os
@@ -19,8 +20,8 @@ LIB = os.path.join(HERE, "libzstdmt_b200.so")
 HSRC = os.path.join(HERE, "harness")
 LIB_GEN = os.path.join(HERE, "libzmt_datagen.so")
 LIB_MEMIO = os.path.join(HERE, "libzmt_memio.so")
-LIB_ZLAZY = os.path.join(ROOT, "oracle", "libzlazy_twin.so")
-LIB_L4HC = os.path.join(ROOT, "oracle", "liblz4hc_twin.so")
+LIB_TWIN = os.path.join(ROOT, "oracle", "libchain_twin.so")
+LIB_TWIN_NAMES = [os.path.join(ROOT, "oracle", f) for f in ("libzlazy_twin.so", "liblz4hc_twin.so")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -90,18 +91,18 @@ def build_oracle(force=False):
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("oracle build failed")
-    # CPU twin of the zstd level 6-12 search class (shares its rule header with the kernels)
-    src, rule = os.path.join(ROOT, "oracle", "zstd_lazy_twin.c"), os.path.join(CSRC, "zstd_lazy_rule.h")
-    if force or _stale(LIB_ZLAZY, [src, rule]):
-        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_ZLAZY, src], cwd=ROOT, capture_output=True, text=True)
+    # CPU twin of the zstd level 6-12 and LZ4 level 10-12 classes (shares their rule headers with the kernels)
+    src, rules = os.path.join(ROOT, "oracle", "chain_twin.c"), [os.path.join(CSRC, f) for f in ("lz4_hc_rule.h", "zstd_lazy_rule.h")]
+    if force or _stale(LIB_TWIN, [src] + rules):
+        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_TWIN, src], cwd=ROOT, capture_output=True, text=True)
         if r.returncode != 0:
-            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/libzlazy_twin.so")
-    # CPU twin of the LZ4 level 10-12 class (its rule header includes the zstd one)
-    src, rules = os.path.join(ROOT, "oracle", "lz4_hc_twin.c"), [os.path.join(CSRC, f) for f in ("lz4_hc_rule.h", "zstd_lazy_rule.h")]
-    if force or _stale(LIB_L4HC, [src] + rules):
-        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_L4HC, src], cwd=ROOT, capture_output=True, text=True)
-        if r.returncode != 0:
-            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/liblz4hc_twin.so")
+            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building oracle/libchain_twin.so")
+    for name in LIB_TWIN_NAMES:
+        target = os.path.basename(LIB_TWIN)
+        if not (os.path.islink(name) and os.readlink(name) == target):
+            tmp = name + ".tmp.%d" % os.getpid()
+            os.symlink(target, tmp)
+            os.replace(tmp, name)
 
 
 def build_cli():

@@ -1,13 +1,12 @@
 // lz4_hc.cuh — the LZ4 high-compression class of levels 10-12: hash chains over the whole chunk, a lazy parse and
-// linked 64 KiB blocks (rule: lz4_hc_rule.h; CPU twin: oracle/lz4_hc_twin.c).  Included by lz4_kernels.cu after
+// linked 64 KiB blocks (rule: lz4_hc_rule.h; CPU twin: oracle/chain_twin.c).  Included by lz4_kernels.cu after
 // zstd_lazy.cuh, whose hash, sort, prev[] and search kernels it runs with the LZ4 block and margins; the block kernel
 // below writes the same per-block slots as lz4_blocks_pipe_kernel, so the LZ4 frame kernels take it from there.
 //
 //   lz4_hc_blocks_kernel  one CTA per 64 KiB LZ4 block.  The block is parsed in four 16 KiB quarters, in order, each by
-//                         the range scheme of zstd_lazy_blocks_kernel (nx[] / ex[] over 64-position ranges, chained
-//                         entries, fold flags); the parse position is carried from one quarter into the next.  Each
-//                         quarter's sequences are sized, scanned and written with c_emit_seq; the last one stays open,
-//                         since a match of the next quarter may still fold into it.
+//                         the range parse of zstd_lazy.cuh; the parse position is carried from one quarter into the
+//                         next.  Each quarter's sequences are sized, scanned and written with c_emit_seq; the last one
+//                         stays open, since a match of the next quarter may still fold into it.
 #pragma once
 #include "lz4_hc_rule.h"
 
@@ -17,11 +16,10 @@
 
 struct L4hLong { uint32_t longl[2 * L4H_MAXLONG]; };         // c_emit_seq's job list
 
+static_assert(L4H_Q == ZL_BLOCK, "a quarter is the parse unit of zstd_lazy.cuh");
+
 struct __align__(16) L4hSmem {
-    uint16_t nx[ZL_PAD(L4H_Q)];           // next free position of the parse from p (quarter-relative)
-    uint16_t ex[ZL_PAD(L4H_Q)];           // first position at or past the end of p's range that the parse reaches from p
-    uint16_t entry[256];                  // first position of the true parse in each range (0xFFFF: none)
-    uint32_t fold[256];                   // the range's entry match folds into the sequence before it
+    ZlParse  P;                           // the parse of the current quarter (quarter-relative positions)
     uint32_t sq[L4H_MAXSEQ];              // sequence: match start (block-relative) | offset << 16
     uint32_t sl[L4H_MAXSEQ];              //           merged match length
     L4hLong  K;
@@ -58,76 +56,30 @@ lz4_hc_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t
         for (uint32_t q0 = 0; q0 < n; q0 += L4H_Q) {
             const uint32_t nb = n - q0 < L4H_Q ? n - q0 : L4H_Q;
             const uint32_t* qb = bb + q0;
-            for (uint32_t p = tid; p < nb; p += NT) {
-                const uint32_t m = qb[p];
-                uint32_t x = p + 1;
-                if (m && !l4h_defer(m, qb[p + 1], qb[p + 2], lazy)) x = p + l4h_len(m);   // a match implies p + 12 <= n
-                S.nx[ZL_PAD(p)] = (uint16_t)x;
-            }
-            S.entry[tid] = 0xFFFF; S.fold[tid] = 0;
+            zl_parse_nx<l4h_defer>(S.P, qb, nb, lazy);
             CTA_SYNC();
             const uint32_t r0 = tid * ZL_RANGE, r1 = r0 + ZL_RANGE < nb ? r0 + ZL_RANGE : nb;
-            for (uint32_t p = r1; p > r0;) { p--; const uint32_t x = S.nx[ZL_PAD(p)]; S.ex[ZL_PAD(p)] = (uint16_t)(x >= r1 ? x : S.ex[ZL_PAD(x)]); }
+            zl_parse_ex(S.P, r0, r1);
             CTA_SYNC();
             if (tid == 0) {
-                uint32_t p = pos - q0;                   // < nb: a carried position ends a match, so it is <= n - 5
-                if (open && S.nx[ZL_PAD(p)] != p + 1 && (S.sq[0] & 0xFFFFu) + S.sl[0] == pos && (S.sq[0] >> 16) == (qb[p] >> ZL_LEN_BITS))
-                    S.fold[p / ZL_RANGE] = 1;            // the entry match continues the sequence left open
-                for (; p < nb; p = S.ex[ZL_PAD(p)]) S.entry[p / ZL_RANGE] = (uint16_t)p;
-                S.pos = q0 + p;
+                const uint32_t p = pos - q0;             // < nb: a carried position ends a match, so it is <= n - 5
+                if (open && S.P.nx[ZL_PAD(p)] != p + 1 && (S.sq[0] & 0xFFFFu) + S.sl[0] == pos && (S.sq[0] >> 16) == zl_off(qb[p]))
+                    S.P.fold[p / ZL_RANGE] = 1;          // the entry match continues the sequence left open
+                S.pos = q0 + zl_parse_entries(S.P, p, nb);
             }
             CTA_SYNC();
-
-            // ---- walk 1: new sequences of the range; flag a fold at the next range's entry
-            const uint32_t e = S.entry[tid];
-            uint32_t nseq = 0;
-            bool ematch = false;
-            if (e != 0xFFFFu) {
-                uint32_t poff = 0;
-                for (uint32_t p = e; p < r1;) {
-                    const uint32_t x = S.nx[ZL_PAD(p)];
-                    if (x == p + 1) poff = 0;
-                    else {
-                        const uint32_t off = qb[p] >> ZL_LEN_BITS;
-                        if (p == e) ematch = true;
-                        if (off != poff) nseq++;
-                        poff = off;
-                        if (x >= r1 && x < nb && S.nx[ZL_PAD(x)] != x + 1 && (qb[x] >> ZL_LEN_BITS) == off) S.fold[x / ZL_RANGE] = 1;
-                    }
-                    p = x;
-                }
-            }
+            const uint32_t e = S.P.entry[tid];
+            const ZlCount c = zl_parse_count(S.P, qb, e, r1, nb);
             pos = S.pos;
             CTA_SYNC();
-            const bool efold = ematch && S.fold[tid];
-            if (efold) nseq--;
+            const bool efold = c.ematch && S.P.fold[tid];
             uint32_t tot;
-            const uint32_t pre = open + block_exscan(nseq, S.scanws, &tot);
-
-            // ---- walk 2: write the sequences (a fold at the entry, and folds before the range's first new sequence, go
-            // to the sequence of an earlier range or quarter: added once its owner has written it)
-            uint32_t si = pre, carry = 0;
-            if (e != 0xFFFFu) {
-                uint32_t poff = 0, qs = 0, ql = 0;
-                bool own = false;
-                for (uint32_t p = e; p < r1;) {
-                    const uint32_t x = S.nx[ZL_PAD(p)];
-                    if (x == p + 1) poff = 0;
-                    else {
-                        const uint32_t off = qb[p] >> ZL_LEN_BITS, len = x - p;
-                        if (p == e ? efold : off == poff) { if (own) ql += len; else carry += len; }
-                        else {
-                            if (own) { S.sq[si] = qs; S.sl[si] = ql; si++; }
-                            qs = (q0 + p) | (off << 16); ql = len; own = true;
-                        }
-                        poff = off;
-                    }
-                    p = x;
-                }
-                if (own) { S.sq[si] = qs; S.sl[si] = ql; }
-            }
+            const uint32_t pre = open + block_exscan(c.nseq - efold, S.scanws, &tot);
+            const uint32_t carry = zl_parse_emit(S.P, qb, e, r1, efold, pre, 0,
+                [&] (uint32_t si, uint32_t st, uint32_t, uint32_t off, uint32_t len) { S.sq[si] = (q0 + st) | (off << 16); S.sl[si] = len; },
+                [] (uint32_t) {});
             CTA_SYNC();
-            if (carry) atomicAdd(&S.sl[pre - 1], carry);
+            if (carry) atomicAdd(&S.sl[pre - 1], carry);     // a fold into the sequence of an earlier range or quarter
             CTA_SYNC();
 
             // ---- emit every sequence but the last, which stays open unless this is the block's last quarter

@@ -1,6 +1,6 @@
 /* lz4_hc_rule.h — the parse rule of the LZ4 high-compression class for levels 10-12.
  *
- * One definition shared by the GPU pipeline (lz4_hc.cuh) and its CPU twin (oracle/lz4_hc_twin.c); plain C so both
+ * One definition shared by the GPU pipeline (lz4_hc.cuh) and its CPU twin (oracle/chain_twin.c); plain C so both
  * compilers take it.  The rule, per chunk (= one LZ4F frame with linked 64 KiB blocks, FLG 0x4C, 0x44 when empty):
  *   blocks  : 64 KiB, the chunk's last one may be short; the parse of each block starts at its first byte.  A match
  *             starts at p only if p + 12 <= blockEnd (MFLIMIT) and ends at or before blockEnd - 5 (LASTLITERALS), so a
@@ -42,14 +42,12 @@ ZL_HD L4hParams l4h_params(int level)
     return p;
 }
 
-/* best[] packs length | offset << ZL_LEN_BITS, as in the zstd class */
-ZL_HD uint32_t l4h_len(uint32_t m) { return m & ((1u << ZL_LEN_BITS) - 1); }
-
-/* the lazy decision at a free position whose match is m (nonzero): 1 = emit a literal, 0 = take m */
+/* the lazy decision at a free position whose match is m (nonzero; best[] packed as in the zstd class): 1 = emit a
+ * literal, 0 = take m */
 ZL_HD int l4h_defer(uint32_t m, uint32_t m1, uint32_t m2, uint32_t lazy)
 {
-    const uint32_t l = l4h_len(m);
-    return l4h_len(m1) > l + 1 || (lazy >= 2 && l4h_len(m2) > l + 2);
+    const uint32_t l = zl_len(m);
+    return zl_len(m1) > l + 1 || (lazy >= 2 && zl_len(m2) > l + 2);
 }
 
 #endif

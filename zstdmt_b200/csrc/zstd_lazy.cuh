@@ -1,5 +1,5 @@
 // zstd_lazy.cuh — the zstd search class of levels 6-12: hash chains over the whole chunk and a lazy parse
-// (rule: zstd_lazy_rule.h; CPU twin: oracle/zstd_lazy_twin.c).  Included by lz4_kernels.cu after the level-3 encoder;
+// (rule: zstd_lazy_rule.h; CPU twin: oracle/chain_twin.c).  Included by lz4_kernels.cu after the level-3 encoder;
 // it feeds the same entropy stage (z_encode_block) and the same frame kernels.
 //
 // Per group of chunks (at most ZL_GROUP_BYTES of positions, so the per-position arrays stay bounded):
@@ -91,15 +91,104 @@ zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint3
     best[i] = res;
 }
 
+// ---- the parallel lazy parse of one 16 KiB unit (a zstd block, or a quarter of an LZ4 block).  The parse is a walk
+// over nx[]: nx[p] = p + 1 (literal) or p + length (match), and nx[p] depends only on best[p .. p+2].  Thread t owns the
+// range [64 t, 64 t + 64): it resolves ex[] backwards over its range (64 steps), thread 0 chains the ranges' entries
+// (<= 256 dependent loads), then every thread re-walks its range from its true entry twice — to count, then to emit.
+// A match that folds into the sequence before it (literal length 0, same offset) is found by its own range when the
+// two are in one range; a range's entry match is flagged by the range the parse came from.  The kernels call the steps
+// below between their own CTA_SYNC()s and keep their own scans.
+struct ZlParse {
+    uint16_t nx[ZL_PAD(ZL_BLOCK)];        // next free position of the parse from p
+    uint16_t ex[ZL_PAD(ZL_BLOCK)];        // first position at or past the end of p's range that the parse reaches from p
+    uint16_t entry[256];                  // first position of the true parse in each range (0xFFFF: none)
+    uint32_t fold[256];                   // the range's entry match folds into the sequence before it
+};
+
+// nx[] of the unit's nb positions (bb: their best[]) under the class's lazy decision; entry[] and fold[] reset.
+// best[p] != 0 only where p + minMatch <= the block's end (zstd: minMatch >= 4, the block is the unit; LZ4: p + 12 <=
+// the end of its 64 KiB block), so best[p+1] and best[p+2] are read without bounds checks: they lie inside the unit,
+// or for LZ4 inside the same block.
+template <int (*DEFER)(uint32_t, uint32_t, uint32_t, uint32_t)>
+__device__ __forceinline__ void zl_parse_nx(ZlParse& P, const uint32_t* bb, uint32_t nb, uint32_t lazy)
+{
+    for (uint32_t p = threadIdx.x; p < nb; p += 256) {
+        const uint32_t m = bb[p];
+        uint32_t x = p + 1;
+        if (m && !DEFER(m, bb[p + 1], lazy >= 2 ? bb[p + 2] : 0, lazy)) x = p + zl_len(m);
+        P.nx[ZL_PAD(p)] = (uint16_t)x;
+    }
+    P.entry[threadIdx.x] = 0xFFFF; P.fold[threadIdx.x] = 0;
+}
+
+// ex[] over this thread's range [r0, r1)
+__device__ __forceinline__ void zl_parse_ex(ZlParse& P, uint32_t r0, uint32_t r1)
+{
+    for (uint32_t p = r1; p > r0;) { p--; const uint32_t x = P.nx[ZL_PAD(p)]; P.ex[ZL_PAD(p)] = (uint16_t)(x >= r1 ? x : P.ex[ZL_PAD(x)]); }
+}
+
+// thread 0: entry[] of the ranges the parse reaches from p; returns the first position at or past the unit's end
+__device__ __forceinline__ uint32_t zl_parse_entries(ZlParse& P, uint32_t p, uint32_t nb)
+{
+    for (; p < nb; p = P.ex[ZL_PAD(p)]) P.entry[p / ZL_RANGE] = (uint16_t)p;
+    return p;
+}
+
+struct ZlCount { uint32_t nseq, nlit, lend; bool ematch; };
+
+// walk 1 of the range [e, r1) from its entry e (0xFFFF: none, nothing to walk): new sequences, literals, the last
+// match end, whether the entry is a match; flags a fold at the next range's entry
+__device__ __forceinline__ ZlCount zl_parse_count(ZlParse& P, const uint32_t* bb, uint32_t e, uint32_t r1, uint32_t nb)
+{
+    ZlCount c = {0, 0, 0, false};
+    uint32_t poff = 0;
+    for (uint32_t p = e; p < r1;) {
+        const uint32_t x = P.nx[ZL_PAD(p)];
+        if (x == p + 1) { c.nlit++; poff = 0; }
+        else {
+            const uint32_t off = zl_off(bb[p]);
+            if (p == e) c.ematch = true;
+            if (off != poff) c.nseq++;
+            poff = off; c.lend = x;
+            if (x >= r1 && x < nb && P.nx[ZL_PAD(x)] != x + 1 && zl_off(bb[x]) == off) P.fold[x / ZL_RANGE] = 1;
+        }
+        p = x;
+    }
+    return c;
+}
+
+// walk 2: put(si, start, anchor, off, merged length) for each sequence the range opens, numbered from si; lit(p) for
+// each literal; anchor: the end of the last match before the range.  A fold at the entry (efold), and folds before the
+// range's first new sequence, belong to the sequence of an earlier range: their length is returned, for the caller to
+// add once that sequence's owner has written it.
+template <class Put, class Lit>
+__device__ __forceinline__ uint32_t zl_parse_emit(const ZlParse& P, const uint32_t* bb, uint32_t e, uint32_t r1, bool efold,
+                                                  uint32_t si, uint32_t anchor, Put put, Lit lit)
+{
+    uint32_t poff = 0, carry = 0, qs = 0, qa = 0, qo = 0, ql = 0;
+    bool open = false;
+    for (uint32_t p = e; p < r1;) {
+        const uint32_t x = P.nx[ZL_PAD(p)];
+        if (x == p + 1) { lit(p); poff = 0; }
+        else {
+            const uint32_t off = zl_off(bb[p]), len = x - p;
+            if (p == e ? efold : off == poff) { if (open) ql += len; else carry += len; }
+            else {
+                if (open) put(si++, qs, qa, qo, ql);
+                qs = p; qa = anchor; qo = off; ql = len; open = true;
+            }
+            poff = off; anchor = x;
+        }
+        p = x;
+    }
+    if (open) put(si, qs, qa, qo, ql);
+    return carry;
+}
+
 struct __align__(16) ZlSmem {
     uint8_t blk[ZL_BLOCK];                        // the block (literals and the raw fallback)
     union {
-        struct {
-            uint16_t nx[ZL_PAD(ZL_BLOCK)];        // next free position of the parse from p
-            uint16_t ex[ZL_PAD(ZL_BLOCK)];        // first position at or past the end of p's range that the parse reaches from p
-            uint16_t entry[256];                  // first position of the true parse in each range (0xFFFF: none)
-            uint32_t fold[256];                   // the range's entry match folds into the sequence before it
-        } p;
+        ZlParse p;
         ZEnt ent;
     };
     ZFseShared fse;
@@ -123,12 +212,7 @@ __device__ __forceinline__ uint32_t zl_block_exmax(uint32_t v, uint32_t* ws)
     return ex;
 }
 
-// The lazy parse of one 16 KiB block is a walk over nx[]: nx[p] = p + 1 (literal) or p + length (match), and nx[p]
-// depends only on best[p .. p+2].  Thread t owns the range [64 t, 64 t + 64): it resolves ex[] backwards over its range
-// (64 steps), thread 0 chains the ranges' entries (<= 256 dependent loads), then every thread re-walks its range from
-// its true entry twice — to count, then to emit.  A match that folds into the sequence before it (literal length 0,
-// same offset) is found by its own range when the two are in one range; a range's entry match is flagged by the range
-// the parse came from.
+// Each 16 KiB block: the range parse above, then the sequences and literals to the CTA's ZScratch and z_encode_block.
 __global__ void __launch_bounds__(256, 2)
 zstd_lazy_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
                         uint32_t bpc, uint32_t c0, uint32_t nwin, uint32_t lazy, const uint32_t* __restrict__ best,
@@ -159,73 +243,26 @@ zstd_lazy_blocks_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint3
             const uint32_t* bb = bw + b0;
             CTA_SYNC();                                          // the previous block's entropy stage is done with the union
             for (uint32_t i = tid; i < nb; i += NT) S.blk[i] = src[b0 + i];
-            for (uint32_t p = tid; p < nb; p += NT) {
-                const uint32_t m = bb[p];
-                uint32_t x = p + 1;
-                if (m) {
-                    const int32_t g = zl_gain(m);
-                    const uint32_t m1 = p + 1 < nb ? bb[p + 1] : 0, m2 = (lazy >= 2 && p + 2 < nb) ? bb[p + 2] : 0;
-                    if (!(m1 && zl_gain(m1) > g + 4) && !(m2 && zl_gain(m2) > g + 7)) x = p + (m & ((1u << ZL_LEN_BITS) - 1));
-                }
-                S.p.nx[ZL_PAD(p)] = (uint16_t)x;
-            }
-            S.p.entry[tid] = 0xFFFF; S.p.fold[tid] = 0;
+            zl_parse_nx<zl_defer>(S.p, bb, nb, lazy);
             CTA_SYNC();
             const uint32_t r0 = tid * ZL_RANGE, r1 = r0 + ZL_RANGE < nb ? r0 + ZL_RANGE : nb;
-            for (uint32_t p = r1; p > r0;) { p--; const uint32_t x = S.p.nx[ZL_PAD(p)]; S.p.ex[ZL_PAD(p)] = (uint16_t)(x >= r1 ? x : S.p.ex[ZL_PAD(x)]); }
+            zl_parse_ex(S.p, r0, r1);
             CTA_SYNC();
-            if (tid == 0) for (uint32_t p = 0; p < nb; p = S.p.ex[ZL_PAD(p)]) S.p.entry[p / ZL_RANGE] = (uint16_t)p;
+            if (tid == 0) zl_parse_entries(S.p, 0, nb);
             CTA_SYNC();
-
-            // ---- walk 1: sequences, literals and the last match end of the range; flag a fold at the next range's entry
             const uint32_t e = S.p.entry[tid];
-            uint32_t nseq = 0, nlit = 0, lend = 0;
-            bool ematch = false;
-            if (e != 0xFFFFu) {
-                uint32_t poff = 0;
-                for (uint32_t p = e; p < r1;) {
-                    const uint32_t x = S.p.nx[ZL_PAD(p)];
-                    if (x == p + 1) { nlit++; poff = 0; }
-                    else {
-                        const uint32_t off = bb[p] >> ZL_LEN_BITS;
-                        if (p == e) ematch = true;
-                        if (off != poff) nseq++;
-                        poff = off; lend = x;
-                        if (x >= r1 && x < nb && S.p.nx[ZL_PAD(x)] != x + 1 && (bb[x] >> ZL_LEN_BITS) == off) S.p.fold[x / ZL_RANGE] = 1;
-                    }
-                    p = x;
-                }
-            }
+            const ZlCount c = zl_parse_count(S.p, bb, e, r1, nb);
             CTA_SYNC();
-            const bool efold = ematch && S.p.fold[tid];
-            if (efold) nseq--;
+            const bool efold = c.ematch && S.p.fold[tid];
             uint32_t tot;
-            const uint32_t pre = block_exscan((nseq << 16) | nlit, S.scanws, &tot);
-            const uint32_t anchor0 = zl_block_exmax(lend, S.scanws + 36);
-
-            // ---- walk 2: emit (a fold at the entry, and folds before the range's first new sequence, go to the sequence
-            // of an earlier range: added once the owner has written it)
-            uint32_t si = pre >> 16, li = pre & 0xFFFFu, carry = 0;
-            if (e != 0xFFFFu) {
-                uint32_t poff = 0, anchor = anchor0;
-                bool open = false;
-                ZSeq q = {0, 0, 0};                                  // mlen <= 16 KiB: the merge cannot overflow it
-                for (uint32_t p = e; p < r1;) {
-                    const uint32_t x = S.p.nx[ZL_PAD(p)];
-                    if (x == p + 1) { zs->lit[li++] = S.blk[p]; poff = 0; }
-                    else {
-                        const uint32_t off = bb[p] >> ZL_LEN_BITS, len = x - p;
-                        if (p == e ? efold : off == poff) { if (open) q.mlen += len; else carry += len; }
-                        else {
-                            if (open) zs->seq[si++] = q;
-                            q.litlen = (p - anchor) | ((off >> 16) << 24); q.off = (uint16_t)off; q.mlen = (uint16_t)len; open = true;
-                        }
-                        poff = off; anchor = x;
-                    }
-                    p = x;
-                }
-                if (open) zs->seq[si] = q;
-            }
+            const uint32_t pre = block_exscan(((c.nseq - efold) << 16) | c.nlit, S.scanws, &tot);
+            const uint32_t anchor0 = zl_block_exmax(c.lend, S.scanws + 36);
+            uint32_t li = pre & 0xFFFFu;
+            const uint32_t carry = zl_parse_emit(S.p, bb, e, r1, efold, pre >> 16, anchor0,
+                [&] (uint32_t si, uint32_t st, uint32_t a, uint32_t off, uint32_t len) {   // len <= 16 KiB: fits mlen
+                    zs->seq[si] = ZSeq{(st - a) | ((off >> 16) << 24), (uint16_t)off, (uint16_t)len};
+                },
+                [&] (uint32_t p) { zs->lit[li++] = S.blk[p]; });
             CTA_SYNC();
             if (carry) atomicAdd(reinterpret_cast<uint32_t*>(&zs->seq[(pre >> 16) - 1].off), carry << 16);     // mlen = the word's high half
             CTA_SYNC();

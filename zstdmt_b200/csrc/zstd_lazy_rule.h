@@ -1,6 +1,6 @@
 /* zstd_lazy_rule.h — the parse rule of the zstd search class for levels 6-12 (and 13-22, which use level 12's row).
  *
- * One definition shared by the GPU pipeline (zstd_lazy.cuh) and its CPU twin (oracle/zstd_lazy_twin.c); plain C so
+ * One definition shared by the GPU pipeline (zstd_lazy.cuh) and its CPU twin (oracle/chain_twin.c); plain C so
  * both compilers take it.  The rule, per chunk (= one single-segment frame):
  *   blocks  : 16 KiB zstd blocks, the last one may be short; the parse of each block starts at its first byte and no
  *             match crosses its end.
@@ -60,6 +60,17 @@ ZL_HD uint32_t zl_highbit(uint32_t v)
     return 31 - __builtin_clz(v);
 #endif
 }
-ZL_HD int32_t zl_gain(uint32_t m) { return (int32_t)(4 * (m & ((1u << ZL_LEN_BITS) - 1))) - (int32_t)zl_highbit((m >> ZL_LEN_BITS) + 3); }
+
+/* best[] packs length | offset << ZL_LEN_BITS */
+ZL_HD uint32_t zl_len(uint32_t m) { return m & ((1u << ZL_LEN_BITS) - 1); }
+ZL_HD uint32_t zl_off(uint32_t m) { return m >> ZL_LEN_BITS; }
+ZL_HD int32_t zl_gain(uint32_t m) { return (int32_t)(4 * zl_len(m)) - (int32_t)zl_highbit(zl_off(m) + 3); }
+
+/* the lazy decision at a free position whose match is m (nonzero): 1 = emit a literal, 0 = take m */
+ZL_HD int zl_defer(uint32_t m, uint32_t m1, uint32_t m2, uint32_t lazy)
+{
+    const int32_t g = zl_gain(m);
+    return (m1 && zl_gain(m1) > g + 4) || (lazy >= 2 && m2 && zl_gain(m2) > g + 7);
+}
 
 #endif
