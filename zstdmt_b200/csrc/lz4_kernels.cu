@@ -75,7 +75,8 @@ struct __align__(16) LzStage {
 struct __align__(16) PipeTile {
     uint16_t off[C_TILE];                 // candidate offset per tile position (0 = none)
     uint32_t M[C_TILE / 32];              // has-candidate bits
-    uint32_t V[C_TILE / 32];              // visited-by-own-chain bits
+    uint32_t V[C_TILE / 32];              // visited-by-own-chain bits (chain k writes the 16-bit half k)
+    uint32_t len4[C_TILE / 8];            // L - 4 of the candidate piece at each position a chain walk took, 4 bits each
     uint8_t  min_[C_CHAINS];              // entry position of a chain on the true path, relative to its own segment (< 16)
     uint32_t pathmask[C_CHAINS / 32];     // chains on the true path
     uint32_t k0, e_din, do_parse, pad;    // entry chain, offset of the match open at the entry, tile has work
@@ -96,7 +97,7 @@ struct LzFront {
 struct LzBack {
     uint32_t Sel[C_TILE / 32];            // pieces on the true greedy chain
     uint32_t Cont[C_TILE / 32];           // ... that continue the previous piece's match across a segment boundary
-    uint8_t  len[C_TILE];                 // piece length per selected piece start (written by the marking walk)
+    uint8_t  clen[C_CHAINS];              // per segment: length of the Cont piece at its start (written by the marking walk)
     uint16_t piece[C_MAXPIECE];           // tile-relative start of the r-th selected piece
     union {                               // segprev is read by head detection, before the heads are written
         uint16_t hidx[C_TILE / 4];        // heads: one per sequence, sequences hold a match of >= 4 bytes
@@ -123,15 +124,23 @@ __device__ __forceinline__ uint32_t c_extend(const uint8_t* s, uint32_t p, uint3
 // Walk one speculative chain through the tile.  The greedy parse is evaluated piecewise: a match is cut at
 // the first segment boundary that leaves it >= 4 bytes, and continues ("inside", din = its offset) into the
 // next segment, so no lane ever compares more than 19 bytes per step.  Pieces are merged again at emission.
-//   MODE 0: own segment only (sets V, exit state -> X.xfree/X.xdin)                      X: LzFront
-//   MODE 1: continuation until it merges into another chain or leaves the tile (-> X.link/X.mpos)
-//   MODE 2: re-walk of a chain that is on the true path: marks X.Sel/X.Cont and the piece lengths X.len
-//           (same steps as MODE 0 + 1)                                                    X: LzBack
+// A candidate piece's length L (4..19) depends only on its start q (offset, cut, limit), not on the chain that takes it,
+// so the front end records L - 4 per start in T.len4 and the marking walk reads it back; only a Cont piece, whose
+// length depends on the offset carried in, is measured again there.
+//   MODE 0: own segment only (V bits and T.len4 of its 16 positions as plain stores, exit state -> X.xfree/X.xdin)
+//                                                                                         X: LzFront
+//   MODE 1: continuation until it merges into another chain or leaves the tile (-> X.link/X.mpos; ORs the lengths of
+//           its pieces into T.len4: chains that continue alike take the same pieces, and a position walk 0 took is a
+//           merge, so the only writers that meet write the same nibble)
+//   MODE 2: re-walk of a chain that is on the true path, from where the path enters it: marks X.Sel/X.Cont and the
+//           Cont lengths X.clen.  The own segment's pieces are its V bits from there on (one step), the continuation
+//           takes the steps of MODE 1 with the lengths from T.len4, so only Cont steps compare bytes.     X: LzBack
 template <int MODE, class OUT>
 __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, uint32_t k, uint32_t p, uint32_t din, uint32_t t0, uint32_t limit)
 {
     const uint32_t t1 = t0 + C_TILE;
     uint32_t lk = 0xFFFFFFFFu, mp = 0;
+    uint32_t vb = 0, lo = 0, hi = 0;                 // MODE 0: V bits and len4 words of the own segment
     bool done = false;
     while (!done) {                                  // single exit: the warp reconverges before the next barrier
         if (p >= t1) { lk = C_END; mp = p; done = true; continue; }
@@ -145,11 +154,30 @@ __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, u
             uint32_t cap = p < limit ? limit - p : 0; if (cap > C_SEG) cap = C_SEG;
             const uint32_t E = c_extend(in, p, din, cap);
             if constexpr (MODE == 2) {
-                if (E) { atomicOr(&X.Sel[rel >> 5], 1u << (rel & 31)); atomicOr(&X.Cont[rel >> 5], 1u << (rel & 31)); X.len[rel] = (uint8_t)E; }
+                if (E) { atomicOr(&X.Sel[rel >> 5], 1u << (rel & 31)); atomicOr(&X.Cont[rel >> 5], 1u << (rel & 31)); X.clen[j] = (uint8_t)E; }
             }
             p += E;
             if (E != C_SEG) din = 0;
             continue;
+        }
+        if constexpr (MODE == 2) {
+            if (j == k) {
+                // Free in the own segment: the path entered this chain on its walk-0 trajectory, so walk 0's pieces
+                // from p on are its V bits.  Mark them at once and leave the segment where walk 0 left it.
+                const uint32_t s0 = rel & ~(C_SEG - 1);
+                const uint32_t own = (uint32_t)reinterpret_cast<const uint16_t*>(T.V)[k] & (0xFFFFu << (rel & 15));
+                p = t0 + s0 + C_SEG;                                  // no piece left: free at the segment's end
+                if (own) {
+                    atomicOr(&X.Sel[rel >> 5], own << (rel & 16));
+                    const uint32_t qr = s0 + 31 - __clz(own), q = t0 + qr;
+                    uint32_t B = t0 + s0 + C_SEG;
+                    if (B - q < 4) B += C_SEG;
+                    const uint32_t e = q + 4 + ((T.len4[qr >> 3] >> (4 * (qr & 7))) & 15u);
+                    if (e == B) din = T.off[qr];                      // still inside the match at the boundary
+                    if (e > p) p = e;
+                }
+                continue;
+            }
         }
         if (MODE != 0 && j != k && (rel & (C_SEG - 1)) == 0) { lk = j; mp = p; done = true; continue; }
         uint32_t bits = (T.M[rel >> 5] >> (rel & 16)) & 0xFFFFu;     // this segment's 16 candidate bits
@@ -158,8 +186,7 @@ __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, u
             const uint32_t nx = t0 + (j + 1) * C_SEG;
             if (MODE == 0) { mp = nx; done = true; }
             else if (j + 1 == C_CHAINS) { lk = C_END; mp = t1; done = true; }
-            else if (j != k) { lk = j + 1; mp = nx; done = true; }
-            else p = nx;
+            else { lk = j + 1; mp = nx; done = true; }                 // (MODE 1 and 2 reach here outside their own segment)
             continue;
         }
         const uint32_t qr = (rel & ~15u) + (__ffs(bits) - 1), q = t0 + qr;
@@ -167,14 +194,25 @@ __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, u
         const uint32_t d = T.off[qr];
         uint32_t B = (q & ~(C_SEG - 1)) + C_SEG;                     // cut at the first boundary leaving >= 4 bytes
         if (B - q < 4) B += C_SEG;
-        const uint32_t end = B < limit ? B : limit;
-        const uint32_t L = 4 + c_extend(in, q + 4, d, end - (q + 4));  // first 4 bytes are known equal; q + 4 <= limit always
-        if constexpr (MODE == 2) { atomicOr(&X.Sel[qr >> 5], 1u << (qr & 31)); X.len[qr] = (uint8_t)L; }
-        if constexpr (MODE == 0) atomicOr(&T.V[qr >> 5], 1u << (qr & 31));
+        uint32_t L;
+        if constexpr (MODE == 2) {
+            L = 4 + ((T.len4[qr >> 3] >> (4 * (qr & 7))) & 15u);
+            atomicOr(&X.Sel[qr >> 5], 1u << (qr & 31));
+        } else {
+            const uint32_t end = B < limit ? B : limit;
+            L = 4 + c_extend(in, q + 4, d, end - (q + 4));              // first 4 bytes are known equal; q + 4 <= limit always
+            const uint32_t nib = (L - 4) << (4 * (qr & 7));
+            if constexpr (MODE == 0) { vb |= 1u << (qr & 15); if (qr & 8) hi |= nib; else lo |= nib; }
+            else atomicOr(&T.len4[qr >> 3], nib);
+        }
         p = q + L;
         if (p == B) din = d;                                          // reached the boundary: still inside the match
     }
-    if constexpr (MODE == 0) { X.xfree[k] = mp; X.xdin[k] = (uint16_t)din; }
+    if constexpr (MODE == 0) {
+        reinterpret_cast<uint16_t*>(T.V)[k] = (uint16_t)vb;
+        *reinterpret_cast<uint2*>(&T.len4[2 * k]) = make_uint2(lo, hi);
+        X.xfree[k] = mp; X.xdin[k] = (uint16_t)din;
+    }
     if constexpr (MODE == 1) { X.link[k] = (uint16_t)lk; X.mpos[k] = mp; if (lk == C_END) X.xdin[k] = (uint16_t)din; }
 }
 

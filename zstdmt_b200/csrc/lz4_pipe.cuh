@@ -12,10 +12,12 @@
 // Every phase below is run by one team of P_TEAM threads and takes that team's barrier id: PB_A / PB_B here, 0 in the
 // Zstandard encoder, whose CTA is one team.
 //
-// Shared memory: only what crosses the teams is double-buffered (PipeTile: off, M, V, entry positions, path mask: 9.5 KB
-// per buffer).  Piece lengths do not cross: the front end does not store them, the marking walk of the back end
-// recomputes them for the true-path pieces only (it has the slack), which keeps the 32-bit hash table and its
-// single-pass atomicMax.  (A 16-bit table needs a CAS loop or a two-pass atomicMax per insert, both more instructions.)
+// Shared memory: only what crosses the teams is double-buffered (PipeTile: off, M, V, the 4-bit candidate piece lengths
+// len4, entry positions, path mask: 11.3 KB per buffer).  The chain walks measure every candidate piece once and the
+// marking walk of the back end reads the lengths back, so it compares bytes only for the continuation (Cont) pieces at
+// segment starts, whose length depends on the offset carried in (LzBack::clen, one byte per segment).  That keeps the
+// 32-bit hash table and its single-pass atomicMax within two CTAs per SM.  (A 16-bit table needs a CAS loop or a
+// two-pass atomicMax per insert, both more instructions.)
 #pragma once
 
 #define P_TEAM      256u
@@ -134,14 +136,13 @@ __device__ __forceinline__ void lz_stage(LzStage& St, uint32_t* tab, uint64_t* m
 }
 
 // ---------------------------------------------------------------- front end
-// Candidate rounds of the tile at t0 (4 rounds of 1024 positions): fills T.off and T.M, clears T.V.  Returns, uniform
+// Candidate rounds of the tile at t0 (4 rounds of 1024 positions): fills T.off and T.M.  Returns, uniform
 // over the team, whether the tile has a candidate.  any[2] holds that flag per tile parity b; any[b ^ 1] is cleared in
 // round 0, once every reader of the previous tile's flag is past the round's first barrier.
 template <uint32_t BARID>
 __device__ __forceinline__ bool lz_candidates(const uint8_t* in, uint32_t* tab, PipeTile& T, uint32_t* any, uint32_t b,
                                               uint32_t t0, uint32_t n, uint32_t ttid, uint32_t lane)
 {
-    if (ttid < C_TILE / 32) T.V[ttid] = 0;
     uint32_t anyM = 0;
 #pragma unroll 1
     for (uint32_t r = 0; r < C_TILE / C_ROUND; r++) {
@@ -231,7 +232,11 @@ __device__ __forceinline__ bool lz_chains(const uint8_t* in, PipeTile& T, LzFron
     const uint32_t seg0 = t0 + ttid * C_SEG;
     const bool alive = ttid >= k0;
     if (alive) c_walk<0>(in, T, F, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
-    else F.link[ttid] = (uint16_t)ttid;                 // dead: self link, never reached
+    else {                                               // dead: self link, never reached; no V bits, no pieces
+        F.link[ttid] = (uint16_t)ttid;
+        reinterpret_cast<uint16_t*>(T.V)[ttid] = 0;
+        *reinterpret_cast<uint2*>(&T.len4[2 * ttid]) = make_uint2(0u, 0u);
+    }
     team_sync<BARID>();
     ZMT_PHASE_TEAM(BARID, ttid, 3);
     if (alive) c_walk<1>(in, T, F, ttid, F.xfree[ttid], F.xdin[ttid], t0, limit);
@@ -276,7 +281,13 @@ __device__ __forceinline__ bool lz_chains(const uint8_t* in, PipeTile& T, LzFron
 // pending sequence: the last one found so far; its match may still grow in the next tile, so it is emitted one tile late
 struct LzPending { uint32_t valid, lit, start, off, end; };
 
-// Marks the pieces of the true path (c_walk recomputes their lengths), lists them, and finds the HEADS: piece r starts
+// length of the selected piece at tile position pr: a Cont piece's from the marking walk, any other from the front end
+__device__ __forceinline__ uint32_t lz_piece_len(const PipeTile& T, const LzBack& K, uint32_t pr)
+{
+    return ((K.Cont[pr >> 5] >> (pr & 31)) & 1u) ? K.clen[pr / C_SEG] : 4u + ((T.len4[pr >> 3] >> (4 * (pr & 7))) & 15u);
+}
+
+// Marks the pieces of the true path (c_walk reads their lengths), lists them, and finds the HEADS: piece r starts
 // a sequence unless it continues the previous piece's match -- flagged continuation, or contiguous with the same
 // offset (the effective offset of a flagged piece is that of the nearest unflagged piece before it).  Returns the
 // number of heads nh (0 when nothing is marked); the pending match grows over the pieces before the first head.
@@ -320,7 +331,7 @@ __device__ __forceinline__ uint32_t lz_heads(const uint8_t* in, PipeTile& T, LzB
                 if (r == 0) { pend = pd.valid ? pd.end : 0xFFFFFFFFu; poff = pd.off; }
                 else {
                     const uint32_t pb = K.piece[r - 1];
-                    pend = t0 + pb + K.len[pb];
+                    pend = t0 + pb + lz_piece_len(T, K, pb);
                     if (!((K.Cont[pb >> 5] >> (pb & 31)) & 1)) poff = T.off[pb];
                     else {                      // Cont pieces start at a segment boundary (c_walk cuts there)
                         const uint32_t sp = K.segprev[pb / C_SEG];
@@ -340,9 +351,9 @@ __device__ __forceinline__ uint32_t lz_heads(const uint8_t* in, PipeTile& T, LzB
     }
     team_sync<BARID>();
     const uint32_t lastp = K.piece[np - 1];
-    tile_end = t0 + lastp + K.len[lastp];                     // end of the last piece of this tile
+    tile_end = t0 + lastp + lz_piece_len(T, K, lastp);       // end of the last piece of this tile
     if (nh == 0) pd.end = tile_end;                           // every piece extends the pending sequence
-    else if (pd.valid && K.hidx[0] > 0) { const uint32_t pb = K.piece[K.hidx[0] - 1]; pd.end = t0 + pb + K.len[pb]; }
+    else if (pd.valid && K.hidx[0] > 0) { const uint32_t pb = K.piece[K.hidx[0] - 1]; pd.end = t0 + pb + lz_piece_len(T, K, pb); }
     return nh;
 }
 
@@ -365,9 +376,9 @@ __device__ __forceinline__ LzRun lz_seq_run(const PipeTile& T, const LzBack& K, 
                 const uint32_t h = sidx - pd.valid;          // head index, h <= nh-2
                 const uint32_t pi = K.hidx[h], pr = K.piece[pi];
                 const uint32_t pl = K.piece[K.hidx[h + 1] - 1];
-                st = t0 + pr; of = T.off[pr]; en = t0 + pl + K.len[pl];
+                st = t0 + pr; of = T.off[pr]; en = t0 + pl + lz_piece_len(T, K, pl);
                 if (h == 0) ls = pd.valid ? pd.end : pd.lit;     // pd.lit doubles as "end of everything emitted so far"
-                else { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + K.len[pp]; }
+                else { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + lz_piece_len(T, K, pp); }
             }
             R.lit0[k] = ls; R.lit[k] = st - ls; R.off[k] = of; R.len[k] = en - st; R.cnt++;
         }
@@ -380,7 +391,7 @@ __device__ __forceinline__ void lz_next_pending(const PipeTile& T, const LzBack&
 {
     const uint32_t pi = K.hidx[nh - 1], pr = K.piece[pi];
     uint32_t ls;
-    if (nh >= 2 || pd.valid) { if (pi > 0) { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + K.len[pp]; } else ls = pd.end; }
+    if (nh >= 2 || pd.valid) { if (pi > 0) { const uint32_t pp = K.piece[pi - 1]; ls = t0 + pp + lz_piece_len(T, K, pp); } else ls = pd.end; }
     else ls = pd.lit;                          // first sequence of the block: literals start where emission stands (0)
     pd.valid = 1; pd.lit = ls; pd.start = t0 + pr; pd.off = T.off[pr]; pd.end = tile_end;
 }
