@@ -185,6 +185,72 @@ int      zmt_lz4_decompress_segments_device(const void* d_in, uint64_t in_bytes,
 int      zmt_lz4f_segment_host(const uint8_t* seg, size_t n, size_t start, uint32_t flg, uint32_t bd, size_t max_in, uint64_t max_out,
                                size_t* end, uint64_t* room, uint32_t* last);
 
+/* ---- zstd frames of any size in bounded memory ----
+ * A zstd frame decoded as a chain of segments, each a run of whole blocks (what ZSTD_decompressStream does through two
+ * fixed buffers when the reference streams a plain .zst file, lib/zstd-mt_decompress.c:552-687).  Four kinds of state
+ * cross a cut:
+ *   - the window: matches of a segment may reach up to Window_Size bytes back, into earlier segments;
+ *   - the repeat offsets;
+ *   - the tables a block may inherit (treeless literals, Repeat_Mode sequence tables): the block that last described the
+ *     Huffman tree and the last FSE / RLE describer of each of the LL, OF and ML tables — at most four blocks;
+ *   - the XXH64 content checksum and the content size.
+ *
+ * zmt_zstd_segment_host walks one segment on the host, resuming where the walk state `w` stands (zero it for a new
+ * frame).  seg[0..n) holds the frame's bytes from frame offset w->pos on, as far as they are known; base_off is where
+ * seg[0] lies in the decoder's input.  The segment runs to the first block boundary at or past seg + max_in, or to where
+ * its blocks reach max_out bytes of room, or to the frame's end, and holds at least one block.  Its descriptors go to
+ * blocks_out[*nblocks_io...] (below max_blocks), scratch from *scratch_used on, as for zmt_zstd_scan_frame_host.  A later
+ * segment first gets one descriptor per table source it carries (zmt_zstd_segment_sources): type 3, no content, never
+ * decoded or executed, named by the blocks that inherit its tables.  Their bytes must lie directly below seg[0] in the
+ * decoder's input, in the order the sources are listed.  On ZMT_ST_OK: *end = the segment's length, *room = the output
+ * room it needs (128 KiB per compressed block), *flags = the ZF bits for d_frame_seq (the dependent-block route is always
+ * set), *last = 1 if it ends the frame (content checksum included), and `w` stands at the next segment.  ZMT_ST_TRUNCATED:
+ * the segment's bytes are not all in seg[0..n) yet (read on); `w` is unchanged then, as on any other error. */
+typedef struct {
+    uint64_t pos;             /* frame offset of the next block header (0: the frame header comes first) */
+    uint64_t content_size;    /* Frame_Content_Size, ~0 without one */
+    uint64_t window;          /* Window_Size (RFC 8878 3.1.1.1.2; Frame_Content_Size for a Single_Segment frame) */
+    uint32_t flags;           /* ZF bits of the frame so far: 1 dependent blocks, 2 content checksum, 4 no content size */
+    uint32_t nblk;            /* blocks of the frame walked so far */
+    uint32_t done;            /* 1: the frame's last block and checksum were walked */
+    uint32_t reserved;
+    /* the four table sources: 0 the Huffman tree, 1-3 the LL / OF / ML tables.  src_off = frame offset of the describing
+     * block's content, src_len = its size; src_off = ~0: none yet, ~1: the predefined table (sequence tables only) */
+    uint64_t src_off[4];
+    uint32_t src_len[4];
+} zmt_zstd_walk;
+int      zmt_zstd_segment_host(const uint8_t* seg, size_t n, uint64_t base_off, uint32_t frame_idx, zmt_zstd_walk* w,
+                               size_t max_in, uint64_t max_out, void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
+                               uint64_t* scratch_used, size_t* end, uint64_t* room, uint32_t* flags, uint32_t* last);
+/* The table sources a segment starting at `w` carries: distinct describing blocks in frame order, off[i] / len[i] (frame
+ * offset and size of block i's content, at most four).  Returns their count; their bytes, back to back, are the carry
+ * area below the segment. */
+uint32_t zmt_zstd_segment_sources(const zmt_zstd_walk* w, uint64_t* off, uint32_t* len);
+/* Decoding: the arguments of zmt_zstd_decompress_device, every frame of the batch a segment.  d_seg[f] carries frame f's
+ * state: the caller zeroes it before the first segment and sets `flags` and `history` for every segment; the device
+ * owns the other fields.  Segment f's content goes to d_out + d_out_off[f]; the last `history` bytes the frame decoded so
+ * far (min(Window_Size, produced)) must lie directly below, in place before the call.  d_expect[f] of a first segment is
+ * the frame's content size (~0 without one), kept in the record; a later segment's entry is not read.  d_frame_seq[f]
+ * must carry the dependent-block bit (zmt_zstd_segment_host sets it).  Every segment seeds the repeat offsets from the
+ * record and stores them back, and folds its content into the running XXH64; the content size and the content checksum
+ * are checked on the last segment.  d_out_size[f] is the segment's decoded size.  A segment with FIRST | LAST is a whole
+ * frame. */
+typedef struct {
+    uint64_t history;         /* in: decoded bytes of the frame directly below d_out + d_out_off[f] (0 for the first segment) */
+    uint64_t produced;        /* device: content bytes of the frame's segments so far */
+    uint64_t content_size;    /* device: the header's content size, ~0 without one */
+    uint32_t flags;           /* in: ZMT_SEG_* */
+    uint32_t rep[3];          /* device: the repeat offsets behind the segments so far */
+    uint64_t acc[4];          /* device: XXH64 accumulators */
+    uint32_t pending_len;     /* device: bytes in pending[] */
+    uint32_t reserved;
+    uint8_t  pending[32];     /* device: content bytes not yet folded into acc[] */
+} zmt_zstd_segment;
+int      zmt_zstd_decompress_segments_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                             const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out,
+                                             const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* d_seg,
+                                             void* d_work, void* stream);
+
 /* ---- multi-GPU: one LZ4MT_* / ZSTDCB_* call deals its batches round-robin over the devices named by the
  * environment variable ZSTDMT_GPUS ("all" or "0,1,..."; default: the calling thread's current device) and re-serialises
  * the frames on the host.  zmt_device_batches(dev) = batches submitted to that device since the library was loaded. */

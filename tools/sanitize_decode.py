@@ -1,5 +1,6 @@
 """Small decode workloads for compute-sanitizer (memcheck / racecheck): LZ4 own + reference-framed (linked) streams, zstd own +
-libzstd-framed streams, through the device API and the callback API.  python tools/sanitize_decode.py [MiB]"""
+libzstd-framed streams, through the device API and the callback API; a libzstd frame decoded as segments through the device
+API and through the callback API in 1 MiB batches.  python tools/sanitize_decode.py [MiB]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -33,3 +34,15 @@ for codec, fr in ((z.CODEC_LZ4, rf), (z.CODEC_ZSTD, zrf)):
     rc, back, st = z.decompress_mem(codec, fr, n + 16, threads=4)
     assert rc == 0 and np.array_equal(back, src)
 print("callback API ok")
+# zstd segments: a libzstd frame (level 3, content checksum, no content size) cut at block boundaries, then as a plain
+# stream in 1 MiB batches
+from test_gpu_plain_streams import zstd_adv
+from test_zstd_frame_segments import header_walk
+zf1 = zstd_adv(src, 3, checksum=1, pieces=[n // 2, n - n // 2])
+cuts = [a + k for a, k, _ in header_walk(zf1)["blocks"]][:-1]
+back, st = z.zstd_decode_segments(zf1, cuts[:: max(1, len(cuts) // 6)])
+assert st == 0 and np.array_equal(back, src)
+os.environ["ZSTDMT_B200_PLAIN_MB"] = "1"
+rc, back, st = z.decompress_mem(z.CODEC_ZSTD, zf1, n + 16, threads=4, inputsize=1 << 20)
+assert rc == 0 and np.array_equal(back, src)
+print("zstd segments ok")

@@ -82,6 +82,13 @@ def lib():
     L.zmt_lz4_decompress_segments_device.argtypes = [c_vp, c_u64, c_vp, c_vp, c_u32, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.zmt_lz4f_segment_host.restype = ctypes.c_int
     L.zmt_lz4f_segment_host.argtypes = [c_vp, c_sz, c_sz, c_u32, c_u32, c_sz, c_u64, ctypes.POINTER(c_sz), ctypes.POINTER(c_u64), ctypes.POINTER(c_u32)]
+    L.zmt_zstd_decompress_segments_device.restype = ctypes.c_int
+    L.zmt_zstd_decompress_segments_device.argtypes = [c_vp, c_vp, c_u32, c_vp, c_vp, c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_segment_host.restype = ctypes.c_int
+    L.zmt_zstd_segment_host.argtypes = [c_vp, c_sz, c_u64, c_u32, ctypes.POINTER(ZstdWalk), c_sz, c_u64, c_vp, ctypes.POINTER(c_u32), c_u32,
+                                        ctypes.POINTER(c_u64), ctypes.POINTER(c_sz), ctypes.POINTER(c_u64), ctypes.POINTER(c_u32), ctypes.POINTER(c_u32)]
+    L.zmt_zstd_segment_sources.restype = c_u32
+    L.zmt_zstd_segment_sources.argtypes = [ctypes.POINTER(ZstdWalk), ctypes.POINTER(c_u64), ctypes.POINTER(c_u32)]
     L.zmt_index_workspace_bytes.restype = c_sz; L.zmt_index_workspace_bytes.argtypes = [c_u32]
     L.zmt_lz4_index_device.restype = ctypes.c_int
     L.zmt_lz4_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
@@ -410,6 +417,96 @@ def lz4_decode_segments(frame, cuts, device="cuda"):
         n = int(osz.item())
         parts.append(out[H:H + n].cpu().numpy())
         hist = torch.cat([hist, out[H:H + n]])[-H:].clone()
+        prev = end
+    return np.concatenate(parts) if parts else np.zeros(0, np.uint8), 0
+
+
+class ZstdWalk(ctypes.Structure):
+    """zmt_zstd_walk (include/zstdmt_b200_dev.h): where the segment walk of a zstd frame stands, and the frame's table sources."""
+    _fields_ = [("pos", c_u64), ("content_size", c_u64), ("window", c_u64), ("flags", c_u32), ("nblk", c_u32), ("done", c_u32),
+                ("reserved", c_u32), ("src_off", c_u64 * 4), ("src_len", c_u32 * 4)]
+
+
+class ZstdSegment(ctypes.Structure):
+    """zmt_zstd_segment (include/zstdmt_b200_dev.h): the device state of a zstd frame decoded as a chain of segments."""
+    _fields_ = [("history", c_u64), ("produced", c_u64), ("content_size", c_u64), ("flags", c_u32), ("rep", c_u32 * 3),
+                ("acc", c_u64 * 4), ("pending_len", c_u32), ("reserved", c_u32), ("pending", ctypes.c_uint8 * 32)]
+
+
+def zstd_segment_sources(walk):
+    """zmt_zstd_segment_sources: [(frame offset, length)] of the table sources a segment starting at `walk` carries."""
+    off, ln = (c_u64 * 4)(), (c_u32 * 4)()
+    k = lib().zmt_zstd_segment_sources(ctypes.byref(walk), off, ln)
+    return [(int(off[i]), int(ln[i])) for i in range(k)]
+
+
+def zstd_segment(seg_bytes, walk, max_in, max_out, base_off=0, frame_idx=0):
+    """zmt_zstd_segment_host on the frame's bytes from walk.pos on: (status, end, room, flags, last, descriptors).  `walk`
+    (a ZstdWalk) advances on success.  descriptors: the segment's block descriptors as bytes (zmt_zstd_blk_desc_bytes()
+    each), the carried table sources first; seg_bytes[0] lies at base_off in the decoder input, the carry area below."""
+    L = lib()
+    b = np.ascontiguousarray(seg_bytes, dtype=np.uint8)
+    dsz = L.zmt_zstd_blk_desc_bytes()
+    cap = int(min(b.size, max_in + (1 << 17)) // 3 + 16)
+    while True:
+        out = np.zeros(cap * dsz, np.uint8)
+        nb, scr, end, room, flags, last = c_u32(0), c_u64(0), c_sz(0), c_u64(0), c_u32(0), c_u32(0)
+        rc = L.zmt_zstd_segment_host(b.ctypes.data, b.size, base_off, frame_idx, ctypes.byref(walk), max_in, max_out, out.ctypes.data,
+                                     ctypes.byref(nb), cap, ctypes.byref(scr), ctypes.byref(end), ctypes.byref(room), ctypes.byref(flags),
+                                     ctypes.byref(last))
+        if rc != 6:                                          # ZMT_ST_DST_SMALL: a larger table
+            return rc, end.value, room.value, flags.value, last.value, out[: nb.value * dsz], scr.value
+        cap *= 2
+
+
+def zstd_decode_segments(frame, cuts, device="cuda"):
+    """Decodes one zstd frame (host bytes) through zmt_zstd_decompress_segments_device as the chain of segments that ends
+    at the frame offsets `cuts` (block boundaries, increasing; the frame's length is appended).  Each segment's input is
+    its carried table sources followed by its bytes; its output goes above the frame's last min(Window_Size, produced)
+    content bytes, copied below it first.  Returns (content, status): the decoded bytes (numpy) and the ZMT_ST_* of the
+    first failing segment, or 0."""
+    torch = _torch(); L = lib()
+    fb = np.ascontiguousarray(frame, dtype=np.uint8)
+    seg = torch.zeros(ctypes.sizeof(ZstdSegment), dtype=torch.uint8, device=device)
+    w = ZstdWalk()
+    ends = [int(c) for c in cuts] + [fb.size]
+    parts, prev, hist = [], 0, torch.zeros(0, dtype=torch.uint8, device=device)
+    for k, end in enumerate(ends):
+        first, last = k == 0, k == len(ends) - 1
+        carry = b"".join(fb[o:o + n].tobytes() for o, n in zstd_segment_sources(w))
+        rc, e2, room, flags, is_last, blk, scr = zstd_segment(fb[prev:], w, end - prev, 1 << 62, base_off=len(carry))
+        if rc != 0 or e2 != end - prev or bool(is_last) != last:
+            raise ValueError("cut %d is not a block boundary (walk: rc %d end %d last %d)" % (end, rc, prev + e2, is_last))
+        nblk = blk.size // L.zmt_zstd_blk_desc_bytes()
+        d_in = torch.zeros(len(carry) + (end - prev) + 256, dtype=torch.uint8, device=device)
+        d_in[:len(carry) + end - prev] = torch.from_numpy(np.frombuffer(carry + fb[prev:end].tobytes(), np.uint8).copy()).to(device)
+        H = hist.numel()
+        out = torch.zeros(H + room + 256, dtype=torch.uint8, device=device)
+        if H:
+            out[:H] = hist
+        d_blk = torch.from_numpy(blk.copy()).to(device)
+        first_blk = torch.tensor([0, nblk], dtype=torch.int32, device=device)
+        expect = torch.tensor([-1 if flags & 4 else w.content_size], dtype=torch.int64, device=device) if first else torch.full((1,), -1, dtype=torch.int64, device=device)
+        fseq = torch.tensor([flags], dtype=torch.int32, device=device)
+        ooff = torch.tensor([H, H + room], dtype=torch.int64, device=device)
+        osz = torch.zeros(1, dtype=torch.int64, device=device)
+        st = torch.zeros(1, dtype=torch.int32, device=device)
+        work = torch.empty(L.zmt_zstdd_workspace_bytes(1, nblk, scr), dtype=torch.uint8, device=device)
+        rec = ZstdSegment.from_buffer_copy(bytes(seg.cpu().numpy()))
+        rec.history, rec.flags = H, (SEG_FIRST if first else 0) | (SEG_LAST if last else 0)
+        seg.copy_(torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8))
+        s = torch.cuda.current_stream()
+        rc = L.zmt_zstd_decompress_segments_device(d_in.data_ptr(), d_blk.data_ptr(), nblk, first_blk.data_ptr(), expect.data_ptr(), fseq.data_ptr(), 1,
+                                                   out.data_ptr(), ooff.data_ptr(), osz.data_ptr(), st.data_ptr(), seg.data_ptr(), work.data_ptr(),
+                                                   s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("zmt_zstd_decompress_segments_device failed: %s" % ST_NAMES.get(rc, rc))
+        torch.cuda.synchronize()
+        if int(st.item()) != 0:
+            return np.concatenate(parts) if parts else np.zeros(0, np.uint8), int(st.item())
+        n = int(osz.item())
+        parts.append(out[H:H + n].cpu().numpy())
+        hist = torch.cat([hist, out[H:H + n]])[-w.window:].clone() if w.window else hist[:0]
         prev = end
     return np.concatenate(parts) if parts else np.zeros(0, np.uint8), 0
 

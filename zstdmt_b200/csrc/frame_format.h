@@ -118,52 +118,105 @@ struct ZDSeq { uint32_t ll; uint32_t off; uint32_t ml; uint32_t pad; };
 #define ZF_CHECKSUM  2u     // 4-byte content checksum (low 32 bits of XXH64) follows the last block
 #define ZF_NO_SIZE   4u     // no Frame_Content_Size: the reported size is an upper bound (128 KiB per compressed block)
 
-// Walks one zstd frame in frame[0..n) (frame header + 3-byte block headers + the two section headers of every
-// compressed block).  `base_off` = offset of the frame's first byte in the decoder's input buffer.
-// W = true writes one descriptor per accepted block at blocks_out[*nblocks_io++] (below index max_blocks); W = false
-// only counts them.  Either way *nblocks_io advances by the block count, *scratch_used by the entropy scratch the
-// blocks take (their seq_off / lit_off), *flags receives the ZF_* bits and, on success, *content_size the frame content
-// size (the block bound without a content-size field).  *end = the frame's length on success, else the offset of the
-// header element the walk stopped at.  Bytes behind the frame are the caller's business.  Returns ZMT_ST_*.
-template <bool W>
-ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
-                           uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size,
-                           uint32_t* flags, size_t* end)
+// segments (zmt_zstd_segment_host): a table source carried from an earlier segment.  Only its bytes are used, by the
+// blocks that name it in *_src: regen 0, nseq 0, never decoded or executed.
+#define ZB_SRC 3u
+#define ZW_NONE   (~0ull)       // zmt_zstd_walk::src_off: no describer yet
+#define ZW_PREDEF (~1ull)       // zmt_zstd_walk::src_off: the predefined table
+
+// The table sources a segment starting at w carries: the distinct describing blocks of w->src_off, in frame order.
+ZMT_HD uint32_t zstd_walk_sources(const zmt_zstd_walk* w, uint64_t* off, uint32_t* len)
 {
-    *flags = 0; *end = 0;
-    if (n < 6 || zf_rd32(frame) != ZMT_ZSTD_MAGIC) return n < 6 ? ZMT_ST_TRUNCATED : ZMT_ST_BAD_MAGIC;
-    const uint32_t fhd = frame[4], fcs = fhd >> 6, single = (fhd >> 5) & 1, did = fhd & 3;
-    if (fhd & 0x08) return ZMT_ST_BAD_HEADER;
-    const bool has_chk = (fhd & 0x04) != 0;                          // XXH64 content checksum after the last block (verified on the device)
-    if (did) return ZMT_ST_UNSUPPORTED;                               // dictionaries: not on the reference path
-    size_t pos = 5 + (single ? 0 : 1);
-    const size_t fl = fcs == 0 ? (single ? 1 : 0) : fcs == 1 ? 2 : fcs == 2 ? 4 : 8;
-    if (n < pos + fl) return ZMT_ST_TRUNCATED;
-    uint64_t cs = 0;
-    if (fl == 1) cs = frame[pos]; else if (fl == 2) cs = (uint64_t)(frame[pos] | (frame[pos + 1] << 8)) + 256;
-    else if (fl == 4) cs = zf_rd32(frame + pos); else if (fl == 8) cs = zf_rd64(frame + pos);
-    pos += fl;
-    const bool no_size = fl == 0;                                     // streamed frame: size from the blocks (bound: 128 KiB per compressed block)
-    uint64_t bound = 0;
-    if (has_chk) *flags |= ZF_CHECKSUM;
-    if (no_size) *flags |= ZF_NO_SIZE;
-    bool first = true;
-    uint32_t last_huf = ZB_NONE, cur_src[3] = { ZB_NONE, ZB_NONE, ZB_NONE };     // block that last described the Huffman tree / each sequence table
+    uint32_t k = 0;
+    if (w->pos == 0) return 0;
+    for (uint32_t t = 0; t < 4; t++) {
+        const uint64_t o = w->src_off[t];
+        bool dup = o >= ZW_PREDEF;
+        for (uint32_t i = 0; i < k; i++) dup = dup || off[i] == o;
+        if (dup) continue;
+        uint32_t i = k++;
+        for (; i > 0 && off[i - 1] > o; i--) { off[i] = off[i - 1]; len[i] = len[i - 1]; }
+        off[i] = o; len[i] = w->src_len[t];
+    }
+    return k;
+}
+
+// Walks the blocks of one zstd frame from where *w stands: p[0..n) are the frame's bytes from frame offset w->pos on
+// (w->pos == 0: the frame header comes first and resets *w), `base_off` = where p[0] lies in the decoder's input buffer.
+// Stops at the first block boundary at or past p + pos_stop or where the blocks of this call reach bound_stop bytes of
+// room (after one block at least), or at the frame's end (w->done, content checksum included).  A call that resumes a
+// frame first emits one ZB_SRC descriptor per table source (zstd_walk_sources), whose bytes the caller places directly
+// below p[0], in that order.  W = true writes one descriptor per block at blocks_out[*nblocks_io++] (below index
+// max_blocks); W = false only counts them.  Either way *nblocks_io advances by the descriptor count, *scratch_used by the
+// entropy scratch the blocks take (their seq_off / lit_off), w->flags collects the ZF_* bits, *bound gets the room of
+// the call's blocks (128 KiB per compressed block).  w->pos = the frame offset the walk stopped at: the next block header,
+// the frame's length at its end, or on failure the header element it could not take.  Returns ZMT_ST_*.
+template <bool W>
+ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
+                            uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, zmt_zstd_walk* w,
+                            size_t pos_stop, uint64_t bound_stop, uint64_t* bound)
+{
+    const uint64_t at0 = w->pos;
+    size_t pos = 0;
+    uint64_t bnd = 0;
+    uint32_t walked = 0;
+    *bound = 0;
+    if (at0 == 0) {
+        w->flags = 0; w->nblk = 0; w->done = 0; w->reserved = 0; w->content_size = ZW_NONE; w->window = 0;
+        for (uint32_t t = 0; t < 4; t++) { w->src_off[t] = ZW_NONE; w->src_len[t] = 0; }
+        if (n < 6 || zf_rd32(p) != ZMT_ZSTD_MAGIC) return n < 6 ? ZMT_ST_TRUNCATED : ZMT_ST_BAD_MAGIC;
+        const uint32_t fhd = p[4], fcs = fhd >> 6, single = (fhd >> 5) & 1, did = fhd & 3;
+        if (fhd & 0x08) return ZMT_ST_BAD_HEADER;
+        if (did) return ZMT_ST_UNSUPPORTED;                               // dictionaries: not on the reference path
+        pos = 5 + (single ? 0 : 1);
+        const size_t fl = fcs == 0 ? (single ? 1 : 0) : fcs == 1 ? 2 : fcs == 2 ? 4 : 8;
+        if (n < pos + fl) return ZMT_ST_TRUNCATED;
+        uint64_t cs = 0;
+        if (fl == 1) cs = p[pos]; else if (fl == 2) cs = (uint64_t)(p[pos] | (p[pos + 1] << 8)) + 256;
+        else if (fl == 4) cs = zf_rd32(p + pos); else if (fl == 8) cs = zf_rd64(p + pos);
+        if (single) w->window = cs;                                       // RFC 8878 3.1.1.1.2
+        else { const uint32_t wd = p[5]; const uint64_t wb = 1ull << (10 + (wd >> 3)); w->window = wb + (wb >> 3) * (wd & 7); }
+        pos += fl;
+        if (fhd & 0x04) w->flags |= ZF_CHECKSUM;                         // XXH64 content checksum after the last block (verified on the device)
+        if (fl == 0) w->flags |= ZF_NO_SIZE;                              // streamed frame: size from the blocks (bound: 128 KiB per compressed block)
+        else w->content_size = cs;
+    }
+    // block that describes the Huffman tree / each sequence table in use, as a descriptor index of this call
+    uint32_t cur[4];
+    for (uint32_t t = 0; t < 4; t++) cur[t] = w->src_off[t] == ZW_PREDEF ? ZB_PREDEF : ZB_NONE;
+    if (at0 != 0) {
+        uint64_t so[4]; uint32_t sl[4];
+        const uint32_t ns = zstd_walk_sources(w, so, sl);
+        uint64_t at = base_off;
+        for (uint32_t i = 0; i < ns; i++) at -= sl[i];
+        for (uint32_t i = 0; i < ns; i++) {
+            if (*nblocks_io >= max_blocks) return ZMT_ST_DST_SMALL;
+            ZBlk B = ZBlk();
+            B.frame = frame_idx; B.type = ZB_SRC; B.comp_off = at; B.comp_size = sl[i];
+            B.seq_off = B.lit_off = *scratch_used;
+            B.huf_src = B.ll_src = B.of_src = B.ml_src = ZB_SELF;
+            for (uint32_t t = 0; t < 4; t++) if (w->src_off[t] == so[i]) cur[t] = *nblocks_io;
+            if (W) blocks_out[*nblocks_io] = B;
+            (*nblocks_io)++;
+            at += sl[i];
+        }
+    }
     for (;;) {
-        *end = pos;
+        w->pos = at0 + pos;
+        if (walked && (pos >= pos_stop || bnd >= bound_stop)) { *bound = bnd; return ZMT_ST_OK; }
         if (n - pos < 3) return ZMT_ST_TRUNCATED;
-        const uint32_t bh = frame[pos] | (frame[pos + 1] << 8) | ((uint32_t)frame[pos + 2] << 16); pos += 3;
+        const uint32_t bh = p[pos] | (p[pos + 1] << 8) | ((uint32_t)p[pos + 2] << 16); pos += 3;
         const uint32_t last = bh & 1, type = (bh >> 1) & 3, bs = bh >> 3;
         if (type == 3 || bs > 128 * 1024) return ZMT_ST_BLOCK;
         if (*nblocks_io >= max_blocks) return ZMT_ST_DST_SMALL;
         ZBlk B = ZBlk();                                              // no padding: every byte is zeroed
-        B.frame = frame_idx; B.type = type; B.first = first ? 1 : 0; B.comp_off = base_off + pos;
-        bound += type == ZB_CMP ? 128 * 1024 : bs;
+        B.frame = frame_idx; B.type = type; B.first = w->nblk == 0 ? 1 : 0; B.comp_off = base_off + pos;
+        bnd += type == ZB_CMP ? 128 * 1024 : bs;
         if (type == ZB_RAW) { if (n - pos < bs) return ZMT_ST_TRUNCATED; B.comp_size = bs; B.regen_hint = bs; pos += bs; }
         else if (type == ZB_RLE) { if (n - pos < 1) return ZMT_ST_TRUNCATED; B.comp_size = 1; B.regen_hint = bs; pos += 1; }
         else {
             if (n - pos < bs || bs < 2) return ZMT_ST_TRUNCATED;
-            const uint8_t* s = frame + pos;
+            const uint8_t* s = p + pos;
             const uint32_t b0 = s[0], lt = b0 & 3, sf = (b0 >> 2) & 3;
             uint32_t lregen, lcomp, lhdr;
             if (lt < 2) {
@@ -187,19 +240,21 @@ ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, ui
             // any non-predefined sequence table mode may be followed by Repeat_Mode -> frame-sequential pass
             {
                 const uint32_t used = q0 == 0 ? 1u : q0 < 128 ? 1u : q0 < 255 ? 2u : 3u;
-                if (lt == 3) *flags |= ZF_NEEDS_SEQ;
-                if (nseq && qn > used && q[used] != 0) *flags |= ZF_NEEDS_SEQ;
+                if (lt == 3) w->flags |= ZF_NEEDS_SEQ;
+                if (nseq && qn > used && q[used] != 0) w->flags |= ZF_NEEDS_SEQ;
                 const uint32_t me = *nblocks_io;
                 B.huf_src = ZB_SELF;
-                if (lt == 2) last_huf = me; else if (lt == 3) B.huf_src = last_huf;
+                if (lt == 2) { cur[0] = me; w->src_off[0] = at0 + pos; w->src_len[0] = bs; }
+                else if (lt == 3) B.huf_src = cur[0];
                 B.ll_src = B.of_src = B.ml_src = ZB_SELF;
                 if (nseq && qn > used) {
                     uint32_t src[3];
 #pragma unroll
                     for (uint32_t t = 0; t < 3; t++) {
                         const uint32_t mode = (q[used] >> (6 - 2 * t)) & 3;
-                        if (mode == 0) cur_src[t] = ZB_PREDEF; else if (mode != 3) cur_src[t] = me;
-                        src[t] = (mode == 3) ? cur_src[t] : (mode == 0 ? ZB_PREDEF : ZB_SELF);
+                        if (mode == 0) { cur[t + 1] = ZB_PREDEF; w->src_off[t + 1] = ZW_PREDEF; w->src_len[t + 1] = 0; }
+                        else if (mode != 3) { cur[t + 1] = me; w->src_off[t + 1] = at0 + pos; w->src_len[t + 1] = bs; }
+                        src[t] = (mode == 3) ? cur[t + 1] : (mode == 0 ? ZB_PREDEF : ZB_SELF);
                     }
                     B.ll_src = src[0]; B.of_src = src[1]; B.ml_src = src[2];
                 }
@@ -211,12 +266,35 @@ ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, ui
         }
         if (W) blocks_out[*nblocks_io] = B;
         (*nblocks_io)++;
-        first = false;
+        w->nblk++; walked++;
         if (last) break;
     }
-    *end = pos;
-    if (has_chk) { if (n - pos < 4) return ZMT_ST_TRUNCATED; pos += 4; }
-    *content_size = no_size ? bound : cs;
-    *end = pos;
+    w->pos = at0 + pos;
+    if (w->flags & ZF_CHECKSUM) { if (n - pos < 4) return ZMT_ST_TRUNCATED; pos += 4; }
+    w->pos = at0 + pos;
+    w->done = 1;
+    *bound = bnd;
     return ZMT_ST_OK;
+}
+
+// Walks one zstd frame in frame[0..n) (frame header + 3-byte block headers + the two section headers of every
+// compressed block).  `base_off` = offset of the frame's first byte in the decoder's input buffer.
+// W = true writes one descriptor per accepted block at blocks_out[*nblocks_io++] (below index max_blocks); W = false
+// only counts them.  Either way *nblocks_io advances by the block count, *scratch_used by the entropy scratch the
+// blocks take (their seq_off / lit_off), *flags receives the ZF_* bits and, on success, *content_size the frame content
+// size (the block bound without a content-size field).  *end = the frame's length on success, else the offset of the
+// header element the walk stopped at.  Bytes behind the frame are the caller's business.  Returns ZMT_ST_*.
+// The frame is one segment of zstd_walk_blocks that runs to its end.
+template <bool W>
+ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
+                           uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size,
+                           uint32_t* flags, size_t* end)
+{
+    zmt_zstd_walk w = {};
+    uint64_t bound = 0;
+    const int r = zstd_walk_blocks<W>(frame, n, base_off, frame_idx, blocks_out, nblocks_io, max_blocks, scratch_used, &w,
+                                      ~(size_t)0, ~0ull, &bound);
+    *flags = w.flags; *end = (size_t)w.pos;
+    if (r == ZMT_ST_OK) *content_size = (w.flags & ZF_NO_SIZE) ? bound : w.content_size;
+    return r;
 }

@@ -620,10 +620,11 @@ size_t read_some(const ErrCodes& E, GenRdWr* rw, void* dst, size_t want, size_t*
 }
 
 // One decode step on `st`: the batch's tables (packed into h_tab, `cap` entries; the device copy at d_tab) and, for zstd,
-// its block descriptors go to the device, the batch is decoded (with `seg`: as one segment of an LZ4F frame), and its
-// status and sizes come back into h_tab.  The batch's input must be in place on the stream before.  Returns ZMT_ST_*.
+// its block descriptors go to the device, the batch is decoded (with `seg` / `zseg`: as one segment of an LZ4F / a zstd
+// frame), and its status and sizes come back into h_tab.  The batch's input must be in place on the stream before.
+// Returns ZMT_ST_*.
 int decode_step(bool is_zstd, const FrameList& fl, uint8_t* h_tab, uint8_t* d_tab, size_t cap, const void* h_blk, void* d_blk,
-                const void* d_in, size_t in_bytes, void* d_out, void* d_work, zmt_lz4_segment* seg, cudaStream_t st)
+                const void* d_in, size_t in_bytes, void* d_out, void* d_work, zmt_lz4_segment* seg, zmt_zstd_segment* zseg, cudaStream_t st)
 {
     const Tables Th = tables_at(h_tab, cap), Td = tables_at(d_tab, cap);
     const uint32_t n = fl.n(), nslots = (uint32_t)fl.nslots;
@@ -631,7 +632,9 @@ int decode_step(bool is_zstd, const FrameList& fl, uint8_t* h_tab, uint8_t* d_ta
     if (cudaMemcpyAsync(d_tab, h_tab, tables_bytes(cap), cudaMemcpyHostToDevice, st) != cudaSuccess ||
         (is_zstd && fl.nblk && cudaMemcpyAsync(d_blk, h_blk, (size_t)fl.nblk * sizeof(ZBlk), cudaMemcpyHostToDevice, st) != cudaSuccess))
         return ZMT_ST_CUDA;
-    const int r = is_zstd ? zmt_zstd_decompress_device(d_in, d_blk, fl.nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size, Td.status, d_work, st)
+    const int r = is_zstd ? (zseg ? zmt_zstd_decompress_segments_device(d_in, d_blk, fl.nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size,
+                                                                        Td.status, zseg, d_work, st)
+                                  : zmt_zstd_decompress_device(d_in, d_blk, fl.nblk, Td.first_blk, Td.expect, Td.per_frame, n, d_out, Td.out_off, Td.out_size, Td.status, d_work, st))
                 : seg ? zmt_lz4_decompress_segments_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, seg, d_work, st)
                       : zmt_lz4_decompress_device(d_in, in_bytes, Td.frame_off, Td.per_frame, n, nslots, d_out, Td.out_off, Td.out_size, Td.status, d_work, st);
     if (r != ZMT_ST_OK) return r;
@@ -657,8 +660,8 @@ struct DevBuf {
 // .lz4 / .zst file, i.e. codec frames back to back without the 12-byte size headers.  Frame lengths are only known after
 // walking the block headers, so the host reads ahead, cuts the bytes it holds into complete frames, and decodes them in
 // batches of at most ~`batch` input bytes with the same GPU kernels; the consumed bytes are dropped before the next read.
-// An LZ4F frame larger than a batch is decoded in segments (lz4_segments), so LZ4 memory is O(batch + 64 KiB); a zstd
-// frame must fit in host and device memory as a whole.  Single-threaded: a batch's frames are written before the next read.
+// A frame larger than a batch is decoded in segments (lz4_segments, zstd_segments), so memory is O(batch + 64 KiB) for
+// LZ4 and O(batch + window) for zstd.  Single-threaded: a batch's frames are written before the next read.
 struct PlainStream {
     Ctx* c; GenRdWr* rw;
     const bool is_zstd;
@@ -667,7 +670,7 @@ struct PlainStream {
     size_t pos = 0;                         // parse position inside in[12..]
     bool eof = false;
     cudaStream_t st = nullptr;
-    DevBuf d_in, d_out, d_tab, d_blk, d_work, d_seg, d_hist;         // d_seg, d_hist: LZ4F frames decoded in segments
+    DevBuf d_in, d_out, d_tab, d_blk, d_work, d_seg, d_hist;         // d_seg, d_hist: frames decoded in segments
     std::vector<uint8_t> h_tab, out;        // the batch's tables (status and sizes come back here) and decoded bytes
     std::vector<ZBlk> blocks;               // zstd: the batch's block table
     FrameList fl;
@@ -713,7 +716,7 @@ struct PlainStream {
     // Decodes the batch `fl`: src[0 .. in_bytes - lo) goes to d_in + lo (the device addresses the frames at their offsets in
     // the batch input), the decode step runs, and the output room [out_off[0], out_end) comes back into `out` with the
     // status and sizes (in h_tab), in one stream synchronisation.
-    size_t decode(const uint8_t* src, size_t lo, size_t in_bytes, zmt_lz4_segment* seg)
+    size_t decode(const uint8_t* src, size_t lo, size_t in_bytes, zmt_lz4_segment* seg, zmt_zstd_segment* zseg = nullptr)
     {
         const uint32_t nf = fl.n();
         const uint64_t out_at = fl.out_off[0], room = fl.out_end() - out_at;
@@ -725,7 +728,7 @@ struct PlainStream {
         out.resize(room ? room : 1);
         cudaError_t ce = cudaMemcpyAsync((uint8_t*)d_in.p + lo, src, in_bytes - lo, cudaMemcpyHostToDevice, st);
         const int rc = ce == cudaSuccess ? decode_step(is_zstd, fl, h_tab.data(), (uint8_t*)d_tab.p, nf, blocks.data(), d_blk.p, d_in.p, in_bytes,
-                                                       d_out.p, d_work.p, seg, st) : ZMT_ST_CUDA;
+                                                       d_out.p, d_work.p, seg, zseg, st) : ZMT_ST_CUDA;
         if (rc == ZMT_ST_OK && room) ce = cudaMemcpyAsync(out.data(), (uint8_t*)d_out.p + out_at, room, cudaMemcpyDeviceToHost, st);
         if (rc == ZMT_ST_OK && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
         if (rc != ZMT_ST_OK || ce != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
@@ -786,6 +789,92 @@ struct PlainStream {
             if (last) return 0;
         }
     }
+
+    // The same for one zstd frame (zmt_zstd_decompress_segments_device).  What crosses a cut:
+    //   - the window: the last min(Window_Size, produced) content bytes, saved to d_hist behind each segment and copied
+    //     back directly below the next segment's output (the two ranges overlap when a segment is shorter than the window);
+    //   - the table sources: the bytes of the (at most four) blocks that describe the tables the next blocks may inherit,
+    //     kept in `carry` and placed in front of the segment's bytes in d_in, where the walk's ZB_SRC descriptors name them;
+    //   - repeat offsets, XXH64 state, content size and produced bytes: in the device record d_seg.
+    // Memory stays O(batch + window).
+    size_t zstd_segments()
+    {
+        if (!d_seg.need(sizeof(zmt_zstd_segment))) return c->E->mem;
+        if (cudaMemsetAsync(d_seg.p, 0, sizeof(zmt_zstd_segment), st) != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
+        zmt_zstd_segment* ds = (zmt_zstd_segment*)d_seg.p;
+        zmt_zstd_walk w = {};
+        std::vector<uint8_t> carry, next;
+        uint64_t produced = 0;
+        if (blocks.size() < 4096) blocks.resize(4096);
+        for (bool first = true;; first = false) {
+            // ---- the next segment: whole blocks up to a batch of input / four of output room
+            const uint64_t seg_at = w.pos;
+            uint64_t so[4]; uint32_t sl[4];
+            const uint32_t ns = zstd_walk_sources(&w, so, sl);
+            zmt_zstd_walk t;
+            uint32_t nb; uint64_t scr, room;
+            for (;;) {
+                t = w; nb = 0; scr = 0;
+                const int r = zstd_walk_blocks<true>(in.data() + 12 + pos, in.size() - 12 - pos, 12 + carry.size(), 0, blocks.data(), &nb,
+                                                     (uint32_t)blocks.size(), &scr, &t, batch, 4 * (uint64_t)batch, &room);
+                if (r == ZMT_ST_OK) break;
+                if (r == ZMT_ST_DST_SMALL) { blocks.resize(2 * blocks.size()); continue; }
+                if (r != ZMT_ST_TRUNCATED) return frame_error(c, r);
+                if (eof) return frame_error(c, ZMT_ST_TRUNCATED);
+                const size_t e = read_to(12 + pos + batch + piece);
+                if (e) return e;
+            }
+            const size_t end = (size_t)(t.pos - seg_at);
+            const bool last = t.done != 0;
+            // ---- decode it: a batch of one frame, [carry | segment bytes] at d_in + 12, its output at d_out + hlen above the history
+            const uint64_t hlen = produced < w.window ? produced : w.window;
+            const uint32_t flags = (first ? ZMT_SEG_FIRST : 0u) | (last ? ZMT_SEG_LAST : 0u);
+            if (!d_out.need(hlen + room + 256) || !d_in.need(12 + carry.size() + end + 256)) return c->E->mem;
+            cudaError_t ce = cudaMemcpyAsync(&ds->history, &hlen, sizeof(hlen), cudaMemcpyHostToDevice, st);
+            if (ce == cudaSuccess) ce = cudaMemcpyAsync(&ds->flags, &flags, sizeof(flags), cudaMemcpyHostToDevice, st);
+            if (ce == cudaSuccess && hlen) ce = cudaMemcpyAsync(d_out.p, d_hist.p, hlen, cudaMemcpyDeviceToDevice, st);
+            if (ce == cudaSuccess && !carry.empty()) ce = cudaMemcpyAsync((uint8_t*)d_in.p + 12, carry.data(), carry.size(), cudaMemcpyHostToDevice, st);
+            if (ce != cudaSuccess) { cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA); }
+            fl.clear(hlen);
+            fl.push(0, t.flags | ZF_NEEDS_SEQ, room, (t.flags & ZF_NO_SIZE) ? ~0ull : t.content_size, nb, scr);
+            const size_t e = decode(in.data() + 12 + pos, 12 + carry.size(), 12 + carry.size() + end, nullptr, ds);
+            if (e) return e;
+            const Tables T = tables_at(h_tab.data(), 1);
+            if (T.status[0] != ZMT_ST_OK) return frame_error(c, T.status[0]);
+            const uint64_t osz = T.out_size[0];
+            if (osz > room) return frame_error(c, ZMT_ST_DST_SMALL);
+            // ---- the history of the next segment: the last Window_Size bytes of [history | this segment], queued behind
+            //      this segment, ahead of the next one (a reallocation of d_out in between synchronises in cudaFree)
+            const uint64_t hnext = hlen + osz < t.window ? hlen + osz : t.window;
+            if (!last && hnext) {
+                if (!d_hist.need(hnext)) return c->E->mem;
+                if (cudaMemcpyAsync(d_hist.p, (uint8_t*)d_out.p + hlen + osz - hnext, hnext, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+                    cudaGetLastError(); return frame_error(c, ZMT_ST_CUDA);
+                }
+            }
+            const size_t we = write(out.data(), osz);
+            if (we) return we;
+            produced += osz;
+            // ---- the table sources of the next segment: from this segment's bytes, or carried on from the current ones
+            if (!last) {
+                uint64_t to[4]; uint32_t tln[4];
+                const uint32_t nt = zstd_walk_sources(&t, to, tln);
+                next.clear();
+                for (uint32_t i = 0; i < nt; i++) {
+                    const uint8_t* b = nullptr;
+                    if (to[i] >= seg_at) b = in.data() + 12 + pos + (to[i] - seg_at);
+                    else for (uint32_t k = 0, at = 0; k < ns; at += sl[k], k++) if (so[k] == to[i]) b = carry.data() + at;
+                    if (!b) return frame_error(c, ZMT_ST_BLOCK);
+                    next.insert(next.end(), b, b + tln[i]);
+                }
+                carry.swap(next);
+            }
+            in.erase(in.begin() + 12, in.begin() + 12 + (long)(pos + end));       // drop the decoded segment
+            pos = 0;
+            w = t;
+            if (last) return 0;
+        }
+    }
 };
 
 size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_t have)
@@ -842,6 +931,18 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                 pos += len;
             } else {
                 if (magic < 0xFD2FB522u || magic > ZMT_ZSTD_MAGIC) return E.data_error;
+                {
+                    // a frame whose blocks reach a batch of input or four of output before its end: decoded in segments,
+                    // after the frames in front of it
+                    zmt_zstd_walk sw = {}; uint32_t nb = 0; uint64_t scr = 0, room = 0;
+                    if (zstd_walk_blocks<false>(s + pos, n - pos, 0, 0, nullptr, &nb, 0xFFFFFFFFu, &scr, &sw, S.batch, 4 * (uint64_t)S.batch, &room) == ZMT_ST_OK &&
+                        !sw.done) {
+                        if (fl.n()) break;
+                        const size_t e = S.zstd_segments();
+                        if (e) return e;
+                        segmented = true; break;
+                    }
+                }
                 ZWalk w;
                 int zr = zstd_blocks(fl, s + pos, n - pos, 12 + pos, S.blocks.data(), (uint32_t)S.blocks.size(), true, w);
                 if (zr == ZMT_ST_DST_SMALL) {                     // block table full: grow it and walk once more
@@ -874,8 +975,6 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
             // ---- read ahead: at least one more piece, up to a batch beyond the parse position
             size_t goal = in.size() + S.piece;
             if (goal < 12 + pos + S.batch) goal = 12 + pos + S.batch;
-            // one zstd frame larger than a batch: read ahead geometrically (an LZ4 frame that large is decoded in segments)
-            if (S.is_zstd && in.size() - 12 - pos >= S.batch) goal = in.size() + (in.size() - 12 - pos) / 2;
             const size_t e = S.read_to(goal);
             if (e) return e;
         } else if (S.eof && pos >= in.size() - 12) break;
@@ -1077,7 +1176,7 @@ size_t decompress_run(Ctx* c, GenRdWr* rw)
     };
     po.submit = [&](Slot& s) -> int {
         if (cudaMemcpyAsync(s.d_in, s.h_in, s.in_used, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) return ZMT_ST_CUDA;
-        const int st = decode_step(is_zstd, s.frames, s.h_tab, s.d_tab, s.tab_cap, s.h_blk, s.d_blk, s.d_in, s.in_used, s.d_out, s.d_work, nullptr, s.stream);
+        const int st = decode_step(is_zstd, s.frames, s.h_tab, s.d_tab, s.tab_cap, s.h_blk, s.d_blk, s.d_in, s.in_used, s.d_out, s.d_work, nullptr, nullptr, s.stream);
         if (st != ZMT_ST_OK) return st;
         return cudaEventRecord(s.ev, s.stream) == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
     };

@@ -20,6 +20,9 @@
 //                            the `done` flags of the blocks it reads from.  Ticket order, dependency test and match copies
 //                            are match_exec.cuh's, shared with the LZ4 decoder
 //   zstd_checksum_kernel     one warp per frame with a content checksum: XXH64 of the regenerated frame
+// zmt_zstd_decompress_segments_device runs the same kernels on segments of frames (zmt_zstd_segment): repeat offsets, the
+// content size and the running XXH64 come from the record and go back to it, matches may reach the history below the
+// segment's output, and ZB_SRC descriptors carry the bytes of earlier segments' table describers.
 // Host side (zmt_zstd_scan_frame_host): walks frame + block headers (3 bytes per block + the two section headers), sizes the
 // scratch, names per block the block whose header describes each table it uses, flags per frame (state, checksum, no size).
 //
@@ -610,7 +613,7 @@ zstd_literals_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ bl
     if (ok && ltype == 3) {
         const ZBlk S = blocks[B.huf_src];
         uint32_t sh, sc, sr, st, ssf;
-        if (S.type != ZB_CMP || !zd_lit_header(in + S.comp_off, S.comp_size, &sh, &sc, &sr, &st, &ssf) || st != 2 || sc < 1) ok = false;
+        if ((S.type != ZB_CMP && S.type != ZB_SRC) || !zd_lit_header(in + S.comp_off, S.comp_size, &sh, &sc, &sr, &st, &ssf) || st != 2 || sc < 1) ok = false;
         else { dlp = in + S.comp_off + sh; dcomp = sc; }
     }
     // ---- weights
@@ -830,7 +833,7 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
         else {
             const ZBlk S = blocks[B.huf_src];
             uint32_t lhdr, lcomp, lregen, lt, sf, tb;
-            if (S.type != ZB_CMP || !zd_lit_header(in + S.comp_off, S.comp_size, &lhdr, &lcomp, &lregen, &lt, &sf) || lt != 2 || lcomp < 1) bad = 1;
+            if ((S.type != ZB_CMP && S.type != ZB_SRC) || !zd_lit_header(in + S.comp_off, S.comp_size, &lhdr, &lcomp, &lregen, &lt, &sf) || lt != 2 || lcomp < 1) bad = 1;
             else if (zd_huf_build(W, in + S.comp_off + lhdr, lcomp, lane, &tb)) bad = 1;
         }
     }
@@ -844,7 +847,7 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
                 if (srcs[t] == ZB_SELF || srcs[t] == ZB_PREDEF) continue;
                 if (srcs[t] >= nblocks) { r = 1; break; }
                 const ZBlk S = blocks[srcs[t]];
-                if (S.type != ZB_CMP || !zd_inherit_table(*refs[t], t, in + S.comp_off, S.comp_size, W)) r = 1;
+                if ((S.type != ZB_CMP && S.type != ZB_SRC) || !zd_inherit_table(*refs[t], t, in + S.comp_off, S.comp_size, W)) r = 1;
             }
         }
         bad = __shfl_sync(ZMT_FULL_MASK, r, 0);
@@ -866,15 +869,17 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
 // One WARP per frame: the repeat-offset rule (RFC 8878 3.1.1.5) over the frame's sequences in order.  Records written by the
 // block-parallel pass carry the coded offset value and pad = 1.  32 records are loaded at once (coalesced); the rule itself
 // is a serial state machine over (r0, r1, r2), walked by all lanes in lockstep with the records passed by shuffle; lane j
-// keeps the resolved offset of record j and stores it.
+// keeps the resolved offset of record j and stores it.  A segment (seg != nullptr) after the first starts from the offsets
+// the previous segment left in its record, and every segment stores its own back.
 __global__ void __launch_bounds__(32 * ZD_WARPS)
 zstd_resolve_offsets_kernel(const ZBlk* __restrict__ blocks, const uint32_t* __restrict__ frame_first_blk, const uint32_t* __restrict__ frame_seq,
-                            uint8_t* __restrict__ scratch, uint32_t* __restrict__ status, uint32_t nframes)
+                            uint8_t* __restrict__ scratch, uint32_t* __restrict__ status, zmt_zstd_segment* __restrict__ seg, uint32_t nframes)
 {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t f = blockIdx.x * ZD_WARPS + (threadIdx.x >> 5);
     if (f >= nframes || !(frame_seq[f] & ZF_NEEDS_SEQ) || (status[f] & 0xFF) != 0) return;
     uint32_t r0 = 1, r1 = 4, r2 = 8;
+    if (seg && !(seg[f].flags & ZMT_SEG_FIRST)) { r0 = seg[f].rep[0]; r1 = seg[f].rep[1]; r2 = seg[f].rep[2]; }
     for (uint32_t b = frame_first_blk[f]; b < frame_first_blk[f + 1]; b++) {
         const ZBlk B = blocks[b];
         if (B.type != ZB_CMP || B.nseq == 0) continue;
@@ -917,6 +922,7 @@ zstd_resolve_offsets_kernel(const ZBlk* __restrict__ blocks, const uint32_t* __r
             if (lane < cnt) { uint32_t* w = reinterpret_cast<uint32_t*>(seqs + base + lane); w[1] = mine; w[3] = 0; }
         }
     }
+    if (seg && lane == 0) { seg[f].rep[0] = r0; seg[f].rep[1] = r1; seg[f].rep[2] = r2; }
 }
 
 // ---------------------------------------------------------------- kernel 1b: frame-sequential entropy decode
@@ -955,10 +961,12 @@ zstd_entropy_seq_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
 }
 
 // ---------------------------------------------------------------- kernel 2: output offsets per block
+// A segment (seg != nullptr) checks the frame's content so far against the content size the first segment recorded: more
+// is what the whole frame reports as a full output, less is a wrong content size once the last segment is in.
 __global__ void zstd_offsets_kernel(const ZBlk* __restrict__ blocks, uint32_t nblocks, const uint32_t* __restrict__ frame_first_blk,
                                     const uint32_t* __restrict__ regen, uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                                     const uint64_t* __restrict__ expect, unsigned long long* __restrict__ out_size, uint32_t* __restrict__ status,
-                                    uint32_t nframes)
+                                    zmt_zstd_segment* __restrict__ seg, uint32_t nframes)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
@@ -967,8 +975,18 @@ __global__ void zstd_offsets_kernel(const ZBlk* __restrict__ blocks, uint32_t nb
     const uint64_t cap = out_off[f + 1] - out_off[f];
     for (uint32_t b = b0; b < b1; b++) { blk_out[b] = out_off[f] + pos; pos += regen[b]; }
     out_size[f] = pos;
+    if ((status[f] & 0xFF) != 0) return;
+    if (seg) {
+        zmt_zstd_segment& S = seg[f];
+        const bool first = (S.flags & ZMT_SEG_FIRST) != 0;
+        if (first) S.content_size = expect[f];
+        const uint64_t exp = S.content_size, total = (first ? 0 : S.produced) + pos;
+        if (pos > cap || (exp != ~0ull && total > exp)) status[f] = ZMT_ST_DST_SMALL;
+        else if ((S.flags & ZMT_SEG_LAST) && exp != ~0ull && total != exp) status[f] = ZMT_ST_CONTENT_SIZE;
+        return;
+    }
     // expect = ~0: the frame header carries no content size (streamed frames); the room then is only a bound
-    if ((status[f] & 0xFF) == 0 && ((expect[f] != ~0ull && pos != expect[f]) || pos > cap)) status[f] = pos > cap ? ZMT_ST_DST_SMALL : ZMT_ST_CONTENT_SIZE;
+    if ((expect[f] != ~0ull && pos != expect[f]) || pos > cap) status[f] = pos > cap ? ZMT_ST_DST_SMALL : ZMT_ST_CONTENT_SIZE;
 }
 
 // ---------------------------------------------------------------- kernel 3: sequence execution
@@ -978,7 +996,8 @@ __global__ void zstd_offsets_kernel(const ZBlk* __restrict__ blocks, uint32_t nb
 // lower indices of the same frame — is held by a warp that is already running.
 __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, const uint8_t* __restrict__ scratch,
                          const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
-                         uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, uint8_t* S)
+                         uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, const zmt_zstd_segment* __restrict__ seg,
+                         uint8_t* S)
 {
     const ZBlk B = blocks[b];
     volatile uint32_t* vdone = done;
@@ -989,14 +1008,15 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
     const uint32_t rg = regen[b];
     if (B.type == ZB_RAW) { const uint8_t* s = in + B.comp_off; for (uint32_t i = lane; i < rg; i += 32) dst[i] = s[i]; }
     else if (B.type == ZB_RLE) { const uint8_t v = in[B.comp_off]; for (uint32_t i = lane; i < rg; i += 32) dst[i] = v; }
-    else {
+    else if (B.type == ZB_CMP) {                              // (ZB_SRC: a carried table source, nothing to execute)
         const uint8_t* lit = scratch + B.lit_off;
         const ZDSeq* seqs = reinterpret_cast<const ZDSeq*>(scratch + B.seq_off);
         uint32_t op = 0, lp = 0;
         bool bad = false;
         uint32_t waited_to = b;                              // blocks [waited_to, b) are known complete
         const uint64_t blk_abs = blk_out[b];                 // absolute output address of this block
-        const uint64_t blk_in_frame = blk_abs - frame_base;
+        // bytes of the frame before this block: a segment's matches may also reach the history placed below its output
+        const uint64_t blk_in_frame = blk_abs - frame_base + (seg ? seg[B.frame].history : 0);
         // Up to MX_STEP sequences per step: one coalesced load of the records, positions from two warp scans.  Everything the
         // step regenerates — at most MX_SPAN bytes, else the step is cut shorter — goes to global memory and to the step
         // window (MxWin): every lane copies its own literal run (literals come from the scratch, no ordering among them),
@@ -1096,7 +1116,8 @@ __global__ void __launch_bounds__(32 * ZX_WARPS)
 zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, uint32_t nblocks, const uint8_t* __restrict__ scratch,
                     const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                     uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, unsigned long long* __restrict__ ticket,
-                    const uint32_t* __restrict__ frame_first_blk, const unsigned long long* __restrict__ wbase, uint32_t nframes)
+                    const uint32_t* __restrict__ frame_first_blk, const unsigned long long* __restrict__ wbase, const zmt_zstd_segment* __restrict__ seg,
+                    uint32_t nframes)
 {
     __shared__ __align__(16) uint8_t stage[ZX_WARPS][MX_SPAN];
     const uint32_t lane = threadIdx.x & 31;
@@ -1107,7 +1128,7 @@ zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blo
         uint32_t b;
         if (!mx_ticket_unit(T, tk, frame_first_blk, b)) continue;
         if (b >= nblocks) continue;
-        zx_block(b, lane, in, blocks, scratch, regen, blk_out, out_off, out, done, status, stage[threadIdx.x >> 5]);
+        zx_block(b, lane, in, blocks, scratch, regen, blk_out, out_off, out, done, status, seg, stage[threadIdx.x >> 5]);
         __syncwarp();
     }
 }
@@ -1116,6 +1137,10 @@ zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blo
 // One warp per frame that carries a checksum (what the stock zstd CLI writes by default; the reference path —
 // ZSTD_compress, zstd-mt_compress.c:284-286 — never does).  Lanes 0..3 run the four accumulator chains, each over its
 // 8-byte word of every 32-byte stripe; eight stripes are loaded ahead of their use.
+// A frame decoded in segments (seg != nullptr) runs the hash across them: the bytes pending from the previous segment are
+// topped up to a stripe first, what is left behind the last whole stripe waits in the record for the next segment, and the
+// last segment finalises and compares.  Every segment advances `produced`, with a checksum or without.  A whole frame is
+// a first and last segment whose state lives in registers.
 #define XP64_1 0x9E3779B185EBCA87ull
 #define XP64_2 0xC2B2AE3D27D4EB4Full
 #define XP64_3 0x165667B19E3779F9ull
@@ -1136,47 +1161,79 @@ __device__ __forceinline__ uint64_t ldg_le64u(const uint8_t* p)
 __global__ void __launch_bounds__(32 * ZD_WARPS)
 zstd_checksum_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, const uint32_t* __restrict__ frame_first_blk,
                      const uint32_t* __restrict__ frame_seq, const uint8_t* __restrict__ out, const uint64_t* __restrict__ out_off,
-                     const unsigned long long* __restrict__ out_size, uint32_t* __restrict__ status, uint32_t nframes)
+                     const unsigned long long* __restrict__ out_size, uint32_t* __restrict__ status, zmt_zstd_segment* __restrict__ seg,
+                     uint32_t nframes)
 {
-    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t lane = threadIdx.x & 31, j = lane & 3;
     const uint32_t f = blockIdx.x * ZD_WARPS + (threadIdx.x >> 5);
-    if (f >= nframes || !(frame_seq[f] & ZF_CHECKSUM) || (status[f] & 0xFF) != 0) return;
+    if (f >= nframes || (status[f] & 0xFF) != 0) return;
     const uint32_t b1 = frame_first_blk[f + 1];
     if (b1 == frame_first_blk[f]) return;
-    const ZBlk BL = blocks[b1 - 1];
+    const bool first = !seg || (seg[f].flags & ZMT_SEG_FIRST), last = !seg || (seg[f].flags & ZMT_SEG_LAST);
     const uint8_t* p = out + out_off[f];
     const uint64_t n = out_size[f];
-    uint64_t h;
-    if (n >= 32) {
-        const uint32_t j = lane & 3;
-        uint64_t acc = j == 0 ? XP64_1 + XP64_2 : j == 1 ? XP64_2 : j == 2 ? 0ull : 0ull - XP64_1;
-        const uint64_t ns = n >> 5;
-        uint64_t s = 0;
-        if (lane < 4) {
-            for (; s + 8 <= ns; s += 8) {
-                uint64_t v[8];
-#pragma unroll
-                for (int k = 0; k < 8; k++) v[k] = ldg_le64u(p + ((s + k) << 5) + 8 * j);
-#pragma unroll
-                for (int k = 0; k < 8; k++) acc = xxh64_round(acc, v[k]);
-            }
-            for (; s < ns; s++) acc = xxh64_round(acc, ldg_le64u(p + (s << 5) + 8 * j));
+    const uint64_t total = (first ? 0 : seg[f].produced) + n;
+    if (!(frame_seq[f] & ZF_CHECKSUM)) { if (seg && lane == 0) seg[f].produced = total; return; }
+    uint8_t* pend = seg ? seg[f].pending : nullptr;
+    uint32_t pl = first ? 0u : seg[f].pending_len;
+    uint64_t acc = !first ? seg[f].acc[j] : j == 0 ? XP64_1 + XP64_2 : j == 1 ? XP64_2 : j == 2 ? 0ull : 0ull - XP64_1;
+    uint64_t k = 0;                                          // bytes of this segment that top up the pending stripe
+    if (pl) {
+        k = n < 32 - pl ? n : 32 - pl;
+        if (pl + k == 32) {                                  // a whole stripe: its word j is pending bytes, then this segment's
+            uint64_t v = 0;
+            for (uint32_t i = 0; i < 8; i++) { const uint32_t q = 8 * j + i; v |= (uint64_t)(q < pl ? pend[q] : p[q - pl]) << (8 * i); }
+            acc = xxh64_round(acc, v);
+            pl = 0;
         }
-        const uint64_t a1 = __shfl_sync(0xFFFFFFFFu, acc, 0), a2 = __shfl_sync(0xFFFFFFFFu, acc, 1), a3 = __shfl_sync(0xFFFFFFFFu, acc, 2), a4 = __shfl_sync(0xFFFFFFFFu, acc, 3);
+    }
+    const uint64_t ns = (n - k) >> 5;
+    if (lane < 4) {
+        const uint8_t* ps = p + k;
+        uint64_t s = 0;
+        for (; s + 8 <= ns; s += 8) {
+            uint64_t v[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) v[i] = ldg_le64u(ps + ((s + i) << 5) + 8 * j);
+#pragma unroll
+            for (int i = 0; i < 8; i++) acc = xxh64_round(acc, v[i]);
+        }
+        for (; s < ns; s++) acc = xxh64_round(acc, ldg_le64u(ps + (s << 5) + 8 * j));
+    }
+    const uint64_t a1 = __shfl_sync(0xFFFFFFFFu, acc, 0), a2 = __shfl_sync(0xFFFFFFFFu, acc, 1), a3 = __shfl_sync(0xFFFFFFFFu, acc, 2), a4 = __shfl_sync(0xFFFFFFFFu, acc, 3);
+    if (lane != 0) return;
+    // the bytes behind the last whole stripe: the pending ones topped up by all of this segment, or this segment's tail
+    uint8_t t[32];
+    uint32_t tl;
+    if (pl) { for (uint32_t i = 0; i < pl; i++) t[i] = pend[i]; for (uint32_t i = 0; i < (uint32_t)k; i++) t[pl + i] = p[i]; tl = pl + (uint32_t)k; }
+    else { const uint64_t t0 = k + (ns << 5); tl = (uint32_t)(n - t0); for (uint32_t i = 0; i < tl; i++) t[i] = p[t0 + i]; }
+    if (!last) {
+        zmt_zstd_segment& S = seg[f];
+        S.acc[0] = a1; S.acc[1] = a2; S.acc[2] = a3; S.acc[3] = a4;
+        for (uint32_t i = 0; i < tl; i++) S.pending[i] = t[i];
+        S.pending_len = tl; S.produced = total;
+        return;
+    }
+    if (seg) seg[f].produced = total;
+    uint64_t h;
+    if (total >= 32) {
         h = rotl64(a1, 1) + rotl64(a2, 7) + rotl64(a3, 12) + rotl64(a4, 18);
         h = xxh64_merge(h, a1); h = xxh64_merge(h, a2); h = xxh64_merge(h, a3); h = xxh64_merge(h, a4);
     } else h = XP64_5;
-    if (lane == 0) {
-        h += n;
-        const uint8_t* q = p + (n & ~31ull); const uint8_t* end = p + n;
-        while (q + 8 <= end) { h ^= xxh64_round(0, ldg_le64u(q)); h = rotl64(h, 27) * XP64_1 + XP64_4; q += 8; }
-        if (q + 4 <= end) { h ^= (uint64_t)((uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24)) * XP64_1; h = rotl64(h, 23) * XP64_2 + XP64_3; q += 4; }
-        while (q < end) { h ^= (*q) * XP64_5; h = rotl64(h, 11) * XP64_1; q++; }
-        h ^= h >> 33; h *= XP64_2; h ^= h >> 29; h *= XP64_3; h ^= h >> 32;
-        const uint8_t* c = in + BL.comp_off + BL.comp_size;
-        const uint32_t stored = (uint32_t)c[0] | ((uint32_t)c[1] << 8) | ((uint32_t)c[2] << 16) | ((uint32_t)c[3] << 24);
-        if (stored != (uint32_t)h) zd_fail(status, f, ZMT_ST_CONTENT_CHECKSUM);
+    h += total;
+    uint32_t q = 0;
+    for (; q + 8 <= tl; q += 8) {
+        uint64_t v = 0;
+        for (uint32_t i = 0; i < 8; i++) v |= (uint64_t)t[q + i] << (8 * i);
+        h ^= xxh64_round(0, v); h = rotl64(h, 27) * XP64_1 + XP64_4;
     }
+    if (q + 4 <= tl) { h ^= (uint64_t)((uint32_t)t[q] | ((uint32_t)t[q + 1] << 8) | ((uint32_t)t[q + 2] << 16) | ((uint32_t)t[q + 3] << 24)) * XP64_1; h = rotl64(h, 23) * XP64_2 + XP64_3; q += 4; }
+    for (; q < tl; q++) { h ^= t[q] * XP64_5; h = rotl64(h, 11) * XP64_1; }
+    h ^= h >> 33; h *= XP64_2; h ^= h >> 29; h *= XP64_3; h ^= h >> 32;
+    const ZBlk BL = blocks[b1 - 1];
+    const uint8_t* c = in + BL.comp_off + BL.comp_size;
+    const uint32_t stored = (uint32_t)c[0] | ((uint32_t)c[1] << 8) | ((uint32_t)c[2] << 16) | ((uint32_t)c[3] << 24);
+    if (stored != (uint32_t)h) zd_fail(status, f, ZMT_ST_CONTENT_CHECKSUM);
 }
 
 // ================================================================ host side
@@ -1237,11 +1294,29 @@ extern "C" size_t zmt_zstdd_workspace_bytes(uint32_t nframes, uint32_t nblocks, 
            + 256 + ticket_table_bytes(nframes) + 3 * (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) + scratch_bytes + 1024;
 }
 
+// Walk one segment of a zstd frame on the host (zstd_walk_blocks in frame_format.h), committing the walk state only when
+// the segment is complete.
+extern "C" int zmt_zstd_segment_host(const uint8_t* seg, size_t n, uint64_t base_off, uint32_t frame_idx, zmt_zstd_walk* w,
+                                     size_t max_in, uint64_t max_out, void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
+                                     uint64_t* scratch_used, size_t* end, uint64_t* room, uint32_t* flags, uint32_t* last)
+{
+    zmt_zstd_walk t = *w;
+    uint32_t nb = *nblocks_io; uint64_t scr = *scratch_used, bound = 0;
+    const int r = zstd_walk_blocks<true>(seg, n, base_off, frame_idx, (ZBlk*)blocks_out, &nb, max_blocks, &scr, &t, max_in, max_out, &bound);
+    if (r != ZMT_ST_OK) return r;
+    *end = (size_t)(t.pos - w->pos); *room = bound; *flags = t.flags | ZF_NEEDS_SEQ; *last = t.done;
+    *w = t; *nblocks_io = nb; *scratch_used = scr;
+    return ZMT_ST_OK;
+}
+
+extern "C" uint32_t zmt_zstd_segment_sources(const zmt_zstd_walk* w, uint64_t* off, uint32_t* len) { return zstd_walk_sources(w, off, len); }
+
 // d_blocks: nblocks descriptors (device copy of what zmt_zstd_scan_frame_host produced); d_frame_first_blk: nframes+1;
-// d_expect: content size per frame (from the frame headers)
-extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
-                                          const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off,
-                                          uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream_)
+// d_expect: content size per frame (from the frame headers).  seg = nullptr: whole frames (zmt_zstd_decompress_device);
+// else every frame of the batch is a segment with its record in seg[f] (zmt_zstd_decompress_segments_device)
+static int zstd_decompress_launch(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                  const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off,
+                                  uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* seg, void* d_work, void* stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0) return ZMT_ST_OK;
@@ -1274,22 +1349,41 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
                                                                                            seq_done, seq_ml, lit_done);
         zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen,
                                                                                            d_status, lit_done);
-        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, scratch, d_status, nframes);
+        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, scratch, d_status,
+                                                                                                   seg, nframes);
         zstd_entropy_seq_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
                                                                                            scratch, regen, d_status, nframes);
     }
     zstd_offsets_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>((const ZBlk*)d_blocks, nblocks, d_frame_first_blk, regen, blk_out, d_out_off, d_expect,
-                                                                   (unsigned long long*)d_out_size, d_status, nframes);
+                                                                   (unsigned long long*)d_out_size, d_status, seg, nframes);
     if (nblocks) {
         const uint32_t gmax = (uint32_t)(zmt_sm_count() * (2048 / (32 * ZX_WARPS)));
         const uint32_t gneed = (nblocks + ZX_WARPS - 1) / ZX_WARPS;
         cudaMemsetAsync(xticket, 0, 8, stream);
         ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, xwbase);
         zstd_execute_kernel<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, scratch, regen, blk_out,
-                                                                                     d_out_off, (uint8_t*)d_out, done, d_status, xticket, d_frame_first_blk, xwbase, nframes);
+                                                                                     d_out_off, (uint8_t*)d_out, done, d_status, xticket, d_frame_first_blk, xwbase, seg, nframes);
         zstd_checksum_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
-                                                                                           (const uint8_t*)d_out, d_out_off, (const unsigned long long*)d_out_size, d_status, nframes);
+                                                                                           (const uint8_t*)d_out, d_out_off, (const unsigned long long*)d_out_size, d_status, seg, nframes);
     }
     zmt_prof_mark(ZMT_K_ZSTD_DECODE, stream, 1);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                          const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off,
+                                          uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream)
+{
+    return zstd_decompress_launch(d_in, d_blocks, nblocks, d_frame_first_blk, d_expect, d_frame_seq, nframes, d_out, d_out_off, d_out_size, d_status,
+                                  nullptr, d_work, stream);
+}
+
+extern "C" int zmt_zstd_decompress_segments_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                                   const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out,
+                                                   const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* d_seg,
+                                                   void* d_work, void* stream)
+{
+    if (!d_seg && nframes) return ZMT_ST_BAD_ARG;
+    return zstd_decompress_launch(d_in, d_blocks, nblocks, d_frame_first_blk, d_expect, d_frame_seq, nframes, d_out, d_out_off, d_out_size, d_status,
+                                  d_seg, d_work, stream);
 }
