@@ -24,6 +24,7 @@ def orc():
         L.orc_lz4f_decode.restype = ctypes.c_int; L.orc_lz4f_decode.argtypes = [c_vp, c_sz, c_vp, c_sz, ctypes.POINTER(c_sz), ctypes.POINTER(c_sz)]
         L.orc_zstd_decode.restype = ctypes.c_int; L.orc_zstd_decode.argtypes = [c_vp, c_sz, c_vp, c_sz, ctypes.POINTER(c_sz), ctypes.POINTER(c_sz)]
         L.orc_lz4_block_compress_b200.restype = c_sz; L.orc_lz4_block_compress_b200.argtypes = [c_vp, c_sz, c_vp, c_sz]
+        L.orc_lz4_b200_offsets.restype = None; L.orc_lz4_b200_offsets.argtypes = [c_vp, c_sz, c_vp]
         L.orc_lz4_block_bound.restype = c_sz; L.orc_lz4_block_bound.argtypes = [c_sz]
         L.orc_lz4_block_decode.restype = ctypes.c_long; L.orc_lz4_block_decode.argtypes = [c_vp, c_sz, c_vp, c_sz, c_sz]
         L.orc_mt_scan.restype = ctypes.c_long; L.orc_mt_scan.argtypes = [c_vp, c_sz, c_vp, c_vp, c_sz]
@@ -83,6 +84,23 @@ def orc_encode_lz4(data, chunk=1 << 20):
     cap = data.size + data.size // 100 + 4096 + 64 * (data.size // chunk + 2)
     out = np.empty(cap, np.uint8)
     n = orc().orc_mt_encode_lz4_b200(data.ctypes.data, data.size, chunk, out.ctypes.data, cap)
+    return out[:n].copy()
+
+
+def lz4_b200_offsets(block):
+    """orc_lz4_b200_offsets: the candidate offset of every position of one block (<= 64 KiB; 0 = none)."""
+    block = _arr(block)
+    off = np.zeros(max(block.size, 1), np.uint16)
+    orc().orc_lz4_b200_offsets(block.ctypes.data, block.size, off.ctypes.data)
+    return off[: block.size]
+
+
+def lz4_block_b200(block):
+    """orc_lz4_block_compress_b200: the CPU twin's LZ4 block (before the stored-block rule of the frame)."""
+    block = _arr(block)
+    cap = orc().orc_lz4_block_bound(65536)
+    out = np.empty(cap, np.uint8)
+    n = orc().orc_lz4_block_compress_b200(block.ctypes.data, block.size, out.ctypes.data, cap)
     return out[:n].copy()
 
 
