@@ -148,6 +148,43 @@ int    zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_f
 int    zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
                               const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream);
 
+/* ---- Frame index on the device for plain streams: the same tables and summary from an ordinary .lz4 / .zst file in
+ * HBM (codec frames back to back as the lz4 and zstd tools write them, without container headers; skippable frames,
+ * magic 0x184D2A50..0x184D2A5F + LE32 size + payload, anywhere between them).  Arguments, workspace, max_frames and
+ * ZMT_ST_DST_SMALL as for the container calls above.  One thread walks the stream: a frame's end is only known by
+ * walking its block headers (one dependent load per block header).  Each frame start is decided as the callback API's
+ * plain path decides it on the same bytes.  Skippable frames are not frames of the index: nframes counts codec frames,
+ * so a container-framed stream is also a valid plain stream, each 12-byte header a skippable frame of size 4.
+ *
+ * Layout convention.  The tables are written for a base 12 bytes below the stream, so that the decode calls address a
+ * frame as they address one behind a container header: d_frame_off[f] = frame f's offset in the plain stream,
+ * d_frame_csize[f] = its length, and the zstd descriptors' offsets are relative to d_in - 12.  Call
+ * zmt_zstd_blocks_device, zmt_lz4_decompress_device (with in_bytes + 12) and zmt_zstd_decompress_device unchanged with
+ * d_in - 12.  None of them reads below base + 12, where the stream starts: every read is at
+ * base + frame_off + 12 or a descriptor's offset on, apart from aligned 8- and 16-byte loads of the decoders, whose
+ * aligned word always holds a stream byte and so never leaves the caller's allocation.
+ *
+ * info.status, the plain path's decision at the first frame start that fails (the walk ends there: the next frame's
+ * start is not known behind it); bad_frame = the frames accepted before it, bad_offset in stream coordinates:
+ *   ZMT_ST_TRUNCATED    fewer than 4 bytes at a frame start, or a skippable frame whose size runs past the end; an LZ4F
+ *                       header shorter than 7 bytes (the frame's start) / LZ4F: the header or a block runs past the end
+ *                       (the block header the walk could not read, or in_bytes)
+ *   ZMT_ST_BAD_MAGIC    neither a skippable frame nor the codec's magic, zstd legacy magics included (the frame's start)
+ *   ZMT_ST_BAD_HEADER   LZ4F: FLG version other than 01, or a block-size id below 4 (the frame's start)
+ *   ZMT_ST_CONTENT_SIZE LZ4F: a content size above the bound of its blocks (the frame's start)
+ *   zstd: what zmt_zstd_scan_frame_host returns for the frame (BAD_HEADER, UNSUPPORTED for a dictionary ID, BLOCK,
+ *                       TRUNCATED), bad_offset = the header element the walk stopped at
+ *   ZMT_ST_UNSUPPORTED  a frame of 2^32 bytes or more (the frame's start): the decode calls' frame_csize is 32-bit; the
+ *                       callback API decodes such a frame in segments
+ *   ZMT_ST_DST_SMALL    as above
+ * ZMT_ST_TRAILING cannot occur: bytes behind a frame are the next frame.  An empty stream, or one of skippable frames
+ * only, is ZMT_ST_OK with nframes = 0. */
+int    zmt_lz4_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                  uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream);
+int    zmt_zstd_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                   uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                   uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream);
+
 /* ---- LZ4F frames of any size in bounded memory ----
  * An LZ4F frame of any size, decoded as a chain of segments, each a run of whole blocks (what LZ4F_decompress does
  * through two fixed buffers when the reference streams a plain .lz4 file, lib/lz4-mt_decompress.c:391-483).  Frame f of
@@ -267,7 +304,7 @@ enum { ZMT_K_LZ4_COMPRESS = 0, ZMT_K_XXH32, ZMT_K_LZ4_SIZES, ZMT_K_SCAN, ZMT_K_L
  * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK)
  * LZ4 levels 10-12: hash, sort and search as zstd's (ZMT_K_ZL_HASH / SORT / SEARCH), ZMT_K_L4H_BLOCKS = lazy parse +
  * LZ4 sequences; checksum, sizes, scan and pack as level 1's
- * ZMT_K_FRAME_INDEX = one index call (container walk, frame pass, scans, summary) or one zmt_zstd_blocks_device call */
+ * ZMT_K_FRAME_INDEX = one index call (container or plain walk, frame pass, scans, summary) or one zmt_zstd_blocks_device call */
 void zmt_prof_begin(void);
 int  zmt_prof_end(double* ms, int* count, int max_ids);
 

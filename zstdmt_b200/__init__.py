@@ -94,6 +94,10 @@ def lib():
     L.zmt_lz4_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.zmt_zstd_index_device.restype = ctypes.c_int
     L.zmt_zstd_index_device.argtypes = [c_vp, c_u64, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_lz4_index_plain_device.restype = ctypes.c_int
+    L.zmt_lz4_index_plain_device.argtypes = L.zmt_lz4_index_device.argtypes
+    L.zmt_zstd_index_plain_device.restype = ctypes.c_int
+    L.zmt_zstd_index_plain_device.argtypes = L.zmt_zstd_index_device.argtypes
     L.zmt_zstd_blocks_device.restype = ctypes.c_int
     L.zmt_zstd_blocks_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_vp]
     for pre, api in (("LZ4MT", "lz4"), ("ZSTDCB", "zstd"), ("ZSTDMT", "zstd")):
@@ -220,13 +224,19 @@ class FrameIndex(ctypes.Structure):
         return "FrameIndex(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
 
 
-def _device_index(d_framed, max_frames, stream, zstd):
-    """Run zmt_{lz4,zstd}_index_device over a framed stream in device memory.  Only the summary struct is read back; on
-    ZMT_ST_DST_SMALL the index runs once more with the exact frame count.  Returns (summary, device tables by name)."""
+# The plain index writes its tables for a base this many bytes below the stream: the decode calls address a frame as
+# one behind a 12-byte container header (include/zstdmt_b200_dev.h, "Layout convention").
+PLAIN_PAD = 12
+
+
+def _device_index(d_framed, max_frames, stream, zstd, plain=False):
+    """Run zmt_{lz4,zstd}_index_device (plain: zmt_{lz4,zstd}_index_plain_device) over a stream in device memory.  Only
+    the summary struct is read back; on ZMT_ST_DST_SMALL the index runs once more with the exact frame count.  Returns
+    (summary, device tables by name)."""
     torch = _torch(); L = lib()
     s = stream if stream is not None else torch.cuda.current_stream()
     dev, nbytes = d_framed.device, d_framed.numel()
-    cap = int(max_frames) if max_frames is not None else min(nbytes // 12, 1 << 16)
+    cap = int(max_frames) if max_frames is not None else min(nbytes // (9 if plain else 12), 1 << 16)
     for attempt in range(2):
         e = lambda n, dt: torch.empty(max(n, 1), dtype=dt, device=dev)
         t = {"frame_off": e(cap, torch.int64), "frame_csize": e(cap, torch.int32), "out_off": e(cap + 1, torch.int64)}
@@ -240,11 +250,13 @@ def _device_index(d_framed, max_frames, stream, zstd):
         d_info = torch.zeros(ctypes.sizeof(FrameIndex), dtype=torch.uint8, device=dev)
         p = lambda k: t[k].data_ptr()
         if zstd:
-            rc = L.zmt_zstd_index_device(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("first_blk"), p("frame_scratch"),
-                                         p("expect"), p("frame_seq"), p("out_off"), d_info.data_ptr(), work.data_ptr(), s.cuda_stream)
+            fn = L.zmt_zstd_index_plain_device if plain else L.zmt_zstd_index_device
+            rc = fn(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("first_blk"), p("frame_scratch"),
+                    p("expect"), p("frame_seq"), p("out_off"), d_info.data_ptr(), work.data_ptr(), s.cuda_stream)
         else:
-            rc = L.zmt_lz4_index_device(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("out_off"), d_info.data_ptr(),
-                                        work.data_ptr(), s.cuda_stream)
+            fn = L.zmt_lz4_index_plain_device if plain else L.zmt_lz4_index_device
+            rc = fn(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("out_off"), d_info.data_ptr(),
+                    work.data_ptr(), s.cuda_stream)
         if rc != 0:
             raise RuntimeError("frame index failed: %s" % ST_NAMES.get(rc, rc))
         s.synchronize()
@@ -254,7 +266,8 @@ def _device_index(d_framed, max_frames, stream, zstd):
             continue
         break
     if info.status != 0:
-        raise ValueError("framed stream rejected: %s in frame %d at offset %d" % (ST_NAMES.get(info.status, info.status), info.bad_frame, info.bad_offset))
+        raise ValueError("%s stream rejected: %s in frame %d at offset %d" % ("plain" if plain else "framed", ST_NAMES.get(info.status, info.status),
+                                                                            info.bad_frame, info.bad_offset))
     return info, t
 
 
@@ -309,7 +322,8 @@ class ZstdDeviceCompressor:
 
 
 class Lz4DeviceDecompressor:
-    """zmt_lz4_decompress_device over a device-resident framed stream."""
+    """zmt_lz4_decompress_device over a device-resident framed stream (from_device: also a plain .lz4 stream)."""
+    pad = 0                 # bytes from the decoder's base to the stream (PLAIN_PAD for a plain stream)
 
     def __init__(self, frame_off, frame_csize, out_sizes, device="cuda"):
         torch = _torch(); L = lib()
@@ -328,27 +342,30 @@ class Lz4DeviceDecompressor:
         self.work = torch.empty(L.zmt_lz4d_workspace_bytes(self.n, self.nslots, self.in_bytes_cap), dtype=torch.uint8, device=device)
 
     @classmethod
-    def from_device(cls, d_framed, max_frames=None, stream=None):
+    def from_device(cls, d_framed, max_frames=None, stream=None, plain=False):
         """A decoder for a framed stream that is already in device memory: the frame tables are built on the GPU
         (zmt_lz4_index_device) and only the summary comes back to the host, as .index_info.  run(d_framed) decodes.
         max_frames sizes the first attempt (default: up to 65536 frames); a larger stream is indexed once more at its
-        exact count.  Raises ValueError naming the status, frame and offset of a stream the index rejects."""
+        exact count.  Raises ValueError naming the status, frame and offset of a stream the index rejects.
+        plain=True: d_framed is a plain .lz4 stream (LZ4F and skippable frames back to back, zmt_lz4_index_plain_device);
+        frame offsets are then the frames' own, and run() passes the decoder the base the tables are written for."""
         torch = _torch(); L = lib()
-        info, t = _device_index(d_framed, max_frames, stream, zstd=False)
+        info, t = _device_index(d_framed, max_frames, stream, zstd=False, plain=plain)
         self = cls.__new__(cls)
+        self.pad = PLAIN_PAD if plain else 0
         self.index_info, self.n, self.nslots, self.out_total = info, info.nframes, max(info.nblocks, 1), info.out_bytes
         self.d_off, self.d_cs, self.d_out_off = t["frame_off"], t["frame_csize"], t["out_off"]
         self.out = torch.empty(max(self.out_total, 1), dtype=torch.uint8, device=d_framed.device)
         self.out_size = torch.zeros(max(self.n, 1), dtype=torch.int64, device=d_framed.device)
         self.status = torch.zeros(max(self.n, 1), dtype=torch.int32, device=d_framed.device)
-        self.in_bytes_cap = d_framed.numel()
+        self.in_bytes_cap = d_framed.numel() + self.pad
         self.work = torch.empty(L.zmt_lz4d_workspace_bytes(self.n, self.nslots, self.in_bytes_cap), dtype=torch.uint8, device=d_framed.device)
         return self
 
     def run(self, d_framed, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_lz4_decompress_device(d_framed.data_ptr(), d_framed.numel(), self.d_off.data_ptr(), self.d_cs.data_ptr(), self.n,
+        rc = lib().zmt_lz4_decompress_device(d_framed.data_ptr() - self.pad, d_framed.numel() + self.pad, self.d_off.data_ptr(), self.d_cs.data_ptr(), self.n,
                                              self.nslots, self.out.data_ptr(), self.d_out_off.data_ptr(), self.out_size.data_ptr(),
                                              self.status.data_ptr(), self.work.data_ptr(), s.cuda_stream)
         if rc != 0:
@@ -516,6 +533,8 @@ class ZstdDeviceDecompressor:
     (zmt_zstd_scan_frame_host: frame + block headers only), as the host pipeline does while reading; from_device builds
     it on the GPU from a stream already in device memory."""
 
+    pad = 0                 # as Lz4DeviceDecompressor.pad
+
     def __init__(self, framed_host, device="cuda"):
         torch = _torch(); L = lib()
         fb = np.ascontiguousarray(framed_host, dtype=np.uint8)
@@ -553,19 +572,21 @@ class ZstdDeviceDecompressor:
         self.work = torch.empty(L.zmt_zstdd_workspace_bytes(self.n, self.nblk, scr.value), dtype=torch.uint8, device=device)
 
     @classmethod
-    def from_device(cls, d_framed, max_frames=None, stream=None):
+    def from_device(cls, d_framed, max_frames=None, stream=None, plain=False):
         """A decoder for a framed stream that is already in device memory: the frame tables and the block table are built
         on the GPU (zmt_zstd_index_device, zmt_zstd_blocks_device) and only the summary comes back to the host, as
-        .index_info.  run(d_framed) decodes.  max_frames and the errors as Lz4DeviceDecompressor.from_device."""
+        .index_info.  run(d_framed) decodes.  max_frames, plain and the errors as Lz4DeviceDecompressor.from_device
+        (plain: a .zst stream, zmt_zstd_index_plain_device)."""
         torch = _torch(); L = lib()
         s = stream if stream is not None else torch.cuda.current_stream()
-        info, t = _device_index(d_framed, max_frames, s, zstd=True)
+        info, t = _device_index(d_framed, max_frames, s, zstd=True, plain=plain)
         dev = d_framed.device
         self = cls.__new__(cls)
+        self.pad = PLAIN_PAD if plain else 0
         self.index_info, self.n, self.nblk, self.out_total = info, info.nframes, info.nblocks, info.out_bytes
         self.d_first, self.d_expect, self.d_fseq, self.d_out_off = t["first_blk"], t["expect"], t["frame_seq"], t["out_off"]
         self.d_blocks = torch.empty(max(1, self.nblk) * L.zmt_zstd_blk_desc_bytes(), dtype=torch.uint8, device=dev)
-        rc = L.zmt_zstd_blocks_device(d_framed.data_ptr(), self.n, t["frame_off"].data_ptr(), t["frame_csize"].data_ptr(), self.d_first.data_ptr(),
+        rc = L.zmt_zstd_blocks_device(d_framed.data_ptr() - self.pad, self.n, t["frame_off"].data_ptr(), t["frame_csize"].data_ptr(), self.d_first.data_ptr(),
                                       t["frame_scratch"].data_ptr(), self.d_blocks.data_ptr(), self.nblk, s.cuda_stream)
         if rc != 0:
             raise RuntimeError("zmt_zstd_blocks_device failed: %s" % ST_NAMES.get(rc, rc))
@@ -579,7 +600,7 @@ class ZstdDeviceDecompressor:
     def run(self, d_framed, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_zstd_decompress_device(d_framed.data_ptr(), self.d_blocks.data_ptr(), self.nblk, self.d_first.data_ptr(), self.d_expect.data_ptr(),
+        rc = lib().zmt_zstd_decompress_device(d_framed.data_ptr() - self.pad, self.d_blocks.data_ptr(), self.nblk, self.d_first.data_ptr(), self.d_expect.data_ptr(),
                                               self.d_fseq.data_ptr(), self.n, self.out.data_ptr(), self.d_out_off.data_ptr(), self.out_size.data_ptr(), self.status.data_ptr(),
                                               self.work.data_ptr(), s.cuda_stream)
         if rc != 0:

@@ -20,6 +20,7 @@
 
 ZMT_HD uint32_t zf_rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 ZMT_HD uint64_t zf_rd64(const uint8_t* p) { return (uint64_t)zf_rd32(p) | ((uint64_t)zf_rd32(p + 4) << 32); }
+ZMT_HD uint32_t zf_rd24(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16); }
 
 // ---------------------------------------------------------------- LZ4F
 // Bytes of an LZ4F frame header with this FLG byte: magic, FLG, BD, [content size], [dictionary ID], header checksum.
@@ -88,6 +89,53 @@ ZMT_HD bool lz4f_out_size(const uint8_t* p, size_t n, uint64_t* out)
 
 // LZ4 decoder block-table slots a frame with this much room takes (the nslots argument sums them)
 ZMT_HD uint64_t lz4_frame_slots(uint64_t room) { const uint64_t nb = (room + 65535) / 65536; return nb ? nb : 1; }
+
+// ---------------------------------------------------------------- plain streams
+// An ordinary .lz4 / .zst file: codec frames and skippable frames (magic 0x184D2A50..0x184D2A5F, LE32 size, payload) back
+// to back, without container headers.  A frame's end is only known by walking its block headers.  The host's plain path
+// (decompress_single_stream) and the device's plain index (frame_index.cu) take the same decision at every frame start
+// from the two functions below and, for a zstd frame, zstd_frame_walk.
+
+// The first decision at a frame start: p[0..n) = the stream's bytes from there.  ZMT_ST_OK: *skip = the length of a
+// skippable frame (8 + its size), or 0 for a codec frame whose head is usable.  ZMT_ST_TRUNCATED: fewer than 4 bytes, a
+// skippable frame whose size runs past n, or an LZ4F header shorter than 7 bytes.  ZMT_ST_BAD_MAGIC: neither a skippable
+// frame nor the codec's magic (zstd: 0xFD2FB522..0xFD2FB528; the walk then rejects the legacy versions with BAD_MAGIC).
+// ZMT_ST_BAD_HEADER: an LZ4F FLG version other than 01, or a block-size id below 4.
+ZMT_HD int plain_frame_head(const uint8_t* p, size_t n, bool zstd, uint64_t* skip)
+{
+    *skip = 0;
+    if (n < 4) return ZMT_ST_TRUNCATED;
+    const uint32_t magic = zf_rd32(p);
+    if ((magic & 0xFFFFFFF0u) == ZMT_CONTAINER_MAGIC) {
+        if (n < 8 || n - 8 < zf_rd32(p + 4)) return ZMT_ST_TRUNCATED;
+        *skip = 8 + (uint64_t)zf_rd32(p + 4);
+        return ZMT_ST_OK;
+    }
+    if (zstd) return magic >= 0xFD2FB522u && magic <= ZMT_ZSTD_MAGIC ? ZMT_ST_OK : ZMT_ST_BAD_MAGIC;
+    if (magic != ZMT_LZ4F_MAGIC) return ZMT_ST_BAD_MAGIC;
+    if (n < 7) return ZMT_ST_TRUNCATED;
+    if ((p[4] >> 6) != 1 || ((p[5] >> 4) & 7) < 4) return ZMT_ST_BAD_HEADER;
+    return ZMT_ST_OK;
+}
+
+// The rest of the decision for an LZ4F frame whose head passed: p[0..n) = the stream's bytes from the frame start.
+// ZMT_ST_OK: *len = the frame's length (content checksum included), *room = its content size, or the block bound
+// (blockMaxSize per compressed block) without one.  ZMT_ST_TRUNCATED: the header or a block runs past n; *stop = the
+// block header the walk could not read, or n.  ZMT_ST_CONTENT_SIZE: a content size above the block bound (*stop = 0):
+// the field is untrusted, and a plain frame has no payload size to bound it by but its own blocks.
+ZMT_HD int lz4f_plain_frame(const uint8_t* p, size_t n, uint64_t* len, uint64_t* room, uint64_t* stop)
+{
+    Lz4fWalk w; w.pos = lz4f_header_len(p[4]); w.bound = 0; w.nblk = 0; w.done = 0;
+    *stop = 0;
+    if (!lz4f_walk_blocks(p, n, p[4], p[5], &w, ~(size_t)0, ~0ull) || w.pos > n) { *stop = w.pos < n ? w.pos : n; return ZMT_ST_TRUNCATED; }
+    *len = w.pos; *room = w.bound;
+    if (p[4] & 8) {
+        const uint64_t cs = zf_rd64(p + 6);
+        if (cs > w.bound) return ZMT_ST_CONTENT_SIZE;
+        *room = cs;
+    }
+    return ZMT_ST_OK;
+}
 
 // ---------------------------------------------------------------- zstd block descriptors (the zstd decoder's block table)
 #define ZB_RAW 0u
@@ -201,11 +249,14 @@ ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint3
             at += sl[i];
         }
     }
+    uint32_t bh_next = 0;                                             // the next block header, when loaded ahead (have_next)
+    bool have_next = false;
     for (;;) {
         w->pos = at0 + pos;
         if (walked && (pos >= pos_stop || bnd >= bound_stop)) { *bound = bnd; return ZMT_ST_OK; }
         if (n - pos < 3) return ZMT_ST_TRUNCATED;
-        const uint32_t bh = p[pos] | (p[pos + 1] << 8) | ((uint32_t)p[pos + 2] << 16); pos += 3;
+        const uint32_t bh = have_next ? bh_next : zf_rd24(p + pos); pos += 3;
+        have_next = false;
         const uint32_t last = bh & 1, type = (bh >> 1) & 3, bs = bh >> 3;
         if (type == 3 || bs > 128 * 1024) return ZMT_ST_BLOCK;
         if (*nblocks_io >= max_blocks) return ZMT_ST_DST_SMALL;
@@ -216,6 +267,9 @@ ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint3
         else if (type == ZB_RLE) { if (n - pos < 1) return ZMT_ST_TRUNCATED; B.comp_size = 1; B.regen_hint = bs; pos += 1; }
         else {
             if (n - pos < bs || bs < 2) return ZMT_ST_TRUNCATED;
+            // the walk is a chain of dependent loads: the next block header's goes out before this block's section
+            // headers are parsed, so a compressed block costs one load latency, not three
+            if (!last && n - pos - bs >= 3) { bh_next = zf_rd24(p + pos + bs); have_next = true; }
             const uint8_t* s = p + pos;
             const uint32_t b0 = s[0], lt = b0 & 3, sf = (b0 >> 2) & 3;
             uint32_t lregen, lcomp, lhdr;

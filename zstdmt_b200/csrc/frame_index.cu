@@ -1,12 +1,18 @@
-// frame_index.cu — the decoders' tables, built on the GPU from a container-framed stream that is already in HBM.
+// frame_index.cu — the decoders' tables, built on the GPU from a stream that is already in HBM.
 //
 // zmt_lz4_decompress_device and zmt_zstd_decompress_device take per-frame tables (and, for zstd, a block table) that the
 // host pipeline builds while its reader walks the headers.  A caller whose stream reaches HBM some other way (GPUDirect
 // Storage, NCCL, our own device compressor) builds them here instead, and the host learns only a summary to size its
-// allocations with:
+// allocations with.  Container-framed streams:
 //   zidx_walk_kernel          one thread follows the chain of 12-byte container headers (one dependent load per frame)
 //   zidx_lz4_frames_kernel    one thread per frame: the LZ4F room rule (lz4f_out_size) and the block-table slot count
 //   zidx_zstd_frames_kernel   one thread per frame: the counting walk of zstd_frame_walk (blocks, scratch, content size, flags)
+// Plain streams (.lz4 / .zst files: codec frames and skippable frames back to back), where a frame's end is only known
+// by walking its block headers:
+//   zidx_plain_walk_kernel    one thread walks the stream with the host plain path's rule (plain_frame_head, then
+//                             lz4f_plain_frame or the counting walk of zstd_frame_walk) and writes every per-frame entry
+//   zidx_plain_tail_kernel    one thread per entry: zeroes the entries behind the stored frames for the scans
+// Both then share:
 //   cub::DeviceScan           exclusive sums in place: output offsets, first block, scratch bases, slots
 //   zidx_summary_kernel       one thread: the first failure in stream order and the totals (zmt_frame_index)
 //   zidx_zstd_blocks_kernel   one thread per frame: the writing walk of zstd_frame_walk fills the ZBlk table
@@ -20,14 +26,14 @@ extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels
 namespace {
 
 constexpr uint32_t kThreads = 128;
-constexpr uint64_t kMaxIndexBytes = 3ull * 0xFFFFFFFFull;     // frames (>= 12 B), zstd blocks (>= 3 B) and LZ4 slots then fit in 32 bits
+constexpr uint64_t kMaxIndexBytes = 3ull * 0xFFFFFFFFull;     // frames (>= 9 B), zstd blocks (>= 3 B) and LZ4 slots then fit in 32 bits
 
 struct IdxCtl {
-    uint32_t nframes;       // container headers accepted
-    uint32_t cstatus;       // ZMT_ST_* of the container walk
+    uint32_t nframes;       // frames the walk accepted
+    uint32_t cstatus;       // ZMT_ST_* of the walk
     uint32_t first_bad;     // lowest frame index whose per-frame pass failed (~0: none)
     uint32_t pad;
-    uint64_t coff;          // stream offset where the container walk stopped
+    uint64_t coff;          // stream offset where the walk stopped (on failure: where in the failing frame)
     uint64_t max_off;       // offset of frame max_frames' header (the first one not stored)
 };
 
@@ -119,6 +125,60 @@ zidx_zstd_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restri
     if (f < max_frames) { expect[f] = (flags & ZF_NO_SIZE) ? ~0ull : cs; frame_seq[f] = flags; }
 }
 
+// The plain stream in[0..in_bytes): skippable frames are stepped over, every codec frame is decided by the host plain
+// path's rule, and the first failure ends the walk (the next frame's start is not known behind it).  Frame f < max_frames
+// gets its offset, length, room and (LZ4) slot count or (zstd) block count, scratch, expect and flags; the scans make the
+// counts bases.  The decode calls take frame_csize as 32 bits: a frame of 2^32 bytes or more is ZMT_ST_UNSUPPORTED.
+template <bool Z>
+__global__ void zidx_plain_walk_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t max_frames, uint64_t* __restrict__ frame_off,
+                                       uint32_t* __restrict__ frame_csize, uint64_t* __restrict__ out_off, uint64_t* __restrict__ slots,
+                                       uint32_t* __restrict__ first_blk, uint64_t* __restrict__ frame_scratch, uint64_t* __restrict__ expect,
+                                       uint32_t* __restrict__ frame_seq, IdxCtl* __restrict__ ctl)
+{
+    uint64_t pos = 0, max_off = 0, at = 0;
+    uint32_t n = 0, st = ZMT_ST_OK;
+    while (pos < in_bytes) {
+        const uint8_t* p = in + pos;
+        const uint64_t rem = in_bytes - pos;
+        uint64_t skip = 0;
+        st = (uint32_t)plain_frame_head(p, rem, Z, &skip);
+        if (st != ZMT_ST_OK) { at = pos; break; }
+        if (skip) { pos += skip; continue; }
+        uint64_t len = 0, room = 0, scr = 0;
+        uint32_t nb = 0, flags = 0;
+        if (Z) {
+            size_t end = 0;
+            st = (uint32_t)zstd_frame_walk<false>(p, rem, 0, 0, nullptr, &nb, 0xFFFFFFFFu, &scr, &room, &flags, &end);
+            len = end; at = pos + end;
+        } else {
+            uint64_t stop = 0;
+            st = (uint32_t)lz4f_plain_frame(p, rem, &len, &room, &stop);
+            at = pos + stop;
+        }
+        if (st != ZMT_ST_OK) break;
+        if (len > 0xFFFFFFFFull) { st = ZMT_ST_UNSUPPORTED; at = pos; break; }
+        if (n < max_frames) {
+            frame_off[n] = pos; frame_csize[n] = (uint32_t)len; out_off[n] = room;
+            if (Z) { first_blk[n] = nb; frame_scratch[n] = scr; expect[n] = (flags & ZF_NO_SIZE) ? ~0ull : room; frame_seq[n] = flags; }
+            else slots[n] = lz4_frame_slots(room);
+        } else if (n == max_frames) max_off = pos;
+        n++; pos += len;
+    }
+    ctl->nframes = n; ctl->cstatus = st; ctl->first_bad = 0xFFFFFFFFu; ctl->coff = st == ZMT_ST_OK ? pos : at; ctl->max_off = max_off;
+}
+
+// f in [min(nframes, max_frames), max_frames]: the entries behind the stored frames are zeroed, as the frame passes of
+// the container path do, so the scans over max_frames + 1 entries leave the totals at index min(nframes, max_frames)
+__global__ void __launch_bounds__(kThreads)
+zidx_plain_tail_kernel(IdxWork k, uint32_t max_frames, uint64_t* __restrict__ out_off, uint32_t* __restrict__ first_blk, uint64_t* __restrict__ frame_scratch)
+{
+    const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+    if (f > max_frames || f < min(k.ctl->nframes, max_frames)) return;
+    out_off[f] = 0;
+    if (first_blk) { first_blk[f] = 0; frame_scratch[f] = 0; }
+    else k.slots[f] = 0;
+}
+
 __global__ void zidx_summary_kernel(IdxWork k, uint32_t max_frames, const uint64_t* __restrict__ out_off, const uint32_t* __restrict__ first_blk,
                                     const uint64_t* __restrict__ frame_scratch, zmt_frame_index* __restrict__ info)
 {
@@ -149,10 +209,11 @@ zidx_zstd_blocks_kernel(const uint8_t* __restrict__ in, uint32_t nframes, const 
     zstd_frame_walk<true>(in + p, frame_csize[f], p, f, blocks, &nb, lim, &scr, &cs, &flags, &end);
 }
 
-// The common part of both index calls: container walk, per-frame pass, scans, summary.
-template <typename FramePass>
+// The common part of the index calls: the walk, the per-frame pass, scans, summary.  walk(k) enqueues the walk,
+// pass(grid, k) the per-frame pass over max_frames + 1 entries.
+template <typename Walk, typename FramePass>
 int index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize, uint64_t* d_out_off,
-                 uint32_t* d_first_blk, uint64_t* d_frame_scratch, zmt_frame_index* d_info, void* d_work, cudaStream_t stream, FramePass pass)
+                 uint32_t* d_first_blk, uint64_t* d_frame_scratch, zmt_frame_index* d_info, void* d_work, cudaStream_t stream, Walk walk, FramePass pass)
 {
     if (in_bytes > kMaxIndexBytes || max_frames >= 0x7FFFFFFFu || !d_info || !d_work || !d_out_off || (max_frames && (!d_frame_off || !d_frame_csize)))
         return ZMT_ST_BAD_ARG;
@@ -161,7 +222,7 @@ int index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint6
     const IdxWork k = carve(d_work, max_frames, tb);
     const int nitems = (int)max_frames + 1;
     zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
-    zidx_walk_kernel<<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k.ctl);
+    walk(k);
     pass((max_frames + kThreads) / kThreads, k);
     size_t t = k.tmp_bytes;
     bool ok = cub::DeviceScan::ExclusiveSum(k.tmp, t, d_out_off, nitems, stream) == cudaSuccess;
@@ -174,6 +235,11 @@ int index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint6
     zidx_summary_kernel<<<1, 1, 0, stream>>>(k, max_frames, d_out_off, d_first_blk, d_frame_scratch, d_info);
     zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return ok && cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+void container_walk(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize, IdxWork k, cudaStream_t stream)
+{
+    zidx_walk_kernel<<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k.ctl);
 }
 
 }  // namespace
@@ -191,6 +257,7 @@ extern "C" int zmt_lz4_index_device(const void* d_in, uint64_t in_bytes, uint32_
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, nullptr, nullptr, d_info, d_work, stream,
+                        [&](IdxWork k) { container_walk(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k, stream); },
                         [&](uint32_t grid, IdxWork k) {
                             zidx_lz4_frames_kernel<<<grid, kThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, d_frame_csize, d_out_off, k, max_frames);
                         });
@@ -203,9 +270,38 @@ extern "C" int zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!d_frame_first_blk || !d_frame_scratch || (max_frames && (!d_expect || !d_frame_seq))) return ZMT_ST_BAD_ARG;
     return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, d_frame_first_blk, d_frame_scratch, d_info, d_work, stream,
+                        [&](IdxWork k) { container_walk(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k, stream); },
                         [&](uint32_t grid, IdxWork k) {
                             zidx_zstd_frames_kernel<<<grid, kThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, d_frame_csize, d_frame_first_blk,
                                                                                  d_frame_scratch, d_expect, d_frame_seq, d_out_off, k, max_frames);
+                        });
+}
+
+extern "C" int zmt_lz4_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                          uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, nullptr, nullptr, d_info, d_work, stream,
+                        [&](IdxWork k) {
+                            zidx_plain_walk_kernel<false><<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off,
+                                                                               k.slots, nullptr, nullptr, nullptr, nullptr, k.ctl);
+                        },
+                        [&](uint32_t grid, IdxWork k) { zidx_plain_tail_kernel<<<grid, kThreads, 0, stream>>>(k, max_frames, d_out_off, nullptr, nullptr); });
+}
+
+extern "C" int zmt_zstd_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                           uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                           uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!d_frame_first_blk || !d_frame_scratch || (max_frames && (!d_expect || !d_frame_seq))) return ZMT_ST_BAD_ARG;
+    return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, d_frame_first_blk, d_frame_scratch, d_info, d_work, stream,
+                        [&](IdxWork k) {
+                            zidx_plain_walk_kernel<true><<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off,
+                                                                              k.slots, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq, k.ctl);
+                        },
+                        [&](uint32_t grid, IdxWork k) {
+                            zidx_plain_tail_kernel<<<grid, kThreads, 0, stream>>>(k, max_frames, d_out_off, d_frame_first_blk, d_frame_scratch);
                         });
 }
 

@@ -898,17 +898,16 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
             const uint8_t* s = in.data() + 12; const size_t n = in.size() - 12;
             if (pos >= n) { need_more = !S.eof; break; }
             if (fl.n() && pos - batch_start >= S.batch) break;
-            if (n - pos < 4) { if (S.eof) return E.data_error; need_more = true; break; }
-            const uint32_t magic = zf_rd32(s + pos);
-            if ((magic & 0xFFFFFFF0u) == ZMT_CONTAINER_MAGIC) {    // skippable frame: magic, LE32 size, payload
-                if (n - pos < 8 || n - pos - 8 < zf_rd32(s + pos + 4)) { if (S.eof) return E.data_error; need_more = true; break; }
-                pos += 8 + (size_t)zf_rd32(s + pos + 4); continue;
-            }
+            // the frame start: a skippable frame, or a codec frame whose head is usable (the rule the device's plain
+            // index takes too, frame_format.h); a start cut short or a foreign magic is a data error of the stream
+            uint64_t skip = 0;
+            const int h = plain_frame_head(s + pos, n - pos, S.is_zstd, &skip);
+            if (h == ZMT_ST_TRUNCATED) { if (S.eof) return E.data_error; need_more = true; break; }
+            if (h == ZMT_ST_BAD_MAGIC) return E.data_error;
+            if (h != ZMT_ST_OK) return frame_error(c, h);
+            if (skip) { pos += (size_t)skip; continue; }
             if (!S.is_zstd) {
-                if (magic != ZMT_LZ4F_MAGIC) return E.data_error;
-                if (n - pos < 7) { if (S.eof) return E.data_error; need_more = true; break; }
-                const uint32_t flg = s[pos + 4], bd = s[pos + 5], id = (bd >> 4) & 7;
-                if ((flg >> 6) != 1 || id < 4) return frame_error(c, ZMT_ST_BAD_HEADER);
+                const uint32_t flg = s[pos + 4], bd = s[pos + 5];
                 {
                     // a frame whose blocks reach a batch of input or four of output before its end: decoded in segments,
                     // after the frames in front of it
@@ -920,17 +919,16 @@ size_t decompress_single_stream(Ctx* c, GenRdWr* rw, const uint8_t* first, size_
                         segmented = true; break;
                     }
                 }
-                size_t len = 0; uint64_t bound = 0;
-                if (!lz4f_walk(s + pos, n - pos, &len, &bound) || len > n - pos) {
+                uint64_t len = 0, osz = 0, stop = 0;
+                const int r = lz4f_plain_frame(s + pos, n - pos, &len, &osz, &stop);
+                if (r == ZMT_ST_TRUNCATED) {
                     if (S.eof) return frame_error(c, ZMT_ST_TRUNCATED);
                     need_more = true; break;
                 }
-                uint64_t osz = bound;
-                if (flg & 8) { osz = zf_rd64(s + pos + 6); if (osz > bound) return frame_error(c, ZMT_ST_CONTENT_SIZE); }    // untrusted field, bounded by the block walk
+                if (r != ZMT_ST_OK) return frame_error(c, r);
                 fl.push(pos, (uint32_t)len, osz);
-                pos += len;
+                pos += (size_t)len;
             } else {
-                if (magic < 0xFD2FB522u || magic > ZMT_ZSTD_MAGIC) return E.data_error;
                 {
                     // a frame whose blocks reach a batch of input or four of output before its end: decoded in segments,
                     // after the frames in front of it
