@@ -288,6 +288,79 @@ int      zmt_zstd_decompress_segments_device(const void* d_in, const void* d_blo
                                              const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* d_seg,
                                              void* d_work, void* stream);
 
+/* ---- Range reads: byte ranges of a stream's content, decoding only the frames that hold them ----
+ * On top of the device index above (container or plain; for a plain stream pass d_in - 12 as to the decode calls).  The
+ * unit of access is the frame: a frame's content is only known by decoding it whole, so every frame a range touches is
+ * decoded once per batch, however many ranges touch it, and every other frame is not read at all.
+ *
+ * Content table, once per stream: d_content_off[0..nframes] = the exclusive prefix of the frames' content sizes, each
+ * from the frame's own header (LZ4F FLG bit 3 + LE64 field; zstd Frame_Content_Size, i.e. d_expect of the zstd index).
+ * The summary is a zmt_frame_index: status, bad_frame (nframes when OK), bad_offset = d_frame_off[bad_frame],
+ * nframes, out_bytes = the total content; nblocks and scratch_bytes are 0.  status:
+ *   ZMT_ST_UNSUPPORTED   a frame without a content size (the lz4 CLI's default, zstd written to a pipe): its content
+ *                        position cannot be known without decoding every frame before it
+ *   ZMT_ST_CONTENT_SIZE  a stated content size above 32768 bytes per compressed byte, more than either format can
+ *                        produce: a damaged header, which would wrap the table
+ * The first such frame in stream order is named.  d_work: zmt_range_workspace_bytes(nframes, 0).
+ *
+ * Plan, once per batch: d_ranges = nranges pairs {start, length} in content coordinates, in any order, overlapping,
+ * repeated or empty.  A range [start, start + length) is bad (ZMT_ST_BAD_ARG) when it ends past the content or
+ * start + length overflows; a bad range takes no room in dst.  The plan finds the frames each good range touches, marks
+ * them, and writes the decode tables of the marked frames (the "selected" frames, in stream order) into d_work, which
+ * must then stay untouched until the batch's read call.  d_dst_off[0..nranges] = the exclusive prefix of the lengths of
+ * the good ranges: range r's bytes go to dst + d_dst_off[r].  The host reads back the zmt_range_plan summary and sizes
+ * the read's buffers from it; the workspace only depends on nframes and nranges.
+ *
+ * Read, once per batch, with the plan's d_work and a host copy of its summary:
+ *   LZ4    a kernel packs the selected frames (a 12-byte container header and the payload each) into the read
+ *          workspace, and zmt_lz4_decompress_device decodes that packed stream, so its match records cover only the
+ *          selected frames' compressed bytes, not the stream's;
+ *   zstd   zmt_zstd_blocks_device builds the selected frames' block table and zmt_zstd_decompress_device decodes them
+ *          in place in d_in (its workspace does not depend on the input's size);
+ * both decode into d_scratch (plan.scratch_bytes: the selected frames' content back to back), then a gather kernel
+ * copies every good range to dst + d_dst_off[r] (any alignment) in pieces of at most 64 KiB.  d_range_status[r]:
+ *   ZMT_ST_OK, ZMT_ST_BAD_ARG for a bad range (its dst bytes are not written), or the decoder's status of the first frame
+ *   the range touches that failed (BLOCK, CONTENT_CHECKSUM, ...; its dst bytes are not written).
+ * Selected frames are decoded whole, so their content checksums (and LZ4F block checksums) are verified as in a
+ * whole-stream decode.  A damaged frame no range of the batch touches is not decoded, and so its damage is not reported.
+ * Memory per batch: the plan's workspace is O(nframes + nranges); the read's workspace (zmt_*_range_read_workspace_bytes)
+ * and d_scratch are O(selected compressed bytes + selected content), never O(stream):
+ *   LZ4    256-aligned packed_bytes + zmt_lz4d_workspace_bytes(nsel, nunits, packed_bytes)
+ *   zstd   256-aligned nunits * zmt_zstd_blk_desc_bytes() + zmt_zstdd_workspace_bytes(nsel, nunits, dec_scratch)
+ * All calls return ZMT_ST_OK once enqueued, ZMT_ST_BAD_ARG or ZMT_ST_CUDA. */
+typedef struct {
+    uint32_t status;        /* ZMT_ST_OK, or ZMT_ST_BAD_ARG when a range is bad (the other ranges are planned and read) */
+    uint32_t bad_range;     /* the first bad range (== nranges when none) */
+    uint32_t nframes;       /* the plan's arguments, for the read call */
+    uint32_t nranges;
+    uint32_t nsel;          /* selected frames: the frames the good ranges touch */
+    uint32_t nunits;        /* LZ4: block-table slots of the selected frames; zstd: their blocks */
+    uint64_t packed_bytes;  /* LZ4: bytes of the packed stream of the selected frames (0 for zstd) */
+    uint64_t scratch_bytes; /* the selected frames' content: the size of d_scratch */
+    uint64_t dec_scratch;   /* zstd: the selected frames' entropy scratch (third argument of zmt_zstdd_workspace_bytes) */
+    uint64_t dst_bytes;     /* d_dst_off[nranges]: the size of dst */
+    uint64_t npieces;       /* gather pieces (at most 64 KiB each) */
+} zmt_range_plan;
+
+size_t   zmt_range_workspace_bytes(uint32_t nframes, uint32_t nranges);
+int      zmt_lz4_content_offsets_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                        uint64_t* d_content_off, zmt_frame_index* d_info, void* d_work, void* stream);
+int      zmt_zstd_content_offsets_device(uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, const uint64_t* d_expect,
+                                         uint64_t* d_content_off, zmt_frame_index* d_info, void* d_work, void* stream);
+int      zmt_lz4_range_plan_device(uint32_t nframes, const uint32_t* d_frame_csize, const uint64_t* d_content_off, const uint64_t* d_ranges,
+                                   uint32_t nranges, uint64_t* d_dst_off, zmt_range_plan* d_plan, void* d_work, void* stream);
+int      zmt_zstd_range_plan_device(uint32_t nframes, const uint32_t* d_frame_csize, const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch,
+                                    const uint64_t* d_content_off, const uint64_t* d_ranges, uint32_t nranges, uint64_t* d_dst_off,
+                                    zmt_range_plan* d_plan, void* d_work, void* stream);
+size_t   zmt_lz4_range_read_workspace_bytes(const zmt_range_plan* plan);
+size_t   zmt_zstd_range_read_workspace_bytes(const zmt_range_plan* plan);
+int      zmt_lz4_range_read_device(const void* d_in, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, const zmt_range_plan* plan,
+                                   void* d_dst, const uint64_t* d_dst_off, uint32_t* d_range_status, void* d_scratch, void* d_read_work,
+                                   void* d_work, void* stream);
+int      zmt_zstd_range_read_device(const void* d_in, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, const uint64_t* d_expect,
+                                    const uint32_t* d_frame_seq, const zmt_range_plan* plan, void* d_dst, const uint64_t* d_dst_off,
+                                    uint32_t* d_range_status, void* d_scratch, void* d_read_work, void* d_work, void* stream);
+
 /* ---- multi-GPU: one LZ4MT_* / ZSTDCB_* call deals its batches round-robin over the devices named by the
  * environment variable ZSTDMT_GPUS ("all" or "0,1,..."; default: the calling thread's current device) and re-serialises
  * the frames on the host.  zmt_device_batches(dev) = batches submitted to that device since the library was loaded. */
@@ -304,7 +377,9 @@ enum { ZMT_K_LZ4_COMPRESS = 0, ZMT_K_XXH32, ZMT_K_LZ4_SIZES, ZMT_K_SCAN, ZMT_K_L
  * ZMT_K_ZL_BLOCKS = lazy parse + entropy stage (the frame pack stays ZMT_K_ZSTD_PACK)
  * LZ4 levels 10-12: hash, sort and search as zstd's (ZMT_K_ZL_HASH / SORT / SEARCH), ZMT_K_L4H_BLOCKS = lazy parse +
  * LZ4 sequences; checksum, sizes, scan and pack as level 1's
- * ZMT_K_FRAME_INDEX = one index call (container or plain walk, frame pass, scans, summary) or one zmt_zstd_blocks_device call */
+ * ZMT_K_FRAME_INDEX = one index call (container or plain walk, frame pass, scans, summary) or one zmt_zstd_blocks_device call;
+ * range reads report here too, as the index's consumers: one content-table or plan call, and the pack stage and the
+ * status + gather stage of a read call (the decoders inside a read call report under their own ids) */
 void zmt_prof_begin(void);
 int  zmt_prof_end(double* ms, int* count, int max_ids);
 

@@ -100,6 +100,21 @@ def lib():
     L.zmt_zstd_index_plain_device.argtypes = L.zmt_zstd_index_device.argtypes
     L.zmt_zstd_blocks_device.restype = ctypes.c_int
     L.zmt_zstd_blocks_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_vp]
+    L.zmt_range_workspace_bytes.restype = c_sz; L.zmt_range_workspace_bytes.argtypes = [c_u32, c_u32]
+    L.zmt_lz4_content_offsets_device.restype = ctypes.c_int
+    L.zmt_lz4_content_offsets_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_content_offsets_device.restype = ctypes.c_int
+    L.zmt_zstd_content_offsets_device.argtypes = [c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_lz4_range_plan_device.restype = ctypes.c_int
+    L.zmt_lz4_range_plan_device.argtypes = [c_u32, c_vp, c_vp, c_vp, c_u32, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_range_plan_device.restype = ctypes.c_int
+    L.zmt_zstd_range_plan_device.argtypes = [c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_vp, c_vp, c_vp, c_vp]
+    for k in ("lz4", "zstd"):
+        f = getattr(L, "zmt_%s_range_read_workspace_bytes" % k); f.restype = c_sz; f.argtypes = [ctypes.POINTER(RangePlan)]
+    L.zmt_lz4_range_read_device.restype = ctypes.c_int
+    L.zmt_lz4_range_read_device.argtypes = [c_vp, c_vp, c_vp, ctypes.POINTER(RangePlan), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.zmt_zstd_range_read_device.restype = ctypes.c_int
+    L.zmt_zstd_range_read_device.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.POINTER(RangePlan), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     for pre, api in (("LZ4MT", "lz4"), ("ZSTDCB", "zstd"), ("ZSTDMT", "zstd")):
         getattr(L, pre + "_createCCtx").restype = c_vp; getattr(L, pre + "_createCCtx").argtypes = [ctypes.c_int] * 3
         getattr(L, pre + "_createDCtx").restype = c_vp; getattr(L, pre + "_createDCtx").argtypes = [ctypes.c_int] * 2
@@ -222,6 +237,15 @@ class FrameIndex(ctypes.Structure):
 
     def __repr__(self):
         return "FrameIndex(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
+
+
+class RangePlan(ctypes.Structure):
+    """zmt_range_plan (include/zstdmt_b200_dev.h): the summary of a range-read plan, read back once per batch."""
+    _fields_ = [("status", c_u32), ("bad_range", c_u32), ("nframes", c_u32), ("nranges", c_u32), ("nsel", c_u32), ("nunits", c_u32),
+                ("packed_bytes", c_u64), ("scratch_bytes", c_u64), ("dec_scratch", c_u64), ("dst_bytes", c_u64), ("npieces", c_u64)]
+
+    def __repr__(self):
+        return "RangePlan(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
 
 
 # The plain index writes its tables for a base this many bytes below the stream: the decode calls address a frame as
@@ -606,3 +630,99 @@ class ZstdDeviceDecompressor:
         if rc != 0:
             raise RuntimeError("zmt_zstd_decompress_device failed: %s" % ST_NAMES.get(rc, rc))
         return self.out, self.status
+
+
+class RangeReader:
+    """Byte ranges of a compressed stream that is already in device memory, decoding only the frames that hold them.
+
+    The constructor indexes the stream once on the GPU (as from_device does; plain=True for a plain .lz4 / .zst stream)
+    and builds its content table: the content offset of every frame, from the sizes the frames' headers state.  A stream
+    with a frame that states no content size cannot be range-read: ValueError names the status and the frame.
+    read(ranges) takes an int64 (M, 2) tensor of (start, length) pairs in content coordinates, on the CPU or the GPU, and
+    returns CUDA tensors (bytes, dst_off, status): range r's bytes are bytes[dst_off[r]:dst_off[r + 1]], status[r] is its
+    ZMT_ST_* code.  Every frame a range touches is decoded once per batch, the others are not read.  Buffers are kept
+    across batches and grown when a batch needs more; .plan is the last batch's RangePlan summary."""
+
+    def __init__(self, d_stream, codec, plain=False, max_frames=None, stream=None):
+        torch = _torch(); L = lib()
+        if codec in ("lz4", CODEC_LZ4):
+            self.zstd = False
+        elif codec in ("zstd", CODEC_ZSTD):
+            self.zstd = True
+        else:
+            raise ValueError("unknown codec %r" % (codec,))
+        s = stream if stream is not None else torch.cuda.current_stream()
+        self.d_stream, self.dev = d_stream, d_stream.device
+        self.pad = PLAIN_PAD if plain else 0
+        self.index_info, self.t = _device_index(d_stream, max_frames, s, zstd=self.zstd, plain=plain)
+        self.n = self.index_info.nframes
+        self.content_off = torch.empty(self.n + 1, dtype=torch.int64, device=self.dev)
+        d_info = torch.zeros(ctypes.sizeof(FrameIndex), dtype=torch.uint8, device=self.dev)
+        self.work = torch.empty(L.zmt_range_workspace_bytes(self.n, 0), dtype=torch.uint8, device=self.dev)
+        p = lambda k: self.t[k].data_ptr()
+        if self.zstd:
+            rc = L.zmt_zstd_content_offsets_device(self.n, p("frame_off"), p("frame_csize"), p("expect"), self.content_off.data_ptr(),
+                                                   d_info.data_ptr(), self.work.data_ptr(), s.cuda_stream)
+        else:
+            rc = L.zmt_lz4_content_offsets_device(self._base(), self.n, p("frame_off"), p("frame_csize"), self.content_off.data_ptr(),
+                                                  d_info.data_ptr(), self.work.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("content table failed: %s" % ST_NAMES.get(rc, rc))
+        s.synchronize()
+        self.content_info = FrameIndex.from_buffer_copy(d_info.cpu().numpy().tobytes())
+        if self.content_info.status != 0:
+            raise ValueError("stream cannot be range-read: %s in frame %d at offset %d" % (
+                ST_NAMES.get(self.content_info.status, self.content_info.status), self.content_info.bad_frame, self.content_info.bad_offset))
+        self.content_size = self.content_info.out_bytes
+        self.scratch = torch.empty(1, dtype=torch.uint8, device=self.dev)
+        self.read_work = torch.empty(1, dtype=torch.uint8, device=self.dev)
+        self.plan = None
+        self.read_work_bytes = 0
+
+    def _base(self):
+        return self.d_stream.data_ptr() - self.pad
+
+    def _grow(self, name, nbytes):
+        torch = _torch()
+        if getattr(self, name).numel() < nbytes:
+            setattr(self, name, torch.empty(nbytes, dtype=torch.uint8, device=self.dev))
+        return getattr(self, name)
+
+    def read(self, ranges, stream=None):
+        torch = _torch(); L = lib()
+        s = stream if stream is not None else torch.cuda.current_stream()
+        r = torch.as_tensor(ranges)
+        if r.dtype != torch.int64 or r.dim() != 2 or r.shape[1] != 2:
+            raise ValueError("ranges must be an int64 (M, 2) tensor of (start, length)")
+        r = r.to(self.dev).contiguous()
+        m = r.shape[0]
+        work = self._grow("work", L.zmt_range_workspace_bytes(self.n, m))
+        dst_off = torch.empty(m + 1, dtype=torch.int64, device=self.dev)
+        d_plan = torch.zeros(ctypes.sizeof(RangePlan), dtype=torch.uint8, device=self.dev)
+        p = lambda k: self.t[k].data_ptr()
+        if self.zstd:
+            rc = L.zmt_zstd_range_plan_device(self.n, p("frame_csize"), p("first_blk"), p("frame_scratch"), self.content_off.data_ptr(), r.data_ptr(), m,
+                                              dst_off.data_ptr(), d_plan.data_ptr(), work.data_ptr(), s.cuda_stream)
+        else:
+            rc = L.zmt_lz4_range_plan_device(self.n, p("frame_csize"), self.content_off.data_ptr(), r.data_ptr(), m, dst_off.data_ptr(),
+                                             d_plan.data_ptr(), work.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("range plan failed: %s" % ST_NAMES.get(rc, rc))
+        s.synchronize()
+        plan = RangePlan.from_buffer_copy(d_plan.cpu().numpy().tobytes())
+        self.plan = plan
+        scratch = self._grow("scratch", max(plan.scratch_bytes, 1))
+        ws = (L.zmt_zstd_range_read_workspace_bytes if self.zstd else L.zmt_lz4_range_read_workspace_bytes)(ctypes.byref(plan))
+        self.read_work_bytes = ws
+        read_work = self._grow("read_work", max(ws, 1))
+        out = torch.empty(max(plan.dst_bytes, 1), dtype=torch.uint8, device=self.dev)
+        status = torch.empty(max(m, 1), dtype=torch.int32, device=self.dev)
+        if self.zstd:
+            rc = L.zmt_zstd_range_read_device(self._base(), p("frame_off"), p("frame_csize"), p("expect"), p("frame_seq"), ctypes.byref(plan), out.data_ptr(),
+                                              dst_off.data_ptr(), status.data_ptr(), scratch.data_ptr(), read_work.data_ptr(), work.data_ptr(), s.cuda_stream)
+        else:
+            rc = L.zmt_lz4_range_read_device(self._base(), p("frame_off"), p("frame_csize"), ctypes.byref(plan), out.data_ptr(), dst_off.data_ptr(),
+                                             status.data_ptr(), scratch.data_ptr(), read_work.data_ptr(), work.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("range read failed: %s" % ST_NAMES.get(rc, rc))
+        return out[: plan.dst_bytes], dst_off, status[:m]

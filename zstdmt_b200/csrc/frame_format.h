@@ -65,6 +65,28 @@ ZMT_HD bool lz4f_walk(const uint8_t* p, size_t n, size_t* len, uint64_t* bound)
     return ok;
 }
 
+// The content size an LZ4F frame's header states: p[0..n) = the frame from its magic.  true: FLG bit 3 is set and the
+// 8-byte field lies inside p[0..n), *cs = its value (untrusted).  false: not an LZ4F frame, no such field, or the header
+// is cut short before it.  Both the decoders' room rule below and the range reads' content table read it here.
+ZMT_HD bool lz4f_content_size(const uint8_t* p, size_t n, uint64_t* cs)
+{
+    if (n < 15 || zf_rd32(p) != ZMT_LZ4F_MAGIC || !(p[4] & 0x08)) return false;
+    *cs = zf_rd64(p + 6);
+    return true;
+}
+
+// The content size of an LZ4F frame known without decoding it: the header's field, or 0 for a frame without one whose
+// first block header is the end mark (liblz4 states no content size for an empty input).  false: neither.
+ZMT_HD bool lz4f_known_content_size(const uint8_t* p, size_t n, uint64_t* cs)
+{
+    if (lz4f_content_size(p, n, cs)) return true;
+    if (n < 7 || zf_rd32(p) != ZMT_LZ4F_MAGIC) return false;
+    const size_t h = lz4f_header_len(p[4]);
+    if (n < h + 4 || zf_rd32(p + h) != 0) return false;
+    *cs = 0;
+    return true;
+}
+
 // The room one LZ4 payload of n bytes gets in the output, from its own header (pt_decompress sizes the buffer from
 // LE64 @ payload+6, lz4-mt_decompress.c:329-335).  Returns false if the header is unusable (ZMT_ST_BAD_HEADER).
 // A payload without the LZ4F magic gets room 0: the decoder reports its precise status.
@@ -73,10 +95,10 @@ ZMT_HD bool lz4f_out_size(const uint8_t* p, size_t n, uint64_t* out)
     if (n < 7 || zf_rd32(p) != ZMT_LZ4F_MAGIC) { *out = 0; return true; }
     const uint32_t flg = p[4], bd = p[5];
     if (flg & 0x08) {
-        if (n < 15) return false;
+        uint64_t v = 0;
+        if (!lz4f_content_size(p, n, &v)) return false;
         // untrusted field: LZ4 cannot expand by more than 255x, anything larger is a corrupt header (the reference
         // fails its malloc there); without this bound a huge value would wrap the running output offsets
-        const uint64_t v = zf_rd64(p + 6);
         if (v > (uint64_t)n * 255 + 65536) return false;
         *out = v; return true;
     }
@@ -129,8 +151,8 @@ ZMT_HD int lz4f_plain_frame(const uint8_t* p, size_t n, uint64_t* len, uint64_t*
     *stop = 0;
     if (!lz4f_walk_blocks(p, n, p[4], p[5], &w, ~(size_t)0, ~0ull) || w.pos > n) { *stop = w.pos < n ? w.pos : n; return ZMT_ST_TRUNCATED; }
     *len = w.pos; *room = w.bound;
-    if (p[4] & 8) {
-        const uint64_t cs = zf_rd64(p + 6);
+    uint64_t cs = 0;
+    if (lz4f_content_size(p, n, &cs)) {
         if (cs > w.bound) return ZMT_ST_CONTENT_SIZE;
         *room = cs;
     }
