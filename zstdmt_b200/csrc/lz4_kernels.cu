@@ -107,52 +107,72 @@ struct LzBack {
                                                            // 4096/37 + 1 pending per tile -- and 255-runs of match lengths >= 1290 (count, offset | 1<<31)
 };
 
-// number of bytes (<= cap) for which s[p + i] == s[p + i - d].  Word compares only: the last, partial word gets a
-// sentinel bit at byte `cap` (reads run at most 3 bytes past p + cap: LzStage::in carries 32 pad bytes).
-__device__ __forceinline__ uint32_t c_extend(const uint8_t* s, uint32_t p, uint32_t d, uint32_t cap)
+// the 16 bytes at s + pos, any alignment: five aligned words
+__device__ __forceinline__ uint4 lds128u(const uint8_t* s, uint32_t pos)
 {
-    uint32_t L = 0;
-    for (;;) {
-        uint32_t x = lds32u(s, p + L) ^ lds32u(s, p + L - d);
-        const uint32_t rem = cap - L;
-        if (rem < 4) x |= 1u << (8 * rem);
-        if (x) return L + ((__ffs(x) - 1) >> 3);
-        L += 4;
-    }
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(s) + (pos >> 2);
+    const uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3], w4 = w[4], sh = 8 * (pos & 3);
+    return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
+}
+
+// number of leading bytes (<= cap <= 16) in which the 16-byte strings a and b agree: one mismatch scan, no loop
+__device__ __forceinline__ uint32_t c_agree16(uint4 a, uint4 b, uint32_t cap)
+{
+    const uint32_t x0 = a.x ^ b.x, x1 = a.y ^ b.y, x2 = a.z ^ b.z, x3 = a.w ^ b.w;
+    // index of the first differing bit (128: none), by selects: __clz(__brev(0)) is 32
+    uint32_t m = 96 + __clz(__brev(x3));
+    m = x2 ? 64 + __clz(__brev(x2)) : m;
+    m = x1 ? 32 + __clz(__brev(x1)) : m;
+    m = x0 ? __clz(__brev(x0)) : m;
+    m >>= 3;
+    return m < cap ? m : cap;
+}
+
+// Length (<= cap <= 16) of a continuation piece: the bytes from the segment boundary p on that still match at offset d.
+// Both 16-byte strings are loaded at once (p is 16-aligned, LzStage::in too; reads run at most 19 bytes past p - d).
+__device__ __forceinline__ uint32_t c_cont_len(const uint8_t* s, uint32_t p, uint32_t d, uint32_t cap)
+{
+    return c_agree16(*reinterpret_cast<const uint4*>(s + p), lds128u(s, p - d), cap);
+}
+
+// L - 4 of the candidate piece at q (offset d, 4 bytes known equal), up to end = min(cut, limit) (q + 4 <= end <= q + 19):
+// both 16-byte strings loaded at once, one mismatch scan
+__device__ __forceinline__ uint32_t c_piece_len4(const uint8_t* s, uint32_t q, uint32_t d, uint32_t end)
+{
+    return c_agree16(lds128u(s, q + 4), lds128u(s, q + 4 - d), end - (q + 4));
 }
 
 // Walk one speculative chain through the tile.  The greedy parse is evaluated piecewise: a match is cut at
 // the first segment boundary that leaves it >= 4 bytes, and continues ("inside", din = its offset) into the
-// next segment, so no lane ever compares more than 19 bytes per step.  Pieces are merged again at emission.
+// next segment, so no lane ever compares more than 19 bytes per step, in one compare (c_piece_len4, c_cont_len).
+// Pieces are merged again at emission.
 // A candidate piece's length L (4..19) depends only on its start q (offset, cut, limit), not on the chain that takes it,
 // so the front end records L - 4 per start in T.len4 and the marking walk reads it back; only a Cont piece, whose
 // length depends on the offset carried in, is measured again there.
-//   MODE 0: own segment only (V bits and T.len4 of its 16 positions as plain stores, exit state -> X.xfree/X.xdin)
-//                                                                                         X: LzFront
+// Walk 0 (c_walk0) covers the own segment; c_walk covers the rest:
 //   MODE 1: continuation until it merges into another chain or leaves the tile (-> X.link/X.mpos; ORs the lengths of
 //           its pieces into T.len4: chains that continue alike take the same pieces, and a position walk 0 took is a
-//           merge, so the only writers that meet write the same nibble)
+//           merge, so the only writers that meet write the same nibble)                              X: LzFront
 //   MODE 2: re-walk of a chain that is on the true path, from where the path enters it: marks X.Sel/X.Cont and the
 //           Cont lengths X.clen.  The own segment's pieces are its V bits from there on (one step), the continuation
 //           takes the steps of MODE 1 with the lengths from T.len4, so only Cont steps compare bytes.     X: LzBack
 template <int MODE, class OUT>
 __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, uint32_t k, uint32_t p, uint32_t din, uint32_t t0, uint32_t limit)
 {
+    static_assert(MODE == 1 || MODE == 2, "walk 0 is c_walk0");
     const uint32_t t1 = t0 + C_TILE;
     uint32_t lk = 0xFFFFFFFFu, mp = 0;
-    uint32_t vb = 0, lo = 0, hi = 0;                 // MODE 0: V bits and len4 words of the own segment
     bool done = false;
     while (!done) {                                  // single exit: the warp reconverges before the next barrier
         if (p >= t1) { lk = C_END; mp = p; done = true; continue; }
         const uint32_t rel = p - t0, j = rel / C_SEG;
-        if (MODE == 0 && j != k) { mp = p; done = true; continue; }
         if (din) {
             // inside a match with offset din that covered everything up to the boundary p
-            if (MODE != 0 && j != k && ((T.M[rel >> 5] >> (rel & 31)) & 1) && T.off[rel] == din) {
+            if (j != k && ((T.M[rel >> 5] >> (rel & 31)) & 1) && T.off[rel] == din) {
                 lk = j; mp = p; done = true; continue;          // chain j's own first step is this very match
             }
             uint32_t cap = p < limit ? limit - p : 0; if (cap > C_SEG) cap = C_SEG;
-            const uint32_t E = c_extend(in, p, din, cap);
+            const uint32_t E = c_cont_len(in, p, din, cap);
             if constexpr (MODE == 2) {
                 if (E) { atomicOr(&X.Sel[rel >> 5], 1u << (rel & 31)); atomicOr(&X.Cont[rel >> 5], 1u << (rel & 31)); X.clen[j] = (uint8_t)E; }
             }
@@ -179,41 +199,64 @@ __device__ __forceinline__ void c_walk(const uint8_t* in, PipeTile& T, OUT& X, u
                 continue;
             }
         }
-        if (MODE != 0 && j != k && (rel & (C_SEG - 1)) == 0) { lk = j; mp = p; done = true; continue; }
+        if (j != k && (rel & (C_SEG - 1)) == 0) { lk = j; mp = p; done = true; continue; }
         uint32_t bits = (T.M[rel >> 5] >> (rel & 16)) & 0xFFFFu;     // this segment's 16 candidate bits
         bits &= 0xFFFFu << (rel & 15);
         if (!bits) {                                                   // segment exhausted: free at its end
-            const uint32_t nx = t0 + (j + 1) * C_SEG;
-            if (MODE == 0) { mp = nx; done = true; }
-            else if (j + 1 == C_CHAINS) { lk = C_END; mp = t1; done = true; }
-            else { lk = j + 1; mp = nx; done = true; }                 // (MODE 1 and 2 reach here outside their own segment)
+            if (j + 1 == C_CHAINS) { lk = C_END; mp = t1; done = true; }
+            else { lk = j + 1; mp = t0 + (j + 1) * C_SEG; done = true; }   // (reached outside the own segment only)
             continue;
         }
         const uint32_t qr = (rel & ~15u) + (__ffs(bits) - 1), q = t0 + qr;
-        if (MODE != 0 && j != k && ((T.V[qr >> 5] >> (qr & 31)) & 1)) { lk = j; mp = q; done = true; continue; }
-        const uint32_t d = T.off[qr];
+        if (j != k && ((T.V[qr >> 5] >> (qr & 31)) & 1)) { lk = j; mp = q; done = true; continue; }
         uint32_t B = (q & ~(C_SEG - 1)) + C_SEG;                     // cut at the first boundary leaving >= 4 bytes
         if (B - q < 4) B += C_SEG;
-        uint32_t L;
+        const uint32_t d = T.off[qr];
+        uint32_t L4;
         if constexpr (MODE == 2) {
-            L = 4 + ((T.len4[qr >> 3] >> (4 * (qr & 7))) & 15u);
+            L4 = (T.len4[qr >> 3] >> (4 * (qr & 7))) & 15u;
             atomicOr(&X.Sel[qr >> 5], 1u << (qr & 31));
         } else {
-            const uint32_t end = B < limit ? B : limit;
-            L = 4 + c_extend(in, q + 4, d, end - (q + 4));              // first 4 bytes are known equal; q + 4 <= limit always
-            const uint32_t nib = (L - 4) << (4 * (qr & 7));
-            if constexpr (MODE == 0) { vb |= 1u << (qr & 15); if (qr & 8) hi |= nib; else lo |= nib; }
-            else atomicOr(&T.len4[qr >> 3], nib);
+            L4 = c_piece_len4(in, q, d, B < limit ? B : limit);       // q + 4 <= limit always
+            atomicOr(&T.len4[qr >> 3], L4 << (4 * (qr & 7)));
         }
-        p = q + L;
+        p = q + 4 + L4;
         if (p == B) din = d;                                          // reached the boundary: still inside the match
     }
-    if constexpr (MODE == 0) {
-        reinterpret_cast<uint16_t*>(T.V)[k] = (uint16_t)vb;
-        *reinterpret_cast<uint2*>(&T.len4[2 * k]) = make_uint2(lo, hi);
-        X.xfree[k] = mp; X.xdin[k] = (uint16_t)din;
-    }
     if constexpr (MODE == 1) { X.link[k] = (uint16_t)lk; X.mpos[k] = mp; if (lk == C_END) X.xdin[k] = (uint16_t)din; }
+}
+
+// Walk 0 of chain k: its own segment only, from p (the segment start, or the tile's entry e in chain k0, with the
+// offset din of the match open there).  The segment's 16 M bits are loaded once; a step loads the piece's offset and
+// measures it in one compare.  Writes the chain's V half, the two len4 words of its segment (plain stores) and its exit
+// state (X.xfree/X.xdin).
+__device__ __forceinline__ void c_walk0(const uint8_t* in, PipeTile& T, LzFront& X, uint32_t k, uint32_t p, uint32_t din, uint32_t t0, uint32_t limit)
+{
+    const uint32_t s0 = t0 + k * C_SEG, s1 = s0 + C_SEG;
+    const uint32_t mb = reinterpret_cast<const uint16_t*>(T.M)[k];
+    uint32_t vb = 0, lo = 0, hi = 0;
+    if (din) {                                       // entered at the segment start inside a match
+        uint32_t cap = p < limit ? limit - p : 0; if (cap > C_SEG) cap = C_SEG;
+        const uint32_t E = c_cont_len(in, p, din, cap);
+        p += E;
+        if (E != C_SEG) din = 0;
+    }
+    while (p < s1) {                                 // free inside the segment (din != 0 only at p == s1)
+        const uint32_t bits = mb & (0xFFFFu << (p - s0));
+        if (!bits) { p = s1; break; }                // segment exhausted: free at its end
+        const uint32_t qr = __ffs(bits) - 1, q = s0 + qr;
+        uint32_t B = s0 + C_SEG;                     // cut at the first boundary leaving >= 4 bytes
+        if (B - q < 4) B += C_SEG;
+        const uint32_t d = T.off[q - t0];
+        const uint32_t L4 = c_piece_len4(in, q, d, B < limit ? B : limit);   // q + 4 <= limit always
+        vb |= 1u << qr;
+        if (qr & 8) hi |= L4 << (4 * (qr & 7)); else lo |= L4 << (4 * qr);
+        p = q + 4 + L4;
+        if (p == B) din = d;                         // reached the boundary: still inside the match
+    }
+    reinterpret_cast<uint16_t*>(T.V)[k] = (uint16_t)vb;
+    *reinterpret_cast<uint2*>(&T.len4[2 * k]) = make_uint2(lo, hi);
+    X.xfree[k] = p; X.xdin[k] = (uint16_t)din;
 }
 
 __device__ __forceinline__ uint32_t c_seq_size(uint32_t lit, uint32_t L)

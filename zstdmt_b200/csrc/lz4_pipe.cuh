@@ -231,7 +231,7 @@ __device__ __forceinline__ bool lz_chains(const uint8_t* in, PipeTile& T, LzFron
     const uint32_t k0 = (e - t0) / C_SEG;
     const uint32_t seg0 = t0 + ttid * C_SEG;
     const bool alive = ttid >= k0;
-    if (alive) c_walk<0>(in, T, F, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
+    if (alive) c_walk0(in, T, F, ttid, ttid == k0 ? e : seg0, ttid == k0 ? e_din : 0u, t0, limit);
     else {                                               // dead: self link, never reached; no V bits, no pieces
         F.link[ttid] = (uint16_t)ttid;
         reinterpret_cast<uint16_t*>(T.V)[ttid] = 0;
