@@ -88,15 +88,16 @@ def test_plan_struct_matches_the_header():
     assert ctypes.sizeof(z.RangePlan) == 64
 
 
-def test_range_reads_report_under_the_frame_index_id():
-    """Range reads add no profiling id: they report under ZMT_K_FRAME_INDEX, whose place and doc line say so."""
+def test_range_read_scopes_report_under_the_frame_index_id():
+    """Range reads add no profiling id: every profiling scope in range_read.cu reports under ZMT_K_FRAME_INDEX, whose
+    place and doc line say so."""
     ids = re.search(r"enum \{(.*?)\};", _header(), flags=re.S).group(1)
     names = [re.sub(r"\s*=.*", "", x).strip() for x in ids.split(",")]
     assert names.index("ZMT_K_FRAME_INDEX") == 16 and names[-1] == "ZMT_K_COUNT" and "ZMT_K_RANGE" not in names
     doc = open(os.path.join(os.path.dirname(GOLD), "..", "include", "zstdmt_b200_dev.h")).read()
     assert re.search(r"ZMT_K_FRAME_INDEX = one index call[^/]*range reads report here too", doc, flags=re.S)
     src = open(os.path.join(os.path.dirname(GOLD), "..", "zstdmt_b200", "csrc", "range_read.cu")).read()
-    assert "zmt_prof_mark(ZMT_K_FRAME_INDEX" in src
+    assert set(re.findall(r"ZmtProfScope\s+\w+\((ZMT_K_\w+)", src)) == {"ZMT_K_FRAME_INDEX"}
 
 
 def test_read_workspace_is_that_of_the_selected_frames():

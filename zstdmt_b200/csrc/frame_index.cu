@@ -18,10 +18,9 @@
 //   zidx_zstd_blocks_kernel   one thread per frame: the writing walk of zstd_frame_walk fills the ZBlk table
 // The header formats live in frame_format.h, shared with the host walkers, so both sources of tables agree byte for byte.
 #include <stdint.h>
-#include <cub/device/device_scan.cuh>
+#include "cub_scan.h"
 #include "frame_format.h"
-
-extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
+#include "launch.h"
 
 namespace {
 
@@ -37,29 +36,20 @@ struct IdxCtl {
     uint64_t max_off;       // offset of frame max_frames' header (the first one not stored)
 };
 
-__host__ __device__ inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
-
 struct IdxWork { IdxCtl* ctl; uint32_t* fstat; uint64_t* fstop; uint64_t* slots; void* tmp; size_t tmp_bytes; };
 
-// workspace: ctl | per-frame status | per-frame stop offset | LZ4 slots (max_frames + 1) | cub scan storage
-size_t scan_tmp_bytes(uint32_t max_frames)
+// workspace (ZmtCarve, launch.h): ctl | per-frame status | per-frame stop offset | LZ4 slots (max_frames + 1) | cub scan
+// storage.  Returns its size, 0 when cub cannot size its scans.
+size_t carve(void* d_work, uint32_t max_frames, IdxWork* k)
 {
-    size_t t64 = 0, t32 = 0;
-    if (cub::DeviceScan::ExclusiveSum(nullptr, t64, (uint64_t*)nullptr, (int)max_frames + 1) != cudaSuccess ||
-        cub::DeviceScan::ExclusiveSum(nullptr, t32, (uint32_t*)nullptr, (int)max_frames + 1) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return t64 > t32 ? t64 : t32;
-}
-
-IdxWork carve(void* d_work, uint32_t max_frames, size_t tmp_bytes)
-{
-    uint8_t* w = (uint8_t*)d_work;
-    IdxWork k;
-    k.ctl = (IdxCtl*)w; w += 256;
-    k.fstat = (uint32_t*)w; w += a256((uint64_t)max_frames * 4);
-    k.fstop = (uint64_t*)w; w += a256((uint64_t)max_frames * 8);
-    k.slots = (uint64_t*)w; w += a256(((uint64_t)max_frames + 1) * 8);
-    k.tmp = w; k.tmp_bytes = tmp_bytes;
-    return k;
+    ZmtCarve c{(uint8_t*)d_work, 0};
+    k->ctl = c.take<IdxCtl>(256);
+    k->fstat = c.take<uint32_t>(a256((uint64_t)max_frames * 4));
+    k->fstop = c.take<uint64_t>(a256((uint64_t)max_frames * 8));
+    k->slots = c.take<uint64_t>(a256(((uint64_t)max_frames + 1) * 8));
+    k->tmp_bytes = scan_tmp_bytes(max_frames + 1);
+    k->tmp = c.take<void>(k->tmp_bytes);
+    return k->tmp_bytes ? (size_t)c.off : 0;
 }
 
 __global__ void zidx_walk_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t max_frames, uint64_t* __restrict__ frame_off,
@@ -217,23 +207,16 @@ int index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint6
 {
     if (in_bytes > kMaxIndexBytes || max_frames >= 0x7FFFFFFFu || !d_info || !d_work || !d_out_off || (max_frames && (!d_frame_off || !d_frame_csize)))
         return ZMT_ST_BAD_ARG;
-    const size_t tb = scan_tmp_bytes(max_frames);
-    if (!tb) return ZMT_ST_CUDA;
-    const IdxWork k = carve(d_work, max_frames, tb);
-    const int nitems = (int)max_frames + 1;
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    IdxWork k;
+    if (!carve(d_work, max_frames, &k)) return ZMT_ST_CUDA;
+    const uint64_t n = (uint64_t)max_frames + 1;
+    ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
     walk(k);
     pass((max_frames + kThreads) / kThreads, k);
-    size_t t = k.tmp_bytes;
-    bool ok = cub::DeviceScan::ExclusiveSum(k.tmp, t, d_out_off, nitems, stream) == cudaSuccess;
-    if (d_first_blk) {
-        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, d_first_blk, nitems, stream) == cudaSuccess;
-        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, d_frame_scratch, nitems, stream) == cudaSuccess;
-    } else {
-        t = k.tmp_bytes; ok = ok && cub::DeviceScan::ExclusiveSum(k.tmp, t, k.slots, nitems, stream) == cudaSuccess;
-    }
+    bool ok = exclusive_sum(k, d_out_off, n, stream);
+    if (d_first_blk) ok = ok && exclusive_sum(k, d_first_blk, n, stream) && exclusive_sum(k, d_frame_scratch, n, stream);
+    else ok = ok && exclusive_sum(k, k.slots, n, stream);
     zidx_summary_kernel<<<1, 1, 0, stream>>>(k, max_frames, d_out_off, d_first_blk, d_frame_scratch, d_info);
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return ok && cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
@@ -247,9 +230,8 @@ void container_walk(const void* d_in, uint64_t in_bytes, uint32_t max_frames, ui
 extern "C" size_t zmt_index_workspace_bytes(uint32_t max_frames)
 {
     if (max_frames >= 0x7FFFFFFFu) return 0;
-    const size_t tb = scan_tmp_bytes(max_frames);
-    if (!tb) return 0;
-    return 256 + a256((uint64_t)max_frames * 4) + a256((uint64_t)max_frames * 8) + a256(((uint64_t)max_frames + 1) * 8) + tb;
+    IdxWork k;
+    return carve(nullptr, max_frames, &k);
 }
 
 extern "C" int zmt_lz4_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
@@ -311,9 +293,8 @@ extern "C" int zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const 
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0 || nblocks == 0) return ZMT_ST_OK;
     if (!d_in || !d_frame_off || !d_frame_csize || !d_frame_first_blk || !d_frame_scratch || !d_blocks) return ZMT_ST_BAD_ARG;
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
     zidx_zstd_blocks_kernel<<<(nframes + kThreads - 1) / kThreads, kThreads, 0, stream>>>((const uint8_t*)d_in, nframes, d_frame_off, d_frame_csize,
                                                                                          d_frame_first_blk, d_frame_scratch, (ZBlk*)d_blocks, nblocks);
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }

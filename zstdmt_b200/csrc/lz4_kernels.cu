@@ -36,6 +36,7 @@
 #include "common.cuh"
 #include "frame_format.h"
 #include "host_common.h"
+#include "launch.h"
 #include "zmt_dev.h"
 #include "zstd_entropy.cuh"
 
@@ -762,15 +763,12 @@ static int zstd_tables_init()
 // ============================================================================ host launchers
 // ZSTDMT_B200_DEBUG_SYNC=1: synchronise after every kernel and name the one that failed (debug only)
 // ---- optional per-kernel timing (zmt_prof_begin / zmt_prof_end): CUDA events recorded on the launching
-// stream around every kernel while enabled; used by bench.py for the roofline of the dominant kernel.
+// stream around every kernel while enabled (ZmtProfScope, launch.h); used by bench.py for the roofline of the dominant kernel.
 struct ZmtProfRec { int id; cudaEvent_t a, b; };
 static bool g_prof_on = false;
 static std::vector<ZmtProfRec> g_prof;
-struct ZmtProfScope {
-    cudaStream_t st; cudaEvent_t a = nullptr, b = nullptr; int id;
-    ZmtProfScope(int id_, cudaStream_t s) : st(s), id(id_) { if (g_prof_on) { cudaEventCreate(&a); cudaEventCreate(&b); cudaEventRecord(a, st); } }
-    ~ZmtProfScope() { if (a) { cudaEventRecord(b, st); g_prof.push_back({id, a, b}); } }
-};
+cudaEvent_t zmt_prof_open(cudaStream_t st) { cudaEvent_t a = nullptr; if (g_prof_on) { cudaEventCreate(&a); cudaEventRecord(a, st); } return a; }
+void zmt_prof_close(int id, cudaEvent_t a, cudaStream_t st) { cudaEvent_t b; cudaEventCreate(&b); cudaEventRecord(b, st); g_prof.push_back({id, a, b}); }
 extern "C" void zmt_prof_begin(void) { for (auto& r : g_prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); } g_prof.clear(); g_prof_on = true; }
 // ms[id] = summed device time, count[id] = launches (the caller synchronises the stream first)
 extern "C" int zmt_prof_end(double* ms, int* count, int max_ids)
@@ -795,16 +793,6 @@ extern "C" int zmt_phase_probe_take(unsigned long long* out)
     return cudaMemcpyToSymbol(zmt_phase_cycles, zero, sizeof(zero)) != cudaSuccess;
 }
 #endif
-
-// begin / end marks for code outside this file (zstd_decode.cu): same records as ZmtProfScope
-static cudaEvent_t g_mark_a[ZMT_K_COUNT];
-extern "C" void zmt_prof_mark(int id, void* stream, int end)
-{
-    if (!g_prof_on || id < 0 || id >= ZMT_K_COUNT) return;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (!end) { cudaEventCreate(&g_mark_a[id]); cudaEventRecord(g_mark_a[id], st); }
-    else { cudaEvent_t b; cudaEventCreate(&b); cudaEventRecord(b, st); g_prof.push_back({id, g_mark_a[id], b}); }
-}
 
 static bool zmt_dbg_check(cudaStream_t st, const char* what)
 {
@@ -843,7 +831,6 @@ extern "C" uint32_t zmt_chunk_count(uint64_t in_bytes, uint32_t chunk_size)
     return n > 0x7FFFFFFFull ? 0 : (uint32_t)n;
 }
 
-static inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
 static inline uint32_t zmt_bpc(uint32_t chunk_size) { return (uint32_t)(((uint64_t)chunk_size + LZ4_BLK - 1) / LZ4_BLK); }   // 64 KiB blocks per chunk
 
 #define ZSTD_MAX_GRID (132u * 2u * 4u)       // the workspace holds one ZScratch per CTA of the largest grid (H100 SXM: 132 SMs)
@@ -885,14 +872,8 @@ static int zmt_batch(ZmtBatch& b, const void* d_in, uint64_t in_bytes, uint32_t 
     return ZMT_ST_OK;
 }
 
-// ---------------------------------------------------------------- encoder workspaces
-// One layout function per codec places the slots from `base`; with base == nullptr it only adds up their sizes.  The
-// *_workspace_bytes functions and the launchers both call it, so the size a caller allocates is the size the launcher carves.
+// ---------------------------------------------------------------- encoder workspaces (ZmtCarve, launch.h)
 // npos: the positions of one group for the chain classes, 0 for the others.
-struct ZmtCarve {
-    uint8_t* base; uint64_t off;
-    template <class T> T* take(uint64_t bytes) { T* p = base ? (T*)(base + off) : nullptr; off += bytes; return p; }
-};
 
 // chain classes: keys, values, prev and best of one group, then the radix sort's temporary storage
 struct ZlChainWs { uint32_t* arr[4]; void* sort_tmp; size_t sort_cap; };
@@ -1126,14 +1107,30 @@ extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uin
     return zmt_zstd_compress_level_device(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, 3, d_work, d_out, d_frame_off, stream_);
 }
 
-// workspace: stored[] | computed[] | needs_seq[] | ticket, any-FLG.BC flag | slot counts | first_slot | block table | progress | match records
-extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, uint64_t in_bytes)
+// The decoder's workspace (ZmtCarve, launch.h).  zeroed: the bytes from stored[] through any_bchk, cleared before the kernels run.
+struct Lz4dWs {
+    uint32_t* stored; uint32_t* computed; uint32_t* needs_seq; unsigned long long* ticket; uint32_t* any_bchk; uint64_t zeroed;
+    unsigned long long* wbase; uint64_t* slot_cnt; uint64_t* first_slot; LzBlk* tab; uint32_t* prog; unsigned long long* rec;
+};
+static uint64_t lz4d_layout(uint8_t* base, uint32_t nframes, uint32_t nslots, uint64_t in_bytes, Lz4dWs& w)
 {
-    uint64_t sz = 3 * a256((uint64_t)nframes * 4) + 256 + 2 * a256(((uint64_t)nframes + 1) * 8) + ticket_table_bytes(nframes);
-    sz += a256((uint64_t)nslots * sizeof(LzBlk)) + a256((uint64_t)nslots * 4);
-    sz += a256((in_bytes / 3 + 8) * 8);
-    return (size_t)sz + 1024;
+    ZmtCarve c{base, 0};
+    w.stored = c.take<uint32_t>(a256((uint64_t)nframes * 4));
+    w.computed = c.take<uint32_t>(a256((uint64_t)nframes * 4));
+    w.needs_seq = c.take<uint32_t>(a256((uint64_t)nframes * 4));
+    w.ticket = c.take<unsigned long long>(8);
+    w.any_bchk = c.take<uint32_t>(248);                                 // any frame with FLG.BC set
+    w.zeroed = c.off;
+    w.wbase = c.take<unsigned long long>(ticket_table_bytes(nframes));
+    w.slot_cnt = c.take<uint64_t>(a256(((uint64_t)nframes + 1) * 8));
+    w.first_slot = c.take<uint64_t>(a256(((uint64_t)nframes + 1) * 8));
+    w.tab = c.take<LzBlk>(a256((uint64_t)nslots * sizeof(LzBlk)));
+    w.prog = c.take<uint32_t>(a256((uint64_t)nslots * 4));
+    w.rec = c.take<unsigned long long>(a256((in_bytes / 3 + 8) * 8));   // a match record per 3 input bytes at most: a token and an offset take 3
+    return c.off + 1024;
 }
+
+extern "C" size_t zmt_lz4d_workspace_bytes(uint32_t nframes, uint32_t nslots, uint64_t in_bytes) { Lz4dWs w; return (size_t)lz4d_layout(nullptr, nframes, nslots, in_bytes, w); }
 
 // seg = nullptr: whole frames (zmt_lz4_decompress_device); else every frame of the batch is a segment
 static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize, uint32_t nframes,
@@ -1143,35 +1140,27 @@ static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0) return ZMT_ST_OK;
     if (nslots < nframes) return ZMT_ST_BAD_ARG;
-    uint8_t* w = (uint8_t*)d_work;
-    uint32_t* stored = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
-    uint32_t* computed = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
-    uint32_t* needs_seq = (uint32_t*)w; w += a256((uint64_t)nframes * 4);
-    unsigned long long* ticket = (unsigned long long*)w;
-    uint32_t* any_bchk = (uint32_t*)(ticket + 1); w += 256;
-    unsigned long long* wbase = (unsigned long long*)w; w += ticket_table_bytes(nframes);
-    uint64_t* slot_cnt = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
-    uint64_t* first_slot = (uint64_t*)w; w += a256(((uint64_t)nframes + 1) * 8);
-    LzBlk* tab = (LzBlk*)w; w += a256((uint64_t)nslots * sizeof(LzBlk));
-    uint32_t* prog = (uint32_t*)w; w += a256((uint64_t)nslots * 4);
-    unsigned long long* rec = (unsigned long long*)w;
+    Lz4dWs w;
+    lz4d_layout((uint8_t*)d_work, nframes, nslots, in_bytes, w);
     cudaMemsetAsync(d_status, 0, (size_t)nframes * 4, stream);
     cudaMemsetAsync(d_out_size, 0, (size_t)nframes * 8, stream);
-    cudaMemsetAsync(stored, 0, 3 * a256((uint64_t)nframes * 4) + 256, stream);      // stored, computed, needs_seq, ticket
+    cudaMemsetAsync(w.stored, 0, w.zeroed, stream);
     const uint8_t* in = (const uint8_t*)d_in;
-    lz4_slot_counts_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(d_out_off, nframes, slot_cnt);
-    scan_u64_kernel<<<1, 1024, 0, stream>>>(slot_cnt, first_slot, nframes);
-    ticket_windows_kernel<<<1, 256, 0, stream>>>(first_slot, nframes, wbase);
-    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, first_slot, nslots, tab, prog, d_status, stored, needs_seq, any_bchk, seg, nframes);
+    lz4_slot_counts_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(d_out_off, nframes, w.slot_cnt);
+    scan_u64_kernel<<<1, 1024, 0, stream>>>(w.slot_cnt, w.first_slot, nframes);
+    ticket_windows_kernel<<<1, 256, 0, stream>>>(w.first_slot, nframes, w.wbase);
+    lz4_scan_frames_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>(in, d_frame_off, d_frame_csize, d_out_off, w.first_slot, nslots, w.tab, w.prog, d_status,
+                                                                      w.stored, w.needs_seq, w.any_bchk, seg, nframes);
     zmt_dbg_check(stream, "lz4_scan_frames_kernel");
     {
         const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8), need = (nslots + X_WARPS - 1) / X_WARPS;
-        lz4_block_checksum_kernel<<<need < maxg ? need : maxg, 32 * X_WARPS, 0, stream>>>(in, d_frame_off, first_slot, tab, d_status, any_bchk, nframes, nslots);
+        lz4_block_checksum_kernel<<<need < maxg ? need : maxg, 32 * X_WARPS, 0, stream>>>(in, d_frame_off, w.first_slot, w.tab, d_status, w.any_bchk, nframes, nslots);
     }
     zmt_dbg_check(stream, "lz4_block_checksum_kernel");
     { ZmtProfScope ps(ZMT_K_LZ4_DECODE, stream);
     lz4_parse_blocks_kernel<<<(nslots + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(
-        in, in + in_bytes, d_frame_off, (uint8_t*)d_out, d_out_off, first_slot, tab, rec, (unsigned long long*)d_out_size, d_status, needs_seq, seg, nframes, nslots); }
+        in, in + in_bytes, d_frame_off, (uint8_t*)d_out, d_out_off, w.first_slot, w.tab, w.rec, (unsigned long long*)d_out_size, d_status, w.needs_seq, seg, nframes,
+        nslots); }
     zmt_dbg_check(stream, "lz4_parse_blocks_kernel");
     {
         const uint32_t maxg = (uint32_t)(zmt_sm_count() * 8);
@@ -1180,18 +1169,18 @@ static int lz4_decompress_launch(const void* d_in, uint64_t in_bytes, const uint
         // the shared-memory step window turns a chain of matches feeding each other into SMEM round trips instead of L2 ones
         // (DESIGN.md §3.2)
         lz4_exec_blocks_kernel<<<need < maxg ? need : maxg, 32 * LZD_WARPS, 0, stream>>>(
-            (uint8_t*)d_out, d_out_off, d_frame_off, first_slot, tab, rec, prog, d_status, needs_seq, ticket, wbase, nframes, nslots);
+            (uint8_t*)d_out, d_out_off, d_frame_off, w.first_slot, w.tab, w.rec, w.prog, d_status, w.needs_seq, w.ticket, w.wbase, nframes, nslots);
     }
     zmt_dbg_check(stream, "lz4_exec_blocks_kernel");
     lz4_decode_frames_seq_kernel<<<(nframes + LZD_WARPS - 1) / LZD_WARPS, 32 * LZD_WARPS, 0, stream>>>(
-        in, in + in_bytes, d_frame_off, d_frame_csize, (uint8_t*)d_out, d_out_off, (unsigned long long*)d_out_size, d_status, needs_seq, seg, nframes);
+        in, in + in_bytes, d_frame_off, d_frame_csize, (uint8_t*)d_out, d_out_off, (unsigned long long*)d_out_size, d_status, w.needs_seq, seg, nframes);
     zmt_dbg_check(stream, "lz4_decode_frames_seq_kernel");
     { ZmtProfScope ps(ZMT_K_XXH32_DEC, stream);
     if (seg) lz4_segment_xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off,
-                                                                                                     (const unsigned long long*)d_out_size, d_status, seg, computed, nframes);
-    else xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off, d_out_size, nullptr, 0, 0, computed, nframes); }
+                                                                                                     (const unsigned long long*)d_out_size, d_status, seg, w.computed, nframes);
+    else xxh32_kernel<<<(nframes + X_WARPS - 1) / X_WARPS, 32 * X_WARPS, 0, stream>>>((const uint8_t*)d_out, d_out_off, d_out_size, nullptr, 0, 0, w.computed, nframes); }
     lz4_verify_kernel<<<(nframes + 255) / 256, 256, 0, stream>>>(in, d_frame_off, d_frame_csize, d_status,
-                                                                (const unsigned long long*)d_out_size, stored, computed, seg, nframes);
+                                                                (const unsigned long long*)d_out_size, w.stored, w.computed, seg, nframes);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 

@@ -3,6 +3,7 @@
 // Here: the ticket order, the step constants, the dependency test and the copies.  Record formats, literals, validation
 // and the waits on earlier blocks stay with the callers; nothing here knows which codec calls it.
 #pragma once
+#include "launch.h"
 
 #define MX_STEP     32u           // match records per step: one per lane
 #define MX_SPAN     2048u         // bytes of output a step may span: staged in shared memory
@@ -24,7 +25,7 @@
 // frame-major order (flag in the top bit of its base).
 #define MX_FRAME_MAJOR (1ull << 63)
 // bytes of the window-base table wbase[] in a workspace (one entry per window and the total, rounded to 256)
-static inline size_t ticket_table_bytes(uint32_t nframes) { return (size_t)((((uint64_t)nframes / MX_TICKET_WIN + 2) * 8 + 255) & ~255ull); }
+static inline size_t ticket_table_bytes(uint32_t nframes) { return (size_t)a256(((uint64_t)nframes / MX_TICKET_WIN + 2) * 8); }
 
 template <typename Idx>
 __global__ void __launch_bounds__(256)

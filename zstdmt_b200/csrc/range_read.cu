@@ -22,10 +22,9 @@
 //                  rr_status_kernel      one thread per range: its status (a search over the failure prefix) and source
 //                  rr_gather_kernel      a CTA per piece of at most 64 KiB: the range's bytes to dst + dst_off[r]
 #include <stdint.h>
-#include <cub/device/device_scan.cuh>
+#include "cub_scan.h"
 #include "frame_format.h"
-
-extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
+#include "launch.h"
 
 namespace {
 
@@ -35,7 +34,6 @@ constexpr uint64_t kPiece = 64 * 1024;                  // gather piece: the mos
 constexpr uint64_t kPackPiece = 128 * 1024;             // pack: the most one CTA copies of one frame
 constexpr uint64_t kMaxExpand = 32768;                  // content bytes per compressed byte no frame can exceed (zstd RLE: 4 B -> 128 KiB)
 
-__host__ __device__ inline uint64_t a256(uint64_t x) { return (x + 255) & ~255ull; }
 __host__ __device__ inline uint64_t a16(uint64_t x) { return (x + 15) & ~15ull; }
 
 struct RangeCtl {
@@ -79,20 +77,13 @@ struct RangeWork {
     size_t    tmp_bytes;
 };
 
-size_t scan_tmp_bytes(uint32_t nitems)
-{
-    size_t a = 0, b = 0;
-    if (cub::DeviceScan::ExclusiveSum(nullptr, a, (uint64_t*)nullptr, (int)nitems) != cudaSuccess ||
-        cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (int)nitems) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return a > b ? a : b;
-}
-
 template <typename T>
-T* take(uint8_t*& w, uint64_t n) { T* p = (T*)w; w += a256(n * sizeof(T)); return p; }
+T* take(ZmtCarve& w, uint64_t n) { return w.take<T>(a256(n * sizeof(T))); }
 
+// returns the workspace's size (ZmtCarve, launch.h), 0 when cub cannot size its scans
 size_t carve(void* d_work, uint32_t nframes, uint32_t nranges, RangeWork* k)
 {
-    uint8_t* w = (uint8_t*)d_work;
+    ZmtCarve w{(uint8_t*)d_work, 0};
     const uint64_t F = (uint64_t)nframes + 1, R = (uint64_t)nranges + 1;
     k->ctl = take<RangeCtl>(w, 1);
     k->cover = take<uint32_t>(w, F); k->selx = take<uint32_t>(w, F); k->f_out = take<uint64_t>(w, F); k->f_pack = take<uint64_t>(w, F);
@@ -103,19 +94,12 @@ size_t carve(void* d_work, uint32_t nframes, uint32_t nranges, RangeWork* k)
     k->sel_status = take<uint32_t>(w, F); k->sel_fail = take<uint32_t>(w, F);
     k->r_fa = take<uint32_t>(w, R); k->r_fb = take<uint32_t>(w, R); k->r_skip = take<uint64_t>(w, R); k->r_len = take<uint64_t>(w, R);
     k->r_st = take<uint32_t>(w, R); k->r_src = take<uint64_t>(w, R); k->r_piece = take<uint64_t>(w, R);
-    k->tmp = w;
     k->tmp_bytes = scan_tmp_bytes((uint32_t)(F > R ? F : R));
-    return k->tmp_bytes ? (size_t)(w - (uint8_t*)d_work) + k->tmp_bytes : 0;
+    k->tmp = w.take<void>(k->tmp_bytes);
+    return k->tmp_bytes ? (size_t)w.off : 0;
 }
 
 bool too_many(uint32_t nframes, uint32_t nranges) { return nframes >= 0x7FFFFFFFu || nranges >= 0x7FFFFFFFu; }
-
-template <typename T>
-bool exclusive(const RangeWork& k, T* a, uint64_t n, cudaStream_t st)
-{
-    size_t t = k.tmp_bytes;
-    return cub::DeviceScan::ExclusiveSum(k.tmp, t, a, (int)n, st) == cudaSuccess;
-}
 
 // ---------------------------------------------------------------- content table
 // f < nframes: frame f's content size (LZ4: from its LZ4F header; zstd: the index's d_expect, ~0 without a size), or 0
@@ -162,13 +146,12 @@ int content_offsets(const void* d_in, uint32_t nframes, const uint64_t* d_frame_
     if (nframes && (!d_frame_off || !d_frame_csize || (Z ? !d_expect : !d_in))) return ZMT_ST_BAD_ARG;
     RangeWork k;
     if (!carve(d_work, nframes, 0, &k)) return ZMT_ST_CUDA;
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
     cudaMemsetAsync(k.ctl, 0xFF, sizeof(RangeCtl), stream);
     rr_content_kernel<Z><<<(nframes + kThreads) / kThreads, kThreads, 0, stream>>>((const uint8_t*)d_in, nframes, d_frame_off, d_frame_csize,
                                                                                   d_expect, d_content_off, k.selx, k.ctl);
-    const bool ok = exclusive(k, d_content_off, (uint64_t)nframes + 1, stream);
+    const bool ok = exclusive_sum(k, d_content_off, (uint64_t)nframes + 1, stream);
     rr_content_summary<<<1, 1, 0, stream>>>(nframes, d_frame_off, d_content_off, k.selx, k.ctl, d_info);
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return ok && cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
@@ -268,18 +251,17 @@ int range_plan(uint32_t nframes, const uint32_t* d_frame_csize, const uint32_t* 
     RangeWork k;
     if (!carve(d_work, nframes, nranges, &k)) return ZMT_ST_CUDA;
     const uint64_t F = (uint64_t)nframes + 1, R = (uint64_t)nranges + 1;
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
     cudaMemsetAsync(k.ctl, 0xFF, sizeof(RangeCtl), stream);
     cudaMemsetAsync(k.cover, 0, F * sizeof(uint32_t), stream);
     rr_ranges_kernel<<<(nranges + kThreads) / kThreads, kThreads, 0, stream>>>(nframes, d_content_off, d_ranges, nranges, d_dst_off, k);
-    bool ok = exclusive(k, k.cover, F, stream);
+    bool ok = exclusive_sum(k, k.cover, F, stream);
     rr_frames_kernel<Z><<<(nframes + kThreads) / kThreads, kThreads, 0, stream>>>(nframes, d_frame_csize, d_first_blk, d_frame_scratch, d_content_off, k);
-    ok = ok && exclusive(k, k.selx, F, stream) && exclusive(k, k.f_out, F, stream) && exclusive(k, k.f_units, F, stream);
-    ok = ok && (Z ? exclusive(k, k.f_scr, F, stream) : exclusive(k, k.f_pack, F, stream));
-    ok = ok && exclusive(k, d_dst_off, R, stream) && exclusive(k, k.r_piece, R, stream);
+    ok = ok && exclusive_sum(k, k.selx, F, stream) && exclusive_sum(k, k.f_out, F, stream) && exclusive_sum(k, k.f_units, F, stream);
+    ok = ok && (Z ? exclusive_sum(k, k.f_scr, F, stream) : exclusive_sum(k, k.f_pack, F, stream));
+    ok = ok && exclusive_sum(k, d_dst_off, R, stream) && exclusive_sum(k, k.r_piece, R, stream);
     rr_compact_kernel<Z><<<(nframes + kThreads) / kThreads, kThreads, 0, stream>>>(nframes, d_frame_csize, k);
     rr_plan_summary<<<1, 1, 0, stream>>>(nframes, nranges, d_dst_off, k, d_plan);
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return ok && cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
@@ -406,13 +388,12 @@ bool plan_ok(const zmt_range_plan* plan) { return plan && !too_many(plan->nframe
 bool finish_read(const zmt_range_plan* plan, const RangeWork& k, void* d_dst, const uint64_t* d_dst_off, uint32_t* d_range_status,
                  const void* d_scratch, cudaStream_t stream)
 {
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
+    ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
     rr_fail_kernel<<<(plan->nsel + kThreads) / kThreads, kThreads, 0, stream>>>(plan->nsel, k);
-    const bool ok = exclusive(k, k.sel_fail, (uint64_t)plan->nsel + 1, stream);
+    const bool ok = exclusive_sum(k, k.sel_fail, (uint64_t)plan->nsel + 1, stream);
     if (plan->nranges) rr_status_kernel<<<(plan->nranges + kThreads - 1) / kThreads, kThreads, 0, stream>>>(plan->nranges, d_range_status, k);
     if (plan->npieces) rr_gather_kernel<<<(uint32_t)plan->npieces, kCopyThreads, 0, stream>>>(plan->nranges, (const uint8_t*)d_scratch, (uint8_t*)d_dst,
                                                                                               d_dst_off, d_range_status, k);
-    zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
     return ok;
 }
 
@@ -480,9 +461,8 @@ extern "C" int zmt_lz4_range_read_device(const void* d_in, const uint64_t* d_fra
         void* dec_work = packed + a256(plan->packed_bytes);
         // pieces of the average selected frame: frames cut from one input at one chunk size get a CTA per piece
         const uint64_t ys = (plan->packed_bytes / plan->nsel + kPackPiece - 1) / kPackPiece;
-        zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 0);
-        rr_pack_kernel<<<dim3(plan->nsel, (uint32_t)(ys < 1 ? 1 : ys > 65535 ? 65535 : ys)), kCopyThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, packed, k);
-        zmt_prof_mark(ZMT_K_FRAME_INDEX, stream, 1);
+        { ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
+        rr_pack_kernel<<<dim3(plan->nsel, (uint32_t)(ys < 1 ? 1 : ys > 65535 ? 65535 : ys)), kCopyThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, packed, k); }
         rc = zmt_lz4_decompress_device(packed, plan->packed_bytes, k.sel_frame_off, k.sel_csize, plan->nsel, plan->nunits, d_scratch,
                                        k.sel_out_off, k.sel_out_size, k.sel_status, dec_work, stream);
     }

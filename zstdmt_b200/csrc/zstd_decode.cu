@@ -39,10 +39,9 @@
 #include "common.cuh"
 #include "frame_format.h"
 #include "host_common.h"
+#include "launch.h"
 #include "match_exec.cuh"
 #include "zmt_dev.h"
-
-extern "C" void zmt_prof_mark(int id, void* stream, int end);     // lz4_kernels.cu: record a begin / end event when profiling is armed
 
 // ---------------------------------------------------------------- predefined FSE decode tables
 struct ZFseDTable { uint8_t sym[64]; uint8_t nb[64]; uint16_t base[64]; uint32_t log; };
@@ -1287,12 +1286,27 @@ extern "C" int zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t
 
 extern "C" size_t zmt_zstd_blk_desc_bytes(void) { return sizeof(ZBlk); }
 
-// workspace: [regen u32 x nblocks][done u32 x nblocks][blk_out u64 x nblocks][expect u64 x nframes][scratch ...]
-extern "C" size_t zmt_zstdd_workspace_bytes(uint32_t nframes, uint32_t nblocks, uint64_t scratch_bytes)
+// The decoder's workspace (ZmtCarve, launch.h): per-block flags and sizes, the execute pass's tickets, the entropy scratch.
+struct ZstddWs {
+    uint32_t* regen; uint32_t* done; uint64_t* blk_out; unsigned long long* xticket; unsigned long long* xwbase;
+    uint32_t* seq_done; uint32_t* seq_ml; uint32_t* lit_done; uint8_t* scratch;
+};
+static uint64_t zstdd_layout(uint8_t* base, uint32_t nframes, uint32_t nblocks, uint64_t scratch_bytes, ZstddWs& w)
 {
-    return (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) * 2 + (((uint64_t)nblocks * 8 + 255) & ~255ull) + (((uint64_t)nframes * 8 + 255) & ~255ull)
-           + 256 + ticket_table_bytes(nframes) + 3 * (size_t)(((uint64_t)nblocks * 4 + 255) & ~255ull) + scratch_bytes + 1024;
+    ZmtCarve c{base, 0};
+    w.regen = c.take<uint32_t>(a256((uint64_t)nblocks * 4));
+    w.done = c.take<uint32_t>(a256((uint64_t)nblocks * 4));
+    w.blk_out = c.take<uint64_t>(a256((uint64_t)nblocks * 8));
+    w.xticket = c.take<unsigned long long>(256);
+    w.xwbase = c.take<unsigned long long>(ticket_table_bytes(nframes));
+    w.seq_done = c.take<uint32_t>(a256((uint64_t)nblocks * 4));
+    w.seq_ml = c.take<uint32_t>(a256((uint64_t)nblocks * 4));
+    w.lit_done = c.take<uint32_t>(a256((uint64_t)nblocks * 4));
+    w.scratch = c.take<uint8_t>(scratch_bytes);
+    return c.off + 1024;
 }
+
+extern "C" size_t zmt_zstdd_workspace_bytes(uint32_t nframes, uint32_t nblocks, uint64_t scratch_bytes) { ZstddWs w; return (size_t)zstdd_layout(nullptr, nframes, nblocks, scratch_bytes, w); }
 
 // Walk one segment of a zstd frame on the host (zstd_walk_blocks in frame_format.h), committing the walk state only when
 // the segment is complete.
@@ -1321,52 +1335,42 @@ static int zstd_decompress_launch(const void* d_in, const void* d_blocks, uint32
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0) return ZMT_ST_OK;
     const int ti = zd_tables_init(); if (ti != ZMT_ST_OK) return ti;
-    uint8_t* w = (uint8_t*)d_work;
-    uint32_t* regen = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint32_t* done = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint64_t* blk_out = (uint64_t*)w; w += (((uint64_t)nblocks * 8 + 255) & ~255ull);
-    w += (((uint64_t)nframes * 8 + 255) & ~255ull);
-    unsigned long long* xticket = (unsigned long long*)w; w += 256;
-    unsigned long long* xwbase = (unsigned long long*)w; w += ticket_table_bytes(nframes);
-    uint32_t* seq_done = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint32_t* seq_ml = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint32_t* lit_done = (uint32_t*)w; w += (((uint64_t)nblocks * 4 + 255) & ~255ull);
-    uint8_t* scratch = w;
+    ZstddWs w;
+    zstdd_layout((uint8_t*)d_work, nframes, nblocks, 0, w);
     cudaMemsetAsync(d_status, 0, (size_t)nframes * 4, stream);
-    cudaMemsetAsync(regen, 0, (size_t)nblocks * 4, stream);
-    cudaMemsetAsync(done, 0, (size_t)nblocks * 4, stream);
-    zmt_prof_mark(ZMT_K_ZSTD_DECODE, stream, 0);
+    cudaMemsetAsync(w.regen, 0, (size_t)nblocks * 4, stream);
+    cudaMemsetAsync(w.done, 0, (size_t)nblocks * 4, stream);
+    ZmtProfScope ps(ZMT_K_ZSTD_DECODE, stream);
     if (nblocks) {
-        cudaMemsetAsync(seq_done, 0, (size_t)nblocks * 4, stream);
-        cudaMemsetAsync(lit_done, 0, (size_t)nblocks * 4, stream);
+        cudaMemsetAsync(w.seq_done, 0, (size_t)nblocks * 4, stream);
+        cudaMemsetAsync(w.lit_done, 0, (size_t)nblocks * 4, stream);
         const size_t lsm = sizeof(ZLitGroup) * ZL_GROUPS * ZL_WARPS;
         cudaFuncSetAttribute(zstd_literals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm);
         const uint32_t per = ZL_GROUPS * ZL_WARPS;
-        zstd_literals_kernel<<<(nblocks + per - 1) / per, 32 * ZL_WARPS, lsm, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, lit_done);
-        zstd_seq_predef_kernel<<<(nblocks + ZS_THREADS - 1) / ZS_THREADS, ZS_THREADS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch,
-                                                                                           seq_done, seq_ml, d_status);
-        zstd_entropy_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen, d_status,
-                                                                                           seq_done, seq_ml, lit_done);
-        zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, scratch, regen,
-                                                                                           d_status, lit_done);
-        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, scratch, d_status,
+        zstd_literals_kernel<<<(nblocks + per - 1) / per, 32 * ZL_WARPS, lsm, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.lit_done);
+        zstd_seq_predef_kernel<<<(nblocks + ZS_THREADS - 1) / ZS_THREADS, ZS_THREADS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch,
+                                                                                           w.seq_done, w.seq_ml, d_status);
+        zstd_entropy_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.regen, d_status,
+                                                                                           w.seq_done, w.seq_ml, w.lit_done);
+        zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.regen,
+                                                                                           d_status, w.lit_done);
+        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, w.scratch, d_status,
                                                                                                    seg, nframes);
         zstd_entropy_seq_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
-                                                                                           scratch, regen, d_status, nframes);
+                                                                                           w.scratch, w.regen, d_status, nframes);
     }
-    zstd_offsets_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>((const ZBlk*)d_blocks, nblocks, d_frame_first_blk, regen, blk_out, d_out_off, d_expect,
+    zstd_offsets_kernel<<<(nframes + 127) / 128, 128, 0, stream>>>((const ZBlk*)d_blocks, nblocks, d_frame_first_blk, w.regen, w.blk_out, d_out_off, d_expect,
                                                                    (unsigned long long*)d_out_size, d_status, seg, nframes);
     if (nblocks) {
         const uint32_t gmax = (uint32_t)(zmt_sm_count() * (2048 / (32 * ZX_WARPS)));
         const uint32_t gneed = (nblocks + ZX_WARPS - 1) / ZX_WARPS;
-        cudaMemsetAsync(xticket, 0, 8, stream);
-        ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, xwbase);
-        zstd_execute_kernel<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, scratch, regen, blk_out,
-                                                                                     d_out_off, (uint8_t*)d_out, done, d_status, xticket, d_frame_first_blk, xwbase, seg, nframes);
+        cudaMemsetAsync(w.xticket, 0, 8, stream);
+        ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, w.xwbase);
+        zstd_execute_kernel<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, w.scratch, w.regen, w.blk_out,
+                                                                                     d_out_off, (uint8_t*)d_out, w.done, d_status, w.xticket, d_frame_first_blk, w.xwbase, seg, nframes);
         zstd_checksum_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
                                                                                            (const uint8_t*)d_out, d_out_off, (const unsigned long long*)d_out_size, d_status, seg, nframes);
     }
-    zmt_prof_mark(ZMT_K_ZSTD_DECODE, stream, 1);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
