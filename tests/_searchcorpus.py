@@ -514,10 +514,10 @@ def far_copies(rng, buf, b0, lengths):
 
 def zstd_bitbuf():
     """Two 16 KiB blocks of level 6 made of back-to-back far copies (offset code 20, no literals) on both sides of the
-    entropy stage's 12 KiB bit buffer: block 128 of 5-byte copies, whose sequence bits certainly overflow it while the
-    compressed block would still be smaller than its content (so it is stored raw for the overflow alone), and block 129
-    of 6- and 7-byte copies whose sequence bits certainly fit, with less than 2 KiB to spare."""
-    from test_gpu_zstd_encoder import raw_bounds, seq_bit_bounds
+    entropy stage's 12 KiB bit buffer: block 128 of 5-byte copies, whose sequence bits overflow it while the compressed
+    block would still be smaller than its content (so the twin stores it raw for the overflow alone), and block 129 of
+    6- and 7-byte copies whose sequence bits fit, with less than 2 KiB to spare."""
+    import _zenc as ze
     rng = np.random.default_rng(900)
     buf = rnd(rng, (1 << 21) + 3 * ZB)
     over = [5] * (ZB // 5 - 1) + [5 + ZB % 5]
@@ -531,16 +531,14 @@ def zstd_bitbuf():
     A, B = (1 << 21) // ZB, (1 << 21) // ZB + 1
 
     def check(level, ev, seqs, best):
-        ra = [tuple(r) for r in seqs[0][A].tolist()]
-        rb = [tuple(r) for r in seqs[0][B].tolist()]
+        ra, rb = seqs[0][A].astype(np.int64), seqs[0][B].astype(np.int64)
         for rows, plan in ((ra, over), (rb, under)):           # a copy whose source overlaps another's may match nearer
-            assert abs(len(rows) - len(plan)) <= 4 and sum(r[0] for r in rows) <= 4
-            assert sum(r[1] > (1 << 20) for r in rows) >= len(plan) - 8
-        upper, overflow = raw_bounds(ZB, ra)
-        assert overflow and upper < ZB
-        upper, overflow = raw_bounds(ZB, rb)
-        lo, hi = seq_bit_bounds(rb)
-        assert not overflow and upper < ZB and Z_BITBUF - 2048 < hi // 8 + 1 + 8 <= Z_BITBUF
+            assert abs(len(rows) - len(plan)) <= 4 and rows[:, 0].sum() <= 4
+            assert (rows[:, 1] > (1 << 20)).sum() >= len(plan) - 8
+        ta, tb = (ze.block_b200(r, ze.literals_of(buf[k * ZB: (k + 1) * ZB], r), buf[k * ZB: (k + 1) * ZB], False)[1]
+                  for k, r in ((A, ra), (B, rb)))
+        assert ta.raw_reason == ze.RAW_BITBUF and ta.bsize < ZB
+        assert tb.raw_reason == 0 and Z_BITBUF - 2048 < tb.seq_body + 8 <= Z_BITBUF
 
     def gpu_check(level, rep):
         assert rep.types[A] == 0 and rep.types[B] == 2 and rep.raw_bitbuf == 1

@@ -4,7 +4,8 @@
       and the sub-blocks are cut where _zenc.sub_blocks says;
   (b) the Huffman code: the traced code lengths are those of _zenc.huf_lengths on the block's literal histogram;
   (c) the mode rules of the default build (see check_modes);
-  (d) the round trip: oracle, libzstd (both paths, when oracle/_ref exists) and the GPU decoder.
+  (d) the round trip: oracle, libzstd (both paths, when oracle/_ref exists) and the GPU decoder;
+  (e) the bytes: the framed stream equals _zenc.framed_b200 (the entropy stage's CPU twin on the twin parse).
 Inputs are built here with fixed seeds; each edge case asserts from the trace that it reached its edge."""
 import numpy as np
 import pytest
@@ -12,11 +13,12 @@ import pytest
 import _oracle as o
 import _zenc as ze
 import zstdmt_b200 as z
+from _zxmodel import ML_BASE
 
 pytestmark = pytest.mark.gpu
 ZT = o.ZT
 W = ze.WINDOW
-Z_BITBUF = 3072 * 4              # the entropy stage's bit buffer (Z_BITWORDS words)
+Z_BITBUF = ze.BITBUF             # the entropy stage's bit buffer (Z_BITWORDS words)
 
 
 @pytest.fixture(scope="module")
@@ -56,20 +58,28 @@ def chunks_of(src, chunk, chunk_bytes):
 
 class Report:
     def __init__(self):
-        self.sub = self.raw = self.raw_bitbuf = self.huf = 0
+        self.sub = self.raw = self.huf = 0
         self.blocks = []                 # (trace, block index, start in the frame's content) of every non-empty block
+        self.twin = []                   # (chunk, block, _zenc.BlockTrace) of every block the twin wrote
+        self.raw_by = {}                 # raw blocks by reason, from the twin's traces (_zenc.raw_counts)
+
+    @property
+    def raw_bitbuf(self):
+        return self.raw_by.get("bitbuf", 0)
 
     def share(self):
         return self.raw_bitbuf / max(1, self.sub)
 
 
 def check(torch, src, chunk=1 << 20, chunk_bytes=None):
-    """Compress on the GPU, trace every frame and check (a)-(d).  Returns the Report with every compressed block."""
+    """Compress on the GPU, trace every frame and check (a)-(e).  Returns the Report with every compressed block."""
     framed = gpu_compress(torch, src, chunk, chunk_bytes)
     frames = o.mt_frames(framed)
     parts = chunks_of(src, chunk, chunk_bytes)
     assert len(frames) == len(parts)
     rep = Report()
+    rep.twin = ze.assert_twin(framed, src, chunk, 3, chunk_bytes)
+    rep.raw_by = ze.raw_counts(rep.twin)
     for f, content in zip(frames, parts):
         tr = o.zstd_trace(f)
         assert np.array_equal(tr.content, content)
@@ -130,8 +140,6 @@ def check_windows(tr, content, rep):
             rep.sub += 1
             if tr.blk[b, ZT["type"]] == 0:
                 rep.raw += 1
-                if raw_by_bitbuf(win, a, e, mseq):
-                    rep.raw_bitbuf += 1
                 continue
             q = tr.block_seqs(b).astype(np.int64)
             if len(q):
@@ -155,63 +163,6 @@ def check_huffman(tr, b, rep):
     got = {int(s): mb + 1 - int(w[s]) for s in np.flatnonzero(w)}
     assert mb == wmax and got == want, ("Huffman lengths differ from the twin", b)
     assert ze.kraft(got, mb) == 1 << mb
-
-
-# predefined FSE distributions (RFC 8878 §3.1.1.3.2.2): bits a symbol's state transition can emit at most
-def _max_state_bits(norm, log):
-    return [log if n in (-1, 1) else log - (int(n - 1).bit_length() - 1) for n in norm]
-
-
-LL_MAXB = _max_state_bits([4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1, 1, 1, -1, -1, -1, -1], 6)
-ML_MAXB = _max_state_bits([1, 4, 3, 2, 2, 2, 2, 2, 2] + [1] * 37 + [-1] * 7, 6)
-OF_MAXB = _max_state_bits([1, 1, 1, 1, 1, 1, 2, 2, 2] + [1] * 15 + [-1] * 5, 5)
-LL_BASE = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 20, 22, 24, 28, 32, 40, 48, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536]
-ML_BASE = [3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33, 34, 35, 37, 39, 41, 43, 47, 51, 59, 67, 83, 99, 131, 259, 515, 1027, 2051, 4099, 8195, 16387, 32771, 65539]
-
-
-def _code(base, v):
-    return int(np.searchsorted(base, v, side="right")) - 1
-
-
-def seq_bit_bounds(rows):
-    """Lower and upper bounds of the bits of a block's sequence bitstream, rows (literal length, offset, match length)
-    with explicit offsets (Offset_Value = offset + 3).  A state transition of a predefined FSE table emits maxBitsOut or
-    maxBitsOut - 1 bits (exactly log for a count of 1 or -1); the first symbol of each stream emits none."""
-    lo = hi = 6 + 5 + 6 - (6 + 5 + 6)                               # final states flushed; first symbols emit nothing
-    for ll, off, ml in rows:
-        lc, mc, oc = _code(LL_BASE, ll), _code(ML_BASE, ml), (off + 3).bit_length() - 1
-        extra = (int(LL_BASE[lc + 1] - LL_BASE[lc]) - 1).bit_length() + (int(ML_BASE[mc + 1] - ML_BASE[mc]) - 1).bit_length() + oc
-        mx = LL_MAXB[lc] + ML_MAXB[mc] + OF_MAXB[oc]
-        mn = sum(b if b == lg else b - 1 for b, lg in ((LL_MAXB[lc], 6), (ML_MAXB[mc], 6), (OF_MAXB[oc], 5)))
-        lo += extra + mn; hi += extra + mx
-    return lo + 6 + 5 + 6 - 17, hi + 6 + 5 + 6
-
-
-def raw_bounds(regen, rows):
-    """(upper bound of the compressed block's size, whether its sequence bits certainly overflow the bit buffer)."""
-    nlit = regen - sum(ml for _, _, ml in rows)
-    lo, hi = seq_bit_bounds(rows)
-    return 3 + (nlit + 5) + 4 + hi // 8 + 1, lo // 8 + 1 + 8 > Z_BITBUF
-
-
-def raw_is_justified(regen, rows):
-    """A block of `regen` bytes whose parse is `rows` may be stored raw: the compressed block may not be smaller than
-    its content, or its sequence bits overflow the bit buffer."""
-    upper, overflow = raw_bounds(regen, rows)
-    return upper >= regen or overflow
-
-
-def raw_by_bitbuf(win, a, e, mseq):
-    """True when a sub-block stored raw certainly was so because its sequence bits overflow the bit buffer: bounded from
-    below they overflow it, and bounded from above the compressed block would have been smaller than its content (the
-    other reason to store it raw)."""
-    if not len(mseq):
-        return False
-    rows, p = [], a
-    for s, off, ml in mseq.tolist():
-        rows.append((s - p, off, ml)); p = s + ml
-    upper, overflow = raw_bounds(e - a, rows)
-    return upper < e - a and overflow
 
 
 def check_roundtrip(torch, framed, src):
@@ -424,6 +375,17 @@ def edges():
     return _EDGE
 
 
+def entropy_edge_windows():
+    """The inputs of the entropy-edge corpus (_zentcorpus) that fit one window, each zero-padded to 64 KiB."""
+    import _zentcorpus as zc
+    out = []
+    for c in zc.cases():
+        src = c.built()[0]
+        if src.size <= W:
+            out.append(np.concatenate([src, np.zeros(W - src.size, np.uint8)]))
+    return out
+
+
 def huff_blocks(rep):
     return [(tr, b) for tr, b, _ in rep.blocks if tr.blk[b, ZT["type"]] == 2 and tr.blk[b, ZT["lit_type"]] == 2]
 
@@ -501,8 +463,9 @@ def test_encoder_edge_windows(torch, name, capsys):
     reached(name, rep)
     if name == "tokens":
         with capsys.disabled():
-            print("\n[zstd encoder] tokens: %d of %d sub-blocks stored raw, %d (%.1f %%) because the sequence bits overflow "
-                  "the %d-byte bit buffer" % (rep.raw, rep.sub, rep.raw_bitbuf, 100 * rep.share(), Z_BITBUF))
+            print("\n[zstd encoder] tokens: %d of %d sub-blocks stored raw: %d not smaller than their content, %d (%.1f %%) because "
+                  "the sequence bits overflow the %d-byte bit buffer" % (rep.raw, rep.sub, rep.raw_by["size"], rep.raw_bitbuf,
+                                                                          100 * rep.share(), Z_BITBUF))
 
 
 def test_encoder_literal_sections_around_16k(torch):
@@ -535,11 +498,12 @@ def test_encoder_ragged_chunks_and_short_windows(torch):
 
 def test_encoder_state_does_not_leak_across_windows_of_one_cta(torch, capsys):
     """About 72 MiB: more windows than the persistent grid has CTAs, so CTA c also encodes window c + grid.  The edge
-    windows are laid out so that each of those CTAs meets two different kinds in turn; the rest is the Silesia-like mix."""
+    windows (and the entropy-edge corpus's level-3 inputs) are laid out so that each of those CTAs meets two different
+    kinds in turn; the rest is the Silesia-like mix."""
     sm = torch.cuda.get_device_properties(0).multi_processor_count
     grid = min(sm * 8, 132 * 8)
     E = edges()
-    kinds = [w for name in EDGE_NAMES for w in E[name]]
+    kinds = [w for name in EDGE_NAMES for w in E[name]] + entropy_edge_windows()
     nwin = grid + 96
     src = z.gen_stream(z.GEN_MIX, nwin * W, 1 << 20, first=1)
     for i in range(96):
@@ -547,6 +511,7 @@ def test_encoder_state_does_not_leak_across_windows_of_one_cta(torch, capsys):
         src[(i + grid) * W: (i + grid + 1) * W] = kinds[(i + 1 + i // len(kinds)) % len(kinds)]
     rep = check(torch, src)
     with capsys.disabled():
-        print("\n[zstd encoder] %.1f MiB, grid %d: %d sub-blocks, %d Huffman, %d raw, %d (%.2f %%) raw because the sequence bits "
-              "overflow the bit buffer" % (src.size / 2**20, grid, rep.sub, rep.huf, rep.raw, rep.raw_bitbuf, 100 * rep.share()))
+        print("\n[zstd encoder] %.1f MiB, grid %d: %d sub-blocks, %d Huffman, %d raw: %d not smaller than their content, %d "
+              "(%.2f %%) because the sequence bits overflow the bit buffer" % (src.size / 2**20, grid, rep.sub, rep.huf, rep.raw,
+                                                                              rep.raw_by["size"], rep.raw_bitbuf, 100 * rep.share()))
     assert src.size > grid * W

@@ -2,9 +2,9 @@
 written by zmt_zstd_compress_level_device is traced by the oracle (orc_zstd_trace) and checked:
   - every compressed block's sequences equal the CPU twin's (oracle/chain_twin.c) for that block, offsets explicit;
   - blocks are raw or compressed, 16 KiB (the chunk's last one may be short), predefined modes, own Huffman tree;
-  - every raw block is raw for a reason: on the twin's parse, an upper bound of its compressed size is at least its
-    content, or a lower bound of its sequence bits overflows the entropy stage's bit buffer;
   - the Huffman lengths are _zenc.huf_lengths of the block's literal histogram;
+  - the framed stream equals _zenc.framed_b200 byte for byte (the entropy stage's CPU twin on the twin's parse), so
+    every raw block is raw for the twin's reason;
   - the oracle, libzstd (T=1 and T>1, when oracle/_ref exists) and the GPU decoder restore the frames.
 Inputs are built here with fixed seeds; each edge case asserts from the trace that it reached its edge."""
 import ctypes
@@ -13,9 +13,10 @@ import numpy as np
 import pytest
 
 import _oracle as o
+import _zenc as ze
 import _zlazy as zl
 import zstdmt_b200 as z
-from test_gpu_zstd_encoder import check_huffman, check_modes, check_roundtrip, raw_bounds, raw_is_justified
+from test_gpu_zstd_encoder import check_huffman, check_modes, check_roundtrip
 
 pytestmark = pytest.mark.gpu
 ZT = o.ZT
@@ -55,7 +56,11 @@ class Report:
         self.seqs = []                   # (frame, block start in the frame, traced (ll, off, ml) rows) of every compressed block
         self.types = []
         self.huf = 0
-        self.raw_bitbuf = 0              # raw blocks whose twin parse certainly overflows the bit buffer
+        self.raw_by = {}                 # raw blocks by reason, from the twin's traces (_zenc.raw_counts)
+
+    @property
+    def raw_bitbuf(self):
+        return self.raw_by.get("bitbuf", 0)
 
     def all_seqs(self):
         return np.concatenate([s for _, _, s in self.seqs]) if self.seqs else np.zeros((0, 3), np.int64)
@@ -69,6 +74,8 @@ def check(torch, src, chunk, level, chunk_bytes=None):
     assert len(frames) == len(parts)
     rep = Report()
     rep.framed = framed
+    rep.twin = ze.assert_twin(framed, src, chunk, level, chunk_bytes)
+    rep.raw_by = ze.raw_counts(rep.twin)
     for fi, (f, content) in enumerate(zip(frames, parts)):
         tr = o.zstd_trace(f)
         assert np.array_equal(tr.content, content)
@@ -81,9 +88,6 @@ def check(torch, src, chunk, level, chunk_bytes=None):
         for k, b in enumerate(blocks):
             rep.types.append(int(tr.blk[b, ZT["type"]]))
             if tr.blk[b, ZT["type"]] != 2:
-                rows = [tuple(r) for r in twin[k].astype(np.int64).tolist()]
-                assert raw_is_justified(int(regen[b]), rows), ("raw block the twin's parse would compress", fi, k)
-                rep.raw_bitbuf += raw_bounds(int(regen[b]), rows)[1]
                 continue
             q = tr.block_seqs(b).astype(np.int64)
             assert (q[:, 1] == q[:, 3] + 3).all()                     # Offset_Value = offset + 3: no repeat codes
