@@ -34,6 +34,7 @@
 #define ZMT_ST_UNSUPPORTED      10u
 #define ZMT_ST_CUDA             11u
 #define ZMT_ST_BAD_ARG          12u
+#define ZMT_ST_DICT_WRONG       13u      /* the frame names a Dictionary_ID other than the dictionary given */
 #define ZMT_ST_HAS_CHK          0x100u   /* internal flag between decode and verify kernels */
 
 #ifdef __cplusplus
@@ -123,7 +124,7 @@ int      zmt_zstd_decompress_device(const void* d_in, const void* d_blocks, uint
  *   ZMT_ST_BAD_HEADER   LZ4: an unusable LZ4F header, or a content size above 255 * payload + 65536 (bad_offset = the payload)
  *                       An LZ4 payload without the LZ4F magic gets room 0 and indexes fine; the decoder reports BAD_MAGIC.
  *   zstd: what zmt_zstd_scan_frame_host returns for the frame (BAD_MAGIC, BAD_HEADER, UNSUPPORTED for a dictionary ID,
- *                       BLOCK, TRUNCATED, TRAILING); bad_offset = the frame or block header the walk stopped at, or the
+ *                       BLOCK, TRUNCATED, TRAILING; with a dictionary DICT_WRONG, bad_offset = the frame's start); bad_offset = the frame or block header the walk stopped at, or the
  *                       first trailing byte
  *   ZMT_ST_DST_SMALL    more than max_frames frames: nframes is the true count, bad_frame = max_frames, bad_offset its header
  *   in_bytes == 0       ZMT_ST_OK with nframes = 0
@@ -184,6 +185,63 @@ int    zmt_lz4_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t 
 int    zmt_zstd_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
                                    uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
                                    uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream);
+
+/* ---- zstd frames written with a dictionary (RFC 8878 §5) ----
+ * A dictionary is loaded once on the device and then named by the calls below, which are the calls above plus the
+ * record.  Two kinds are accepted, as libzstd's ZSTD_dct_auto accepts them:
+ *   formatted    magic 0xEC30A437, LE32 Dictionary_ID, the entropy tables (a Huffman tree description in the literals
+ *                section's format, then FSE table descriptions for OF, ML and LL, in that order), three LE32 repeat
+ *                offsets (each non-zero and at most the content size), then the content: the rest of the buffer;
+ *   raw content  any other buffer: Dictionary_ID 0, no tables, repeat offsets {1, 4, 8}, all of it content.
+ * zmt_zstd_ddict_load_device parses and checks the entropy section with one warp, using the decoder's own table
+ * builders and the block format's limits (Huffman codes up to 11 bits, FSE logs 8 for OF and 9 for ML / LL), and writes
+ * the opaque record d_ddict (zmt_zstd_ddict_bytes() bytes of device memory) and the summary d_info.  The record keeps
+ * the address d_dict: the dictionary bytes stay where the caller put them and must outlive every call that names the
+ * record.  No per-frame memory: the frames read the content in place.  d_info->status: ZMT_ST_OK, ZMT_ST_BAD_HEADER
+ * (unusable tables or repeat offsets), ZMT_ST_TRUNCATED (fewer than 12 bytes behind the tables for the repeat offsets);
+ * a record whose load failed makes every frame named against it fail with that status.  Reports under
+ * ZMT_K_ZSTD_DECODE; returns ZMT_ST_OK once enqueued, ZMT_ST_BAD_ARG or ZMT_ST_CUDA.
+ *
+ * The rule is libzstd's ZSTD_decompress_usingDict: every frame of a dictionary batch decodes against the dictionary,
+ * whether its header names the dictionary's ID or names none.  A frame that names another ID fails with
+ * ZMT_ST_DICT_WRONG (the index's bad_offset: the frame's start).  Each frame gets ZF_DICT | ZF_NEEDS_SEQ in d_frame_seq:
+ * the tables and repeat offsets its first blocks may take from the dictionary tie it to the dependent-block route.
+ * Matches may reach as far back as the frame's output so far plus the dictionary's content.
+ *   zmt_zstd_scan_frame_dict_host       zmt_zstd_scan_frame_host with the summary of a loaded dictionary (dict = NULL:
+ *                                       no dictionary, which is zmt_zstd_scan_frame_host itself)
+ *   zmt_zstd_index_dict_device,         the index calls; d_ddict = NULL is the call without a dictionary
+ *   zmt_zstd_index_plain_dict_device
+ *   zmt_zstd_blocks_dict_device         zmt_zstd_blocks_device; byte for byte what zmt_zstd_scan_frame_dict_host writes
+ *   zmt_zstd_decompress_dict_device     zmt_zstd_decompress_device against the dictionary
+ * The calls without a dictionary keep refusing a frame that names a Dictionary_ID with ZMT_ST_UNSUPPORTED, and so does
+ * the segment walk (zmt_zstd_segment_host). */
+#define ZF_DICT 8u                   /* d_frame_seq: the frame decodes against the batch's dictionary */
+typedef struct {
+    uint32_t status;             /* ZMT_ST_OK, ZMT_ST_BAD_HEADER (unusable tables / repeat offsets), ZMT_ST_TRUNCATED */
+    uint32_t dict_id;            /* 0 for raw content */
+    uint32_t kind;               /* 0 raw content, 1 formatted */
+    uint32_t reserved;
+    uint64_t content_bytes;      /* history the frames may reach */
+    uint64_t content_off;        /* where the content starts in the dictionary */
+} zmt_zstd_dict_info;
+size_t zmt_zstd_ddict_bytes(void);
+int    zmt_zstd_ddict_load_device(const void* d_dict, uint64_t dict_bytes, void* d_ddict, zmt_zstd_dict_info* d_info, void* stream);
+int    zmt_zstd_scan_frame_dict_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, void* blocks_out,
+                                     uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size,
+                                     uint32_t* needs_seq, const zmt_zstd_dict_info* dict);
+int    zmt_zstd_index_dict_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                  uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                  uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream, const void* d_ddict);
+int    zmt_zstd_index_plain_dict_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                        uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                        uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream, const void* d_ddict);
+int    zmt_zstd_blocks_dict_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                   const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream,
+                                   const void* d_ddict);
+int    zmt_zstd_decompress_dict_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                       const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out,
+                                       const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream,
+                                       const void* d_ddict);
 
 /* ---- LZ4F frames of any size in bounded memory ----
  * An LZ4F frame of any size, decoded as a chain of segments, each a run of whole blocks (what LZ4F_decompress does

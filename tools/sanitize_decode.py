@@ -1,6 +1,7 @@
 """Small decode workloads for compute-sanitizer (memcheck / racecheck): LZ4 own + reference-framed (linked) streams, zstd own +
 libzstd-framed streams, through the device API and the callback API; a libzstd frame decoded as segments through the device
-API and through the callback API in 1 MiB batches.  python tools/sanitize_decode.py [MiB]"""
+API and through the callback API in 1 MiB batches; zstd frames written against a dictionary through the host scan and the
+device index.  python tools/sanitize_decode.py [MiB]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -46,3 +47,20 @@ os.environ["ZSTDMT_B200_PLAIN_MB"] = "1"
 rc, back, st = z.decompress_mem(z.CODEC_ZSTD, zf1, n + 16, threads=4, inputsize=1 << 20)
 assert rc == 0 and np.array_equal(back, src)
 print("zstd segments ok")
+# zstd frames written against a dictionary (formatted and raw content): host scan, device index of a container and of a
+# plain stream
+import _zdict as zd
+recs = zd.records(5, 400)
+for d, kind in ((zd.train(6, 64 << 10), zd.DCT_AUTO), (np.concatenate(zd.records(7, 20))[: 16 << 10], zd.DCT_RAW)):
+    dct = z.ZstdDictionary(d)
+    frames = [zd.compress(r, d, level=(1, 3, 19)[i % 3], checksum=i & 1, kind=kind) for i, r in enumerate(recs)]
+    for fr, plain in ((zd.container(frames), False), (zd.plain(frames), True)):
+        d_fr = torch.from_numpy(fr).cuda()
+        decs = [z.ZstdDeviceDecompressor.from_device(d_fr, plain=plain, dictionary=dct)]
+        if not plain:
+            decs.append(z.ZstdDeviceDecompressor(fr, dictionary=dct))
+        for dec in decs:
+            out, st = dec.run(d_fr); torch.cuda.synchronize()
+            oo = dec.d_out_off.cpu().numpy()
+            assert int(st.abs().sum()) == 0 and all(np.array_equal(out[int(oo[i]): int(oo[i]) + r.size].cpu().numpy(), r) for i, r in enumerate(recs))
+print("zstd dictionary ok")

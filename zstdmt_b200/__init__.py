@@ -22,7 +22,7 @@ CODEC_LZ4, CODEC_ZSTD = 1, 2
 GEN_ZEROS, GEN_TEXT, GEN_MIX, GEN_RANDOM = 0, 1, 2, 3
 
 ST_NAMES = {0: "ok", 1: "truncated", 2: "bad_magic", 3: "bad_header", 4: "hdr_checksum", 5: "block", 6: "dst_small",
-            7: "content_checksum", 8: "content_size", 9: "trailing", 10: "unsupported", 11: "cuda", 12: "bad_arg"}
+            7: "content_checksum", 8: "content_size", 9: "trailing", 10: "unsupported", 11: "cuda", 12: "bad_arg", 13: "dict_wrong"}
 
 GEN_LIB_PATH = os.path.join(_HERE, "libzmt_datagen.so")
 MEMIO_LIB_PATH = os.path.join(_HERE, "libzmt_memio.so")
@@ -100,6 +100,13 @@ def lib():
     L.zmt_zstd_index_plain_device.argtypes = L.zmt_zstd_index_device.argtypes
     L.zmt_zstd_blocks_device.restype = ctypes.c_int
     L.zmt_zstd_blocks_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_vp]
+    L.zmt_zstd_ddict_bytes.restype = c_sz; L.zmt_zstd_ddict_bytes.argtypes = []
+    L.zmt_zstd_ddict_load_device.restype = ctypes.c_int; L.zmt_zstd_ddict_load_device.argtypes = [c_vp, c_u64, c_vp, c_vp, c_vp]
+    L.zmt_zstd_scan_frame_dict_host.restype = ctypes.c_int
+    L.zmt_zstd_scan_frame_dict_host.argtypes = L.zmt_zstd_scan_frame_host.argtypes + [ctypes.POINTER(DictInfo)]
+    for k in ("index", "index_plain", "blocks", "decompress"):
+        f = getattr(L, "zmt_zstd_%s_dict_device" % k); f.restype = ctypes.c_int
+        f.argtypes = getattr(L, "zmt_zstd_%s_device" % k).argtypes + [c_vp]
     L.zmt_range_workspace_bytes.restype = c_sz; L.zmt_range_workspace_bytes.argtypes = [c_u32, c_u32]
     L.zmt_lz4_content_offsets_device.restype = ctypes.c_int
     L.zmt_lz4_content_offsets_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
@@ -239,6 +246,14 @@ class FrameIndex(ctypes.Structure):
         return "FrameIndex(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
 
 
+class DictInfo(ctypes.Structure):
+    """zmt_zstd_dict_info (include/zstdmt_b200_dev.h): the summary of a dictionary loaded on the device."""
+    _fields_ = [("status", c_u32), ("dict_id", c_u32), ("kind", c_u32), ("reserved", c_u32), ("content_bytes", c_u64), ("content_off", c_u64)]
+
+    def __repr__(self):
+        return "DictInfo(%s)" % ", ".join("%s=%s" % (k, getattr(self, k)) for k, _ in self._fields_)
+
+
 class RangePlan(ctypes.Structure):
     """zmt_range_plan (include/zstdmt_b200_dev.h): the summary of a range-read plan, read back once per batch."""
     _fields_ = [("status", c_u32), ("bad_range", c_u32), ("nframes", c_u32), ("nranges", c_u32), ("nsel", c_u32), ("nunits", c_u32),
@@ -253,10 +268,10 @@ class RangePlan(ctypes.Structure):
 PLAIN_PAD = 12
 
 
-def _device_index(d_framed, max_frames, stream, zstd, plain=False):
-    """Run zmt_{lz4,zstd}_index_device (plain: zmt_{lz4,zstd}_index_plain_device) over a stream in device memory.  Only
-    the summary struct is read back; on ZMT_ST_DST_SMALL the index runs once more with the exact frame count.  Returns
-    (summary, device tables by name)."""
+def _device_index(d_framed, max_frames, stream, zstd, plain=False, dictionary=None):
+    """Run zmt_{lz4,zstd}_index_device (plain: zmt_{lz4,zstd}_index_plain_device; with a ZstdDictionary: the zstd
+    *_dict_device calls) over a stream in device memory.  Only the summary struct is read back; on ZMT_ST_DST_SMALL the
+    index runs once more with the exact frame count.  Returns (summary, device tables by name)."""
     torch = _torch(); L = lib()
     s = stream if stream is not None else torch.cuda.current_stream()
     dev, nbytes = d_framed.device, d_framed.numel()
@@ -274,9 +289,14 @@ def _device_index(d_framed, max_frames, stream, zstd, plain=False):
         d_info = torch.zeros(ctypes.sizeof(FrameIndex), dtype=torch.uint8, device=dev)
         p = lambda k: t[k].data_ptr()
         if zstd:
-            fn = L.zmt_zstd_index_plain_device if plain else L.zmt_zstd_index_device
-            rc = fn(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("first_blk"), p("frame_scratch"),
+            args = (d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("first_blk"), p("frame_scratch"),
                     p("expect"), p("frame_seq"), p("out_off"), d_info.data_ptr(), work.data_ptr(), s.cuda_stream)
+            if dictionary is not None:
+                fn = L.zmt_zstd_index_plain_dict_device if plain else L.zmt_zstd_index_dict_device
+                rc = fn(*args, dictionary.d_ddict.data_ptr())
+            else:
+                fn = L.zmt_zstd_index_plain_device if plain else L.zmt_zstd_index_device
+                rc = fn(*args)
         else:
             fn = L.zmt_lz4_index_plain_device if plain else L.zmt_lz4_index_device
             rc = fn(d_framed.data_ptr(), nbytes, cap, p("frame_off"), p("frame_csize"), p("out_off"), d_info.data_ptr(),
@@ -552,14 +572,38 @@ def zstd_decode_segments(frame, cuts, device="cuda"):
     return np.concatenate(parts) if parts else np.zeros(0, np.uint8), 0
 
 
+class ZstdDictionary:
+    """A zstd dictionary loaded on the device (zmt_zstd_ddict_load_device): `data` (bytes or a uint8 array, formatted or
+    raw content) is copied to the device and stays there with the record for as long as this object lives.  .info is
+    the load's summary (DictInfo); a dictionary the load rejects raises ValueError with the status name."""
+
+    def __init__(self, data, device="cuda", stream=None):
+        torch = _torch(); L = lib()
+        b = np.frombuffer(bytes(data), dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        s = stream if stream is not None else torch.cuda.current_stream()
+        self.nbytes = int(b.size)
+        self.d_dict = torch.from_numpy(np.concatenate([b, np.zeros(1, np.uint8)])).to(device)
+        self.d_ddict = torch.zeros(L.zmt_zstd_ddict_bytes(), dtype=torch.uint8, device=device)
+        d_info = torch.zeros(ctypes.sizeof(DictInfo), dtype=torch.uint8, device=device)
+        rc = L.zmt_zstd_ddict_load_device(self.d_dict.data_ptr(), self.nbytes, self.d_ddict.data_ptr(), d_info.data_ptr(), s.cuda_stream)
+        if rc != 0:
+            raise RuntimeError("zmt_zstd_ddict_load_device failed: %s" % ST_NAMES.get(rc, rc))
+        s.synchronize()
+        self.info = DictInfo.from_buffer_copy(d_info.cpu().numpy().tobytes())
+        if self.info.status != 0:
+            raise ValueError("dictionary rejected: %s" % ST_NAMES.get(self.info.status, self.info.status))
+
+
 class ZstdDeviceDecompressor:
     """zmt_zstd_decompress_device.  The constructor builds the block table on the host from the framed bytes
     (zmt_zstd_scan_frame_host: frame + block headers only), as the host pipeline does while reading; from_device builds
-    it on the GPU from a stream already in device memory."""
+    it on the GPU from a stream already in device memory.  With a ZstdDictionary every frame decodes against it (the
+    *_dict calls); the dictionary must outlive the decompressor, which keeps a reference to it."""
 
     pad = 0                 # as Lz4DeviceDecompressor.pad
+    dictionary = None
 
-    def __init__(self, framed_host, device="cuda"):
+    def __init__(self, framed_host, device="cuda", dictionary=None):
         torch = _torch(); L = lib()
         fb = np.ascontiguousarray(framed_host, dtype=np.uint8)
         offs, sizes = scan_frames(fb)
@@ -574,8 +618,12 @@ class ZstdDeviceDecompressor:
         for i in range(self.n):
             first[i] = nblk.value
             cs = c_u64(0); nsq = c_u32(0)
-            rc = L.zmt_zstd_scan_frame_host(fb[int(offs[i]) + 12:].ctypes.data, int(sizes[i]), int(offs[i]) + 12, i, blocks.ctypes.data,
-                                            ctypes.byref(nblk), cap, ctypes.byref(scr), ctypes.byref(cs), ctypes.byref(nsq))
+            args = (fb[int(offs[i]) + 12:].ctypes.data, int(sizes[i]), int(offs[i]) + 12, i, blocks.ctypes.data,
+                    ctypes.byref(nblk), cap, ctypes.byref(scr), ctypes.byref(cs), ctypes.byref(nsq))
+            if dictionary is not None:
+                rc = L.zmt_zstd_scan_frame_dict_host(*args, ctypes.byref(dictionary.info))
+            else:
+                rc = L.zmt_zstd_scan_frame_host(*args)
             self.scan_status.append(rc)
             expect[i] = cs.value; fseq[i] = nsq.value
         first[self.n] = nblk.value
@@ -594,24 +642,27 @@ class ZstdDeviceDecompressor:
         self.out_size = torch.zeros(max(self.n, 1), dtype=torch.int64, device=device)
         self.status = torch.zeros(max(self.n, 1), dtype=torch.int32, device=device)
         self.work = torch.empty(L.zmt_zstdd_workspace_bytes(self.n, self.nblk, scr.value), dtype=torch.uint8, device=device)
+        self.dictionary = dictionary
 
     @classmethod
-    def from_device(cls, d_framed, max_frames=None, stream=None, plain=False):
+    def from_device(cls, d_framed, max_frames=None, stream=None, plain=False, dictionary=None):
         """A decoder for a framed stream that is already in device memory: the frame tables and the block table are built
         on the GPU (zmt_zstd_index_device, zmt_zstd_blocks_device) and only the summary comes back to the host, as
         .index_info.  run(d_framed) decodes.  max_frames, plain and the errors as Lz4DeviceDecompressor.from_device
         (plain: a .zst stream, zmt_zstd_index_plain_device)."""
         torch = _torch(); L = lib()
         s = stream if stream is not None else torch.cuda.current_stream()
-        info, t = _device_index(d_framed, max_frames, s, zstd=True, plain=plain)
+        info, t = _device_index(d_framed, max_frames, s, zstd=True, plain=plain, dictionary=dictionary)
         dev = d_framed.device
         self = cls.__new__(cls)
         self.pad = PLAIN_PAD if plain else 0
+        self.dictionary = dictionary
         self.index_info, self.n, self.nblk, self.out_total = info, info.nframes, info.nblocks, info.out_bytes
         self.d_first, self.d_expect, self.d_fseq, self.d_out_off = t["first_blk"], t["expect"], t["frame_seq"], t["out_off"]
         self.d_blocks = torch.empty(max(1, self.nblk) * L.zmt_zstd_blk_desc_bytes(), dtype=torch.uint8, device=dev)
-        rc = L.zmt_zstd_blocks_device(d_framed.data_ptr() - self.pad, self.n, t["frame_off"].data_ptr(), t["frame_csize"].data_ptr(), self.d_first.data_ptr(),
-                                      t["frame_scratch"].data_ptr(), self.d_blocks.data_ptr(), self.nblk, s.cuda_stream)
+        rc = L.zmt_zstd_blocks_dict_device(d_framed.data_ptr() - self.pad, self.n, t["frame_off"].data_ptr(), t["frame_csize"].data_ptr(),
+                                           self.d_first.data_ptr(), t["frame_scratch"].data_ptr(), self.d_blocks.data_ptr(), self.nblk, s.cuda_stream,
+                                           dictionary.d_ddict.data_ptr() if dictionary is not None else None)
         if rc != 0:
             raise RuntimeError("zmt_zstd_blocks_device failed: %s" % ST_NAMES.get(rc, rc))
         self.d_frame_off, self.d_frame_csize, self.d_frame_scratch = t["frame_off"], t["frame_csize"], t["frame_scratch"]
@@ -624,9 +675,13 @@ class ZstdDeviceDecompressor:
     def run(self, d_framed, stream=None):
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_zstd_decompress_device(d_framed.data_ptr() - self.pad, self.d_blocks.data_ptr(), self.nblk, self.d_first.data_ptr(), self.d_expect.data_ptr(),
-                                              self.d_fseq.data_ptr(), self.n, self.out.data_ptr(), self.d_out_off.data_ptr(), self.out_size.data_ptr(), self.status.data_ptr(),
-                                              self.work.data_ptr(), s.cuda_stream)
+        args = (d_framed.data_ptr() - self.pad, self.d_blocks.data_ptr(), self.nblk, self.d_first.data_ptr(), self.d_expect.data_ptr(),
+                self.d_fseq.data_ptr(), self.n, self.out.data_ptr(), self.d_out_off.data_ptr(), self.out_size.data_ptr(), self.status.data_ptr(),
+                self.work.data_ptr(), s.cuda_stream)
+        if self.dictionary is not None:
+            rc = lib().zmt_zstd_decompress_dict_device(*args, self.dictionary.d_ddict.data_ptr())
+        else:
+            rc = lib().zmt_zstd_decompress_device(*args)
         if rc != 0:
             raise RuntimeError("zmt_zstd_decompress_device failed: %s" % ST_NAMES.get(rc, rc))
         return self.out, self.status

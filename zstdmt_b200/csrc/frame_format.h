@@ -181,12 +181,23 @@ struct ZBlk {
 #define ZB_SELF   0xFFFFFFFFu
 #define ZB_PREDEF 0xFFFFFFFEu
 #define ZB_NONE   0xFFFFFFFDu
+#define ZB_DICT   0xFFFFFFFCu       // the table comes from the batch's dictionary (a formatted one: ZDDict's descriptions)
 struct ZDSeq { uint32_t ll; uint32_t off; uint32_t ml; uint32_t pad; };
 
-// per-frame flags (the d_frame_seq[] argument of zmt_zstd_decompress_device)
+// per-frame flags (the d_frame_seq[] argument of zmt_zstd_decompress_device; ZF_DICT = 8 is in the public header)
 #define ZF_NEEDS_SEQ 1u     // blocks depend on earlier blocks: frame-sequential entropy pass
 #define ZF_CHECKSUM  2u     // 4-byte content checksum (low 32 bits of XXH64) follows the last block
 #define ZF_NO_SIZE   4u     // no Frame_Content_Size: the reported size is an upper bound (128 KiB per compressed block)
+
+// A loaded dictionary (zmt_zstd_ddict_load_device writes it; callers hold it as opaque device memory).  The walk reads
+// only `info` (status, ID, kind), so the host scan takes the zmt_zstd_dict_info summary in its place.
+struct ZDDict {
+    zmt_zstd_dict_info info;
+    uint64_t dict;              // device address of the dictionary's bytes (the caller's buffer)
+    uint32_t rep[3];            // repeat offsets the frames start from
+    uint32_t huf_off, of_off, ml_off, ll_off;     // formatted: where the four table descriptions start in the dictionary
+    uint32_t rep_off;           // formatted: where the repeat offsets start (the LL description's end)
+};
 
 // segments (zmt_zstd_segment_host): a table source carried from an earlier segment.  Only its bytes are used, by the
 // blocks that name it in *_src: regen 0, nseq 0, never decoded or executed.
@@ -221,10 +232,14 @@ ZMT_HD uint32_t zstd_walk_sources(const zmt_zstd_walk* w, uint64_t* off, uint32_
 // entropy scratch the blocks take (their seq_off / lit_off), w->flags collects the ZF_* bits, *bound gets the room of
 // the call's blocks (128 KiB per compressed block).  w->pos = the frame offset the walk stopped at: the next block header,
 // the frame's length at its end, or on failure the header element it could not take.  Returns ZMT_ST_*.
-template <bool W>
+// dict: the batch's dictionary (D = true).  Without one a frame that names a Dictionary_ID is ZMT_ST_UNSUPPORTED.  With
+// one every frame decodes against it (ZF_DICT | ZF_NEEDS_SEQ) unless it names another ID (ZMT_ST_DICT_WRONG, w->pos = 0),
+// and a formatted dictionary is the describer of all four tables until a block of the frame describes its own (ZB_DICT).
+// Only a whole-frame walk (w->pos == 0) takes a dictionary.  D = false: the walk without one, which never reads dict.
+template <bool W, bool D = false>
 ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
                             uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, zmt_zstd_walk* w,
-                            size_t pos_stop, uint64_t bound_stop, uint64_t* bound)
+                            size_t pos_stop, uint64_t bound_stop, uint64_t* bound, const zmt_zstd_dict_info* dict = nullptr)
 {
     const uint64_t at0 = w->pos;
     size_t pos = 0;
@@ -237,8 +252,19 @@ ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint3
         if (n < 6 || zf_rd32(p) != ZMT_ZSTD_MAGIC) return n < 6 ? ZMT_ST_TRUNCATED : ZMT_ST_BAD_MAGIC;
         const uint32_t fhd = p[4], fcs = fhd >> 6, single = (fhd >> 5) & 1, did = fhd & 3;
         if (fhd & 0x08) return ZMT_ST_BAD_HEADER;
-        if (did) return ZMT_ST_UNSUPPORTED;                               // dictionaries: not on the reference path
+        if (did && !D) return ZMT_ST_UNSUPPORTED;                         // dictionaries: only against a loaded one
         pos = 5 + (single ? 0 : 1);
+        if (D && did) {
+            const size_t dl = did == 3 ? 4 : did;
+            if (n < pos + dl) return ZMT_ST_TRUNCATED;
+            const uint32_t id = dl == 1 ? p[pos] : dl == 2 ? (uint32_t)(p[pos] | (p[pos + 1] << 8)) : zf_rd32(p + pos);
+            if (id != 0 && id != dict->dict_id) return ZMT_ST_DICT_WRONG;  // ZSTD_decompress_usingDict: a frame without an ID takes the dictionary
+            pos += dl;
+        }
+        if (D) {
+            if (dict->status != ZMT_ST_OK) return (int)dict->status;      // a dictionary whose load failed decodes nothing
+            w->flags |= ZF_DICT | ZF_NEEDS_SEQ;
+        }
         const size_t fl = fcs == 0 ? (single ? 1 : 0) : fcs == 1 ? 2 : fcs == 2 ? 4 : 8;
         if (n < pos + fl) return ZMT_ST_TRUNCATED;
         uint64_t cs = 0;
@@ -253,7 +279,7 @@ ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint3
     }
     // block that describes the Huffman tree / each sequence table in use, as a descriptor index of this call
     uint32_t cur[4];
-    for (uint32_t t = 0; t < 4; t++) cur[t] = w->src_off[t] == ZW_PREDEF ? ZB_PREDEF : ZB_NONE;
+    for (uint32_t t = 0; t < 4; t++) cur[t] = w->src_off[t] == ZW_PREDEF ? ZB_PREDEF : (D && dict->kind ? ZB_DICT : ZB_NONE);
     if (at0 != 0) {
         uint64_t so[4]; uint32_t sl[4];
         const uint32_t ns = zstd_walk_sources(w, so, sl);
@@ -361,15 +387,16 @@ ZMT_HD int zstd_walk_blocks(const uint8_t* p, size_t n, uint64_t base_off, uint3
 // size (the block bound without a content-size field).  *end = the frame's length on success, else the offset of the
 // header element the walk stopped at.  Bytes behind the frame are the caller's business.  Returns ZMT_ST_*.
 // The frame is one segment of zstd_walk_blocks that runs to its end.
-template <bool W>
+// D, dict: as for zstd_walk_blocks.
+template <bool W, bool D = false>
 ZMT_HD int zstd_frame_walk(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx, ZBlk* blocks_out,
                            uint32_t* nblocks_io, uint32_t max_blocks, uint64_t* scratch_used, uint64_t* content_size,
-                           uint32_t* flags, size_t* end)
+                           uint32_t* flags, size_t* end, const zmt_zstd_dict_info* dict = nullptr)
 {
     zmt_zstd_walk w = {};
     uint64_t bound = 0;
-    const int r = zstd_walk_blocks<W>(frame, n, base_off, frame_idx, blocks_out, nblocks_io, max_blocks, scratch_used, &w,
-                                      ~(size_t)0, ~0ull, &bound);
+    const int r = zstd_walk_blocks<W, D>(frame, n, base_off, frame_idx, blocks_out, nblocks_io, max_blocks, scratch_used, &w,
+                                         ~(size_t)0, ~0ull, &bound, dict);
     *flags = w.flags; *end = (size_t)w.pos;
     if (r == ZMT_ST_OK) *content_size = (w.flags & ZF_NO_SIZE) ? bound : w.content_size;
     return r;

@@ -17,6 +17,8 @@
 //   zidx_summary_kernel       one thread: the first failure in stream order and the totals (zmt_frame_index)
 //   zidx_zstd_blocks_kernel   one thread per frame: the writing walk of zstd_frame_walk fills the ZBlk table
 // The header formats live in frame_format.h, shared with the host walkers, so both sources of tables agree byte for byte.
+// The zstd kernels take a template flag D: D = true walks against the loaded dictionary dd (the *_dict_device calls),
+// D = false is the walk without one and never reads dd.
 #include <stdint.h>
 #include "cub_scan.h"
 #include "frame_format.h"
@@ -94,10 +96,11 @@ zidx_lz4_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restric
     out_off[f] = room; k.slots[f] = slots;
 }
 
+template <bool D>
 __global__ void __launch_bounds__(kThreads)
 zidx_zstd_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
                         uint32_t* __restrict__ first_blk, uint64_t* __restrict__ frame_scratch, uint64_t* __restrict__ expect,
-                        uint32_t* __restrict__ frame_seq, uint64_t* __restrict__ out_off, IdxWork k, uint32_t max_frames)
+                        uint32_t* __restrict__ frame_seq, uint64_t* __restrict__ out_off, IdxWork k, uint32_t max_frames, const ZDDict* __restrict__ dd)
 {
     const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
     if (f > max_frames) return;
@@ -107,7 +110,7 @@ zidx_zstd_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restri
         const uint64_t p = frame_off[f] + 12;
         const uint32_t n = frame_csize[f];
         size_t end = 0;
-        int r = zstd_frame_walk<false>(in + p, n, p, f, nullptr, &nb, 0xFFFFFFFFu, &scr, &cs, &flags, &end);
+        int r = zstd_frame_walk<false, D>(in + p, n, p, f, nullptr, &nb, 0xFFFFFFFFu, &scr, &cs, &flags, &end, D ? &dd->info : nullptr);
         if (r == ZMT_ST_OK && end != n) r = ZMT_ST_TRAILING;
         if (r != ZMT_ST_OK) { nb = 0; scr = 0; cs = 0; flags = 0; zidx_fail(k, f, (uint32_t)r, p + end); }
     }
@@ -119,11 +122,11 @@ zidx_zstd_frames_kernel(const uint8_t* __restrict__ in, const uint64_t* __restri
 // path's rule, and the first failure ends the walk (the next frame's start is not known behind it).  Frame f < max_frames
 // gets its offset, length, room and (LZ4) slot count or (zstd) block count, scratch, expect and flags; the scans make the
 // counts bases.  The decode calls take frame_csize as 32 bits: a frame of 2^32 bytes or more is ZMT_ST_UNSUPPORTED.
-template <bool Z>
+template <bool Z, bool D>
 __global__ void zidx_plain_walk_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t max_frames, uint64_t* __restrict__ frame_off,
                                        uint32_t* __restrict__ frame_csize, uint64_t* __restrict__ out_off, uint64_t* __restrict__ slots,
                                        uint32_t* __restrict__ first_blk, uint64_t* __restrict__ frame_scratch, uint64_t* __restrict__ expect,
-                                       uint32_t* __restrict__ frame_seq, IdxCtl* __restrict__ ctl)
+                                       uint32_t* __restrict__ frame_seq, IdxCtl* __restrict__ ctl, const ZDDict* __restrict__ dd)
 {
     uint64_t pos = 0, max_off = 0, at = 0;
     uint32_t n = 0, st = ZMT_ST_OK;
@@ -138,7 +141,7 @@ __global__ void zidx_plain_walk_kernel(const uint8_t* __restrict__ in, uint64_t 
         uint32_t nb = 0, flags = 0;
         if (Z) {
             size_t end = 0;
-            st = (uint32_t)zstd_frame_walk<false>(p, rem, 0, 0, nullptr, &nb, 0xFFFFFFFFu, &scr, &room, &flags, &end);
+            st = (uint32_t)zstd_frame_walk<false, D>(p, rem, 0, 0, nullptr, &nb, 0xFFFFFFFFu, &scr, &room, &flags, &end, D ? &dd->info : nullptr);
             len = end; at = pos + end;
         } else {
             uint64_t stop = 0;
@@ -185,9 +188,11 @@ __global__ void zidx_summary_kernel(IdxWork k, uint32_t max_frames, const uint64
     *info = r;
 }
 
+template <bool D>
 __global__ void __launch_bounds__(kThreads)
 zidx_zstd_blocks_kernel(const uint8_t* __restrict__ in, uint32_t nframes, const uint64_t* __restrict__ frame_off, const uint32_t* __restrict__ frame_csize,
-                        const uint32_t* __restrict__ first_blk, const uint64_t* __restrict__ frame_scratch, ZBlk* __restrict__ blocks, uint32_t nblocks)
+                        const uint32_t* __restrict__ first_blk, const uint64_t* __restrict__ frame_scratch, ZBlk* __restrict__ blocks, uint32_t nblocks,
+                        const ZDDict* __restrict__ dd)
 {
     const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
     if (f >= nframes) return;
@@ -196,7 +201,7 @@ zidx_zstd_blocks_kernel(const uint8_t* __restrict__ in, uint32_t nframes, const 
     const uint32_t lim = min(first_blk[f + 1], nblocks);
     uint64_t scr = frame_scratch[f], cs = 0;
     size_t end = 0;
-    zstd_frame_walk<true>(in + p, frame_csize[f], p, f, blocks, &nb, lim, &scr, &cs, &flags, &end);
+    zstd_frame_walk<true, D>(in + p, frame_csize[f], p, f, blocks, &nb, lim, &scr, &cs, &flags, &end, D ? &dd->info : nullptr);
 }
 
 // The common part of the index calls: the walk, the per-frame pass, scans, summary.  walk(k) enqueues the walk,
@@ -245,18 +250,44 @@ extern "C" int zmt_lz4_index_device(const void* d_in, uint64_t in_bytes, uint32_
                         });
 }
 
-extern "C" int zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
-                                     uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
-                                     uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+// The zstd index calls: container (plain = false) or plain stream, against the dictionary dd or without one.
+static int zstd_index(bool plain, const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+               uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq, uint64_t* d_out_off,
+               zmt_frame_index* d_info, void* d_work, cudaStream_t stream, const ZDDict* dd)
 {
-    cudaStream_t stream = (cudaStream_t)stream_;
     if (!d_frame_first_blk || !d_frame_scratch || (max_frames && (!d_expect || !d_frame_seq))) return ZMT_ST_BAD_ARG;
     return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, d_frame_first_blk, d_frame_scratch, d_info, d_work, stream,
-                        [&](IdxWork k) { container_walk(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k, stream); },
+                        [&](IdxWork k) {
+                            if (!plain) container_walk(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, k, stream);
+                            else (dd ? zidx_plain_walk_kernel<true, true> : zidx_plain_walk_kernel<true, false>)<<<1, 1, 0, stream>>>(
+                                (const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, k.slots, d_frame_first_blk,
+                                d_frame_scratch, d_expect, d_frame_seq, k.ctl, dd);
+                        },
                         [&](uint32_t grid, IdxWork k) {
-                            zidx_zstd_frames_kernel<<<grid, kThreads, 0, stream>>>((const uint8_t*)d_in, d_frame_off, d_frame_csize, d_frame_first_blk,
-                                                                                 d_frame_scratch, d_expect, d_frame_seq, d_out_off, k, max_frames);
+                            if (plain) zidx_plain_tail_kernel<<<grid, kThreads, 0, stream>>>(k, max_frames, d_out_off, d_frame_first_blk, d_frame_scratch);
+                            else if (dd) zidx_zstd_frames_kernel<true><<<grid, kThreads, 0, stream>>>(
+                                (const uint8_t*)d_in, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq, d_out_off,
+                                k, max_frames, dd);
+                            else zidx_zstd_frames_kernel<false><<<grid, kThreads, 0, stream>>>(
+                                (const uint8_t*)d_in, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq, d_out_off,
+                                k, max_frames, nullptr);
                         });
+}
+
+extern "C" int zmt_zstd_index_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                     uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                     uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream)
+{
+    return zstd_index(false, d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq,
+                      d_out_off, d_info, d_work, (cudaStream_t)stream, nullptr);
+}
+
+extern "C" int zmt_zstd_index_dict_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                          uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                          uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream, const void* d_ddict)
+{
+    return zstd_index(false, d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq,
+                      d_out_off, d_info, d_work, (cudaStream_t)stream, (const ZDDict*)d_ddict);
 }
 
 extern "C" int zmt_lz4_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
@@ -265,36 +296,44 @@ extern "C" int zmt_lz4_index_plain_device(const void* d_in, uint64_t in_bytes, u
     cudaStream_t stream = (cudaStream_t)stream_;
     return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, nullptr, nullptr, d_info, d_work, stream,
                         [&](IdxWork k) {
-                            zidx_plain_walk_kernel<false><<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off,
-                                                                               k.slots, nullptr, nullptr, nullptr, nullptr, k.ctl);
+                            zidx_plain_walk_kernel<false, false><<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off,
+                                                                               k.slots, nullptr, nullptr, nullptr, nullptr, k.ctl, nullptr);
                         },
                         [&](uint32_t grid, IdxWork k) { zidx_plain_tail_kernel<<<grid, kThreads, 0, stream>>>(k, max_frames, d_out_off, nullptr, nullptr); });
 }
 
 extern "C" int zmt_zstd_index_plain_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
                                            uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
-                                           uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream_)
+                                           uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream)
 {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    if (!d_frame_first_blk || !d_frame_scratch || (max_frames && (!d_expect || !d_frame_seq))) return ZMT_ST_BAD_ARG;
-    return index_device(d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off, d_frame_first_blk, d_frame_scratch, d_info, d_work, stream,
-                        [&](IdxWork k) {
-                            zidx_plain_walk_kernel<true><<<1, 1, 0, stream>>>((const uint8_t*)d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_out_off,
-                                                                              k.slots, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq, k.ctl);
-                        },
-                        [&](uint32_t grid, IdxWork k) {
-                            zidx_plain_tail_kernel<<<grid, kThreads, 0, stream>>>(k, max_frames, d_out_off, d_frame_first_blk, d_frame_scratch);
-                        });
+    return zstd_index(true, d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq,
+                      d_out_off, d_info, d_work, (cudaStream_t)stream, nullptr);
 }
 
-extern "C" int zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
-                                      const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream_)
+extern "C" int zmt_zstd_index_plain_dict_device(const void* d_in, uint64_t in_bytes, uint32_t max_frames, uint64_t* d_frame_off, uint32_t* d_frame_csize,
+                                                uint32_t* d_frame_first_blk, uint64_t* d_frame_scratch, uint64_t* d_expect, uint32_t* d_frame_seq,
+                                                uint64_t* d_out_off, zmt_frame_index* d_info, void* d_work, void* stream, const void* d_ddict)
+{
+    return zstd_index(true, d_in, in_bytes, max_frames, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_expect, d_frame_seq,
+                      d_out_off, d_info, d_work, (cudaStream_t)stream, (const ZDDict*)d_ddict);
+}
+
+extern "C" int zmt_zstd_blocks_dict_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                           const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream_,
+                                           const void* d_ddict)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0 || nblocks == 0) return ZMT_ST_OK;
     if (!d_in || !d_frame_off || !d_frame_csize || !d_frame_first_blk || !d_frame_scratch || !d_blocks) return ZMT_ST_BAD_ARG;
+    const ZDDict* dd = (const ZDDict*)d_ddict;
     ZmtProfScope ps(ZMT_K_FRAME_INDEX, stream);
-    zidx_zstd_blocks_kernel<<<(nframes + kThreads - 1) / kThreads, kThreads, 0, stream>>>((const uint8_t*)d_in, nframes, d_frame_off, d_frame_csize,
-                                                                                         d_frame_first_blk, d_frame_scratch, (ZBlk*)d_blocks, nblocks);
+    (dd ? zidx_zstd_blocks_kernel<true> : zidx_zstd_blocks_kernel<false>)<<<(nframes + kThreads - 1) / kThreads, kThreads, 0, stream>>>(
+        (const uint8_t*)d_in, nframes, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, (ZBlk*)d_blocks, nblocks, dd);
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
+}
+
+extern "C" int zmt_zstd_blocks_device(const void* d_in, uint32_t nframes, const uint64_t* d_frame_off, const uint32_t* d_frame_csize,
+                                      const uint32_t* d_frame_first_blk, const uint64_t* d_frame_scratch, void* d_blocks, uint32_t nblocks, void* stream)
+{
+    return zmt_zstd_blocks_dict_device(d_in, nframes, d_frame_off, d_frame_csize, d_frame_first_blk, d_frame_scratch, d_blocks, nblocks, stream, nullptr);
 }

@@ -1263,6 +1263,7 @@ const char* status_string(size_t st)
     case ZMT_ST_UNSUPPORTED: return "stream type not supported by the GPU path";
     case ZMT_ST_CUDA: return "CUDA runtime / kernel failure";
     case ZMT_ST_BAD_ARG: return "bad argument";
+    case ZMT_ST_DICT_WRONG: return "ERROR_dictionary_wrong";
     }
     return nullptr;
 }

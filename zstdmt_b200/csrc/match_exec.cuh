@@ -110,13 +110,23 @@ __device__ __forceinline__ bool mx_independent(uint32_t lane, bool act, uint32_t
 // Every byte a step regenerates is written to global memory AND to the window; a source byte at or above the step's
 // first output byte is read from the window.  A chain of matches that feed each other then runs at shared-memory
 // latency instead of one L2 round trip per link.
+// A prefix region below the frame: content that precedes the frame's output without being part of it (a dictionary's
+// content).  The copies below take it when instantiated with PRE = true: a source byte at block position q below the
+// frame's first byte fs reads pre_end[q - fs], the region's tail, and a copy that straddles fs is split there.  The
+// caller bounds every source by the frame's output so far plus the region.  PRE = false never reads pre_end / fs.
 struct MxWin {
     uint8_t* dst;             // the block's output in global memory
     uint8_t* S;               // S[wb + p] = window byte of block position p, lo <= p < lo + MX_SPAN
     int32_t wb, lo;           // lo = block position of the step's first output byte
+    const uint8_t* pre_end;   // PRE: one past the prefix region's last byte
+    int32_t fs;               // PRE: block position of the frame's first byte (<= 0)
 };
 
-__device__ __forceinline__ uint8_t mx_src_byte(const MxWin& W, int32_t q) { return q >= W.lo ? W.S[W.wb + q] : W.dst[q]; }
+template <bool PRE = false>
+__device__ __forceinline__ uint8_t mx_src_byte(const MxWin& W, int32_t q)
+{
+    return q >= W.lo ? W.S[W.wb + q] : (PRE && q < W.fs) ? W.pre_end[q - W.fs] : W.dst[q];
+}
 // One lane: bytes [k0, n) of src to d (global memory) and dw (window), loads first, stores after, 8 bytes at a time — a
 // byte-wise load -> store loop pays one L2 latency per byte, this one per 8 bytes.
 __device__ __forceinline__ void mx_lane_copy(uint8_t* d, uint8_t* dw, const uint8_t* src, uint32_t k0, uint32_t n)
@@ -130,7 +140,7 @@ __device__ __forceinline__ void mx_lane_copy(uint8_t* d, uint8_t* dw, const uint
     }
 }
 
-// bytes of the source [sp, sp + ml) that lie below the window
+// bytes of the source [sp, sp + ml) that lie below the window (with PRE: the prefix region's among them too)
 __device__ __forceinline__ int32_t mx_nlow(const MxWin& W, int32_t sp, uint32_t ml)
 {
     return sp >= W.lo ? 0 : (W.lo - sp < (int32_t)ml ? W.lo - sp : (int32_t)ml);
@@ -138,29 +148,36 @@ __device__ __forceinline__ int32_t mx_nlow(const MxWin& W, int32_t sp, uint32_t 
 
 // One lane copies its own independent match of at most MX_OWN bytes: the nlow source bytes below the window come from
 // global memory (those below k0 the caller has copied already), the rest out of the window.
+template <bool PRE = false>
 __device__ __forceinline__ void mx_own_match(const MxWin& W, uint32_t dst, uint32_t ml, uint32_t off, int32_t nlow, int32_t k0)
 {
     const int32_t sp = (int32_t)dst - (int32_t)off;
     uint8_t* d = W.dst + dst; uint8_t* dw = W.S + (W.wb + (int32_t)dst);
-    mx_lane_copy(d, dw, W.dst + sp, (uint32_t)k0, (uint32_t)nlow);
+    if (PRE && sp < W.fs) {                                     // the first np source bytes lie in the prefix region
+        const int32_t np = W.fs - sp < nlow ? W.fs - sp : nlow;
+        mx_lane_copy(d, dw, W.pre_end + (sp - W.fs), (uint32_t)k0, (uint32_t)np);
+        mx_lane_copy(d, dw, W.dst + sp, (uint32_t)(k0 > np ? k0 : np), (uint32_t)nlow);
+    } else
+        mx_lane_copy(d, dw, W.dst + sp, (uint32_t)k0, (uint32_t)nlow);
     for (int32_t k = nlow; k < (int32_t)ml; k++) { const uint8_t x = W.S[W.wb + sp + k]; d[k] = x; dw[k] = x; }
 }
 
 // The whole warp copies one match through the window; called for the matches of a step in order, so the source may be a
 // match of this very step, or the match itself (off < ml).
+template <bool PRE = false>
 __device__ __forceinline__ void mx_warp_match(const MxWin& W, uint32_t dst, uint32_t ml, uint32_t off, uint32_t lane)
 {
     const int32_t qs = (int32_t)dst - (int32_t)off;
     uint8_t* d = W.dst + dst; uint8_t* dw = W.S + (W.wb + (int32_t)dst);
     if (off >= ml) {
-        for (uint32_t k = lane; k < ml; k += 32) { const uint8_t x = mx_src_byte(W, qs + (int32_t)k); d[k] = x; dw[k] = x; }
+        for (uint32_t k = lane; k < ml; k += 32) { const uint8_t x = mx_src_byte<PRE>(W, qs + (int32_t)k); d[k] = x; dw[k] = x; }
     } else if (off >= MX_PERIOD) {                              // overlapping, period >= warp width: 32-byte waves
         for (uint32_t k = 0; k < ml; k += 32) {
-            if (k + lane < ml) { const uint8_t x = mx_src_byte(W, qs + (int32_t)(k + lane)); d[k + lane] = x; dw[k + lane] = x; }
+            if (k + lane < ml) { const uint8_t x = mx_src_byte<PRE>(W, qs + (int32_t)(k + lane)); d[k + lane] = x; dw[k + lane] = x; }
             __syncwarp();
         }
     } else {                                                    // short period: replicate the pattern
-        for (uint32_t k = lane; k < ml; k += 32) { const uint8_t x = mx_src_byte(W, qs + (int32_t)(k % off)); d[k] = x; dw[k] = x; }
+        for (uint32_t k = lane; k < ml; k += 32) { const uint8_t x = mx_src_byte<PRE>(W, qs + (int32_t)(k % off)); d[k] = x; dw[k] = x; }
     }
     __syncwarp();
 }
@@ -173,5 +190,20 @@ __device__ __forceinline__ void mx_warp_match_global(uint8_t* d, uint32_t ml, ui
     if (off >= ml) { for (uint32_t k = lane; k < ml; k += 32) d[k] = m[k]; }
     else if (off >= MX_PERIOD) { for (uint32_t k = 0; k < ml; k += 32) { if (k + lane < ml) d[k + lane] = m[k + lane]; __syncwarp(); } }
     else { for (uint32_t k = lane; k < ml; k += 32) d[k] = m[k % off]; }
+    __syncwarp();
+}
+
+// mx_warp_match_global with a prefix region: `below` = the frame's output below d; a source that starts further back takes
+// its first off - below bytes from the region's tail [pre_end - (off - below), pre_end).
+__device__ __forceinline__ void mx_warp_match_global_pre(uint8_t* d, uint32_t ml, uint32_t off, uint32_t lane, const uint8_t* pre_end, uint64_t below)
+{
+    if (off <= below) { mx_warp_match_global(d, ml, off, lane); return; }
+    const uint8_t* m = d - off;
+    const uint32_t np = (uint32_t)(off - below);
+    const uint8_t* pm = pre_end - np;
+    auto at = [&](uint32_t i) -> uint8_t { return i < np ? pm[i] : m[i]; };
+    if (off >= ml) { for (uint32_t k = lane; k < ml; k += 32) d[k] = at(k); }
+    else if (off >= MX_PERIOD) { for (uint32_t k = 0; k < ml; k += 32) { if (k + lane < ml) d[k + lane] = at(k + lane); __syncwarp(); } }
+    else { for (uint32_t k = lane; k < ml; k += 32) d[k] = at(k % off); }
     __syncwarp();
 }

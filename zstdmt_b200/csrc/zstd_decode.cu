@@ -20,6 +20,10 @@
 //                            the `done` flags of the blocks it reads from.  Ticket order, dependency test and match copies
 //                            are match_exec.cuh's, shared with the LZ4 decoder
 //   zstd_checksum_kernel     one warp per frame with a content checksum: XXH64 of the regenerated frame
+// zmt_zstd_decompress_dict_device runs them against a dictionary (ZDDict, loaded once by zstd_ddict_load_kernel): its
+// frames take the dependent-block route, whose kernels are instantiated with DICT = true — treeless literals and
+// Repeat_Mode tables may name the dictionary's tables (ZB_DICT), repeat offsets start from its three, and matches may read
+// its content below the frame's output (match_exec.cuh's prefix region).  DICT = false is the code without a dictionary.
 // zmt_zstd_decompress_segments_device runs the same kernels on segments of frames (zmt_zstd_segment): repeat offsets, the
 // content size and the running XXH64 come from the record and go back to it, matches may reach the history below the
 // segment's output, and ZB_SRC descriptors carry the bytes of earlier segments' table describers.
@@ -29,7 +33,7 @@
 // Scope (DESIGN.md §7): the full block format of RFC 8878 — raw / RLE / compressed blocks, Huffman literals with direct
 // or FSE-coded weights, 1 or 4 streams, treeless reuse, sequence tables predefined / RLE / FSE-described / repeat,
 // repeat offsets, content checksum, frames without a content size — i.e. what libzstd and the zstd CLI emit (SURVEY.md
-// fact 0.6).  Not handled (reported per frame as ZMT_ST_UNSUPPORTED, never decoded on the CPU): dictionaries.
+// fact 0.6) — and frames written with a dictionary, formatted or raw content (RFC 8878 §5).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -811,9 +815,28 @@ __device__ bool zd_inherit_table(ZTabRef& cur, uint32_t which, const uint8_t* sr
     return false;
 }
 
+// Build sequence table `which` (0 LL, 1 OF, 2 ML) from the dictionary's FSE description of it (a formatted dictionary
+// holds them in the order OF, ML, LL; each ends where the next begins, LL where the repeat offsets begin).  One lane.
+__device__ bool zd_dict_table(ZTabRef& cur, uint32_t which, const ZDDict* dd, ZWarpTabs& W)
+{
+    if (dd->info.status != ZMT_ST_OK || dd->info.kind != 1) return false;
+    uint32_t* const custom[3] = { W.ll, W.of, W.ml };
+    const uint32_t* const predef[3] = { W.pll, W.pof, W.pml };
+    const uint32_t plog[3] = { 6, 5, 6 };
+    const int maxlog[3] = { 9, 8, 9 }, maxsym[3] = { 35, 31, 52 };
+    const uint32_t at = which == 0 ? dd->ll_off : which == 1 ? dd->of_off : dd->ml_off;
+    const uint32_t end = which == 0 ? dd->rep_off : which == 1 ? dd->ml_off : dd->ll_off;
+    const uint8_t* qp = reinterpret_cast<const uint8_t*>(dd->dict) + at;
+    uint32_t qn = end - at;
+    bool need = false;
+    return zd_seq_table(cur, 2, custom[which], predef[which], plog[which], W.norm, qp, qn, maxlog[which], maxsym[which], false, &need);
+}
+
+template <bool DICT>
 __global__ void __launch_bounds__(32 * ZD_WARPS)
 zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, uint32_t nblocks, const uint32_t* __restrict__ frame_seq,
-                        uint8_t* __restrict__ scratch, uint32_t* __restrict__ regen, uint32_t* __restrict__ status, const uint32_t* __restrict__ lit_done)
+                        uint8_t* __restrict__ scratch, uint32_t* __restrict__ regen, uint32_t* __restrict__ status, const uint32_t* __restrict__ lit_done,
+                        const ZDDict* __restrict__ dd)
 {
     __shared__ ZWarpTabs tabs[ZD_WARPS];
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -828,7 +851,12 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
     uint32_t bad = 0;
     // ---- treeless literals: the tree of the block that last described one
     if (!lit_done[b] && B.huf_src != ZB_SELF) {
-        if (B.huf_src >= nblocks) bad = 1;
+        uint32_t tb;
+        if (DICT && B.huf_src == ZB_DICT) {
+            if (dd->info.status != ZMT_ST_OK || dd->info.kind != 1 ||
+                zd_huf_build(W, reinterpret_cast<const uint8_t*>(dd->dict) + dd->huf_off, dd->of_off - dd->huf_off, lane, &tb)) bad = 1;
+        }
+        else if (B.huf_src >= nblocks) bad = 1;
         else {
             const ZBlk S = blocks[B.huf_src];
             uint32_t lhdr, lcomp, lregen, lt, sf, tb;
@@ -844,6 +872,7 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
             ZTabRef* const refs[3] = { &fs.ll, &fs.of, &fs.ml };
             for (uint32_t t = 0; t < 3 && !r; t++) {
                 if (srcs[t] == ZB_SELF || srcs[t] == ZB_PREDEF) continue;
+                if (DICT && srcs[t] == ZB_DICT) { if (!zd_dict_table(*refs[t], t, dd, W)) r = 1; continue; }
                 if (srcs[t] >= nblocks) { r = 1; break; }
                 const ZBlk S = blocks[srcs[t]];
                 if ((S.type != ZB_CMP && S.type != ZB_SRC) || !zd_inherit_table(*refs[t], t, in + S.comp_off, S.comp_size, W)) r = 1;
@@ -869,16 +898,20 @@ zstd_entropy_dep_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__
 // block-parallel pass carry the coded offset value and pad = 1.  32 records are loaded at once (coalesced); the rule itself
 // is a serial state machine over (r0, r1, r2), walked by all lanes in lockstep with the records passed by shuffle; lane j
 // keeps the resolved offset of record j and stores it.  A segment (seg != nullptr) after the first starts from the offsets
-// the previous segment left in its record, and every segment stores its own back.
+// the previous segment left in its record, and every segment stores its own back.  A frame decoded against a dictionary
+// (DICT, ZF_DICT) starts from the dictionary's repeat offsets.
+template <bool DICT>
 __global__ void __launch_bounds__(32 * ZD_WARPS)
 zstd_resolve_offsets_kernel(const ZBlk* __restrict__ blocks, const uint32_t* __restrict__ frame_first_blk, const uint32_t* __restrict__ frame_seq,
-                            uint8_t* __restrict__ scratch, uint32_t* __restrict__ status, zmt_zstd_segment* __restrict__ seg, uint32_t nframes)
+                            uint8_t* __restrict__ scratch, uint32_t* __restrict__ status, zmt_zstd_segment* __restrict__ seg, uint32_t nframes,
+                            const ZDDict* __restrict__ dd)
 {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t f = blockIdx.x * ZD_WARPS + (threadIdx.x >> 5);
     if (f >= nframes || !(frame_seq[f] & ZF_NEEDS_SEQ) || (status[f] & 0xFF) != 0) return;
     uint32_t r0 = 1, r1 = 4, r2 = 8;
     if (seg && !(seg[f].flags & ZMT_SEG_FIRST)) { r0 = seg[f].rep[0]; r1 = seg[f].rep[1]; r2 = seg[f].rep[2]; }
+    if (DICT && (frame_seq[f] & ZF_DICT)) { r0 = dd->rep[0]; r1 = dd->rep[1]; r2 = dd->rep[2]; }
     for (uint32_t b = frame_first_blk[f]; b < frame_first_blk[f + 1]; b++) {
         const ZBlk B = blocks[b];
         if (B.type != ZB_CMP || B.nseq == 0) continue;
@@ -993,10 +1026,15 @@ __global__ void zstd_offsets_kernel(const ZBlk* __restrict__ blocks, uint32_t nb
 #define ZX_LANE_LIT 32u        // a literal run up to this length is copied by its own lane, a longer one by the whole warp
 // One block, one warp.  Blocks are handed out in match_exec.cuh's ticket order, so every block this one may wait for —
 // lower indices of the same frame — is held by a warp that is already running.
+// DICT: the dictionary's content is the prefix region below every frame (match_exec.cuh), so an offset is valid up to the
+// frame's output so far plus the content (libzstd's bound: no window check, a single-segment frame's offsets into the
+// dictionary routinely exceed Window_Size).  A match whose source starts below the frame waits for all earlier blocks of
+// its frame: the part above the frame's start may lie in any of them.
+template <bool DICT>
 __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, const uint8_t* __restrict__ scratch,
                          const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                          uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, const zmt_zstd_segment* __restrict__ seg,
-                         uint8_t* S)
+                         uint8_t* S, const ZDDict* __restrict__ dd)
 {
     const ZBlk B = blocks[b];
     volatile uint32_t* vdone = done;
@@ -1016,11 +1054,19 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
         const uint64_t blk_abs = blk_out[b];                 // absolute output address of this block
         // bytes of the frame before this block: a segment's matches may also reach the history placed below its output
         const uint64_t blk_in_frame = blk_abs - frame_base + (seg ? seg[B.frame].history : 0);
+        uint64_t pre_bytes = 0;                              // DICT: the dictionary content below the frame
+        const uint8_t* pre_end = nullptr;
+        if (DICT) {
+            pre_bytes = dd->info.status == ZMT_ST_OK ? dd->info.content_bytes : 0;
+            pre_end = reinterpret_cast<const uint8_t*>(dd->dict) + dd->info.content_off + pre_bytes;
+        }
+        const uint64_t blk_reach = DICT ? blk_in_frame + pre_bytes : blk_in_frame;     // the farthest a match may reach from the block's start
         // Up to MX_STEP sequences per step: one coalesced load of the records, positions from two warp scans.  Everything the
         // step regenerates — at most MX_SPAN bytes, else the step is cut shorter — goes to global memory and to the step
         // window (MxWin): every lane copies its own literal run (literals come from the scratch, no ordering among them),
         // then the matches run.
         MxWin W; W.dst = dst; W.S = S;
+        if (DICT) { W.pre_end = pre_end; W.fs = blk_in_frame < 0x7FFFFFFFull ? -(int32_t)blk_in_frame : -0x7FFFFFFF; }
         for (uint32_t base = 0; base < B.nseq;) {
             uint32_t cnt = B.nseq - base < MX_STEP ? B.nseq - base : MX_STEP;
             uint32_t ll = 0, off = 0, ml = 0;
@@ -1037,10 +1083,11 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
                 // the first sequence alone is larger than the window: straight in global memory, by the whole warp
                 const uint32_t qll = __shfl_sync(0xFFFFFFFFu, ll, 0), qoff = __shfl_sync(0xFFFFFFFFu, off, 0), qml = __shfl_sync(0xFFFFFFFFu, ml, 0);
                 const uint32_t mp = op + qll;
-                if ((uint64_t)op + qll + qml > rg || (uint64_t)lp + qll > B.regen_hint || qoff == 0 || (uint64_t)qoff > blk_in_frame + mp) { bad = true; break; }
+                if ((uint64_t)op + qll + qml > rg || (uint64_t)lp + qll > B.regen_hint || qoff == 0 || (uint64_t)qoff > blk_reach + mp) { bad = true; break; }
                 for (uint32_t k = lane; k < qll; k += 32) dst[op + k] = lit[lp + k];
                 if (qoff > mp) {
-                    const unsigned long long need = blk_abs + mp - qoff;
+                    // below the frame's start (DICT): the match also reads every earlier block of its frame
+                    const unsigned long long need = (DICT && (uint64_t)qoff > blk_in_frame + mp) ? frame_base : blk_abs + mp - qoff;
                     bool waited = false;
                     while (waited_to > 0 && blocks[waited_to - 1].frame == B.frame && blk_out[waited_to - 1] + regen[waited_to - 1] > need) {
                         waited_to--; waited = true;
@@ -1050,14 +1097,15 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
                     if (waited) __threadfence();
                 }
                 __syncwarp();
-                mx_warp_match_global(dst + mp, qml, qoff, lane);
+                if (DICT) mx_warp_match_global_pre(dst + mp, qml, qoff, lane, pre_end, blk_in_frame + mp);
+                else mx_warp_match_global(dst + mp, qml, qoff, lane);
                 op += qll + qml; lp += qll; base += 1;
                 continue;
             }
             cnt = nfit;
             if (lane >= cnt) { ll = 0; ml = 0; }
             const uint32_t my_op = op + it - (ll + ml), my_lp = lp + il - ll, my_mp = my_op + ll;
-            const bool mybad = lane < cnt && ((uint64_t)my_op + ll + ml > rg || (uint64_t)my_lp + ll > B.regen_hint || off == 0 || (uint64_t)off > blk_in_frame + my_mp);
+            const bool mybad = lane < cnt && ((uint64_t)my_op + ll + ml > rg || (uint64_t)my_lp + ll > B.regen_hint || off == 0 || (uint64_t)off > blk_reach + my_mp);
             const uint32_t badmask = __ballot_sync(0xFFFFFFFFu, mybad);
             const uint32_t lim = badmask ? (uint32_t)(__ffs(badmask) - 1) : cnt;      // sequences of this step that are executed
             W.lo = (int32_t)op; W.wb = -(int32_t)op;                                   // the window starts at the step's first output byte
@@ -1071,7 +1119,7 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
             // ---- matches.  Any source below this block: wait (once per step) for the earlier blocks it touches.
             {
                 unsigned long long need = ~0ull;                            // lowest absolute output address read by this step
-                if (lane < lim && ml && off > my_mp) need = blk_abs + my_mp - off;
+                if (lane < lim && ml && off > my_mp) need = (DICT && (uint64_t)off > blk_in_frame + my_mp) ? frame_base : blk_abs + my_mp - off;
 #pragma unroll
                 for (int x = 16; x > 0; x >>= 1) { const unsigned long long y = __shfl_xor_sync(0xFFFFFFFFu, need, x); need = y < need ? y : need; }
                 if (need != ~0ull) {
@@ -1087,12 +1135,12 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
             __syncwarp();                                                   // this step's literals are in place (global and window)
             const bool act = lane < lim && ml != 0;
             const bool indep = mx_independent(lane, act, my_mp, ml, off);
-            if (indep && ml <= MX_OWN) mx_own_match(W, my_mp, ml, off, mx_nlow(W, (int32_t)my_mp - (int32_t)off, ml), 0);
+            if (indep && ml <= MX_OWN) mx_own_match<DICT>(W, my_mp, ml, off, mx_nlow(W, (int32_t)my_mp - (int32_t)off, ml), 0);
             uint32_t dm = __ballot_sync(0xFFFFFFFFu, act && !(indep && ml <= MX_OWN));   // long independent ones and the dependent ones: in order, whole warp
             if (dm) __syncwarp();
             while (dm) {
                 const int jq = __ffs(dm) - 1; dm &= dm - 1;
-                mx_warp_match(W, __shfl_sync(0xFFFFFFFFu, my_mp, jq), __shfl_sync(0xFFFFFFFFu, ml, jq), __shfl_sync(0xFFFFFFFFu, off, jq), lane);
+                mx_warp_match<DICT>(W, __shfl_sync(0xFFFFFFFFu, my_mp, jq), __shfl_sync(0xFFFFFFFFu, ml, jq), __shfl_sync(0xFFFFFFFFu, off, jq), lane);
             }
             __syncwarp();
             if (badmask) { bad = true; break; }
@@ -1111,12 +1159,13 @@ __device__ void zx_block(uint32_t b, uint32_t lane, const uint8_t* __restrict__ 
     if (lane == 0) { __threadfence(); vdone[b] = 1; }
 }
 
+template <bool DICT>
 __global__ void __launch_bounds__(32 * ZX_WARPS)
 zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blocks, uint32_t nblocks, const uint8_t* __restrict__ scratch,
                     const uint32_t* __restrict__ regen, const uint64_t* __restrict__ blk_out, const uint64_t* __restrict__ out_off,
                     uint8_t* __restrict__ out, uint32_t* __restrict__ done, uint32_t* __restrict__ status, unsigned long long* __restrict__ ticket,
                     const uint32_t* __restrict__ frame_first_blk, const unsigned long long* __restrict__ wbase, const zmt_zstd_segment* __restrict__ seg,
-                    uint32_t nframes)
+                    uint32_t nframes, const ZDDict* __restrict__ dd)
 {
     __shared__ __align__(16) uint8_t stage[ZX_WARPS][MX_SPAN];
     const uint32_t lane = threadIdx.x & 31;
@@ -1127,7 +1176,7 @@ zstd_execute_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ blo
         uint32_t b;
         if (!mx_ticket_unit(T, tk, frame_first_blk, b)) continue;
         if (b >= nblocks) continue;
-        zx_block(b, lane, in, blocks, scratch, regen, blk_out, out_off, out, done, status, seg, stage[threadIdx.x >> 5]);
+        zx_block<DICT>(b, lane, in, blocks, scratch, regen, blk_out, out_off, out, done, status, seg, stage[threadIdx.x >> 5], dd);
         __syncwarp();
     }
 }
@@ -1235,6 +1284,59 @@ zstd_checksum_kernel(const uint8_t* __restrict__ in, const ZBlk* __restrict__ bl
     if (stored != (uint32_t)h) zd_fail(status, f, ZMT_ST_CONTENT_CHECKSUM);
 }
 
+// ---------------------------------------------------------------- dictionary load (RFC 8878 §5), one warp
+// A formatted dictionary: magic, ID, the Huffman tree description (literals-section format), FSE descriptions for OF, ML
+// and LL, three LE32 repeat offsets, content.  The tables are parsed and built with the decoders' own routines and the
+// block format's limits, only to check them: the blocks that name ZB_DICT rebuild them from the offsets recorded here.
+// Anything without the magic is raw content (libzstd's ZSTD_dct_auto).
+#define ZD_DICT_MAGIC 0xEC30A437u
+__global__ void __launch_bounds__(32)
+zstd_ddict_load_kernel(const uint8_t* __restrict__ d, uint64_t n, ZDDict* __restrict__ out, zmt_zstd_dict_info* __restrict__ info)
+{
+    __shared__ ZWarpTabs W;
+    const uint32_t lane = threadIdx.x;
+    ZDDict R;
+    R.info.status = ZMT_ST_OK; R.info.dict_id = 0; R.info.kind = 0; R.info.reserved = 0;
+    R.info.content_bytes = n; R.info.content_off = 0;
+    R.dict = (uint64_t)(uintptr_t)d; R.rep[0] = 1; R.rep[1] = 4; R.rep[2] = 8;
+    R.huf_off = R.of_off = R.ml_off = R.ll_off = R.rep_off = 0;
+    if (n >= 8 && zf_rd32(d) == ZD_DICT_MAGIC) {
+        R.info.kind = 1; R.info.dict_id = zf_rd32(d + 4);
+        const uint32_t avail = n - 8 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)(n - 8);
+        uint32_t st = ZMT_ST_OK, tb = 0;
+        if (avail == 0) st = ZMT_ST_TRUNCATED;
+        else if (zd_huf_build(W, d + 8, avail, lane, &tb)) st = ZMT_ST_BAD_HEADER;
+        if (lane == 0 && st == ZMT_ST_OK) {
+            uint32_t pos = 8 + tb;
+            uint32_t* const tab[3] = { W.of, W.ml, W.ll };
+            uint32_t* const at[3] = { &R.of_off, &R.ml_off, &R.ll_off };
+            const int maxlog[3] = { 8, 9, 9 }, maxsym[3] = { 31, 52, 35 };
+            R.huf_off = 8;
+            for (uint32_t t = 0; t < 3 && st == ZMT_ST_OK; t++) {
+                *at[t] = pos;
+                int nsym = 0, log = 0;
+                const int used = pos < avail + 8 ? zd_read_ncount(d + pos, avail + 8 - pos, W.norm, &nsym, &log, maxlog[t], maxsym[t]) : -1;
+                if (pos >= avail + 8) st = ZMT_ST_TRUNCATED;
+                else if (used < 0 || !zd_fse_build(tab[t], W.norm, nsym, log)) st = ZMT_ST_BAD_HEADER;
+                else pos += (uint32_t)used;
+            }
+            R.rep_off = pos;
+            if (st == ZMT_ST_OK && (uint64_t)avail + 8 - pos < 12) st = ZMT_ST_TRUNCATED;
+            if (st == ZMT_ST_OK) {
+                const uint64_t content = n - pos - 12;
+                for (uint32_t t = 0; t < 3; t++) {
+                    R.rep[t] = zf_rd32(d + pos + 4 * t);
+                    if (R.rep[t] == 0 || R.rep[t] > content) st = ZMT_ST_BAD_HEADER;     // libzstd: each within the content
+                }
+                R.info.content_off = pos + 12; R.info.content_bytes = content;
+            }
+        }
+        st = __shfl_sync(ZMT_FULL_MASK, st, 0);
+        if (st != ZMT_ST_OK) { R.info.status = st; R.info.content_bytes = 0; }
+    }
+    if (lane == 0) { *out = R; *info = R.info; }
+}
+
 // ================================================================ host side
 static void zd_build_dtable(ZFseDTable& T, const int16_t* norm, int nsym, int log)
 {
@@ -1273,15 +1375,36 @@ static int zd_tables_init()
 // Walk one zstd frame on the host (frame header + 3-byte block headers + the two section headers of every
 // compressed block; zstd_frame_walk in frame_format.h).  `base_off` = offset of the frame's first byte inside the batch
 // input buffer.  Appends block descriptors (scratch offsets assigned from *scratch_used).  Returns ZMT_ST_*.
+// dict: the summary of a loaded dictionary, or nullptr (zmt_zstd_scan_frame_host).
+extern "C" int zmt_zstd_scan_frame_dict_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
+                                             void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
+                                             uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq, const zmt_zstd_dict_info* dict)
+{
+    size_t end = 0;
+    const int r = dict ? zstd_frame_walk<true, true>(frame, n, base_off, frame_idx, (ZBlk*)blocks_out, nblocks_io, max_blocks, scratch_used,
+                                                     content_size, needs_seq, &end, dict)
+                       : zstd_frame_walk<true>(frame, n, base_off, frame_idx, (ZBlk*)blocks_out, nblocks_io, max_blocks, scratch_used, content_size,
+                                               needs_seq, &end);
+    if (r != ZMT_ST_OK) return r;
+    return end == n ? ZMT_ST_OK : ZMT_ST_TRAILING;
+}
+
 extern "C" int zmt_zstd_scan_frame_host(const uint8_t* frame, size_t n, uint64_t base_off, uint32_t frame_idx,
                                         void* blocks_out, uint32_t* nblocks_io, uint32_t max_blocks,
                                         uint64_t* scratch_used, uint64_t* content_size, uint32_t* needs_seq)
 {
-    size_t end = 0;
-    const int r = zstd_frame_walk<true>(frame, n, base_off, frame_idx, (ZBlk*)blocks_out, nblocks_io, max_blocks, scratch_used, content_size,
-                                        needs_seq, &end);
-    if (r != ZMT_ST_OK) return r;
-    return end == n ? ZMT_ST_OK : ZMT_ST_TRAILING;
+    return zmt_zstd_scan_frame_dict_host(frame, n, base_off, frame_idx, blocks_out, nblocks_io, max_blocks, scratch_used, content_size, needs_seq, nullptr);
+}
+
+extern "C" size_t zmt_zstd_ddict_bytes(void) { return sizeof(ZDDict); }
+
+extern "C" int zmt_zstd_ddict_load_device(const void* d_dict, uint64_t dict_bytes, void* d_ddict, zmt_zstd_dict_info* d_info, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!d_ddict || !d_info || (dict_bytes && !d_dict)) return ZMT_ST_BAD_ARG;
+    ZmtProfScope ps(ZMT_K_ZSTD_DECODE, stream);
+    zstd_ddict_load_kernel<<<1, 32, 0, stream>>>((const uint8_t*)d_dict, dict_bytes, (ZDDict*)d_ddict, d_info);
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
 extern "C" size_t zmt_zstd_blk_desc_bytes(void) { return sizeof(ZBlk); }
@@ -1327,10 +1450,11 @@ extern "C" uint32_t zmt_zstd_segment_sources(const zmt_zstd_walk* w, uint64_t* o
 
 // d_blocks: nblocks descriptors (device copy of what zmt_zstd_scan_frame_host produced); d_frame_first_blk: nframes+1;
 // d_expect: content size per frame (from the frame headers).  seg = nullptr: whole frames (zmt_zstd_decompress_device);
-// else every frame of the batch is a segment with its record in seg[f] (zmt_zstd_decompress_segments_device)
+// else every frame of the batch is a segment with its record in seg[f] (zmt_zstd_decompress_segments_device).
+// dd: the loaded dictionary of zmt_zstd_decompress_dict_device, or nullptr.
 static int zstd_decompress_launch(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
                                   const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off,
-                                  uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* seg, void* d_work, void* stream_)
+                                  uint64_t* d_out_size, uint32_t* d_status, zmt_zstd_segment* seg, void* d_work, void* stream_, const ZDDict* dd)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (nframes == 0) return ZMT_ST_OK;
@@ -1352,10 +1476,10 @@ static int zstd_decompress_launch(const void* d_in, const void* d_blocks, uint32
                                                                                            w.seq_done, w.seq_ml, d_status);
         zstd_entropy_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.regen, d_status,
                                                                                            w.seq_done, w.seq_ml, w.lit_done);
-        zstd_entropy_dep_kernel<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.regen,
-                                                                                           d_status, w.lit_done);
-        zstd_resolve_offsets_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, w.scratch, d_status,
-                                                                                                   seg, nframes);
+        (dd ? zstd_entropy_dep_kernel<true> : zstd_entropy_dep_kernel<false>)<<<(nblocks + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>(
+            (const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, d_frame_seq, w.scratch, w.regen, d_status, w.lit_done, dd);
+        (dd ? zstd_resolve_offsets_kernel<true> : zstd_resolve_offsets_kernel<false>)<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>(
+            (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq, w.scratch, d_status, seg, nframes, dd);
         zstd_entropy_seq_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
                                                                                            w.scratch, w.regen, d_status, nframes);
     }
@@ -1366,8 +1490,9 @@ static int zstd_decompress_launch(const void* d_in, const void* d_blocks, uint32
         const uint32_t gneed = (nblocks + ZX_WARPS - 1) / ZX_WARPS;
         cudaMemsetAsync(w.xticket, 0, 8, stream);
         ticket_windows_kernel<<<1, 256, 0, stream>>>(d_frame_first_blk, nframes, w.xwbase);
-        zstd_execute_kernel<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, w.scratch, w.regen, w.blk_out,
-                                                                                     d_out_off, (uint8_t*)d_out, w.done, d_status, w.xticket, d_frame_first_blk, w.xwbase, seg, nframes);
+        (dd ? zstd_execute_kernel<true> : zstd_execute_kernel<false>)<<<gneed < gmax ? gneed : gmax, 32 * ZX_WARPS, 0, stream>>>(
+            (const uint8_t*)d_in, (const ZBlk*)d_blocks, nblocks, w.scratch, w.regen, w.blk_out, d_out_off, (uint8_t*)d_out, w.done, d_status, w.xticket,
+            d_frame_first_blk, w.xwbase, seg, nframes, dd);
         zstd_checksum_kernel<<<(nframes + ZD_WARPS - 1) / ZD_WARPS, 32 * ZD_WARPS, 0, stream>>>((const uint8_t*)d_in, (const ZBlk*)d_blocks, d_frame_first_blk, d_frame_seq,
                                                                                            (const uint8_t*)d_out, d_out_off, (const unsigned long long*)d_out_size, d_status, seg, nframes);
     }
@@ -1379,7 +1504,15 @@ extern "C" int zmt_zstd_decompress_device(const void* d_in, const void* d_blocks
                                           uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream)
 {
     return zstd_decompress_launch(d_in, d_blocks, nblocks, d_frame_first_blk, d_expect, d_frame_seq, nframes, d_out, d_out_off, d_out_size, d_status,
-                                  nullptr, d_work, stream);
+                                  nullptr, d_work, stream, nullptr);
+}
+
+extern "C" int zmt_zstd_decompress_dict_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
+                                               const uint64_t* d_expect, const uint32_t* d_frame_seq, uint32_t nframes, void* d_out, const uint64_t* d_out_off,
+                                               uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream, const void* d_ddict)
+{
+    return zstd_decompress_launch(d_in, d_blocks, nblocks, d_frame_first_blk, d_expect, d_frame_seq, nframes, d_out, d_out_off, d_out_size, d_status,
+                                  nullptr, d_work, stream, (const ZDDict*)d_ddict);
 }
 
 extern "C" int zmt_zstd_decompress_segments_device(const void* d_in, const void* d_blocks, uint32_t nblocks, const uint32_t* d_frame_first_blk,
@@ -1389,5 +1522,5 @@ extern "C" int zmt_zstd_decompress_segments_device(const void* d_in, const void*
 {
     if (!d_seg && nframes) return ZMT_ST_BAD_ARG;
     return zstd_decompress_launch(d_in, d_blocks, nblocks, d_frame_first_blk, d_expect, d_frame_seq, nframes, d_out, d_out_off, d_out_size, d_status,
-                                  d_seg, d_work, stream);
+                                  d_seg, d_work, stream, nullptr);
 }
