@@ -243,6 +243,31 @@ int    zmt_zstd_decompress_dict_device(const void* d_in, const void* d_blocks, u
                                        const uint64_t* d_out_off, uint64_t* d_out_size, uint32_t* d_status, void* d_work, void* stream,
                                        const void* d_ddict);
 
+/* ---- Compressing against a zstd dictionary (levels 6-22) ----
+ * zmt_zstd_cdict_build_device indexes the content of a dictionary that zmt_zstd_ddict_load_device has loaded into
+ * d_ddict, on the same stream: it reads the content's address and size from the record on the device (no round trip),
+ * hashes every position q with q + 5 <= the content's length as the search class hashes a chunk's, sorts them, and
+ * writes the opaque index d_cdict (zmt_zstd_cdict_bytes(dict_bytes) bytes of device memory: a 16 MiB head table,
+ * 4 bytes per dictionary byte for the chains and 16 more plus the sort's scratch while it builds).  dict_bytes is the
+ * size the dictionary was loaded with; 2^31 or more is ZMT_ST_BAD_ARG (zmt_zstd_cdict_bytes returns 0).  An index built
+ * on a record whose load failed is empty and names no Dictionary_ID: the frames are those of the call without a
+ * dictionary (the load's zmt_zstd_dict_info reports the failure).  The index keeps the addresses of the record and of
+ * the dictionary's bytes; both must outlive every call that names it.  Reports under ZMT_K_ZL_HASH / ZMT_K_ZL_SORT.
+ *
+ * zmt_zstd_compress_dict_device is zmt_zstd_compress_level_device with the index: same layout contract, workspace
+ * (zmt_zstdc_level_workspace_bytes at the same level) and output bound.  A chunk's hash chain that runs out with steps
+ * and window left continues through the dictionary's content, which sits before every chunk (zstd_lazy_rule.h): matches
+ * may start up to the window behind the chunk's start and end at the content's end at the latest.  Every offset is
+ * written explicitly and the sequence tables are the predefined ones, so a frame uses only the dictionary's content; a
+ * formatted dictionary's ID (not 0) is named in the frame header in 1, 2 or 4 bytes as libzstd writes it, which
+ * zmt_zstdc_out_bound's per-window slack covers.  Levels 1-5 are ZMT_ST_BAD_ARG (the level-3 class has no chains);
+ * d_cdict = NULL is the call without a dictionary, byte for byte. */
+size_t zmt_zstd_cdict_bytes(uint64_t dict_bytes);
+int    zmt_zstd_cdict_build_device(const void* d_ddict, uint64_t dict_bytes, void* d_cdict, void* stream);
+int    zmt_zstd_compress_dict_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                     uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off,
+                                     void* stream, const void* d_cdict);
+
 /* ---- LZ4F frames of any size in bounded memory ----
  * An LZ4F frame of any size, decoded as a chain of segments, each a run of whole blocks (what LZ4F_decompress does
  * through two fixed buffers when the reference streams a plain .lz4 file, lib/lz4-mt_decompress.c:391-483).  Frame f of

@@ -107,6 +107,10 @@ def lib():
     for k in ("index", "index_plain", "blocks", "decompress"):
         f = getattr(L, "zmt_zstd_%s_dict_device" % k); f.restype = ctypes.c_int
         f.argtypes = getattr(L, "zmt_zstd_%s_device" % k).argtypes + [c_vp]
+    L.zmt_zstd_cdict_bytes.restype = c_sz; L.zmt_zstd_cdict_bytes.argtypes = [c_u64]
+    L.zmt_zstd_cdict_build_device.restype = ctypes.c_int; L.zmt_zstd_cdict_build_device.argtypes = [c_vp, c_u64, c_vp, c_vp]
+    L.zmt_zstd_compress_dict_device.restype = ctypes.c_int
+    L.zmt_zstd_compress_dict_device.argtypes = L.zmt_zstd_compress_level_device.argtypes + [c_vp]
     L.zmt_range_workspace_bytes.restype = c_sz; L.zmt_range_workspace_bytes.argtypes = [c_u32, c_u32]
     L.zmt_lz4_content_offsets_device.restype = ctypes.c_int
     L.zmt_lz4_content_offsets_device.argtypes = [c_vp, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
@@ -342,11 +346,15 @@ class Lz4DeviceCompressor:
 
 class ZstdDeviceCompressor:
     """zmt_zstd_compress_level_device: same layout contract as the LZ4 twin, Zstandard frames out.  Levels 1-5 run the
-    level-3 encoder (zmt_zstd_compress_device), levels 6-22 the hash-chain class with a lazy parse."""
+    level-3 encoder (zmt_zstd_compress_device), levels 6-22 the hash-chain class with a lazy parse.  With a
+    ZstdDictionary (levels 6-22) the chains continue into its content and the frames name its ID
+    (zmt_zstd_compress_dict_device); the dictionary must outlive the compressor, which keeps a reference to it."""
 
-    def __init__(self, in_bytes, chunk, device="cuda", level=3):
+    def __init__(self, in_bytes, chunk, device="cuda", level=3, dictionary=None):
         torch = _torch(); L = lib()
-        self.chunk, self.in_bytes, self.level = chunk, in_bytes, level
+        if dictionary is not None and level < 6:
+            raise ValueError("compressing with a dictionary needs level 6 or above (level %d)" % level)
+        self.chunk, self.in_bytes, self.level, self.dictionary = chunk, in_bytes, level, dictionary
         self.nchunks = L.zmt_chunk_count(in_bytes, chunk)
         wb = L.zmt_zstdc_level_workspace_bytes(self.nchunks, chunk, level)
         if wb == 0:
@@ -355,13 +363,27 @@ class ZstdDeviceCompressor:
         self.out = torch.empty(L.zmt_zstdc_out_bound(self.nchunks, chunk), dtype=torch.uint8, device=device)
         self.frame_off = torch.zeros(self.nchunks + 1, dtype=torch.int64, device=device)
 
-    def run(self, d_in, stream=None):
+    def run(self, d_in, stream=None, chunk_bytes=None):
+        """chunk_bytes: a device uint32 tensor of the chunks' lengths (one per chunk; chunk c starts at c * chunk), for a
+        batch of records in fixed slots."""
         torch = _torch()
         s = stream if stream is not None else torch.cuda.current_stream()
-        rc = lib().zmt_zstd_compress_level_device(d_in.data_ptr(), self.in_bytes, self.chunk, None, self.nchunks, self.level,
-                                                  self.work.data_ptr(), self.out.data_ptr(), self.frame_off.data_ptr(), s.cuda_stream)
+        cb = None
+        if chunk_bytes is not None:
+            if (chunk_bytes.dtype not in (torch.int32, torch.uint32) or not chunk_bytes.is_cuda or not chunk_bytes.is_contiguous()
+                    or chunk_bytes.numel() != self.nchunks):
+                raise ValueError("chunk_bytes: a contiguous device tensor of %d 32-bit lengths" % self.nchunks)
+            cb = chunk_bytes.data_ptr()
+        args = (d_in.data_ptr(), self.in_bytes, self.chunk, cb, self.nchunks, self.level, self.work.data_ptr(), self.out.data_ptr(),
+                self.frame_off.data_ptr(), s.cuda_stream)
+        if self.dictionary is not None:
+            name = "zmt_zstd_compress_dict_device"
+            rc = lib().zmt_zstd_compress_dict_device(*args, self.dictionary.cdict(s).data_ptr())
+        else:
+            name = "zmt_zstd_compress_level_device"
+            rc = lib().zmt_zstd_compress_level_device(*args)
         if rc != 0:
-            raise RuntimeError("zmt_zstd_compress_level_device failed: %s" % ST_NAMES.get(rc, rc))
+            raise RuntimeError("%s failed: %s" % (name, ST_NAMES.get(rc, rc)))
         return self.out, self.frame_off
 
 
@@ -575,7 +597,10 @@ def zstd_decode_segments(frame, cuts, device="cuda"):
 class ZstdDictionary:
     """A zstd dictionary loaded on the device (zmt_zstd_ddict_load_device): `data` (bytes or a uint8 array, formatted or
     raw content) is copied to the device and stays there with the record for as long as this object lives.  .info is
-    the load's summary (DictInfo); a dictionary the load rejects raises ValueError with the status name."""
+    the load's summary (DictInfo); a dictionary the load rejects raises ValueError with the status name.  The
+    compression index (16 MiB and more, zmt_zstd_cdict_build_device) is built on first use by a compressor."""
+
+    _cdict = None
 
     def __init__(self, data, device="cuda", stream=None):
         torch = _torch(); L = lib()
@@ -592,6 +617,21 @@ class ZstdDictionary:
         self.info = DictInfo.from_buffer_copy(d_info.cpu().numpy().tobytes())
         if self.info.status != 0:
             raise ValueError("dictionary rejected: %s" % ST_NAMES.get(self.info.status, self.info.status))
+
+    def cdict(self, stream=None):
+        """The compression index (device uint8 tensor), built on `stream` the first time it is asked for."""
+        if self._cdict is None:
+            torch = _torch(); L = lib()
+            s = stream if stream is not None else torch.cuda.current_stream()
+            nb = L.zmt_zstd_cdict_bytes(self.nbytes)
+            if nb == 0:
+                raise ValueError("no compression index for a dictionary of %d bytes" % self.nbytes)
+            cd = torch.empty(nb, dtype=torch.uint8, device=self.d_ddict.device)
+            rc = L.zmt_zstd_cdict_build_device(self.d_ddict.data_ptr(), self.nbytes, cd.data_ptr(), s.cuda_stream)
+            if rc != 0:
+                raise RuntimeError("zmt_zstd_cdict_build_device failed: %s" % ST_NAMES.get(rc, rc))
+            self._cdict = cd
+        return self._cdict
 
 
 class ZstdDeviceDecompressor:

@@ -3,6 +3,7 @@
   zstdmt_b200/libzstdmt_b200.so   CUDA kernels (sm_90a) + host pipeline + C-ABI   [the product]
   zstdmt_b200/libzmt_datagen.so   synthetic input generator (harness/datagen.c)     [bench / test harness, no dependencies]
   zstdmt_b200/libzmt_memio.so     in-memory fn_read / fn_write drivers of the C-ABI [bench / test harness, links the product]
+  zstdmt_b200/libzlazy_dict_twin.so  CPU twin of the zstd search class against a dictionary   [test infrastructure]
   oracle/liboracle.so             CPU restatement                                  [test infrastructure]
   oracle/libchain_twin.so         CPU twin of the chain-search encoders            [test infrastructure]
   oracle/libzlazy_twin.so,        links to libchain_twin.so under the per-class names that test trees and tools
@@ -20,6 +21,7 @@ LIB = os.path.join(HERE, "libzstdmt_b200.so")
 HSRC = os.path.join(HERE, "harness")
 LIB_GEN = os.path.join(HERE, "libzmt_datagen.so")
 LIB_MEMIO = os.path.join(HERE, "libzmt_memio.so")
+LIB_DICT_TWIN = os.path.join(HERE, "libzlazy_dict_twin.so")
 LIB_TWIN = os.path.join(ROOT, "oracle", "libchain_twin.so")
 LIB_TWIN_NAMES = [os.path.join(ROOT, "oracle", f) for f in ("libzlazy_twin.so", "liblz4hc_twin.so")]
 
@@ -73,7 +75,7 @@ def build_product(force=False, verbose=False, defines=(), out_dir=None):
 
 
 def build_harness(force=False):
-    """The two harness libraries (plain gcc).  libzmt_memio.so resolves LZ4MT_* / ZSTDCB_* from the product library."""
+    """The harness libraries (plain gcc).  libzmt_memio.so resolves LZ4MT_* / ZSTDCB_* from the product library."""
     gen_src, io_src = os.path.join(HSRC, "datagen.c"), os.path.join(HSRC, "memio_glue.c")
     if force or _stale(LIB_GEN, [gen_src]):
         r = subprocess.run(["gcc", "-O3", "-fPIC", "-pthread", "-shared", "-o", LIB_GEN, gen_src, "-lpthread"], cwd=ROOT, capture_output=True, text=True)
@@ -84,6 +86,12 @@ def build_harness(force=False):
                             "-Wl,-rpath,$ORIGIN"], cwd=ROOT, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building libzmt_memio.so")
+    # CPU twin of the zstd search class against a dictionary (shares zstd_lazy_rule.h with the kernels)
+    tw_src = os.path.join(HSRC, "zlazy_dict_twin.c")
+    if force or _stale(LIB_DICT_TWIN, [tw_src, os.path.join(CSRC, "zstd_lazy_rule.h")]):
+        r = subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-Wall", "-o", LIB_DICT_TWIN, tw_src], cwd=ROOT, capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr); raise RuntimeError("gcc failed building libzlazy_dict_twin.so")
 
 
 def build_oracle(force=False):

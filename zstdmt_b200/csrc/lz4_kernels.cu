@@ -670,27 +670,36 @@ lz4_frame_pack_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_
 // (SURVEY.md Appendix A: 28 B5 2F FD A0 <LE32 size> for 1 MiB, 28 B5 2F FD 20 00 01 00 00 for empty input).
 __device__ __forceinline__ uint32_t zstd_fcs_bytes(uint64_t n) { return n <= 255 ? 1u : n <= 65791 ? 2u : 4u; }
 
+// Dictionary_ID field: 1, 2 or 4 bytes for IDs below 256, below 65536, or larger (FHD bits 0-1 = 1, 2, 3), none for ID 0
+__device__ __forceinline__ uint32_t zstd_did_bytes(uint32_t id) { return id == 0 ? 0u : id < 256 ? 1u : id < 65536 ? 2u : 4u; }
+
+// DICT: the frames carry the Dictionary_ID of the index cd (compressed against it, zmt_zstd_compress_dict_device)
+template <bool DICT>
 __global__ void zstd_frame_sizes_kernel(const uint32_t* __restrict__ blk_csize, uint64_t in_bytes, uint32_t chunk_size,
-                                        const uint32_t* __restrict__ chunk_bytes, uint32_t bpc, uint32_t nchunks, uint64_t* __restrict__ frame_size)
+                                        const uint32_t* __restrict__ chunk_bytes, uint32_t bpc, uint32_t nchunks, uint64_t* __restrict__ frame_size,
+                                        const ZlCDict* __restrict__ cd)
 {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= nchunks) return;
     const uint64_t cbytes = zmt_chunk_len(chunk_bytes, c, in_bytes, chunk_size);
     uint64_t sz = 12 + 4 + 1 + zstd_fcs_bytes(cbytes);
+    if (DICT) sz += zstd_did_bytes(cd->dict_id);
     if (cbytes == 0) sz += 3;
     for (uint32_t b = 0; b < bpc; b++) sz += blk_csize[c * bpc + b];
     frame_size[c] = sz;
 }
 
+template <bool DICT>
 __global__ void __launch_bounds__(256)
 zstd_frame_pack_kernel(uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes, uint32_t bpc,
                        const uint8_t* __restrict__ tmp, const uint32_t* __restrict__ blk_csize, const uint64_t* __restrict__ frame_off,
-                       uint8_t* __restrict__ out, uint32_t nblocks)
+                       uint8_t* __restrict__ out, uint32_t nblocks, const ZlCDict* __restrict__ cd)
 {
+    const uint32_t did = DICT ? cd->dict_id : 0u, dl = DICT ? zstd_did_bytes(did) : 0u;
     for (uint32_t blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
         const uint32_t c = blk / bpc, b = blk % bpc;
         const uint64_t cbytes = zmt_chunk_len(chunk_bytes, c, in_bytes, chunk_size);
-        const uint32_t fl = zstd_fcs_bytes(cbytes), hdr = 12 + 4 + 1 + fl;
+        const uint32_t fl = zstd_fcs_bytes(cbytes), hdr = 12 + 4 + 1 + dl + fl;
         uint8_t* f = out + frame_off[c];
         const uint32_t cs = blk_csize[blk];
         if (cs == 0 && b != 0) continue;
@@ -701,9 +710,18 @@ zstd_frame_pack_kernel(uint64_t in_bytes, uint32_t chunk_size, const uint32_t* _
             stg_le32(f, 0x184D2A50u); stg_le32(f + 4, 4); stg_le32(f + 8, (uint32_t)(fsz - 12));
             stg_le32(f + 12, 0xFD2FB528u);
             f[16] = fl == 1 ? 0x20 : fl == 2 ? 0x60 : 0xA0;
-            if (fl == 1) f[17] = (uint8_t)cbytes;
-            else if (fl == 2) { const uint32_t v = (uint32_t)cbytes - 256; f[17] = (uint8_t)v; f[18] = (uint8_t)(v >> 8); }
-            else stg_le32(f + 17, (uint32_t)cbytes);
+            if (!DICT || dl == 0) {
+                if (fl == 1) f[17] = (uint8_t)cbytes;
+                else if (fl == 2) { const uint32_t v = (uint32_t)cbytes - 256; f[17] = (uint8_t)v; f[18] = (uint8_t)(v >> 8); }
+                else stg_le32(f + 17, (uint32_t)cbytes);
+            } else {                                                    // FHD, Dictionary_ID, Frame_Content_Size
+                f[16] |= dl == 1 ? 1 : dl == 2 ? 2 : 3;
+                for (uint32_t k = 0; k < dl; k++) f[17 + k] = (uint8_t)(did >> (8 * k));
+                uint8_t* fcs = f + 17 + dl;
+                if (fl == 1) fcs[0] = (uint8_t)cbytes;
+                else if (fl == 2) { const uint32_t v = (uint32_t)cbytes - 256; fcs[0] = (uint8_t)v; fcs[1] = (uint8_t)(v >> 8); }
+                else stg_le32(fcs, (uint32_t)cbytes);
+            }
             if (cbytes == 0) { f[hdr] = 1; f[hdr + 1] = 0; f[hdr + 2] = 0; }        // empty raw last block
         }
         if (cs) coop_copy_g2g(f + pos, tmp + (uint64_t)blk * ZMT_LZ4_TMP_STRIDE, cs, threadIdx.x, blockDim.x);
@@ -843,11 +861,11 @@ static inline uint32_t zl_group_chunks(uint32_t nchunks, uint32_t chunk_size)
     if (g == 0) g = 1;
     return g < nchunks ? g : nchunks;
 }
-static size_t zl_sort_temp_bytes(uint32_t npos)
+static size_t zl_sort_temp_bytes(uint32_t npos, int end_bit = ZL_HASHLOG)
 {
     size_t t = 0;
     cub::DoubleBuffer<uint32_t> k(nullptr, nullptr), v(nullptr, nullptr);
-    if (cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)npos, 0, ZL_HASHLOG) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)npos, 0, end_bit) != cudaSuccess) { cudaGetLastError(); return 0; }
     return t;
 }
 
@@ -948,9 +966,10 @@ extern "C" uint64_t zmt_zstdc_out_bound(uint32_t nchunks, uint32_t chunk_size)
 // ---------------------------------------------------------------- chain search (zstd_lazy.cuh), shared by both chain classes
 // One group of G chunks at a time: hash every position, radix-sort the (hash, position) pairs, link each position to the
 // previous one with its hash (prev[]), walk the chains into best[], then run the class's block kernel over the group's
-// blocks through blocks(c0, nblk, best).
-template <uint32_t BLK, uint32_t START, uint32_t END, class Blocks>
-static int zl_chain_groups(const ZmtBatch& b, const ZlChainWs& ch, uint32_t min_match, uint32_t depth, uint32_t window, cudaStream_t stream, Blocks blocks)
+// blocks through blocks(c0, nblk, best).  DICT: chains continue into the dictionary's index cd.
+template <uint32_t BLK, uint32_t START, uint32_t END, bool DICT = false, class Blocks>
+static int zl_chain_groups(const ZmtBatch& b, const ZlChainWs& ch, uint32_t min_match, uint32_t depth, uint32_t window, cudaStream_t stream, Blocks blocks,
+                           const ZlCDict* cd = nullptr)
 {
     for (uint32_t c0 = 0; c0 < b.nchunks; c0 += b.G) {
         const uint32_t ng = b.nchunks - c0 < b.G ? b.nchunks - c0 : b.G;
@@ -971,8 +990,8 @@ static int zl_chain_groups(const ZmtBatch& b, const ZlChainWs& ch, uint32_t min_
             }
             zmt_dbg_check(stream, "zstd_lazy sort + prev");
             { ZmtProfScope ps(ZMT_K_ZL_SEARCH, stream);
-            zstd_lazy_search_kernel<BLK, START, END><<<g, 256, 0, stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, c0, np, min_match, depth, window,
-                                                                            V.Alternate(), K.Alternate()); }
+            zstd_lazy_search_kernel<BLK, START, END, DICT><<<g, 256, 0, stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, c0, np, min_match, depth,
+                                                                                  window, V.Alternate(), K.Alternate(), cd); }
             zmt_dbg_check(stream, "zstd_lazy_search_kernel");
         }
         blocks(c0, ng * b.bpc, K.Alternate());
@@ -1054,25 +1073,28 @@ extern "C" int zmt_lz4_compress_device(const void* d_in, uint64_t in_bytes, uint
 }
 
 // ---------------------------------------------------------------- zstd compress, levels 1-22 (levels 6-22: zstd_lazy.cuh)
-// frame sizes -> frame offsets -> pack
-static int zstd_frame_tail(const ZmtBatch& b, const ZstdWs& w, uint8_t* out, uint64_t* frame_off, cudaStream_t stream)
+// frame sizes -> frame offsets -> pack; DICT: the frames name the Dictionary_ID of cd
+template <bool DICT>
+static int zstd_frame_tail(const ZmtBatch& b, const ZstdWs& w, uint8_t* out, uint64_t* frame_off, cudaStream_t stream, const ZlCDict* cd)
 {
-    zstd_frame_sizes_kernel<<<(b.nchunks + 255) / 256, 256, 0, stream>>>(w.blk_csize, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, b.nchunks, w.frame_size);
+    zstd_frame_sizes_kernel<DICT><<<(b.nchunks + 255) / 256, 256, 0, stream>>>(w.blk_csize, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, b.nchunks,
+                                                                               w.frame_size, cd);
     zmt_dbg_check(stream, "zstd_frame_sizes_kernel");
     scan_u64_kernel<<<1, 1024, 0, stream>>>(w.frame_size, frame_off, b.nchunks);
     zmt_dbg_check(stream, "scan_u64_kernel");
     const uint32_t maxp = (uint32_t)(zmt_sm_count() * 16);
     { ZmtProfScope ps(ZMT_K_ZSTD_PACK, stream);
-    zstd_frame_pack_kernel<<<b.nblocks < maxp ? b.nblocks : maxp, 256, 0, stream>>>(b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, w.tmp, w.blk_csize, frame_off,
-                                                                                   out, b.nblocks); }
+    zstd_frame_pack_kernel<DICT><<<b.nblocks < maxp ? b.nblocks : maxp, 256, 0, stream>>>(b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, w.tmp, w.blk_csize,
+                                                                                         frame_off, out, b.nblocks, cd); }
     zmt_dbg_check(stream, "zstd_frame_pack_kernel");
     return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
-extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
-                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+// DICT: levels 6-22 only, their chains continuing into the dictionary's index cd
+template <bool DICT>
+static int zstd_compress(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes, uint32_t nchunks, int level,
+                         void* d_work, void* d_out, uint64_t* d_frame_off, cudaStream_t stream, const ZlCDict* cd)
 {
-    cudaStream_t stream = (cudaStream_t)stream_;
     const bool chain = level >= ZL_MIN_LEVEL;
     ZmtBatch b;
     int st = zmt_batch(b, d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, chain);
@@ -1089,16 +1111,78 @@ extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_byte
     } else {
         const ZlParams P = zl_params(level);
         cudaFuncSetAttribute(zstd_lazy_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZlSmem));
-        st = zl_chain_groups<ZL_BLOCK, 0, 0>(b, w.ch, P.min_match, P.depth, zl_window(level), stream,
+        st = zl_chain_groups<ZL_BLOCK, 0, 0, DICT>(b, w.ch, P.min_match, P.depth, zl_window(level), stream,
             [&](uint32_t c0, uint32_t nwin, const uint32_t* best) {
                 { ZmtProfScope ps(ZMT_K_ZL_BLOCKS, stream);
                 zstd_lazy_blocks_kernel<<<zstd_grid(nwin), 256, sizeof(ZlSmem), stream>>>(b.in, b.in_bytes, b.chunk_size, b.chunk_bytes, b.bpc, c0, nwin, P.lazy,
                                                                                            best, w.tmp, w.blk_csize, w.zsc); }
                 zmt_dbg_check(stream, "zstd_lazy_blocks_kernel");
-            });
+            }, cd);
         if (st != ZMT_ST_OK) return st;
     }
-    return zstd_frame_tail(b, w, (uint8_t*)d_out, d_frame_off, stream);
+    return zstd_frame_tail<DICT>(b, w, (uint8_t*)d_out, d_frame_off, stream, cd);
+}
+
+extern "C" int zmt_zstd_compress_level_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                              uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_)
+{
+    return zstd_compress<false>(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, level, d_work, d_out, d_frame_off, (cudaStream_t)stream_, nullptr);
+}
+
+extern "C" int zmt_zstd_compress_dict_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,
+                                             uint32_t nchunks, int level, void* d_work, void* d_out, uint64_t* d_frame_off, void* stream_,
+                                             const void* d_cdict)
+{
+    if (level < ZL_MIN_LEVEL) return ZMT_ST_BAD_ARG;        // the level-3 class has no chains to continue
+    const ZlCDict* cd = (const ZlCDict*)d_cdict;
+    return cd ? zstd_compress<true>(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, level, d_work, d_out, d_frame_off, (cudaStream_t)stream_, cd)
+              : zstd_compress<false>(d_in, in_bytes, chunk_size, d_chunk_bytes, nchunks, level, d_work, d_out, d_frame_off, (cudaStream_t)stream_, nullptr);
+}
+
+// ---- a dictionary's compression index (ZlCDict, zstd_lazy.cuh): the header, head[], prev[] and the sort's pairs and
+// scratch over dict_bytes positions
+#define ZL_CDICT_KEY_BITS (ZL_HASHLOG + 1)          // the hashes and the key of unlinked positions
+struct ZlCDictWs { ZlCDict* hdr; uint32_t* head; uint32_t* prev; uint32_t* arr[4]; void* sort_tmp; size_t sort_cap; };
+static uint64_t zl_cdict_layout(uint8_t* base, uint32_t n, ZlCDictWs& w)
+{
+    ZmtCarve c{base, 0};
+    w.hdr = c.take<ZlCDict>(a256(sizeof(ZlCDict)));
+    w.head = c.take<uint32_t>(4ull << ZL_HASHLOG);
+    w.prev = c.take<uint32_t>(a256(4ull * n));
+    for (int k = 0; k < 4; k++) w.arr[k] = c.take<uint32_t>(a256(4ull * n));
+    w.sort_cap = n ? zl_sort_temp_bytes(n, ZL_CDICT_KEY_BITS) : 0;
+    w.sort_tmp = c.take<void>(a256(w.sort_cap));
+    return c.off;
+}
+
+extern "C" size_t zmt_zstd_cdict_bytes(uint64_t dict_bytes)
+{
+    if (dict_bytes >= (1ull << 31)) return 0;
+    ZlCDictWs w;
+    return (size_t)zl_cdict_layout(nullptr, (uint32_t)dict_bytes, w);
+}
+
+extern "C" int zmt_zstd_cdict_build_device(const void* d_ddict, uint64_t dict_bytes, void* d_cdict, void* stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!d_ddict || !d_cdict || dict_bytes >= (1ull << 31)) return ZMT_ST_BAD_ARG;
+    const uint32_t n = (uint32_t)dict_bytes, mm = zl_params(ZL_MIN_LEVEL).min_match, g = (n + 255) / 256;
+    const ZDDict* dd = (const ZDDict*)d_ddict;
+    ZlCDictWs w;
+    zl_cdict_layout((uint8_t*)d_cdict, n, w);
+    if (cudaMemsetAsync(w.head, 0xFF, 4ull << ZL_HASHLOG, stream) != cudaSuccess) return ZMT_ST_CUDA;
+    if (n) {
+        cub::DoubleBuffer<uint32_t> K(w.arr[0], w.arr[1]), V(w.arr[2], w.arr[3]);
+        { ZmtProfScope ps(ZMT_K_ZL_HASH, stream);
+        zl_cdict_hash_kernel<<<g, 256, 0, stream>>>(dd, n, mm, K.Current(), V.Current()); }
+        ZmtProfScope ps(ZMT_K_ZL_SORT, stream);
+        size_t tb = 0;
+        if (cub::DeviceRadixSort::SortPairs(nullptr, tb, K, V, (int)n, 0, ZL_CDICT_KEY_BITS, stream) != cudaSuccess || tb > w.sort_cap) return ZMT_ST_CUDA;
+        if (cub::DeviceRadixSort::SortPairs(w.sort_tmp, tb, K, V, (int)n, 0, ZL_CDICT_KEY_BITS, stream) != cudaSuccess) return ZMT_ST_CUDA;
+        zl_cdict_link_kernel<<<g, 256, 0, stream>>>(K.Current(), V.Current(), n, w.head, w.prev);
+    }
+    zl_cdict_header_kernel<<<1, 1, 0, stream>>>(dd, mm, w.head, w.prev, w.hdr);
+    return cudaGetLastError() == cudaSuccess ? ZMT_ST_OK : ZMT_ST_CUDA;
 }
 
 extern "C" int zmt_zstd_compress_device(const void* d_in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* d_chunk_bytes,

@@ -1,5 +1,6 @@
 // zstd_lazy.cuh — the zstd search class of levels 6-12: hash chains over the whole chunk and a lazy parse
-// (rule: zstd_lazy_rule.h; CPU twin: oracle/chain_twin.c).  Included by lz4_kernels.cu after the level-3 encoder;
+// (rule: zstd_lazy_rule.h; CPU twins: oracle/chain_twin.c, and harness/zlazy_dict_twin.c against a dictionary).
+// Included by lz4_kernels.cu after the level-3 encoder;
 // it feeds the same entropy stage (z_encode_block) and the same frame kernels.
 //
 // Per group of chunks (at most ZL_GROUP_BYTES of positions, so the per-position arrays stay bounded):
@@ -54,13 +55,72 @@ __device__ __forceinline__ uint32_t zl_ld32(const uint8_t* p)
     return sh ? __funnelshift_r(lo, __ldg(w + 1), sh) : lo;
 }
 
+// ---- a dictionary's compression index (zmt_zstd_cdict_build_device): the chains of its content, hashed as a chunk's
+// positions are.  Position q of the content is linked when q + min_match <= its length; a chunk's chain that runs off the
+// chunk's start continues at head[h(p)] and through prev[] (the rule: zstd_lazy_rule.h).
+struct ZlCDict {
+    uint32_t status;            // the load's status; anything but ZMT_ST_OK leaves the index empty and dict_id 0
+    uint32_t dict_id;           // what the frames name (0: raw content, no Dictionary_ID field)
+    uint32_t min_match;         // the hash the chains were built with
+    uint32_t pad;
+    uint64_t content_bytes;     // dlen; 0 for an empty index
+    const uint8_t* content;     // the content, inside the caller's dictionary buffer
+    const ZDDict* ddict;        // the loaded record the index was built from
+    const uint32_t* head;       // [1 << ZL_HASHLOG] the largest linked position per hash, ZL_NONE where none
+    const uint32_t* prev;       // per position: the next smaller linked position with the same hash, ZL_NONE at the end
+};
+
+// one thread per position below dict_bytes (the content's size is only known on the device): key h(q) for a linked
+// position, 1 << ZL_HASHLOG (outside every hash) for the rest, so they never join a chain
+__global__ void __launch_bounds__(256)
+zl_cdict_hash_kernel(const ZDDict* __restrict__ dd, uint32_t n, uint32_t mm, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t dlen = dd->info.status == ZMT_ST_OK ? dd->info.content_bytes : 0;
+    uint32_t h = 1u << ZL_HASHLOG;
+    if ((uint64_t)i + mm <= dlen) {
+        const uint8_t* p = (const uint8_t*)dd->dict + dd->info.content_off + i;
+        uint64_t v = 0;
+        for (uint32_t k = 0; k < mm; k++) v |= (uint64_t)p[k] << (8 * k);
+        h = zl_hash(v, mm);
+    }
+    keys[i] = h; vals[i] = i;
+}
+
+// over the sorted pairs: prev[] from the neighbour with the same key, head[] from the last position of each run
+__global__ void __launch_bounds__(256)
+zl_cdict_link_kernel(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t n, uint32_t* __restrict__ head,
+                     uint32_t* __restrict__ prev)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = keys[i];
+    if (k >> ZL_HASHLOG) { prev[vals[i]] = ZL_NONE; return; }
+    prev[vals[i]] = (i && keys[i - 1] == k) ? vals[i - 1] : ZL_NONE;
+    if (i + 1 == n || keys[i + 1] != k) head[k] = vals[i];
+}
+
+__global__ void zl_cdict_header_kernel(const ZDDict* __restrict__ dd, uint32_t mm, const uint32_t* head, const uint32_t* prev, ZlCDict* __restrict__ cd)
+{
+    const bool ok = dd->info.status == ZMT_ST_OK;
+    ZlCDict h;
+    h.status = dd->info.status; h.dict_id = ok ? dd->info.dict_id : 0; h.min_match = mm; h.pad = 0;
+    h.content_bytes = ok ? dd->info.content_bytes : 0;
+    h.content = (const uint8_t*)dd->dict + dd->info.content_off;
+    h.ddict = dd; h.head = head; h.prev = prev;
+    *cd = h;
+}
+
 // BLK: the parse unit (zstd: 16 KiB blocks, LZ4: 64 KiB blocks).  START: a match starts at o only if o + START <= the
 // block's end (0: o + mm, the zstd rule; LZ4: 12).  END: matches end at or before the block's end - END (zstd 0, LZ4 5).
-template <uint32_t BLK, uint32_t START, uint32_t END>
+// DICT (zstd only): a chain that runs off the chunk's start with steps and window left continues through the
+// dictionary's index cd.
+template <uint32_t BLK, uint32_t START, uint32_t END, bool DICT = false>
 __global__ void __launch_bounds__(256)
 zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint32_t chunk_size, const uint32_t* __restrict__ chunk_bytes,
                         uint32_t c0, uint32_t npos, uint32_t mm, uint32_t depth, uint32_t W,
-                        const uint32_t* __restrict__ prev, uint32_t* __restrict__ best)
+                        const uint32_t* __restrict__ prev, uint32_t* __restrict__ best, const ZlCDict* __restrict__ cd)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npos) return;
@@ -73,8 +133,8 @@ zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint3
         const uint8_t* base = in + (uint64_t)c * chunk_size;
         const uint8_t* ps = base + o;
         const uint32_t cs0 = i - o;              // group-relative start of the chunk
-        uint32_t bl = 0, bo = 0, q = prev[i];
-        for (uint32_t step = 0; step < depth && q != ZL_NONE && q >= cs0 && i - q <= W; step++, q = prev[q]) {
+        uint32_t bl = 0, bo = 0, q = prev[i], step = 0;
+        for (; step < depth && q != ZL_NONE && q >= cs0 && i - q <= W; step++, q = prev[q]) {
             const uint8_t* qs = base + (q - cs0);
             if (bl && qs[bl] != ps[bl]) continue;                       // cannot be longer than the best so far
             uint32_t l = 0;
@@ -85,6 +145,27 @@ zstd_lazy_search_kernel(const uint8_t* __restrict__ in, uint64_t in_bytes, uint3
                 l += 4;
             }
             if (l >= mm && l > bl) { bl = l; bo = i - q; if (l == cap) break; }
+        }
+        // the chunk's chain ran out (not the depth, the window or a match at the cap): on into the dictionary, where
+        // candidate q lies o + dlen - q back and its match ends at the content's end at the latest
+        if (DICT && step < depth && (q == ZL_NONE || q < cs0) && cd->content_bytes && cd->min_match == mm) {
+            const uint32_t dlen = (uint32_t)cd->content_bytes;
+            const uint8_t* dc = cd->content;
+            uint64_t v = 0;
+            for (uint32_t k = 0; k < mm; k++) v |= (uint64_t)ps[k] << (8 * k);
+            for (q = cd->head[zl_hash(v, mm)]; step < depth && q != ZL_NONE && (uint64_t)o + dlen - q <= W; step++, q = cd->prev[q]) {
+                const uint8_t* qs = dc + q;
+                const uint32_t qcap = dlen - q < cap ? dlen - q : cap;
+                if (bl && (bl >= qcap || qs[bl] != ps[bl])) continue;   // cannot be longer (and qs[bl] may lie past the content)
+                uint32_t l = 0;
+                for (;;) {
+                    if (l + 4 > qcap) { while (l < qcap && qs[l] == ps[l]) l++; break; }
+                    const uint32_t x = zl_ld32(qs + l) ^ zl_ld32(ps + l);
+                    if (x) { l += (uint32_t)(__ffs(x) - 1) >> 3; break; }
+                    l += 4;
+                }
+                if (l >= mm && l > bl) { bl = l; bo = o + dlen - q; if (l == cap) break; }    // the position's cap ends the walk
+            }
         }
         res = bl ? bl | (bo << ZL_LEN_BITS) : 0;
     }

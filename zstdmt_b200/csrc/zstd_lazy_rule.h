@@ -12,6 +12,17 @@
  *   parse   : at a free position p with a match m = best[p]: a literal if gain(best[p+1]) > gain(m) + 4, or, at lazy
  *             depth 2, gain(best[p+2]) > gain(m) + 7; else take m.  gain(m) = 4 len - highbit32(off + 3).
  *   merge   : a sequence with literal length 0 and the offset of the sequence before it is folded into that one.
+ * With a dictionary whose content D is dlen bytes (zmt_zstd_compress_dict_device), the chains run over D ‖ chunk:
+ *   linked  : dictionary position q is in a chain only if q + minMatch <= dlen (no hash spans into the chunk);
+ *   walk    : a chunk position's chain walks the chunk as above; when it runs out, it continues at the largest linked q
+ *             with h(q) == h(p), then through the earlier dictionary positions with that hash.  `depth` counts chunk
+ *             and dictionary steps together;
+ *   distance: p + dlen - q for a dictionary candidate; the walk goes on while it is <= W;
+ *   length  : a dictionary candidate's is capped at min(ZL_LCAP, blockEnd - p, dlen - q) (its match ends at the
+ *             dictionary's end); the walk stops early only on a match of the position's cap min(ZL_LCAP, blockEnd - p);
+ *   ties    : the first candidate met, as above (the smallest distance).
+ * The frame stays single-segment with Frame_Content_Size; a formatted dictionary's ID (not 0) is named in 1, 2 or 4
+ * bytes (IDs < 256, < 65536, larger; FHD bits 0-1 = 1, 2, 3), raw content (ID 0) in none.
  */
 #ifndef ZSTD_LAZY_RULE_H
 #define ZSTD_LAZY_RULE_H
